@@ -1,9 +1,13 @@
 #!/usr/bin/env python
-"""bench.py — hash-join probe rows/sec (BASELINE.json metric) on 1..N B200s.
+"""bench.py — hash-join probe rows/sec (BASELINE.json metric) on 1..N H100s.
 
   python bench.py --gpus 1 --steps K --warmup W                       (N = 1)
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...   (N > 1)
   python bench.py --impl reference ...      the reference algorithm's CPU restatement on the host cores
+  --dump-outputs DIR                         (N = 1) after the timed steps, write what the last timed step computed as
+                                             DIR/<column>.npy (float64, rows in a canonical order, a fixed sample of
+                                             at most 1 Mi rows; join keys as their ids, key * ODD^-1, which float64 holds
+                                             exactly): two builds run with the same arguments compare row for row
 
 N = 1 workload = BASELINE.json configs[1]: hash join 100M ⋈ 10M int64 keys, 8-byte payload, 100 % match,
 output (probe.k, probe.v, build.k, build.v).  A step = one pass of the probe over the whole 100M-row
@@ -42,6 +46,8 @@ sys.path.insert(0, ROOT)
 import numpy as np
 
 ODD = 0x9E3779B97F4A7C15 - (1 << 64)   # odd 64-bit multiplier (as int64): a bijection, keys are unique but not dense
+ODD_INV = pow(ODD % (1 << 64), -1, 1 << 64)
+ODD_INV -= (1 << 64) if ODD_INV >= (1 << 63) else 0   # key * ODD_INV = the key's id (mod 2^64), exact in float64
 BYTES_PER_PROBE_ROW = 64                # SURVEY §8(d): 16 read + 16 gathered + 32 written at 100 % match
 
 
@@ -52,7 +58,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -154,6 +160,24 @@ class ClockSampler:
                     reasons.add(nm)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "samples": len(sm), "reasons": sorted(reasons)}
+
+
+DUMP_ROWS = 1 << 20   # rows kept per dumped column: 4 columns x 1 Mi rows x 8 B = 32 MiB
+
+
+def dump_outputs(out_dir, cols, order_key, rows):
+    """--dump-outputs: writes the result columns `cols` (name -> 1-D device tensor, one entry per result row) as float64
+    DIR/<name>.npy, plus the result row count as output_rows.npy.  Kernels emit rows in a nondeterministic order, so the rows
+    are put in the order of `order_key` (unique per row) first; a longer result is reduced to DUMP_ROWS evenly spaced rows
+    of that order, the same rows in every run with the same arguments."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    order = torch.argsort(order_key)
+    if order.numel() > DUMP_ROWS:
+        order = order[torch.arange(DUMP_ROWS, device=order.device) * (order.numel() - 1) // (DUMP_ROWS - 1)]   # exact int64 spacing
+    for name, t in cols.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t[order].to(torch.float64).cpu().numpy())
+    np.save(os.path.join(out_dir, "output_rows.npy"), np.array([rows], dtype=np.float64))
 
 
 def make_plan(device: int, stream: int):
@@ -268,7 +292,7 @@ def run_reference(args):
                                 f"hash join {args.probe_rows}x{nb} int64 keys (the GPU arm's partitioned join over {world} GPUs, "
                                 f"{args.probe_rows // world}x{nb // world} per GPU), 8-byte payload, 100% match, in ONE host process "
                                 f"(BASELINE configs[4] / 8 per GPU" + ("" if world != 8 else " = the 1Bx100M join") + ")"),
-                   "note": "CPU restatement of TiDB's HashJoinV2 algorithm (oracle/join.cpp), NOT the Go binary: no Go toolchain in this image"
+                   "note": "CPU restatement of TiDB's HashJoinV2 algorithm (oracle/join.cpp), NOT the Go binary: the project has no Go toolchain"
                            + ("; " + note_mem if note_mem else "")},
         "cpu_baseline": {"value": rate, "unit": "rows/s", "cores": threads, "kind": "port",
                          "sample": f"full {nb}-row build ({bsec:.2f}s, untimed) + probe of {sample} rows as 1024-row chunks per step"},
@@ -383,7 +407,7 @@ def run_gpu(args):
     mail_timings = {}
     MAIL_CANDIDATES = {"mail": dict(dma=False, ctas_per_sm=args.scatter_ctas), "mail-dma": dict(dma=True, ctas_per_sm=args.scatter_ctas, copy_streams=args.copy_streams, direct_peers=args.direct_peers),
                        "mail-smcopy": dict(dma=True, ctas_per_sm=args.scatter_ctas, sm_copy=True, sm_copy_ctas=args.sm_copy_ctas),
-                       "mail-hybrid": dict(dma=True, ctas_per_sm=args.scatter_ctas, copy_streams=args.copy_streams, direct_peers=1)}   # measured at 8 GPUs: 1 direct peer 4.07 ms, 2: 4.21, 3: 4.42, 0 (copy engines only): 4.69
+                       "mail-hybrid": dict(dma=True, ctas_per_sm=args.scatter_ctas, copy_streams=args.copy_streams, direct_peers=1)}
 
     def mail_step(xm, sync: bool):
         """ALL SM kernels of a rank on ONE stream, in the order regroup(k+1), probe(k): the shared-memory-heavy scatter never
@@ -414,7 +438,7 @@ def run_gpu(args):
 
     if world > 1 and args.exchange in ("mail", "mail-dma", "mail-hybrid", "mail-smcopy", "auto"):
         from tidb_b200.parallel import MailboxExchange
-        names = ["mail-dma", "mail-hybrid", "mail"] if args.exchange == "auto" else [args.exchange]   # mail-smcopy measured slower (4.75 vs 3.45 ms at N = 2): explicit only
+        names = ["mail-dma", "mail-hybrid", "mail"] if args.exchange == "auto" else [args.exchange]   # mail-smcopy: explicit only
         timings = {}
         for nm in names:
             xm = MailboxExchange(rank, world, local, xstream, 2, npb, slack=args.slack, **MAIL_CANDIDATES[nm])
@@ -507,6 +531,7 @@ def run_gpu(args):
     stream.synchronize()
 
     # ---- timed region: value (device resident) ----------------------------------------------------------------
+    last_out = None
     sampler = ClockSampler(local)
     l0 = join.stats().kernel_launches
     lx0 = (sum(x.launches for x in xch_p) if xch_p else 0) + (xseg.launches if xseg else 0) + (xmail.launches if xmail else 0)
@@ -518,8 +543,11 @@ def run_gpu(args):
         ev0.record(stream)
         if xstream is not None:
             xstream.wait_event(ev0)
-        for _ in range(args.steps):
-            step(False)
+        for s in range(args.steps):
+            if world == 1 and s == args.steps - 1:
+                last_out = join.probe([pk, pv], sync=True)   # the same step; like a caller's call it also returns the row count
+            else:
+                step(False)
         if xmail is not None:
             mail_drain(xmail)
         ev1.record(stream)
@@ -542,15 +570,18 @@ def run_gpu(args):
         xmail.check()
     launches = (join.stats().kernel_launches - l0) + (launches_extra - lx0)
     value = npb * world / (ms_step * 1e-3)
+    if args.dump_outputs:   # before anything else probes: the library reuses its output buffers
+        rows_d, cols_d, _ = last_out
+        o_pk, o_pv, o_bk, o_bv = [dview(p, rows_d) for p in cols_d]
+        with torch.cuda.stream(stream):
+            dump_outputs(args.dump_outputs, {"probe_key_id": o_pk * ODD_INV, "probe_payload": o_pv, "build_key_id": o_bk * ODD_INV,
+                                             "build_payload": o_bv}, o_pv, rows_d)
+        stream.synchronize()
+    l2_mb = torch.cuda.get_device_properties(dev).L2_cache_size / 1e6
 
     # kernel-only duration for the roofline at N = 1 (the step IS the probe kernel + an 8-byte memset)
     roof = None
     traffic = args.ncu_traffic_bytes
-    if traffic is None:
-        try:   # per-launch DRAM bytes of the committed ncu --set full capture of this kernel
-            traffic = float(json.load(open(os.path.join(ROOT, "profiles", "r2_pipeline_traffic.json" if os.environ.get("TG_PROBE_PARTITION", "1") == "1" else "r1_probe_final_traffic.json")))["dram_bytes_per_launch"])
-        except Exception:
-            traffic = None
     if world == 1:
         achieved = BYTES_PER_PROBE_ROW * npb / (ms_step * 1e-3) / 1e9
         roof = {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
@@ -569,8 +600,8 @@ def run_gpu(args):
                 "traffic": None, "peak_source": peak_src + f" x {world} GPUs",
                 "kernel": "per rank and step: k_partition_scatter_bulk<0,2,4> (repartition + NVLink bulk stores) | k_partition_scatter_bulk<1,2,4> + k_probe_inner_u1_seg_lean<1,2,1,0> (L2 pass + segment probe)",
                 "algorithmic_bytes_per_launch": BYTES_PER_PROBE_ROW * npb * world,
-                "nvlink": {"payload_gbs_per_direction_per_gpu": nvl, "reference_gbs": 770.0, "frac": nvl / 770.0,
-                           "note": "16 B per exchanged row; reference = measured peer-copy bandwidth per direction (B200_PROFILING.md)"}}
+                "nvlink": {"payload_gbs_per_direction_per_gpu": nvl, "reference_gbs": 450.0, "frac": nvl / 450.0,
+                           "note": "16 B per exchanged row; reference = H100 SXM data sheet NVLink bandwidth per direction (900 GB/s bidirectional), not measured"}}
 
     # ---- side line (N = 1): the 50 % match variant of the same workload (SURVEY 8d input 2) ---------------------------
     side50 = None
@@ -612,7 +643,7 @@ def run_gpu(args):
             e2e = (run_e2e_mail(args, torch, dist, dev, stream, xstream, rank, world, pk, pv, xmail, join, barrier, dview) if xmail is not None else
                    run_e2e_multi(args, torch, dist, dev, stream, xstream, rank, world, pk, pv, xch_p, bounds, join, barrier))
 
-    # ---- CPU baseline (rank 0, N = 1 only): bounded sample on the box's host cores ------------------------------
+    # ---- CPU baseline (rank 0, N = 1 only): bounded sample on the machine's host cores ------------------------------
     cpu = None
     if world == 1 and not args.skip_cpu:
         sample = min(npb, args.cpu_sample_rows)
@@ -638,7 +669,7 @@ def run_gpu(args):
             "config": {"workload": (f"hash join {npb}x{nb} int64 keys, 8-byte payload, 100% match, output 4 columns (BASELINE configs[1])" if world == 1 else
                                     f"partitioned hash join {npb * world}x{nb * world} int64 keys over {world} GPUs ({npb}x{nb} per GPU, keys uniform over the global key set), "
                                     f"8-byte payload, 100% match, output 4 columns, key-hash exchange over NVLink every step (BASELINE configs[4] / 8 per GPU" + ("" if world != 8 else " = the 1Bx100M join") + ")"),
-                       "l2": "inputs larger than L2 (1.6 GB probe columns + 3.2 GB output + %.0f MB table per step vs 126 MB L2)" % (bstats.table_slots * 16 / 1e6),
+                       "l2": "inputs larger than L2 (1.6 GB probe columns + 3.2 GB output + %.0f MB table per step vs %.0f MB L2)" % (bstats.table_slots * 16 / 1e6, l2_mb),
                        "table": {"slots": bstats.table_slots, "mode": bstats.table_mode, "distinct_keys": bstats.distinct_keys, "build_ms": bstats.build_ms},
                        "exchange": "none" if world == 1 else {"mail": f"MailboxExchange ({mail_choice}): k_partition_scatter_bulk appends to this rank's fixed-capacity region on every peer with bulk stores over NVLink (tg_partition_exchange_cf_ex), counts and buffer-reuse ACKs through device mailboxes (tg_mail_signal / tg_mail_wait): no NCCL, no copy engine, no host wait in a step; exchange stream one step ahead of the probe stream; segmented probe (tg_join_probe_dev_seg)",
                                                                     "cf": "count-free: k_partition_scatter_bulk appends to this rank's fixed-capacity region on every peer over NVLink (tg_partition_exchange_cf), one all-gather of the counts per step, segmented probe (tg_join_probe_dev_seg)",
@@ -883,8 +914,8 @@ def run_e2e_mail(args, torch, dist, dev, stream, xstream, rank, world, pk, pv, x
 # ---------------------------------------------------------------------------------------------------------
 def run_agg(args):
     """Same JSON contract as the join line, metric = aggregated input rows/sec.  A step = one whole aggregation (table
-    init + update + finalize) of the 100M-row batch.  roofline: 16.24 algorithmic bytes per row (SURVEY 8d) over the HBM peak,
-    plus the measured L2-operation floor of this access pattern (profiles/r2_agg_lab.md) as `l2_op_floor_ms`."""
+    init + update + finalize) of the 100M-row batch.  roofline: 16.24 algorithmic bytes per row (SURVEY 8d) over the HBM peak
+    (tools/scratch/agg_lab.cu measures the L2-operation floor of this access pattern)."""
     os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
     import torch
     from tidb_b200 import abi
@@ -914,7 +945,8 @@ def run_agg(args):
         o = _A(); o.__cuda_array_interface__ = {"shape": (m,), "typestr": dt, "data": (p, False), "version": 3}
         return torch.as_tensor(o, device=dev)
 
-    def one(verify=False):
+    def one(verify=False, keep=False):
+        """one whole aggregation; keep=True leaves the handle open and returns it with its result"""
         agg = DeviceAgg(plan)
         with torch.cuda.stream(stream):
             agg.push([keys, x])
@@ -926,6 +958,8 @@ def run_agg(args):
                 exp = torch.zeros(G, dtype=torch.float64, device=dev).scatter_add_(0, keys, x)
                 assert torch.allclose(s_, exp[gk], rtol=1e-6, atol=0)
         st = agg.stats()
+        if keep:
+            return st, agg, rows, cols
         agg.close()
         return st
     for _ in range(max(3, args.warmup) - 1):
@@ -936,13 +970,23 @@ def run_agg(args):
     launches = 0
     with torch.cuda.stream(stream):
         e0.record(stream)
-    for _ in range(args.steps):
-        launches += one().kernel_launches
+    for i in range(args.steps):
+        if i == args.steps - 1:   # the last handle is closed after the timed region, with or without --dump-outputs
+            st, last_agg, rows, cols = one(keep=True)
+        else:
+            st = one()
+        launches += st.kernel_launches
     with torch.cuda.stream(stream):
         e1.record(stream)
     stream.synchronize()
     clocks = sampler.stop()
     ms = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs:
+        gk = view(cols[0], rows, "<i8")
+        with torch.cuda.stream(stream):
+            dump_outputs(args.dump_outputs, {"group_key": gk, "sum": view(cols[1], rows, "<f8"), "count": view(cols[2], rows, "<i8")}, gk, rows)
+        stream.synchronize()
+    last_agg.close()
     # e2e: host chunks through tg_agg_push / tg_agg_next (pinned host memory in, host result out)
     e2e = None
     if not args.skip_e2e:
@@ -981,13 +1025,13 @@ def run_agg(args):
     line = {"metric": "hash-agg input rows/sec", "value": n / (ms * 1e-3), "unit": "rows/s", "n_gpus": 1, "steps": args.steps, "warmup": max(3, args.warmup),
             "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": {"workload": f"HashAggExec SUM/COUNT GROUP BY int64, {n} rows / {G} groups, 1 GPU (BASELINE configs[2])",
-                       "l2": "inputs (1.6 GB) larger than L2; the group table (48 MB) is L2 resident by design"},
+                       # single-key SUM/COUNT table: keys, row counts and sums, 8 B each per slot
+                       "l2": "inputs (1.6 GB) larger than L2; group table %.0f MB vs %.0f MB L2" % (st.table_slots * 24 / 1e6, torch.cuda.get_device_properties(dev).L2_cache_size / 1e6)},
             "clocks": clocks, "gpu_launches": int(launches), "e2e": e2e,
             "roofline": {"bound": "hbm", "achieved": alg / (ms * 1e-3) / 1e9, "peak": hbm_peak, "unit": "GB/s", "frac": alg / (ms * 1e-3) / 1e9 / hbm_peak,
                          "traffic": None, "peak_source": peak_src, "kernel": "k_agg_init + k_agg_update2<false> + k_agg_count + k_agg_finalize (one step)",
                          "algorithmic_bytes_per_launch": alg,
-                         "l2_op_floor_ms": 1.572 * n / 1e8, "frac_of_l2_op_floor": (1.572 * n / 1e8) / ms,
-                         "note": "the table lives in L2: one key gather + two 64-bit REDs per row cost 1.572 ms per 100 M rows on this chip (tools/scratch/agg_lab.cu, profiles/r2_agg_lab.md)"}}
+                         "note": "random table accesses, not the streamed bytes, bound the step: one key gather + two 64-bit REDs per row, in L2 while the table fits there, with HBM sector traffic on top when it does not"}}
     if cpu:
         line["cpu_baseline"] = cpu
     print(json.dumps(line))
@@ -1023,8 +1067,13 @@ def main():
     ap.add_argument("--skip-e2e", action="store_true")
     ap.add_argument("--skip-side", action="store_true", help="skip the 50 %% match side line (N = 1)")
     ap.add_argument("--skip-cpu", action="store_true")
-    ap.add_argument("--ncu-traffic-bytes", type=float, default=None, help="dram bytes per launch from the committed ncu capture")
+    ap.add_argument("--ncu-traffic-bytes", type=float, default=None, help="DRAM bytes per launch of a profiler capture, reported beside the roofline")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="N = 1: write the outputs of the last timed step as DIR/<column>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.gpus != 1 or args.impl != "b200"):
+        ap.error("--dump-outputs is implemented for the GPU path on one GPU (--gpus 1)")
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * tidbgpu.h — C ABI of libtidbgpu.so: the B200 (sm_100a) operator hot path of TiDB's
+ * tidbgpu.h — C ABI of libtidbgpu.so: the H100 (sm_90a) operator hot path of TiDB's
  * chunk-based vectorized executor (hash join build/probe, hash aggregation, VecEval*
  * filter/projection kernels, key-hash repartition for multi-GPU).
  *
@@ -404,7 +404,7 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
             tg_mut_chunk* out, int64_t* nrows, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Key-hash repartition for the multi-GPU exchange (the B200 analogue of the MPP
+ * Key-hash repartition for the multi-GPU exchange (the GPU analogue of the MPP
  * ExchangeSender HashPartition, pkg/planner/core/operator/physicalop/physical_exchange_sender.go:115;
  * in-process analogue: partitionHashSplitter.split, pkg/executor/shuffle.go:450).
  * Device-resident: scatter `ncols` 8-byte columns of `rows` rows into `nparts` contiguous

@@ -1,6 +1,6 @@
 // oracle/agg.cpp — CPU restatement of HashAggExec (TEST INFRASTRUCTURE, see oracle.h).
 //
-// Follows /root/reference/pkg/executor/aggregate:
+// Follows the reference's pkg/executor/aggregate:
 //   agg_hash_executor.go   parallelExec :635, fetchChildData :449, DefaultVal on empty input :654
 //   agg_hash_partial_worker.go  updatePartialResult :256, getPartialResultsOfEachRow :219
 //                               (murmur3.Sum32(key) % finalConcurrency), shuffleIntermData :287

@@ -1,6 +1,6 @@
 // oracle/join.cpp — CPU restatement of HashJoinV2Exec (TEST INFRASTRUCTURE, see oracle.h).
 //
-// Follows, function by function, the Go sources under /root/reference/pkg/executor/join:
+// Follows, function by function, the reference's Go sources under pkg/executor/join:
 //   join_table_meta.go   newTableMeta :184, setupJoinKeys :260, setupColumnOrder :331, getKeyProp :130
 //   row_table_builder.go processOneChunk :138, initHashValueAndPartIndexForOneChunk :103,
 //                        appendToRowTable :530, fillNullMap :375, fillRowData :433

@@ -2,9 +2,9 @@
  * oracle.h — C entry points of liboracle.so.
  *
  * TEST INFRASTRUCTURE, NOT PRODUCT.  This is a CPU restatement (C++17, no deps) of the algorithm of
- * TiDB's chunk-based operator hot path, written from the Go sources under /root/reference as a
- * specification (the reference is pure Go and no Go toolchain exists in this image, so it cannot be
- * compiled or run here: there is no oracle/_ref).  Only tests/, __graft_entry__.smoke() and
+ * TiDB's chunk-based operator hot path, written from the Go sources of pingcap/tidb as a
+ * specification (the reference is pure Go and the project has no Go toolchain, so it is not
+ * compiled or run: there is no oracle/_ref).  Only tests/, __graft_entry__.smoke() and
  * bench.py's cpu_baseline / --impl reference legs may load this library.  libtidbgpu.so never does.
  *
  * PARITY PINNING: the restatement is pinned against every known-answer test the reference's own

@@ -1,7 +1,7 @@
 // oracle/vec.cpp — row-at-a-time restatement of the VecEval* builtins on the path (TEST
 // INFRASTRUCTURE, see oracle.h) plus helpers shared by join.cpp / agg.cpp.
 //
-// Follows /root/reference/pkg/expression:
+// Follows the reference's pkg/expression:
 //   builtin_compare_vec.go  builtinLTIntSig.vecEvalInt :524-561, vecCompareInt :619
 //   builtin_compare_vec_generated.go :54 (real compare through cmp.Compare)
 //   builtin_arithmetic_vec.go  PlusInt :856-990 (plusUU/US/SU/SS), MinusInt :365-411 with

@@ -4,7 +4,7 @@ restatement of the reference's algorithm) produces.  Re-run after an intentional
 
     python tests/golden/make_golden.py
 
-The reference itself (Go) cannot run in this image, so the expected outputs come from the oracle, which is pinned to the
+The reference itself (Go) is not run by this project, so the expected outputs come from the oracle, which is pinned to the
 reference by the known-answer tests in tests/test_oracle_kat.py / test_oracle_join.py / test_oracle_agg_vec.py.  The
 fixtures freeze today's oracle behaviour: tests/test_golden.py fails if either the oracle (CPU) or the CUDA path (GPU)
 drifts from them.  Rows are stored as sorted lists; NULL = null; doubles as repr strings (bit exact)."""

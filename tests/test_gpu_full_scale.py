@@ -1,7 +1,7 @@
 """Parity at BASELINE.json's full sizes, against the oracle (not only size-independent properties):
   configs[1]  hash join 100M x 10M int64 keys, 8-byte payload, 100 % and 50 % match  -> every output row, bit-exact
   configs[2]  HashAgg SUM/COUNT GROUP BY int64, 100M rows / 1M groups (+ 1 % NULL x)  -> COUNT bit-exact, SUM within 1e-6
-The oracle (oracle/join.cpp, oracle/agg.cpp) runs on the host cores of the GPU box; these tests take about two minutes and
+The oracle (oracle/join.cpp, oracle/agg.cpp) runs on the host cores of the GPU machine; these tests take about two minutes and
 ~25 GB of host memory.  TG_SKIP_FULL_SCALE=1 skips them (e.g. on a small host)."""
 import os
 

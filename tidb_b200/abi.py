@@ -1,7 +1,7 @@
 """ctypes mirror of include/tidbgpu.h — the C-ABI of libtidbgpu.so.
 
 The structures here are byte-for-byte the ones a cgo shim would fill (INTEGRATION.md); the Python
-host side exists only because this image has no Go toolchain.  Loading fails loudly when the CUDA
+host side exists only because the project has no Go toolchain.  Loading fails loudly when the CUDA
 library has not been built: there is no CPU fallback anywhere in this package.
 """
 from __future__ import annotations
@@ -154,7 +154,7 @@ def load_lib() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} is missing: run `python -m tidb_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: run `python -m tidb_b200.build` (nvcc, sm_90a). "
             "There is no CPU fallback for the GPU operators.")
     lib = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
     lib.tg_last_error.restype = C.c_char_p

@@ -7,7 +7,8 @@
 //   HashAggFinalWorker merge + AppendFinalResult2Chunk (agg_hash_final_worker.go:73, :121;
 //     func_sum.go:80, func_avg.go:332, func_count.go:43)              → k_agg_finalize
 // There is no partial/final split on one GPU: every row updates the single device-resident group table
-// with atomics (the 1M-group table of config 3 is 32–48 MB and lives in the 126 MB L2).
+// with atomics.  The 1M-group table of config 3 is 48 MB, which does NOT stay resident in the 50 MB L2 of an H100: the
+// step takes about twice as long as with a 24 MB table (DESIGN.md §4.2).
 //
 // Layout: structure-of-arrays open-addressing table — keys[S+2] (int64, sentinel = empty), rows[S+2]
 // (group row count), and one or two 8-byte state arrays per aggregate.  Slot S holds the NULL group
@@ -64,8 +65,8 @@ struct AggTable {
   unsigned long long* tags;
   long long* keyw[TG_MAX_GROUP_COLS + 1];
   int32_t nkw;
-  // element stride of every array above, in 8-byte words: 1 = structure of arrays (single-key tables: hot groups live in
-  // L2 and same-sector atomics would serialise, profiles/r2_agg_lab.md); multi-key tables are ARRAY OF RECORDS
+  // element stride of every array above, in 8-byte words: 1 = structure of arrays (single-key tables: a row's atomics go to
+  // different sectors, and same-sector atomics would serialise); multi-key tables are ARRAY OF RECORDS
   // [tag | key words | rows | states], padded to 32 bytes: their groups are mostly cold (Q3: 2.4 rows per group, a 1.4 GB
   // table), and a row should touch one or two DRAM sectors instead of one per array
   uint32_t stride;
@@ -536,9 +537,12 @@ __device__ __forceinline__ unsigned long long mk_find_or_insert(const AggTable& 
   const unsigned long long ready = h | 3ull, busy = (h & ~3ull) | 1ull;
   uint32_t s = slot32(h, (uint32_t)t.nslots), steps = 0;
   for (;;) {
-    // tag and the first three key words sit in the record's first 32 bytes: ONE L2-coherent 256-bit load (records are 32-byte aligned)
+    // tag and the first three key words sit in the record's first 32 bytes (records are 32-byte aligned): two L2-coherent
+    // 128-bit loads of that one sector (128 bits is the widest load sm_90 has).  A tag that is not yet `ready`, or key words
+    // that do not match, fall through to the ordered loads below.
     unsigned long long cur, k0, k1, k2;
-    asm volatile("ld.global.cg.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(cur), "=l"(k0), "=l"(k1), "=l"(k2) : "l"(&t.tags[(size_t)s * t.stride]) : "memory");
+    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(cur), "=l"(k0) : "l"(&t.tags[(size_t)s * t.stride]) : "memory");
+    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2+16];" : "=l"(k1), "=l"(k2) : "l"(&t.tags[(size_t)s * t.stride]) : "memory");
     if (cur == 0) {
       cur = atomicCAS(&t.tags[(size_t)s * t.stride], 0ull, busy);
       if (cur == 0) {
@@ -627,7 +631,7 @@ struct AggImpl {
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  int nsm = 148;
+  int nsm = 132;
 
   int ncols = 0;
   std::vector<int> types, elem;
@@ -956,7 +960,7 @@ static int update_grouped_v2(AggImpl* a, const GroupKey& gk, const DevCols& cols
 
 // rows [lo, hi): CTA-local partial aggregation, then merge of the partial results into the global table
 static int local_partial_pass(AggImpl* a, const GroupKey& gk, const DevCols& cols, int64_t lo, int64_t hi, unsigned long long* sc) {
-  int local_slots = 1024;   // measured best on B200 (tools/bench_ops.py): bigger tables lose more to occupancy than they gain
+  int local_slots = 1024;   // bigger tables lose more to occupancy than they gain (TG_AGG_LOCAL_SLOTS overrides for sweeps)
   if (const char* e = getenv("TG_AGG_LOCAL_SLOTS")) { int v = atoi(e); if (v == 512 || v == 1024 || v == 2048 || v == 4096) local_slots = v; }
   size_t smem_per_cta = (size_t)(local_slots + 2) * 8 * (2 + a->nstates);
   int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (200u << 10) / smem_per_cta));
@@ -1067,9 +1071,8 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
         int64_t span = hi - done;
         done = hi;
         if (nd) have_deferred = true;
-        // Keep the CTA-local phase while it absorbs a useful share of the rows.  Measured (profiles/r1_agg_notes.md): shared-memory
-        // atomics (LSU) and L2 atomics are different engines; 1000 groups with half of the rows aggregated in shared memory and
-        // half deferred to the L2 path take 2.7 ms, all-L2 5.0 ms, all-shared 9 ms.
+        // Keep the CTA-local phase while it absorbs a useful share of the rows: shared-memory atomics (LSU) and L2 atomics
+        // are different engines, so splitting the rows between them beats sending all of them to either one.
         if (a->local_mode < 0) a->local_mode = (nd * 10 <= (unsigned long long)span * 7) ? 1 : 0;
         if (a->local_mode == 0) break;
       }

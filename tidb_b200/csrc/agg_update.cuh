@@ -1,15 +1,15 @@
 // agg_update.cuh — the round-2 grouped-aggregation update kernels (included by agg.cu after its table structs).
 //
-// What bounds a grouped aggregation on a B200 (tools/scratch/agg_lab.cu, profiles/r2_agg_lab.md; 100 M rows, 1 M groups):
-// the table (24-48 MB) lives in L2, so the cost is L2 OPERATIONS, not HBM bytes — an 8-byte gather costs 0.46 ms per
-// 100 M, a 64-bit RED 0.60-0.70 ms, and they add up (1 gather + 2 RED = 1.57 ms).  Packing a group's words into one
-// 32-byte sector is SLOWER (2.3 ms: same-sector atomics serialise), so the table stays structure-of-arrays.
-// Shared-memory atomics run 230 G/s chip-wide (f64 is a CAS loop), so a CTA-local table pays only while most rows hit
-// it.  Hence ONE kernel with two levels (the reference's partial/final split, agg_hash_partial_worker.go:256 /
+// What bounds a grouped aggregation (tools/scratch/agg_lab.cu measures the primitives; 100 M rows): while the table stays
+// in L2 the cost is L2 OPERATIONS, not HBM bytes — one key gather and two 64-bit REDs per row, and their costs add up.  A
+// table that does not fit L2 (1 M groups = 48 MB on an H100's 50 MB L2) adds random HBM sector traffic on top and takes
+// about twice as long (DESIGN.md §4.2).  Packing a group's words into one 32-byte sector is slower (same-sector atomics serialise), so the table stays
+// structure-of-arrays.  Shared-memory atomics are not free either (f64 is a CAS loop), so a CTA-local table pays only
+// while most rows hit it.  Hence ONE kernel with two levels (the reference's partial/final split, agg_hash_partial_worker.go:256 /
 // agg_hash_final_worker.go:73, with a CTA as the partial worker):
 //   level 1 (LOCAL): a small shared-memory table per CTA absorbs the rows of the keys it holds; a CTA that sees a low
 //                    hit rate after its first tiles switches it off for the rest of its rows (high-cardinality input);
-//   level 2        : everything else goes straight to the global L2 table — R rows per thread, all slot gathers of a
+//   level 2        : everything else goes straight to the global table — R rows per thread, all slot gathers of a
 //                    tile issued before the first compare (memory-level parallelism instead of a dependent chain);
 //   at the end the CTA folds its local groups into the global table (MergePartialResult semantics).
 // Rows / local groups that cannot be inserted within `max_probe` steps (table overfull) are deferred (bitmap) / spilled
@@ -25,7 +25,7 @@ namespace tg {
 // ---- shared-memory atomics on 32-bit shared addresses (generic-address atomics on shared memory are slower) ----------
 __device__ __forceinline__ void sred_add_u64(uint32_t a, unsigned long long v) { asm volatile("red.shared.add.u64 [%0], %1;" ::"r"(a), "l"(v) : "memory"); }
 // +1 on the LOW word of a 64-bit counter: a native 32-bit shared atomic (ATOMS.ADD) instead of the 64-bit CAS loop every
-// 64-bit shared atomic compiles to (ATOMS.CAST.SPIN; lab: 0.15 vs 0.38 ms per 100 M).  Exact while the counter stays below
+// 64-bit shared atomic compiles to (ATOMS.CAST.SPIN).  Exact while the counter stays below
 // 2^32, which a CTA's share of one launch (< 2^31 rows) guarantees.
 __device__ __forceinline__ void sred_inc_lo32(uint32_t a) { asm volatile("red.shared.add.u32 [%0], 1;" ::"r"(a) : "memory"); }
 __device__ __forceinline__ void sred_add_f64(uint32_t a, double v) { asm volatile("red.shared.add.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }

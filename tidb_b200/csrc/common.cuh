@@ -1,4 +1,4 @@
-// common.cuh — shared host/device helpers of libtidbgpu.so (sm_100a only).
+// common.cuh — shared host/device helpers of libtidbgpu.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -49,8 +49,7 @@ inline bool is_int_family(int tp) {
 
 // ---- device buffer (grow-only) ------------------------------------------------------------------
 // Stream-ordered pool allocation (cudaMallocAsync on a per-device service stream, pool never trimmed): a handle's
-// setup otherwise spends milliseconds in cudaMalloc / cudaFree, which also synchronise the whole device
-// (profiles/r1_agg_update_global.md: 1.8 ms kernel inside a 5.2 ms one-shot aggregation).
+// setup otherwise spends milliseconds in cudaMalloc / cudaFree, which also synchronise the whole device.
 cudaStream_t service_stream(int device);
 inline cudaError_t pool_alloc(int dev, void** p, size_t bytes) {
   cudaStream_t st = service_stream(dev);
@@ -146,7 +145,7 @@ inline void bury_handle(H* h) {
 // ---- hashing --------------------------------------------------------------------------------------
 // The reference hashes the serialised key with FNV-1 64 (join/row_table_builder.go:103).  The hash only selects a
 // bucket / partition, never a result, so the GPU is free to use something cheaper.  These kernels turned out to be
-// instruction-bound (profiles/r1_partitioned_*): murmur's 64-bit finaliser plus a 64-bit multiply-high cost ~40 SASS
+// instruction-bound: murmur's 64-bit finaliser plus a 64-bit multiply-high cost ~40 SASS
 // instructions per row.  hash64 is one xor-fold and ONE 64-bit multiply (Fibonacci hashing, ~5 instructions); every
 // range reduction is a 32-bit multiply-high:
 //   slot   = mulhi32(hi32(h), nslots)      table slot, monotone in hi32(h)   (tables are limited to < 2^32 slots)

@@ -98,7 +98,7 @@ struct JoinImpl {
   cudaStream_t d2h_stream = nullptr; // tg_join_next copies results on its own stream: D2H overlaps the next H2D + probe
   bool own_stream = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  int nsm = 148;
+  int nsm = 132;
   double load_factor = 0.5;
   bool default_load_factor = true;
 
@@ -341,7 +341,7 @@ static int setup(JoinImpl* j, const tg_join_desc* d) {
   if (j->n_out > TG_MAX_OUT) return fail(TG_ERR_UNSUPPORTED, "too many output columns");
   j->device = d->device;
   j->default_load_factor = !(d->load_factor > 0.05 && d->load_factor <= 0.95);
-  j->load_factor = (d->load_factor > 0.05 && d->load_factor <= 0.95) ? d->load_factor : 0.35;   // measured best with the lean segment probe (profiles/r2_sweep_probe_lf_parts.jsonl: 1.93 vs 1.96 ms at 0.4, 2.12 at 0.5)
+  j->load_factor = (d->load_factor > 0.05 && d->load_factor <= 0.95) ? d->load_factor : 0.35;   // sparse enough for short probe runs, dense enough for the L2 slices of the partitioned probe
   return TG_OK;
 }
 
@@ -508,9 +508,9 @@ static int build_table(JoinImpl* j) {
     ks.data = j->bkey_syn.p; ks.nulls = j->bkey_syn_nn.as<uint8_t>();
   } else { ks.data = bview.data[b.key_col]; ks.nulls = bview.nulls[b.key_col]; }
   unsigned long long nslots = (unsigned long long)((double)(n > 0 ? n : 1) / j->load_factor) + 32;
-  // the L2 partition pass handles at most TG_MAX_PARTS slices and wants them <= ~33 MB (45 MB slices: 2.10 vs 1.93 ms,
-  // profiles/r2_sweep_probe_lf_parts.jsonl): with the DEFAULT load factor a table that would need more slices is made denser,
-  // down to load factor 0.5, instead of growing its slices
+  // the L2 partition pass handles at most TG_MAX_PARTS slices of <= ~33 MB: with the DEFAULT load factor a table that would
+  // need more slices is made denser, down to load factor 0.5, instead of growing its slices.  (These sizes suit an L2
+  // larger than an H100's; see the partition pass in probe_device.)
   if (j->default_load_factor) {
     const unsigned long long fit = ((unsigned long long)TG_MAX_PARTS * (33ull << 20)) / sizeof(Slot);
     const unsigned long long dense = (unsigned long long)((double)(n > 0 ? n : 1) / 0.5) + 32;
@@ -725,7 +725,7 @@ static bool uq_path_ok(const JoinImpl* j, const DevCols& pview) {
   return true;
 }
 
-// ---- fast-path launch tuning (env overrides are for A/B sweeps on the GPU box; defaults are the measured best) ----
+// ---- fast-path launch tuning (env overrides are for A/B sweeps; the defaults are the production choice) ----
 struct ProbeTuning { int variant; int R; int evict_last; int ctas_per_sm; int partition; int subseg; int parts; int part_min_mb; int part_min_rows; int seg_vec; int seg_lean; int carveout; int tma; int stages; int tma_ctas; int cta_agg; };
 static ProbeTuning probe_tuning() {
   ProbeTuning t;
@@ -734,12 +734,12 @@ static ProbeTuning probe_tuning() {
   t.evict_last = env_int("TG_PROBE_EVICT_LAST", 0);
   t.ctas_per_sm = env_int("TG_PROBE_CTAS_PER_SM", 0);   // 0 = exactly the resident CTA count (occupancy query)
   t.partition = env_int("TG_PROBE_PARTITION", 1);   // regroup big probes into L2-sized partitions first (0 = never, 2 = counted/dense variant)
-  t.subseg = env_int("TG_PROBE_SUBSEG", 0);         // 1 = CTA-private sub-segments in the L2 partition pass (no global cursor atomics): MEASURED SLOWER (scatter 0.62 vs 0.575 ms: 7104 write streams; probe 2.3 vs 1.36 ms: the interleaved empty tails let warps drift across partitions) - kept for the record, off
-  t.parts = env_int("TG_PROBE_PARTS", 0);           // 0 = auto: table slices of <= 32 MB
+  t.subseg = env_int("TG_PROBE_SUBSEG", 0);         // 1 = CTA-private sub-segments in the L2 partition pass (no global cursor atomics): off, slower (thousands of write streams, and the interleaved empty tails let warps drift across partitions)
+  t.parts = env_int("TG_PROBE_PARTS", 0);           // 0 = auto: table slices of <= 32 MB, at most TG_MAX_PARTS
   t.part_min_mb = env_int("TG_PROBE_PART_MIN_MB", 64);
   t.part_min_rows = env_int("TG_PROBE_PART_MIN_ROWS", 1 << 22);
   t.seg_vec = env_int("TG_PROBE_SEG_VEC", 1);            // 128-bit loads/stores in the segment probe
-  t.seg_lean = env_int("TG_PROBE_SEG_LEAN", 1);          // 1 = lean full-tile path (default: 1.954 vs 2.089 ms per step, profiles/r2_sweep_probe.jsonl), 0 = round-1 kernel, 2 = + register prefetch (2.01 ms)
+  t.seg_lean = env_int("TG_PROBE_SEG_LEAN", 1);          // 1 = lean full-tile path (default), 0 = round-1 kernel, 2 = + register prefetch
   t.carveout = env_int("TG_PROBE_CARVEOUT", -1);         // EXPERIMENTAL: preferred shared-memory carve-out (%) of the segment probe kernels, -1 = driver default
   t.tma = 0;                                        // (the TMA-fed probe kernels were removed in round 2)
   t.stages = env_int("TG_PROBE_STAGES", 4);
@@ -789,7 +789,7 @@ template <int NPC, int NKD, int NMD>
 struct LaunchWarp {
   static int run(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t, const SegSpec& seg) {
     constexpr int R = 4;
-    static int resident = 0;   // CTAs of this instantiation one SM holds (register-bound, 3 on sm_100a)
+    static int resident = 0;   // CTAs of this instantiation one SM holds (register-bound)
     if (!resident) {
       int nb = 0;
       if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_probe_inner_u1_w<R, NPC, NKD, NMD>, 256, 0) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 3; }
@@ -873,16 +873,18 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
         if (tune.partition == 1 && src16 && scatter_bulk_enabled() && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
           // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments.
           // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
-          // [p/P, (p+1)/P) — ~32 MB that stay L2 resident while the probe kernel sweeps the segment.  Trades 32 B/row of
-          // extra streaming traffic (0.57 ms per 100 M rows) for ~100 B/row of random HBM traffic (probe 2.5 → 1.45 ms);
-          // profiles/r1_probe_lab.md.  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
+          // [p/P, (p+1)/P) while the probe kernel sweeps the segment.  The pass trades 32 B/row of extra streaming traffic for
+          // random HBM traffic, which only pays while a slice stays L2 resident.  The ~32 MB slices below do not stay
+          // resident in the 50 MB L2 of an H100, where the pass measured no faster than the direct probe (DESIGN.md §4.1);
+          // it stays the default only until smaller slices, which need more than TG_MAX_PARTS partitions, are measured
+          // there.  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
           // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
           int P = tune.parts > 0 ? tune.parts : (int)((table_bytes + (32u << 20) - 1) / (32u << 20));
           if (P > TG_MAX_PARTS) P = TG_MAX_PARTS;
           const int64_t n_main = n / PTILE * PTILE;
           const int nc = 1 + fo.n_pcols;
           // Segment layout.  Default: one segment per partition filled through global cursors.  TG_PROBE_SUBSEG=1 (experiment,
-          // measured slower, profiles/r2_subseg.md): every scatter CTA owns a private sub-segment of each partition —
+          // slower): every scatter CTA owns a private sub-segment of each partition —
           // G = grid, sub-segment (p, b) = rows [(p*G + b) * C, ...) — placed with a shared-memory cursor, no global atomics.
           const int G = tune.subseg ? scatter_bulk_grid_nc(j->device, n_main, nc) : 1;
           const int64_t nsegs = (int64_t)P * G;
@@ -1175,9 +1177,9 @@ int tg_join_open(const tg_join_desc* desc, tg_join** out) {
   TG_CUDA(cudaStreamCreateWithFlags(&j->d2h_stream, cudaStreamNonBlocking));
   j->nsm = device_sm_count(j->device);
   {
-    // L2 fetch granularity (cudaLimitMaxL2FetchGranularity): left at the device default.  Measured (tools/sweep_probe.py,
-    // profiles/r1_sweep.md): capping it at 32 B cuts the HBM bytes of the random gathers but makes the unpartitioned probe
-    // SLOWER (the gathers are bound by DRAM access rate, not bytes); TG_L2_FETCH={32,64,128} overrides for experiments.
+    // L2 fetch granularity (cudaLimitMaxL2FetchGranularity): left at the device default.  Capping it at 32 B cuts the HBM
+    // bytes of the random gathers, but they are bound by DRAM access rate, not bytes; TG_L2_FETCH={32,64,128} overrides
+    // for experiments (tools/sweep_probe.py).
     int gran = env_int("TG_L2_FETCH", 0);
     if (gran == 32 || gran == 64 || gran == 128) { if (cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)gran) != cudaSuccess) cudaGetLastError(); }
   }

@@ -1,4 +1,4 @@
-// join_kernels.cuh — hash-join build / probe kernels for sm_100a.
+// join_kernels.cuh — hash-join build / probe kernels for sm_90a.
 //
 // What they replace in the reference (pkg/executor/join):
 //   build : rowTableBuilder.processOneChunk (row_table_builder.go:138) + subTable.build
@@ -10,7 +10,7 @@
 //                                                                    → k_probe_inner_u1 (fused fast path)
 //                                                                      k_probe_count / k_probe_write
 //
-// Data layout in HBM (B200-first, not the reference's chained row pointers):
+// Data layout in HBM (GPU-first, not the reference's chained row pointers):
 //   * open-addressing table of 16-byte slots {int64 key, u64 meta}, linear probing, one slot per
 //     DISTINCT key; any table size (multiply-high range reduction), one extra slot at index nslots
 //     for the key whose value equals the empty sentinel.
@@ -133,10 +133,12 @@ __device__ __forceinline__ Slot load_slot(const Slot* p) {
   return s;
 }
 
-// both slots of a 32-byte home pair with ONE 256-bit load (LDG.E.256, sm_100+); p must be 32-byte aligned
+// both slots of a 32-byte home pair: two back-to-back 128-bit loads (128 bits is the widest load sm_90 has) of the same
+// 32-byte sector, so the pair still costs one sector fetch; p must be 32-byte aligned
 __device__ __forceinline__ void load_pair(const Slot* p, Slot& a, Slot& b) {
   unsigned long long x0, x1, x2, x3;
-  asm volatile("ld.global.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(x0), "=l"(x1), "=l"(x2), "=l"(x3) : "l"(p));
+  asm volatile("ld.global.v2.u64 {%0, %1}, [%2];" : "=l"(x0), "=l"(x1) : "l"(p));
+  asm volatile("ld.global.v2.u64 {%0, %1}, [%2+16];" : "=l"(x2), "=l"(x3) : "l"(p));
   a.key = (int64_t)x0; a.meta = x1; b.key = (int64_t)x2; b.meta = x3;
 }
 
@@ -416,7 +418,7 @@ k_probe_inner_u1(const int64_t* __restrict__ pkey, DevCols pcols, int64_t n, Tab
 // probe — fused fast path, warp-autonomous and TMA-fed variants.
 // The output shape is a template parameter (NPC probe payload columns, NKD outputs fed by the join key, NMD outputs
 // fed by the build payload): with run-time destination counts ptxas unrolled the store loops into ~360 predicated
-// STG + 350 LDC per kernel (886 M warp instructions for 100 M rows, profiles/r1_partitioned_tma_launches.csv).
+// STG + 350 LDC per kernel.
 // ---------------------------------------------------------------------------------------------
 #define TG_FAST_MAX_PCOLS 3
 #define TG_FAST_MAX_KEYDST 2
@@ -553,7 +555,7 @@ struct SegSpec {
 
 // warp-autonomous: no shared memory, no block barrier; each warp owns tiles of 32×R rows.
 // Launch with exactly the resident CTA count (occupancy × SMs): every extra wave of a persistent grid-stride kernel
-// re-sweeps all partitions of a partition-ordered input and re-fetches the table slices (lab: 1.48 → 1.60 ms).
+// re-sweeps all partitions of a partition-ordered input and re-fetches the table slices.
 template <int R, int NPC, int NKD, int NMD>
 __global__ void __launch_bounds__(256)
 k_probe_inner_u1_w(const int64_t* __restrict__ pkey, int64_t n, TableView t, FastOut out,
@@ -659,11 +661,10 @@ k_probe_inner_u1_seg(const int64_t* __restrict__ pkey, int64_t n, TableView t, F
 }
 
 // ---------------------------------------------------------------------------------------------
-// DEFAULT since round 2 (TG_PROBE_SEG_LEAN=1; 0 = the kernel above, 2 = + register prefetch; measured on the library's data:
-// step 2.089 -> 1.954 ms, profiles/r2_sweep_probe.jsonl): the same segment probe with a lean full-tile path — no per-row `in` flags, no slot array, sentinel-valued
+// DEFAULT (TG_PROBE_SEG_LEAN=1; 0 = the kernel above, 2 = + register prefetch): the same segment probe with a lean
+// full-tile path — no per-row `in` flags, no slot array, sentinel-valued
 // keys detected once per tile (then the tile takes the generic path) — and, with PREFETCH, the next tile's keys/payloads
-// requested before the current tile's gathers are issued.  ncu: the production kernel executes 551 M warp instructions per
-// 100 M rows, the lab kernel 351 M.
+// requested before the current tile's gathers are issued.
 // ---------------------------------------------------------------------------------------------
 template <int NPC, int NKD, int NMD>
 __device__ __forceinline__ void probe_tile_generic(const int64_t* __restrict__ pkey, int64_t base, int64_t limit, const TableView& t,
@@ -803,9 +804,9 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
   }
 }
 
-// (The TMA-fed variant of this kernel — keys/payloads through a cp.async.bulk ring — was removed in round 2: measured no
-// faster in round 1 (the segment probe is bound by L1 gather issue, and every KB of shared memory it holds costs L1), it
-// added 96 instantiations to the library.  tools/scratch/probe_lab.cu keeps the experiment; profiles/r1_probe_lab.md the numbers.)
+// (There is no TMA-fed variant of this kernel — keys/payloads through a cp.async.bulk ring: the segment probe is bound by
+// L1 gather issue, every KB of shared memory such a ring holds costs L1, and it would add 96 instantiations to the library.
+// tools/scratch/probe_lab.cu keeps the experiment.)
 
 // OtherCondition on ONE candidate pair (probe row i, build row `brow` of the row store): true iff every CNF item is
 // non-NULL true (expression.VectorizedFilter over the joined chunk, inner_join_probe.go:72-79)
@@ -1021,8 +1022,8 @@ k_probe_write(int64_t n, const unsigned long long* __restrict__ off, const uint3
 #define UQ_R 4
 __global__ void __launch_bounds__(256)
 k_probe_inner_uq(KeySpec key, DevCols pcols, DevFilter filt, int64_t n, TableView t, OutCols out, unsigned long long* __restrict__ out_cursor) {
-  // ONE output-cursor atomic per 1024-row CTA tile: a per-warp reservation (600 M rows -> 19 M atomics on one address) was
-  // measured to serialise in L2 at ~2 ns each (Q3 J2 probe 38.8 ms); per tile it is 0.6 M
+  // ONE output-cursor atomic per 1024-row CTA tile: a per-warp reservation (600 M rows -> 19 M atomics on one address)
+  // serialises in L2; per tile it is 0.6 M
   __shared__ uint32_t s_cnt[2][UQ_R][8];          // double-buffered by tile parity: two CTA barriers per tile, not three
   __shared__ unsigned long long s_base[2];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1034,7 +1035,7 @@ k_probe_inner_uq(KeySpec key, DevCols pcols, DevFilter filt, int64_t n, TableVie
     Slot v[UQ_R];
     bool valid[UQ_R];
     // the key loads do not depend on the filter: issue them first so that key and filter columns stream in together
-    // (ncu, profiles/r2_q3_kernels.md: the kernel was bound by three dependent DRAM round trips per tile)
+    // (otherwise the kernel is bound by three dependent DRAM round trips per tile)
 #pragma unroll
     for (int r = 0; r < UQ_R; r++) {
       const int64_t i = base + (int64_t)r * 256 + threadIdx.x;

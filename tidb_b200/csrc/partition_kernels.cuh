@@ -229,7 +229,7 @@ k_partition_scatter_tma(int64_t ntiles, PartDst d, unsigned long long* __restric
       uint64_t h = hash64(key[j]);
       uint32_t p = HIGH ? mulhi32((uint32_t)(h >> 32), P) : part_of(h, P);
       // rank inside (tile, destination): one shared-memory atomic per row.  Warp-aggregating it (match_any + leader
-      // election) was measured 1.6x SLOWER end to end (tools/scratch/probe_lab.cu: 0.92 vs 0.58 ms per 100 M rows).
+      // election) costs more instructions than the contention it saves (tools/scratch/probe_lab.cu compares both).
       pr[j] = (p << 16) | atomicAdd(&s_cnt[p], 1u);
     }
     __syncthreads();
@@ -506,7 +506,7 @@ template <bool HIGH, int NC>
 inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d, unsigned long long* cursors, int64_t* launches, int ctas_per_sm = 0) {
   int nsm = device_sm_count(device);
   if (scatter_bulk_enabled()) {
-    // 1024-row tiles: 4 CTAs per SM for NC <= 2 (profiles/r1_scatter_bulk.md)
+    // 1024-row tiles: 4 CTAs per SM for NC <= 2
     constexpr int ITEMS = 4, TILE = PT_BLOCK * ITEMS;
     int64_t ntiles = n / TILE;
     if (ntiles > 0) {

@@ -60,7 +60,7 @@ int device_sm_count(int device) {
   static int cache[64];
   if (device >= 0 && device < 64 && cache[device] > 0) return cache[device];
   int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) { cudaGetLastError(); n = 148; }
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) { cudaGetLastError(); n = 132; }
   if (device >= 0 && device < 64) cache[device] = n;
   return n;
 }

@@ -1,8 +1,7 @@
 // tma.cuh — bulk asynchronous copies (cp.async.bulk, the 1-D TMA path, SASS UBLKCP) + mbarrier helpers.
 //
 // Why: the operators here are HBM-bound streams mixed with random gathers.  One 8-byte LDG in flight per thread
-// cannot cover HBM latency (profiles/r1_probe_first.md: the first probe kernel stalls on long_scoreboard and the
-// plain streaming kernels reach ~2 TB/s).  Bulk copies are issued by one elected thread, need no registers for
+// cannot cover HBM latency (a plain probe kernel stalls on long_scoreboard).  Bulk copies are issued by one elected thread, need no registers for
 // the data in flight, bypass the LSU/L1 miss path, and complete on an mbarrier, so every CTA keeps several
 // 16-32 KB tiles in flight regardless of occupancy.
 #pragma once
@@ -35,8 +34,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Every lane performs its own acquire, then the warp reconverges: try_wait may release lanes of one warp at
 // different times, and the CTA-wide __syncthreads() that follows in the kernels is an ALIGNED barrier — executing it
-// with a diverged warp is undefined (seen on B200: the barrier released early and the stage was refilled under
-// lanes that had not read it yet).
+// with a diverged warp is undefined (the barrier can release early and the stage be refilled under lanes that have
+// not read it yet).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {}
   __syncwarp();

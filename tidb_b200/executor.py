@@ -3,7 +3,7 @@
 The reference's contract is exec.Executor (pkg/executor/internal/exec/executor.go:51-77):
 Open(ctx) / Next(ctx, req *chunk.Chunk) / Close(), children pulled with exec.Next(ctx, child, chk),
 zero rows = EOF.  A cgo shim implementing that interface forwards to the C-ABI exactly like the
-classes below do (INTEGRATION.md shows the Go source); they exist in Python only because this image
+classes below do (INTEGRATION.md shows the Go source); they exist in Python only because the project
 has no Go toolchain.  Names follow the reference: MockDataSource (internal/testutil/testutil.go:63),
 HashJoinV2Exec (join/hash_join_v2.go:608), HashAggExec (aggregate/agg_hash_executor.go:93).
 

@@ -291,7 +291,7 @@ class SegmentExchange:
         self.stage_arr = []
         self.copy_streams = []
         if self.dma:
-            # one stream's copies run back to back on one copy engine (~500 GB/s measured at 8 GPUs); a few streams keep
+            # one stream's copies run back to back on one copy engine; a few streams keep
             # several engines and NVLink paths busy
             self.copy_streams = [torch.cuda.Stream(device=self.dev) for _ in range(min(4, world - 1))]
             for c in range(ncols):
@@ -476,8 +476,8 @@ class MailboxExchange:
         self.dev = torch.device("cuda", device)
         self.dma = bool(dma) and world > 1
         # dma + direct_peers = K: HYBRID transfer.  The regroup kernel stores the rows of the K next ranks (ring order) straight
-        # into those peers over NVLink (SM bulk stores, ~580 GB/s while the kernel runs) and stages the rest for the copy engines
-        # (~400 GB/s per direction under load at 8 GPUs, profiles/r2_trace_8gpu_cs14.txt): the two paths add up, the copy
+        # into those peers over NVLink (SM bulk stores while the kernel runs) and stages the rest for the copy engines: the
+        # two paths add up, the copy
         # engines' share shrinks until it hides behind the probe again
         self.direct = set(((rank + i) % world) for i in range(1, min(int(direct_peers), world - 1) + 1)) if self.dma else set()
         # dma + sm_copy: the staged regions are moved by tg_peer_copy_regions (an SM kernel small enough to sit next to the
@@ -551,8 +551,7 @@ class MailboxExchange:
                         for p in range(world) for c in range(ncols)]
                 self.stage_arr.append((C.c_void_p * len(flat))(*flat))
             # one stream drives one copy engine at a time: the (world-1) x ncols region copies are spread over several streams
-            # (default: one per copy, at most 16).  Measured at 8 GPUs with 4 streams: 430 GB/s per direction, the transfer
-            # (not the SMs) bounded the step (profiles/r2_trace_8gpu_first.txt)
+            # (default: one per copy, at most 16): with a few streams the transfer, not the SMs, bounds the step
             ncs = copy_streams if copy_streams > 0 else min(16, (world - 1) * ncols)
             self.copy_streams = [torch.cuda.Stream(device=self.dev) for _ in range(max(1, ncs))]
             self.dstream = torch.cuda.Stream(device=self.dev)
@@ -613,7 +612,7 @@ class MailboxExchange:
         """enqueue step k's repartition + transfer + count publication; cols[0] must be `key`.
         The SM kernel (regroup / scatter) goes on `compute_stream` (default: the exchange stream given to the constructor).
         Putting it on the SAME stream as the probe keeps the shared-memory-heavy scatter and the L1-hungry probe kernel
-        from ever sharing an SM (profiles/r1_probe_lab.md: the probe runs 2.3x slower under a large carve-out); with
+        from ever sharing an SM (the probe slows down under a large shared-memory carve-out); with
         dma=True the NVLink transfer then overlaps the probe on the copy engines."""
         lib, abi, torch = self.lib, self.abi, self.torch
         k = self.sent_steps

@@ -1,7 +1,7 @@
-// agg_lab.cu — what bounds a 100 M-row / 1 M-group SUM+COUNT aggregation on a B200?
+// agg_lab.cu — what bounds a 100 M-row / 1 M-group SUM+COUNT aggregation on an H100?
 // Scratch tool (round 2): rates of the primitive operations a grouped aggregation can be built from — L2 atomics by
 // width / layout, shared-memory atomics, L2-resident gathers — and of whole-kernel candidates.  Numbers guide agg.cu.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/scratch/agg_lab tools/scratch/agg_lab.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/scratch/agg_lab tools/scratch/agg_lab.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

@@ -1,6 +1,6 @@
-// gather_bench.cu — how many random 32-byte gathers per second can a B200 sustain, as a function of table size,
-// loads in flight per thread, L2 fetch granularity and the mechanism (LDG.256 into registers vs cp.async into shared memory)?
-// Scratch tool: numbers guide the probe kernel's structure (profiles/r1_gather_bench.txt).
+// gather_bench.cu — how many random 32-byte gathers per second can an H100 sustain, as a function of table size,
+// loads in flight per thread, L2 fetch granularity and the mechanism (LDG into registers vs cp.async into shared memory)?
+// Scratch tool: numbers guide the probe kernel's structure.
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -15,7 +15,9 @@ struct alignas(32) Pair { uint64_t a, b, c, d; };
 
 __device__ __forceinline__ Pair ldg256(const Pair* p) {
   Pair r;
-  asm volatile("ld.global.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(r.a), "=l"(r.b), "=l"(r.c), "=l"(r.d) : "l"(p));
+  // two 128-bit loads of one 32-byte sector (sm_90 has no 256-bit load)
+  asm volatile("ld.global.v2.u64 {%0,%1}, [%2];" : "=l"(r.a), "=l"(r.b) : "l"(p));
+  asm volatile("ld.global.v2.u64 {%0,%1}, [%2+16];" : "=l"(r.c), "=l"(r.d) : "l"(p));
   return r;
 }
 
@@ -99,7 +101,7 @@ static float time_ms(F f, int reps = 5) {
 int main() {
   const int64_t n = 100000000;
   unsigned long long* out; CK(cudaMalloc(&out, 8));
-  int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   size_t gran_default = 0; cudaDeviceGetLimit(&gran_default, cudaLimitMaxL2FetchGranularity);
   printf("SMs %d, default L2 fetch granularity %zu\n", sms, gran_default);
   const size_t table_mb[] = {16, 32, 64, 128, 400};

@@ -2,7 +2,7 @@
 // Measures, on the bench workload (100 M probe rows, 10 M build keys, 16-byte slots, load factor 0.4):
 //   S*  pure streaming kernels with the probe's traffic shape (16 B in, 32 B out per row), to find the ceiling
 //   P*  probe kernels on the unpartitioned input and on the input regrouped by L2 partition
-// build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -I include -I tidb_b200/csrc \
+// build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -I include -I tidb_b200/csrc \
 //        tools/scratch/probe_lab.cu tidb_b200/csrc/runtime.cu -o tools/scratch/probe_lab
 #include "join_kernels.cuh"
 #include "partition_kernels.cuh"
@@ -694,7 +694,8 @@ __global__ void __launch_bounds__(256, MINB) k_probe_v3(const int64_t* __restric
 // streamed inputs with evict_first hint (POL & 4)
 __device__ __forceinline__ void load_pair_pol(const Slot* p, Slot& a, Slot& b, u64 pol) {
   u64 x0, x1, x2, x3;
-  asm volatile("ld.global.L2::cache_hint.v4.u64 {%0, %1, %2, %3}, [%4], %5;" : "=l"(x0), "=l"(x1), "=l"(x2), "=l"(x3) : "l"(p), "l"(pol));
+  asm volatile("ld.global.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(x0), "=l"(x1) : "l"(p), "l"(pol));
+  asm volatile("ld.global.L2::cache_hint.v2.u64 {%0, %1}, [%2+16], %3;" : "=l"(x2), "=l"(x3) : "l"(p), "l"(pol));
   a.key = (int64_t)x0; a.meta = x1; b.key = (int64_t)x2; b.meta = x3;
 }
 __device__ __forceinline__ void st16_pol(void* p, ulonglong2 v, u64 pol) {
@@ -1114,7 +1115,7 @@ int main(int argc, char** argv) {
   const double load = argc > 1 ? atof(argv[1]) : 0.4;
   const uint32_t P = argc > 2 ? atoi(argv[2]) : 12;
   const bool all = argc > 3 && std::string(argv[3]) == "all";
-  int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   u64 nslots = ((u64)(nb / load) + 32) & ~1ull;
   printf("n=%lld nb=%lld nslots=%llu (%.0f MB) P=%u slice=%.1f MB\n", (long long)n, (long long)nb, nslots, nslots * 16 / 1048576.0, P, nslots * 16 / 1048576.0 / P);
   int64_t *bk, *pk, *pk_s; u64 *bp, *pv, *pv_s, *o[4], *cursor, *acc; Slot* slots; uint8_t* part; uint32_t* idx;
