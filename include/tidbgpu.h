@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define TIDBGPU_ABI_VERSION 1
+#define TIDBGPU_ABI_VERSION 2
 
 /* ---------------------------------------------------------------------------------------------
  * status codes
@@ -290,10 +290,20 @@ typedef struct tg_join_stats {
   int64_t output_rows;
   int64_t kernel_launches;    /* CUDA kernels launched by this handle                 */
   int32_t table_mode;         /* 0 none, 1 unique-inline, 2 grouped row store         */
-  int32_t reserved;
+  int32_t paths;              /* TG_JOIN_PATH_* bits: kernel families this handle has launched */
   double build_ms, probe_ms;  /* device time measured with CUDA events                */
   int64_t h2d_bytes, d2h_bytes;
 } tg_join_stats;
+/* tg_join_stats.paths */
+enum {
+  TG_JOIN_PATH_PROBE_UQ = 1 << 0,       /* single-pass unique-key probe (k_probe_inner_uq)                       */
+  TG_JOIN_PATH_PROBE_GENERAL = 1 << 1,  /* general count -> scan -> write probe                                  */
+  TG_JOIN_PATH_PROBE_DIRECT = 1 << 2,   /* fused warp probe (k_probe_inner_u1_w), also the gated fallback launch  */
+  TG_JOIN_PATH_PROBE_SEG = 1 << 3,      /* segment probe over L2-partitioned rows (k_probe_inner_u1_seg*)        */
+  TG_JOIN_PATH_PROBE_TILE = 1 << 4,     /* fused CTA-tile probe (k_probe_inner_u1)                               */
+  TG_JOIN_PATH_SCATTER_BULK = 1 << 5,   /* bulk partition scatter (k_partition_scatter_bulk)                     */
+  TG_JOIN_PATH_SCATTER = 1 << 6         /* any other partition scatter kernel                                    */
+};
 int tg_join_get_stats(tg_join* j, tg_join_stats* out);
 
 /* ---------------------------------------------------------------------------------------------
@@ -354,7 +364,20 @@ typedef struct tg_agg_stats {
   int64_t input_rows, groups, table_slots, kernel_launches;
   double update_ms, finalize_ms;
   int64_t h2d_bytes, d2h_bytes;
+  int64_t local_rows;         /* rows the CTA-local (shared-memory) level of the grouped update absorbed       */
+  int32_t paths;              /* TG_AGG_PATH_* bits: kernel families this handle has launched                 */
+  int32_t reserved;
 } tg_agg_stats;
+/* tg_agg_stats.paths */
+enum {
+  TG_AGG_PATH_NOGROUP = 1 << 0,     /* no GROUP BY (k_agg_update_nogroup)                                        */
+  TG_AGG_PATH_V2_GLOBAL = 1 << 1,   /* grouped update, global table only (k_agg_update2<false>)                 */
+  TG_AGG_PATH_V2_LOCAL = 1 << 2,    /* grouped update with the CTA-local level (k_agg_update2<true>)            */
+  TG_AGG_PATH_MULTI_KEY = 1 << 3,   /* several GROUP BY columns (k_agg_update_mk)                                */
+  TG_AGG_PATH_V1_LOCAL = 1 << 4,    /* TG_AGG_V1=1: CTA-local partial pass (k_agg_update_local)                  */
+  TG_AGG_PATH_V1_GLOBAL = 1 << 5,   /* TG_AGG_V1=1: global update (k_agg_update)                                 */
+  TG_AGG_PATH_MERGE = 1 << 6        /* partial results folded into the global table (k_agg_merge)                */
+};
 int tg_agg_get_stats(tg_agg* a, tg_agg_stats* out);
 
 /* ---------------------------------------------------------------------------------------------

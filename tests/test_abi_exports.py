@@ -22,14 +22,27 @@ def lib():
     return abi.load_lib()
 
 
-def test_header_symbols_all_exported(lib):
+def test_header_symbols_all_exported_abi_version_2(lib):
     hdr = open(os.path.join(ROOT, "include", "tidbgpu.h")).read()
     declared = set(re.findall(r"\b(tg_[a-z0-9_]+)\s*\(", hdr))
     assert declared, "no declarations parsed"
     assert declared == set(abi.EXPORTED_SYMBOLS), declared ^ set(abi.EXPORTED_SYMBOLS)
     for name in declared:
         assert hasattr(lib, name), f"{name} is declared in tidbgpu.h but not exported"
-    assert lib.tg_abi_version() == 1
+    assert lib.tg_abi_version() == 2
+
+
+def test_stats_struct_layout_and_path_bits():
+    # tg_join_stats / tg_agg_stats as include/tidbgpu.h lays them out (ABI version 2): the Python mirror must agree byte
+    # for byte, and the path bits must carry the header's values
+    assert C.sizeof(abi.TgJoinStats) == 12 * 8 + 2 * 4 and abi.TgJoinStats.paths.offset == 8 * 8 + 4
+    assert C.sizeof(abi.TgAggStats) == 9 * 8 + 2 * 4 and abi.TgAggStats.local_rows.offset == 8 * 8
+    assert abi.TgAggStats.paths.offset == 9 * 8
+    hdr = open(os.path.join(ROOT, "include", "tidbgpu.h")).read()
+    bits = dict((m.group(1), 1 << int(m.group(2))) for m in re.finditer(r"\bTG_((?:JOIN|AGG)_PATH_[A-Z0-9_]+) = 1 << (\d+)", hdr))
+    assert len(bits) == 14
+    for name, v in bits.items():
+        assert getattr(abi, name) == v, name
 
 
 def test_fixed_len_matches_reference(lib):

@@ -31,6 +31,22 @@ def run_gpu_agg(plan, chunks, required_rows=1024):
     return rows
 
 
+def run_gpu_agg_stats(plan, chunks, required_rows=1024):
+    """run_gpu_agg, plus the handle's tg_agg_stats read before close"""
+    e = HashAggExec(plan, MockDataSource(plan.col_types, chunks))
+    e.open()
+    try:
+        rows = []
+        while True:
+            c = e.next(required_rows)
+            if c.num_rows() == 0:
+                break
+            rows.extend(columns_to_rows([(col.data, col.nulls()) for col in c.columns]))
+        return rows, e.stats()
+    finally:
+        e.close()
+
+
 def run_orc_agg(plan, chunks):
     a = O.OracleAgg(plan, 5, 5)
     n, cols = a.run(chunks)
@@ -138,9 +154,15 @@ def test_agg_config3_shape_reduced():
 @pytest.mark.parametrize("hint,local_env", [(0, None), (300, None), (200_000, None), (0, "0"), (200_000, "2")])
 def test_agg_two_level_paths_vs_oracle(hint, local_env, monkeypatch):
     # the round-2 two-level update (csrc/agg_update.cuh): CTA-local tables + global table, every combination of
-    # hint / forced mode, on skewed keys (a few hot groups + a long tail), NULL groups, the sentinel-valued key, 1 % NULL x
+    # hint / forced mode, on skewed keys (a few hot groups + a long tail), NULL groups, the sentinel-valued key, 1 % NULL x.
+    # The CTA-local level takes at most 4 device states, so the aggregates are split over two plans; tg_agg_stats shows
+    # which level ran
+    monkeypatch.delenv("TG_AGG_LOCAL", raising=False)
+    monkeypatch.delenv("TG_AGG_V1", raising=False)
     if local_env is not None:
         monkeypatch.setenv("TG_AGG_LOCAL", local_env)
+    # the CTA-local level runs for hints up to 4096 groups (or no hint) unless TG_AGG_LOCAL=0; TG_AGG_LOCAL=2 forces it
+    local = local_env == "2" or (local_env != "0" and hint <= 4096)
     rng = np.random.default_rng(11 + hint)
     n = 400_000
     hot = rng.integers(0, 8, n)
@@ -151,10 +173,16 @@ def test_agg_two_level_paths_vs_oracle(hint, local_env, monkeypatch):
     x = np.floor(rng.random(n) * 1e7); xn = rng.random(n) < 0.01
     y = rng.integers(-(1 << 40), 1 << 40, n).astype(np.int64)
     chunks = Chunk([Column(g, gn), Column(x, xn), Column(y)]).split(1 << 16)
-    plan = AggPlan([INT, DBL, INT_NN], [0], [
-        AggFunc(abi.AGG_FIRSTROW, 0), AggFunc(abi.AGG_SUM, 1, abi.TYPE_DOUBLE), AggFunc(abi.AGG_COUNT, 1, abi.TYPE_DOUBLE),
-        AggFunc(abi.AGG_COUNT, -1), AggFunc(abi.AGG_MAX, 2), AggFunc(abi.AGG_MIN, 1, abi.TYPE_DOUBLE)], expected_groups=hint)
-    assert_agg_equal(run_orc_agg(plan, chunks), run_gpu_agg(plan, chunks), {1})
+    for funcs, float_cols in (([AggFunc(abi.AGG_FIRSTROW, 0), AggFunc(abi.AGG_SUM, 1, abi.TYPE_DOUBLE), AggFunc(abi.AGG_COUNT, 1, abi.TYPE_DOUBLE),
+                                AggFunc(abi.AGG_COUNT, -1), AggFunc(abi.AGG_MAX, 2)], {1}),
+                              ([AggFunc(abi.AGG_FIRSTROW, 0), AggFunc(abi.AGG_COUNT, -1), AggFunc(abi.AGG_MIN, 1, abi.TYPE_DOUBLE)], set())):
+        plan = AggPlan([INT, DBL, INT_NN], [0], funcs, expected_groups=hint)
+        got, st = run_gpu_agg_stats(plan, chunks)
+        assert_agg_equal(run_orc_agg(plan, chunks), got, float_cols)
+        if local:
+            assert st.paths & abi.AGG_PATH_V2_LOCAL and st.local_rows > 0, (hex(st.paths), st.local_rows)
+        else:
+            assert st.paths & abi.AGG_PATH_V2_GLOBAL and not st.paths & abi.AGG_PATH_V2_LOCAL and st.local_rows == 0, (hex(st.paths), st.local_rows)
 
 
 @pytest.mark.parametrize("ncols,nullable", [(2, False), (3, True), (4, True)])

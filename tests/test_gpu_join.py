@@ -28,6 +28,22 @@ def run_gpu(plan, left, right, required_rows=1024):
     return rows
 
 
+def run_gpu_stats(plan, left, right, required_rows=1024):
+    """run_gpu, plus the handle's tg_join_stats read before close"""
+    e = HashJoinExec(plan, MockDataSource(plan.left_types, left), MockDataSource(plan.right_types, right))
+    e.open()
+    try:
+        rows = []
+        while True:
+            c = e.next(required_rows)
+            if c.num_rows() == 0:
+                break
+            rows.extend(columns_to_rows([(col_.data, col_.nulls()) for col_ in c.columns]))
+        return rows, e.stats()
+    finally:
+        e.close()
+
+
 def test_device_present():
     lib = abi.load_lib()
     assert lib.tg_device_count() > 0, "GPU tests need a CUDA device"
@@ -235,7 +251,7 @@ def test_gpu_time_join_keys_unique_build_and_gate():
 def test_gpu_unique_key_single_pass_probe(build_is_right, uq, monkeypatch):
     # k_probe_inner_uq: inner join, unique build keys, two NOT NULL build payload columns (row store), probe filters, a probe
     # key column with NULLs that is not output, the sentinel-valued key; TG_PROBE_UQ=0 sends the same plan down the general
-    # count -> scan -> write path, both against the oracle
+    # count -> scan -> write path, both against the oracle, and tg_join_stats.paths shows which path ran
     monkeypatch.setenv("TG_PROBE_UQ", uq)
     rng = np.random.default_rng(77 + int(build_is_right))
     nb, npr = 40_000, 300_000
@@ -255,7 +271,10 @@ def test_gpu_unique_key_single_pass_probe(build_is_right, uq, monkeypatch):
     else:
         plan = JoinPlan(abi.JOIN_INNER, btypes, ptypes, [0], [1], build_is_right=False, lused=[2, 1], rused=[0, 2], probe_filter=pf)
         l, r = build.split(1 << 13), probe.split(1 << 15)
-    assert_rows_equal(run_oracle(plan, l, r), run_gpu(plan, l, r, required_rows=1 << 16))
+    got, st = run_gpu_stats(plan, l, r, required_rows=1 << 16)
+    assert_rows_equal(run_oracle(plan, l, r), got)
+    ran, skipped = (abi.JOIN_PATH_PROBE_UQ, abi.JOIN_PATH_PROBE_GENERAL) if uq == "1" else (abi.JOIN_PATH_PROBE_GENERAL, abi.JOIN_PATH_PROBE_UQ)
+    assert st.paths & ran and not st.paths & skipped, hex(st.paths)
 
 
 @pytest.mark.parametrize("required_rows", [1, 3, 13])
@@ -391,6 +410,24 @@ def test_partial_match_and_stats():
     assert np.array_equal(columns_sorted(ocols), columns_sorted([(g, np.zeros(len(g), dtype=bool)) for g in got]))
 
 
+def _fused_variant_paths(env):
+    """(bits that must be set, bits that must be clear) in tg_join_stats.paths for a test_fused_probe_variants_forced env"""
+    J = abi
+    seg, bulk, other, direct, tile = J.JOIN_PATH_PROBE_SEG, J.JOIN_PATH_SCATTER_BULK, J.JOIN_PATH_SCATTER, J.JOIN_PATH_PROBE_DIRECT, J.JOIN_PATH_PROBE_TILE
+    never = J.JOIN_PATH_PROBE_UQ | J.JOIN_PATH_PROBE_GENERAL
+    if env.get("TG_PROBE_VARIANT") == "0":           # CTA-tile kernel; the partition pass needs the warp kernels
+        return tile, never | direct | seg | bulk | other
+    part = env.get("TG_PROBE_PARTITION", "1")
+    if part == "0":
+        return direct, never | tile | seg | bulk | other
+    if part == "1":                                  # count-free pass: bulk scatter, segment probe (8-byte warp kernel without SEG_VEC)
+        if env.get("TG_PROBE_SEG_VEC") == "0":
+            return direct | bulk, never | tile | seg | other
+        return direct | bulk | seg, never | tile | other
+    scatter, no_scatter = (other, bulk) if env.get("TG_SCATTER_BULK") == "0" else (bulk, other)
+    return direct | scatter, never | tile | seg | no_scatter   # counted pass, then the warp kernel over dense partitions
+
+
 @pytest.mark.parametrize("env", [dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="5"), dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="16"),
                                  dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="7", TG_PROBE_SEG_VEC="0"),
                                  dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="5", TG_PROBE_SEG_LEAN="0"), dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="6", TG_PROBE_SEG_LEAN="2"),
@@ -402,6 +439,8 @@ def test_partial_match_and_stats():
 def test_fused_probe_variants_forced(env, monkeypatch):
     # every launch variant of the fused fast path (L2 partition pass in both layouts, segment kernels, warp kernel, CTA-tile kernel) must
     # give the same multiset; odd sizes exercise the tail tiles; PART_MIN_MB=0 forces the partition pass on a small table
+    for k in ("TG_PROBE_VARIANT", "TG_PROBE_SEG_VEC", "TG_SCATTER_BULK", "TG_PROBE_UQ"):
+        monkeypatch.delenv(k, raising=False)
     for k, v in dict(env, TG_PROBE_PART_MIN_MB="0", TG_PROBE_PART_MIN_ROWS="0").items():
         monkeypatch.setenv(k, v)
     rng = np.random.default_rng(17)
@@ -414,7 +453,18 @@ def test_fused_probe_variants_forced(env, monkeypatch):
     probe = Chunk([Column(pk), Column(np.arange(npr, dtype=np.int64))])
     plan = JoinPlan(abi.JOIN_INNER, [INT_NN, INT_NN], [INT_NN, INT_NN], [0], [0])
     e = HashJoinExec(plan, MockDataSource(plan.left_types, [probe]), MockDataSource(plan.right_types, [build]))
-    chunks = drain(e, 1 << 22)
+    e.open()
+    chunks = []
+    while True:
+        c = e.next(1 << 22)
+        if c.num_rows() == 0:
+            break
+        chunks.append(c)
+    paths = e.stats().paths
+    e.close()
+    # the kernel families this environment selects ran, and no other
+    want, dont = _fused_variant_paths(env)
+    assert paths & want == want and paths & dont == 0, (hex(paths), hex(want), hex(dont))
     got = [np.concatenate([c.columns[i].data for c in chunks]) for i in range(4)]
     order = np.argsort(bk); sb = bk[order]
     pos = np.searchsorted(sb, pk); pos[pos >= nb] = nb - 1

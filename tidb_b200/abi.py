@@ -82,7 +82,7 @@ class TgJoinStats(C.Structure):
     _fields_ = [("build_rows", C.c_int64), ("build_valid_keys", C.c_int64),
                 ("table_slots", C.c_int64), ("distinct_keys", C.c_int64), ("max_dup", C.c_int64),
                 ("probe_rows", C.c_int64), ("output_rows", C.c_int64),
-                ("kernel_launches", C.c_int64), ("table_mode", C.c_int32), ("reserved", C.c_int32),
+                ("kernel_launches", C.c_int64), ("table_mode", C.c_int32), ("paths", C.c_int32),
                 ("build_ms", C.c_double), ("probe_ms", C.c_double),
                 ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64)]
 
@@ -117,7 +117,15 @@ class TgAggDesc(C.Structure):
 class TgAggStats(C.Structure):
     _fields_ = [("input_rows", C.c_int64), ("groups", C.c_int64), ("table_slots", C.c_int64),
                 ("kernel_launches", C.c_int64), ("update_ms", C.c_double),
-                ("finalize_ms", C.c_double), ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64)]
+                ("finalize_ms", C.c_double), ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64),
+                ("local_rows", C.c_int64), ("paths", C.c_int32), ("reserved", C.c_int32)]
+
+
+# tg_join_stats.paths / tg_agg_stats.paths: kernel families a handle has launched
+JOIN_PATH_PROBE_UQ, JOIN_PATH_PROBE_GENERAL, JOIN_PATH_PROBE_DIRECT, JOIN_PATH_PROBE_SEG = 1 << 0, 1 << 1, 1 << 2, 1 << 3
+JOIN_PATH_PROBE_TILE, JOIN_PATH_SCATTER_BULK, JOIN_PATH_SCATTER = 1 << 4, 1 << 5, 1 << 6
+AGG_PATH_NOGROUP, AGG_PATH_V2_GLOBAL, AGG_PATH_V2_LOCAL, AGG_PATH_MULTI_KEY = 1 << 0, 1 << 1, 1 << 2, 1 << 3
+AGG_PATH_V1_LOCAL, AGG_PATH_V1_GLOBAL, AGG_PATH_MERGE = 1 << 4, 1 << 5, 1 << 6
 
 
 # every symbol include/tidbgpu.h declares; tests/test_abi_exports.py checks the .so exports them all

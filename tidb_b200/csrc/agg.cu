@@ -85,6 +85,12 @@ __device__ __forceinline__ double ordered_to_f64(unsigned long long u) {
 }
 __device__ __forceinline__ unsigned long long i64_to_ordered(long long v) { return (unsigned long long)v ^ 0x8000000000000000ull; }
 
+// home slot of a single-column group key in the global table.  Every kernel that places or looks up such a key uses it —
+// the update kernels (k_agg_update, k_agg_update2), the merge of partial results and the rehash into a grown table: a key
+// that a rehash or a merge placed by another function is not found by the next lookup, which inserts a second copy of
+// its group
+__device__ __forceinline__ uint32_t agg_home(long long k, unsigned long long nslots) { return slot32(hash64((unsigned long long)k), (uint32_t)nslots); }
+
 __global__ void k_agg_init(AggTable t, AggSpec spec, unsigned long long n_total) {
   unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
   unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
@@ -174,7 +180,7 @@ k_agg_update(GroupKey gk, DevCols cols, int64_t n, AggTable t, AggSpec spec, uns
       }
       if (k == kEmptyKey) s = t.nslots + 1;
       else {
-        s = slot_of(mix64((uint64_t)k), t.nslots);
+        s = agg_home(k, t.nslots);
         bool defer = false;
         // No global fill counter: one atomic per NEW key on a single address serialised at ~3 ns each (1 M groups =
         // 3 ms, twice the rest of the kernel).  A probe sequence longer than `max_fill` steps means the table is
@@ -361,7 +367,7 @@ k_agg_merge(AggPartials in, int64_t m, AggTable t, AggSpec spec, unsigned long l
     else if (in.kind[i] == 2) s = t.nslots + 1;
     else {
       long long k = in.keys[i];
-      s = slot_of(mix64((uint64_t)k), t.nslots);
+      s = agg_home(k, t.nslots);
       bool defer = false;
       unsigned int steps = 0;
       for (;;) {
@@ -404,7 +410,7 @@ __global__ void k_agg_rehash(AggTable oldt, AggTable newt, AggSpec spec, int nst
     else {
       long long k = oldt.keys[i];
       if (k == kEmptyKey) continue;
-      s = slot_of(mix64((uint64_t)k), newt.nslots);
+      s = agg_home(k, newt.nslots);
       for (;;) {
         unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(&newt.keys[s]), (unsigned long long)kEmptyKey, (unsigned long long)k);
         if (old == (unsigned long long)kEmptyKey) break;
@@ -649,7 +655,7 @@ struct AggImpl {
   DevBuf tbl_mem;
   AggTable tbl{};
   unsigned long long nslots = 0;
-  DevBuf scalars;              // [0] fill [1] n_deferred [2] out cursor
+  DevBuf scalars;              // [0] fill [1] n_deferred [2] out cursor ... [6] rows the CTA-local level absorbed (zeroed with the table) [7] overflow
   DevBuf deferred, partials_mem;
   int64_t expected_groups = 0;
   int local_mode = -1;            // -1 undecided, 0 global atomics only, 1 CTA-local partial aggregation first
@@ -850,6 +856,7 @@ static int merge_partials(AggImpl* a, const AggPartials& pp, unsigned long long 
     unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
     k_agg_merge<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->tbl, a->spec, max_fill, sc, mdef.as<uint32_t>(), only, sc + 4);
     a->stats.kernel_launches++;
+    a->stats.paths |= TG_AGG_PATH_MERGE;
     unsigned long long nd = 0;
     TG_CUDA(cudaMemcpyAsync(&nd, sc + 4, 8, cudaMemcpyDeviceToHost, a->stream));
     TG_CUDA(cudaStreamSynchronize(a->stream));
@@ -888,6 +895,7 @@ static int update_grouped_mk(AggImpl* a, const DevCols& cols, int64_t n, unsigne
     TG_CUDA(cudaMemsetAsync(sc + 1, 0, 8, a->stream));
     k_agg_update_mk<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, 48u, a->deferred.as<uint32_t>(), only, sc + 1);
     a->stats.kernel_launches++;
+    a->stats.paths |= TG_AGG_PATH_MULTI_KEY;
     unsigned long long nd = 0;
     TG_CUDA(cudaMemcpyAsync(&nd, sc + 1, 8, cudaMemcpyDeviceToHost, a->stream));
     TG_CUDA(cudaStreamSynchronize(a->stream));
@@ -910,8 +918,7 @@ static int update_grouped_v2(AggImpl* a, const GroupKey& gk, const DevCols& cols
   TG_TRY(a->deferred.ensure(a->device, dwords * 4 + 16));
   TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
   // CTA-local level: on for small / unknown cardinalities (a CTA turns it off by itself when its hit rate is low)
-  static int env_local = -1, env_slots = 0;
-  if (env_local < 0) { const char* e = getenv("TG_AGG_LOCAL"); env_local = e ? atoi(e) : 1; const char* s2 = getenv("TG_AGG_LOCAL_SLOTS"); env_slots = s2 ? atoi(s2) : 0; }
+  const int env_local = env_int("TG_AGG_LOCAL", 1), env_slots = env_int("TG_AGG_LOCAL_SLOTS", 0);
   bool local = env_local != 0 && a->nstates <= AGG_LOCAL_MAX_STATES && (a->expected_groups == 0 || a->expected_groups <= 4096);
   if (env_local == 2) local = a->nstates <= AGG_LOCAL_MAX_STATES;
   int local_slots = (env_slots == 512 || env_slots == 1024 || env_slots == 2048 || env_slots == 4096) ? env_slots : 2048;
@@ -937,9 +944,11 @@ static int update_grouped_v2(AggImpl* a, const GroupKey& gk, const DevCols& cols
     if (local && round == 0) k_agg_update2<true><<<grid, AGG2_BLOCK, smem, a->stream>>>(p, cols, a->tbl, a->spec);
     else k_agg_update2<false><<<grid, AGG2_BLOCK, 0, a->stream>>>(p, cols, a->tbl, a->spec);
     a->stats.kernel_launches++;
+    a->stats.paths |= (local && round == 0) ? TG_AGG_PATH_V2_LOCAL : TG_AGG_PATH_V2_GLOBAL;
     unsigned long long back[8] = {0};
     TG_CUDA(cudaMemcpyAsync(back, sc, 64, cudaMemcpyDeviceToHost, a->stream));
     TG_CUDA(cudaStreamSynchronize(a->stream));
+    a->stats.local_rows = (int64_t)back[6];   // cumulative since the table was created
     const unsigned long long nd = back[1], spilled = (local && round == 0) ? back[5] : 0;
     if (nd == 0 && spilled == 0) break;
     if (spilled > p.spill_cap) return fail(TG_ERR_CUDA, "internal: aggregation spill buffer overflow");
@@ -980,6 +989,7 @@ static int local_partial_pass(AggImpl* a, const GroupKey& gk, const DevCols& col
   TG_CUDA(cudaFuncSetAttribute(k_agg_update_local, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_agg_update_local<<<grid, 256, smem, a->stream>>>(gk, cols, lo, hi, a->spec, a->nstates, local_slots, pp, a->deferred.as<uint32_t>(), sc + 1);
   a->stats.kernel_launches++;
+  a->stats.paths |= TG_AGG_PATH_V1_LOCAL;
   unsigned long long m = 0;
   TG_CUDA(cudaMemcpyAsync(&m, sc + 3, 8, cudaMemcpyDeviceToHost, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
@@ -995,6 +1005,7 @@ static int local_partial_pass(AggImpl* a, const GroupKey& gk, const DevCols& col
     unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
     k_agg_merge<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->tbl, a->spec, max_fill, sc, mdef.as<uint32_t>(), only, sc + 4);
     a->stats.kernel_launches++;
+    a->stats.paths |= TG_AGG_PATH_MERGE;
     unsigned long long nd = 0;
     TG_CUDA(cudaMemcpyAsync(&nd, sc + 4, 8, cudaMemcpyDeviceToHost, a->stream));
     TG_CUDA(cudaStreamSynchronize(a->stream));
@@ -1032,6 +1043,7 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
   if (a->group_col < 0) {
     k_agg_update_nogroup<<<agrid(a, n, 256, 4), 256, 0, a->stream>>>(cols, n, a->tbl, a->spec);
     a->stats.kernel_launches++;
+    a->stats.paths |= TG_AGG_PATH_NOGROUP;
   } else {
     if (a->nkw) {
       TG_TRY(update_grouped_mk(a, cols, n, sc));
@@ -1042,9 +1054,7 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
       return TG_OK;
     }
     GroupKey gk{cols.data[a->group_col], cols.nulls[a->group_col], a->gk_kind, 0};
-    static int v1 = -1;
-    if (v1 < 0) { const char* e = getenv("TG_AGG_V1"); v1 = e ? atoi(e) : 0; }
-    if (!v1) {
+    if (!env_int("TG_AGG_V1", 0)) {
       TG_TRY(update_grouped_v2(a, gk, cols, n, sc));
       TG_CUDA(cudaEventRecord(a->ev1, a->stream));
       TG_CUDA(cudaStreamSynchronize(a->stream));
@@ -1096,6 +1106,7 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
         unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
         k_agg_update<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, max_fill, sc, a->deferred.as<uint32_t>(), only, sc + 1);
         a->stats.kernel_launches++;
+        a->stats.paths |= TG_AGG_PATH_V1_GLOBAL;
         unsigned long long nd = 0;
         TG_CUDA(cudaMemcpyAsync(&nd, sc + 1, 8, cudaMemcpyDeviceToHost, a->stream));
         TG_CUDA(cudaStreamSynchronize(a->stream));

@@ -243,7 +243,7 @@ k_agg_update2(Agg2Params p, DevCols cols, AggTable t, AggSpec spec) {
 #pragma unroll
     for (int r = 0; r < AGG2_R; r++) {
       cur[r] = 0;
-      if (kind[r] == 0) { slot[r] = slot32(hash64((unsigned long long)key[r]), S); cur[r] = *reinterpret_cast<volatile long long*>(&t.keys[slot[r]]); }
+      if (kind[r] == 0) { slot[r] = agg_home(key[r], S); cur[r] = *reinterpret_cast<volatile long long*>(&t.keys[slot[r]]); }
     }
 #pragma unroll
     for (int r = 0; r < AGG2_R; r++) {
@@ -283,7 +283,7 @@ k_agg_update2(Agg2Params p, DevCols cols, AggTable t, AggSpec spec) {
     if (i == lt.ls) s = t.nslots;
     else if (i == lt.ls + 1) s = t.nslots + 1;
     else {
-      uint32_t sl = slot32(hash64((unsigned long long)k), S);
+      uint32_t sl = agg_home(k, S);
       long long c0 = *reinterpret_cast<volatile long long*>(&t.keys[sl]);
       ok = global_find_or_insert(t, k, sl, c0, p.max_probe);
       s = sl;

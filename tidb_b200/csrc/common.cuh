@@ -31,6 +31,11 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
 
 inline int fail(int code, const std::string& msg) { set_error(msg); return code; }
 
+// integer variant switch from the environment, read at every use (not cached): a process that changes it between calls,
+// such as a test forcing one kernel variant after another, gets the variant it asked for.  One getenv per host-side
+// launch decision.
+inline int env_int(const char* name, int dflt) { const char* v = getenv(name); return (v && *v) ? atoi(v) : dflt; }
+
 // pkg/util/chunk/codec.go:165-179 getFixedLen
 inline int fixed_len(int tp) {
   switch (tp) {

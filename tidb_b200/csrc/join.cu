@@ -152,8 +152,6 @@ struct JoinImpl {
 
 namespace tg {
 
-static int env_int(const char* name, int dflt) { const char* v = getenv(name); return (v && *v) ? atoi(v) : dflt; }
-
 static int grid_for(const JoinImpl* j, int64_t n, int block, int per_sm) {
   int64_t need = (n + block - 1) / block;
   int64_t cap = (int64_t)j->nsm * per_sm;
@@ -715,9 +713,7 @@ static bool fast_path_ok(const JoinImpl* j, const DevCols& pview) {
 // single-pass unique-key probe (k_probe_inner_uq): inner join, every build key unique, no OtherCondition, 8-byte output
 // columns that cannot be NULL (probe used columns without a bitmap in this batch, build columns without NULLs)
 static bool uq_path_ok(const JoinImpl* j, const DevCols& pview) {
-  static int en = -1;
-  if (en < 0) en = env_int("TG_PROBE_UQ", 1);
-  if (!en || j->probe_kind != PK_INNER || j->need_scan || !j->other.empty() || j->stats.max_dup > 1) return false;
+  if (!env_int("TG_PROBE_UQ", 1) ||j->probe_kind != PK_INNER || j->need_scan || !j->other.empty() || j->stats.max_dup > 1) return false;
   if (j->tv.mode != TABLE_U1 && j->tv.mode != TABLE_G) return false;
   for (int c : j->probe.used) if (j->probe.elem[c] != 8 || pview.nulls[c]) return false;
   for (int c : j->build.used) if (j->build.elem[c] != 8 || j->bcols.has_nulls[c]) return false;
@@ -832,9 +828,11 @@ struct LaunchSeg {
 };
 static int launch_probe_warp(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t,
                              const SegSpec& seg = SegSpec{nullptr, 0, 0, 0, nullptr}) {
+  j->stats.paths |= TG_JOIN_PATH_PROBE_DIRECT;
   return dispatch_shape<LaunchWarp>(fo, j, pkey, n, fo, cur, t, seg);
 }
 static int launch_probe_seg(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t, const SegSpec& seg) {
+  j->stats.paths |= TG_JOIN_PATH_PROBE_SEG;
   return dispatch_shape<LaunchSeg>(fo, j, pkey, n, fo, cur, t, seg);
 }
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -914,7 +912,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
             }
             if (in_seg) { d.in_cnt = in_seg->cnt; d.in_cap = in_seg->cap; d.in_tiles_per_seg = (uint32_t)(in_seg->cap / PTILE); }
             TG_TRY(launch_partition_scatter<true>(j->device, j->stream, reinterpret_cast<const long long*>(pkey), nullptr, n_main, d, cursors,
-                                                  &j->stats.kernel_launches));
+                                                  &j->stats.kernel_launches, 0, &j->stats.paths));
             FastOut pf = fo;
             for (int c = 0; c < fo.n_pcols; c++) pf.psrc[c] = j->part_cols[1 + c]->as<unsigned long long>();
             // the 128-bit stores of the segment kernel need 16-byte aligned output columns: results appended behind an odd
@@ -954,7 +952,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
             for (int c = 0; c < fo.n_pcols; c++) d.src[1 + c] = fo.psrc[c];
             for (int c = 0; c < nc; c++) for (int q = 0; q < P; q++) d.dst[q][c] = j->part_cols[c]->p;
             d.dst_base = offs;
-            TG_TRY(launch_partition_scatter<true>(j->device, j->stream, k64, nullptr, n, d, cursors, &j->stats.kernel_launches));
+            TG_TRY(launch_partition_scatter<true>(j->device, j->stream, k64, nullptr, n, d, cursors, &j->stats.kernel_launches, 0, &j->stats.paths));
             pkey = j->part_cols[0]->as<int64_t>();
             for (int c = 0; c < fo.n_pcols; c++) fo.psrc[c] = j->part_cols[1 + c]->as<unsigned long long>();
           }
@@ -973,6 +971,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
         int grid = (int)std::min<int64_t>(tiles, (int64_t)j->nsm * (tune.ctas_per_sm > 0 ? tune.ctas_per_sm : 8));
         k_probe_inner_u1<R><<<grid, 256, 0, j->stream>>>(reinterpret_cast<const int64_t*>(ks.data), pview, n, j->tv, oc, cur);
         j->stats.kernel_launches++;
+        j->stats.paths |= TG_JOIN_PATH_PROBE_TILE;
       }
     }
     if (sync_count) {
@@ -997,6 +996,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
       int grid = (int)std::min<int64_t>(tiles, (int64_t)j->nsm * 8);
       k_probe_inner_uq<<<grid, 256, 0, j->stream>>>(ks, pview, p.filter, n, j->tv, oc, cur);
       j->stats.kernel_launches++;
+      j->stats.paths |= TG_JOIN_PATH_PROBE_UQ;
     }
     // the output row count decides rb.rows (and the next append position): always needed on the host
     unsigned long long got = 0;
@@ -1033,6 +1033,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
     k_probe_count<<<grid_for(j, m, 256, 8), 256, 0, j->stream>>>(sks, sub, p.filter, j->dev_other, m, j->tv, j->probe_kind, j->tmp_cnt.as<uint32_t>(),
                                                                  j->tmp_slot.as<uint32_t>(), j->need_scan ? j->slot_used.as<uint8_t>() : nullptr);
     j->stats.kernel_launches++;
+    j->stats.paths |= TG_JOIN_PATH_PROBE_GENERAL;
     unsigned long long total = 0;
     TG_TRY(scan_counts(j, m, &total));
     if (total) {

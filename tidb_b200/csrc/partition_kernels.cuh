@@ -484,11 +484,7 @@ inline int launch_partition_count(int device, cudaStream_t st, const long long* 
   return TG_OK;
 }
 
-inline int scatter_bulk_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("TG_SCATTER_BULK"); v = e ? atoi(e) : 1; }
-  return v;
-}
+inline int scatter_bulk_enabled() { return env_int("TG_SCATTER_BULK", 1); }
 
 // grid the bulk scatter will use for n rows of NC columns (the CTA-private sub-segment layout depends on it)
 template <int NC>
@@ -503,7 +499,8 @@ inline int scatter_bulk_grid_nc(int device, int64_t n, int nc) {
 }
 
 template <bool HIGH, int NC>
-inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d, unsigned long long* cursors, int64_t* launches, int ctas_per_sm = 0) {
+inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d, unsigned long long* cursors, int64_t* launches, int ctas_per_sm,
+                             int32_t* paths) {
   int nsm = device_sm_count(device);
   if (scatter_bulk_enabled()) {
     // 1024-row tiles: 4 CTAs per SM for NC <= 2
@@ -515,14 +512,14 @@ inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d,
       int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (smem + 1024)));
       // a scatter that runs NEXT TO a probe kernel (exchange of step k+1 under the probe of step k) should leave the SMs'
       // L1 to the probe: TG_SCATTER_CTAS_PER_SM caps the CTAs (and with them the shared-memory carve-out) per SM
-      static int cap_env = -1;
-      if (cap_env < 0) { const char* e = getenv("TG_SCATTER_CTAS_PER_SM"); cap_env = e ? atoi(e) : 0; }
+      const int cap_env = env_int("TG_SCATTER_CTAS_PER_SM", 0);
       if (!HIGH && cap_env > 0 && per_sm > cap_env) per_sm = cap_env;
       if (ctas_per_sm > 0 && per_sm > ctas_per_sm) per_sm = ctas_per_sm;
       int grid = (int)std::min<int64_t>(ntiles, (int64_t)nsm * per_sm);
       if (d.sub_cap > 0 && (uint32_t)grid != d.sub_grid) return fail(TG_ERR_CUDA, "internal: sub-segment layout sized for another grid");
       k_partition_scatter_bulk<HIGH, NC, ITEMS><<<grid, PT_BLOCK, smem, st>>>(ntiles, d, cursors);
       if (launches) (*launches)++;
+      if (paths) *paths |= TG_JOIN_PATH_SCATTER_BULK;
     }
     int64_t done = ntiles * TILE;
     if (done < n) {
@@ -541,6 +538,7 @@ inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d,
     int grid = (int)std::min<int64_t>(ntiles, (int64_t)nsm * 2);
     k_partition_scatter_tma<HIGH, NC><<<grid, PT_BLOCK, smem, st>>>(ntiles, d, cursors);
     if (launches) (*launches)++;
+    if (paths) *paths |= TG_JOIN_PATH_SCATTER;
   }
   int64_t done = ntiles * PT_TILE;
   if (done < n) {
@@ -552,10 +550,12 @@ inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d,
   return TG_OK;
 }
 
-// d.src[0] must be the key column; falls back to the LSU kernel for NULL-able keys, unaligned sources or > 4 columns
+// d.src[0] must be the key column; falls back to the LSU kernel for NULL-able keys, unaligned sources or > 4 columns.
+// `paths` (optional) gains TG_JOIN_PATH_SCATTER_BULK when the bulk kernel ran, TG_JOIN_PATH_SCATTER for the other
+// full-tile kernels (the < 1-tile remainder kernel is not counted)
 template <bool HIGH>
 inline int launch_partition_scatter(int device, cudaStream_t st, const long long* key, const uint8_t* nulls, int64_t n, PartDst& d,
-                                    unsigned long long* cursors, int64_t* launches, int ctas_per_sm = 0) {
+                                    unsigned long long* cursors, int64_t* launches, int ctas_per_sm = 0, int32_t* paths = nullptr) {
   if (n <= 0) return TG_OK;
   bool tma_ok = !nulls && d.ncols <= 4 && d.src[0] == (const void*)key;
   for (int c = 0; c < d.ncols && tma_ok; c++) tma_ok = ptr_aligned16(d.src[c]);
@@ -563,10 +563,10 @@ inline int launch_partition_scatter(int device, cudaStream_t st, const long long
   for (int p = 0; p < d.nparts && tma_ok; p++) for (int c = 0; c < d.ncols && tma_ok; c++) tma_ok = ptr_aligned16(d.dst[p][c]);
   if (tma_ok) {
     switch (d.ncols) {
-      case 1: return launch_scatter_nc<HIGH, 1>(device, st, n, d, cursors, launches, ctas_per_sm);
-      case 2: return launch_scatter_nc<HIGH, 2>(device, st, n, d, cursors, launches, ctas_per_sm);
-      case 3: return launch_scatter_nc<HIGH, 3>(device, st, n, d, cursors, launches, ctas_per_sm);
-      default: return launch_scatter_nc<HIGH, 4>(device, st, n, d, cursors, launches, ctas_per_sm);
+      case 1: return launch_scatter_nc<HIGH, 1>(device, st, n, d, cursors, launches, ctas_per_sm, paths);
+      case 2: return launch_scatter_nc<HIGH, 2>(device, st, n, d, cursors, launches, ctas_per_sm, paths);
+      case 3: return launch_scatter_nc<HIGH, 3>(device, st, n, d, cursors, launches, ctas_per_sm, paths);
+      default: return launch_scatter_nc<HIGH, 4>(device, st, n, d, cursors, launches, ctas_per_sm, paths);
     }
   }
   int nsm = device_sm_count(device);
@@ -574,6 +574,7 @@ inline int launch_partition_scatter(int device, cudaStream_t st, const long long
   int grid = (int)std::min<int64_t>(tiles, (int64_t)nsm * 4);
   k_partition_scatter<HIGH><<<grid, PT_BLOCK, 0, st>>>(key, nulls, n, d, cursors);
   if (launches) (*launches)++;
+  if (paths) *paths |= TG_JOIN_PATH_SCATTER;
   return TG_OK;
 }
 
