@@ -327,7 +327,27 @@ typedef struct tg_agg_func {
    *   TG_ARGEXPR_MUL        arg_col * arg_col2
    *   TG_ARGEXPR_MUL_CSUB   arg_col * (arg_const - arg_col2)      e.g. l_extendedprice * (1 - l_discount)            */
   int32_t arg_expr;
-  int32_t reserved;
+  /* AggFuncDesc.RetTp: GetType() and GetDecimal().  Any ret_type other than TG_TYPE_NEWDECIMAL (0 = not given) keeps the
+   * result type the function has always had here.  TG_TYPE_NEWDECIMAL asks for TiDB's exact DECIMAL result of SUM / AVG
+   * over an integer column (typeInfer4Sum / typeInfer4Avg, aggregation/base_func.go; the shim unwraps the
+   * cast(col AS DECIMAL) that WrapCastForAggArgs puts around it):
+   *   - Complete mode, arg_expr = TG_ARGEXPR_COL, an 8-byte integer-family column, signed or TG_FLAG_UNSIGNED;
+   *     anything else is TG_ERR_UNSUPPORTED.  SUM needs ret_frac = 0 and AVG 0 <= ret_frac <= 30, else TG_ERR_INVALID.
+   *   - SUM is the exact sum (NULL when the group has no non-NULL input, func_sum.go sum4Decimal).  AVG is
+   *     DecimalDiv(sum, count, ret_frac) rounded to ret_frac digits with ModeHalfUp (func_avg.go baseAvgDecimal): the
+   *     quotient is truncated at 9 * ceil(ret_frac / 9) fraction digits, so AVG rounds half away from zero unless ret_frac
+   *     is a multiple of 9, where it truncates toward zero.  NULL when the count is 0.  A result that is zero is never
+   *     negative.
+   *   - The output column holds 40-byte MyDecimal cells (types/mydecimal.go MyDecimal, copied whole into a chunk column):
+   *     int8 digitsInt, int8 digitsFrac, int8 resultFrac, bool negative, int32 wordBuf[9] in base 10^9, most significant
+   *     word first, integer words then fraction words, unused words 0.  The library writes one canonical form:
+   *     digitsInt = 9 * the number of integer words (at least one word, as FromUint makes it), digitsFrac = resultFrac =
+   *     ret_frac.  tg_agg_next fails with TG_ERR_INVALID unless the caller's tg_mut_column.elem_len for that column is 40;
+   *     tg_agg_result_dev returns a device column of 40-byte cells.
+   * The table keeps such a function in three 8-byte words (128-bit sum lo / hi, non-NULL count), so a plan needs at most
+   * 24 state words in all; more is TG_ERR_UNSUPPORTED.                                                                     */
+  int16_t ret_type;
+  int16_t ret_frac;
   double arg_const;
 } tg_agg_func;
 enum { TG_ARGEXPR_COL = 0, TG_ARGEXPR_MUL = 1, TG_ARGEXPR_MUL_CSUB = 2 };

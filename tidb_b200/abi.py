@@ -99,7 +99,7 @@ class TgMailTargets(C.Structure):
 class TgAggFunc(C.Structure):
     _fields_ = [("name", C.c_int32), ("mode", C.c_int32), ("arg_col", C.c_int32),
                 ("arg_type", C.c_int32), ("arg_flag", C.c_uint32), ("arg_col2", C.c_int32),
-                ("arg_expr", C.c_int32), ("reserved", C.c_int32), ("arg_const", C.c_double)]
+                ("arg_expr", C.c_int32), ("ret_type", C.c_int16), ("ret_frac", C.c_int16), ("arg_const", C.c_double)]
 
 
 ARGEXPR_COL, ARGEXPR_MUL, ARGEXPR_MUL_CSUB = 0, 1, 2

@@ -15,6 +15,10 @@ import numpy as np
 from . import abi
 
 
+DECIMAL_CELL = 40   # bytes of one MyDecimal cell in a chunk column
+DECIMAL_DTYPE = np.dtype((np.uint8, DECIMAL_CELL))   # numpy allocates it as (n, 40) uint8
+
+
 def pack_not_null_bitmap(nulls: np.ndarray) -> np.ndarray:
     """bool array (True = NULL) -> Column.nullBitmap bytes (bit 1 = NOT NULL, LSB first)."""
     return np.packbits(~np.asarray(nulls, dtype=bool), bitorder="little")
@@ -27,15 +31,19 @@ def unpack_nulls(bitmap: np.ndarray, n: int) -> np.ndarray:
 
 
 class Column:
-    """One fixed-width chunk.Column.  `data` is a 1-D numpy array of int64/uint64/float64/float32."""
+    """One fixed-width chunk.Column.  `data` is a 1-D numpy array of int64/uint64/float64/float32, or an (n, 40) uint8
+    array of MyDecimal cells (a DECIMAL column: types/mydecimal.go:236, copied whole into the column, column.go:41)."""
 
     def __init__(self, data: np.ndarray, nulls: Optional[np.ndarray] = None):
         data = np.ascontiguousarray(data)
-        if data.dtype.itemsize not in (4, 8):
-            raise ValueError("only 4/8-byte fixed-width columns are modelled")
+        if data.ndim == 2 and data.dtype == np.uint8 and data.shape[1] == DECIMAL_CELL:
+            self.elem_len = DECIMAL_CELL
+        elif data.dtype.itemsize in (4, 8):
+            self.elem_len = int(data.dtype.itemsize)
+        else:
+            raise ValueError("only 4/8-byte fixed-width columns and 40-byte DECIMAL cells are modelled")
         self.data = data
         self.length = int(data.shape[0])
-        self.elem_len = int(data.dtype.itemsize)
         if nulls is not None:
             nulls = np.asarray(nulls, dtype=bool)
             if nulls.shape[0] != self.length:

@@ -17,6 +17,7 @@
 #include <algorithm>
 #include "common.cuh"
 #include "tma.cuh"
+#include "decimal.cuh"
 
 namespace tg {
 
@@ -32,6 +33,8 @@ struct AggFuncDev {
   int32_t final_mode;   // TG_AGGMODE_FINAL: inputs are partial results
   int32_t arg_col2;
   int32_t arg_expr;     // TG_ARGEXPR_*
+  int32_t s2;           // >= 0: DECIMAL SUM / AVG of an integer column, an exact 128-bit sum: s0 its low word, s2 its high word
+  int32_t dec_frac;     // DECIMAL AVG: result scale (AggFuncDesc.RetTp decimal)
   int32_t pad;
   double arg_const;
 };
@@ -85,6 +88,20 @@ __device__ __forceinline__ double ordered_to_f64(unsigned long long u) {
 }
 __device__ __forceinline__ unsigned long long i64_to_ordered(long long v) { return (unsigned long long)v ^ 0x8000000000000000ull; }
 
+// DECIMAL SUM / AVG: adds the 128-bit value (ext:v) to the 128-bit sum (*hi:*lo).  The atomic that wraps the low word sees
+// its own carry, so the sum is exact in any order of the additions.  ext is v's high word: all ones for a negative signed
+// argument, 0 for a non-negative or unsigned one, so non-negative data pays the second atomic only on a carry.  The sum
+// cannot overflow: fewer than 2^63 rows of magnitude at most 2^64 stay below 2^127.
+__device__ __forceinline__ void dec_add(unsigned long long* lo, unsigned long long* hi, unsigned long long v, unsigned long long ext) {
+  const unsigned long long old = atomicAdd(lo, v);
+  const unsigned long long add = ext + (old + v < old ? 1ull : 0ull);
+  if (add) atomicAdd(hi, add);
+}
+// high word of an integer argument as a 128-bit value
+__device__ __forceinline__ unsigned long long dec_ext(const AggFuncDev& f, unsigned long long v) {
+  return f.is_unsigned ? 0ull : (unsigned long long)((long long)v >> 63);
+}
+
 // home slot of a single-column group key in the global table.  Every kernel that places or looks up such a key uses it —
 // the update kernels (k_agg_update, k_agg_update2), the merge of partial results and the rehash into a grown table: a key
 // that a rehash or a merge placed by another function is not found by the next lookup, which inserts a second copy of
@@ -106,6 +123,7 @@ __global__ void k_agg_init(AggTable t, AggSpec spec, unsigned long long n_total)
         t.state[f.s0][(size_t)i * t.stride] = init;
       }
       if (f.s1 >= 0) t.state[f.s1][(size_t)i * t.stride] = 0;
+      if (f.s2 >= 0) t.state[f.s2][(size_t)i * t.stride] = 0;
     }
   }
 }
@@ -124,6 +142,12 @@ __device__ __forceinline__ void agg_apply(const AggTable& t, const AggSpec& spec
         else atomicAdd(&t.state[f.s0][(size_t)s * t.stride], 1ull);
         break;
       case TG_AGG_SUM: {
+        if (f.s2 >= 0) {   // DECIMAL: exact 128-bit sum of the integer argument
+          const unsigned long long v = reinterpret_cast<const unsigned long long*>(cols.data[f.arg_col])[row];
+          dec_add(&t.state[f.s0][(size_t)s * t.stride], &t.state[f.s2][(size_t)s * t.stride], v, dec_ext(f, v));
+          if (f.s1 >= 0) atomicAdd(&t.state[f.s1][(size_t)s * t.stride], 1ull);
+          break;
+        }
         double v;
         if (!agg_arg_real(spec, f, cols, row, v)) break;
         atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][(size_t)s * t.stride]), v);
@@ -131,7 +155,11 @@ __device__ __forceinline__ void agg_apply(const AggTable& t, const AggSpec& spec
         break;
       }
       case TG_AGG_AVG:
-        if (f.final_mode) {   // args: count column, sum column (func_avg.go:405)
+        if (f.s2 >= 0) {
+          const unsigned long long v = reinterpret_cast<const unsigned long long*>(cols.data[f.arg_col])[row];
+          dec_add(&t.state[f.s0][(size_t)s * t.stride], &t.state[f.s2][(size_t)s * t.stride], v, dec_ext(f, v));
+          if (f.s1 >= 0) atomicAdd(&t.state[f.s1][(size_t)s * t.stride], 1ull);
+        } else if (f.final_mode) {   // args: count column, sum column (func_avg.go:405)
           const uint8_t* nb2 = cols.nulls[f.arg_col2];
           if (nb2 && !bit_not_null(nb2, row)) break;
           atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][(size_t)s * t.stride]), reinterpret_cast<const double*>(cols.data[f.arg_col2])[row]);
@@ -223,8 +251,15 @@ k_agg_update_nogroup(DevCols cols, int64_t n, AggTable t, AggSpec spec) {
     if (f.arg_col < 0 || f.s0 < 0) continue;
     const uint8_t* nb = cols.nulls[f.arg_col];
     double fs = 0; unsigned long long cnt = 0, ext = f.name == TG_AGG_MIN ? ~0ull : 0ull, isum = 0;
+    __int128 dsum = 0;   // DECIMAL SUM / AVG: exact
     for (int64_t i = i0; i < n; i += stride) {
       if (nb && !bit_not_null(nb, i)) continue;
+      if (f.s2 >= 0) {
+        const unsigned long long v = reinterpret_cast<const unsigned long long*>(cols.data[f.arg_col])[i];
+        dsum += f.is_unsigned ? (__int128)v : (__int128)(long long)v;
+        cnt++;
+        continue;
+      }
       if (f.name == TG_AGG_AVG && f.final_mode) {
         const uint8_t* nb2 = cols.nulls[f.arg_col2];
         if (nb2 && !bit_not_null(nb2, i)) continue;
@@ -248,6 +283,19 @@ k_agg_update_nogroup(DevCols cols, int64_t n, AggTable t, AggSpec spec) {
         else v = i64_to_ordered(reinterpret_cast<const long long*>(cols.data[f.arg_col])[i]);
         ext = f.name == TG_AGG_MIN ? (v < ext ? v : ext) : (v > ext ? v : ext);
       }
+    }
+    if (f.s2 >= 0) {
+      for (int o = 16; o; o >>= 1) {
+        const unsigned long long lo = __shfl_xor_sync(0xffffffffu, (unsigned long long)dsum, o);
+        const unsigned long long hi = __shfl_xor_sync(0xffffffffu, (unsigned long long)((unsigned __int128)dsum >> 64), o);
+        dsum += (__int128)(((unsigned __int128)hi << 64) | lo);
+        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+      }
+      if (lane == 0 && cnt) {
+        dec_add(&t.state[f.s0][t.nslots], &t.state[f.s2][t.nslots], (unsigned long long)dsum, (unsigned long long)((unsigned __int128)dsum >> 64));
+        if (f.s1 >= 0) atomicAdd(&t.state[f.s1][t.nslots], cnt);
+      }
+      continue;
     }
     for (int o = 16; o; o >>= 1) {
       fs += __shfl_xor_sync(0xffffffffu, fs, o);
@@ -304,6 +352,7 @@ k_agg_update_local(GroupKey gk, DevCols cols, int64_t row_lo, int64_t row_hi, Ag
       const AggFuncDev& f = spec.f[k];
       if (f.s0 >= 0) lt.state[f.s0][i] = f.name == TG_AGG_MIN ? ~0ull : 0ull;
       if (f.s1 >= 0) lt.state[f.s1][i] = 0;
+      if (f.s2 >= 0) lt.state[f.s2][i] = 0;
     }
   }
   if (threadIdx.x == 0) s_fill = 0;
@@ -389,7 +438,10 @@ k_agg_merge(AggPartials in, int64_t m, AggTable t, AggSpec spec, unsigned long l
         unsigned long long v = in.state[f.s0][i];
         switch (f.name) {
           case TG_AGG_COUNT: atomicAdd(&t.state[f.s0][s], v); break;                                                  // countPartial merge func_count.go:481
-          case TG_AGG_SUM: case TG_AGG_AVG: atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v)); break;   // func_sum.go:106, func_avg.go:444
+          case TG_AGG_SUM: case TG_AGG_AVG:   // func_sum.go:106, func_avg.go:444
+            if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, in.state[f.s2][i]);
+            else atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v));
+            break;
           case TG_AGG_MIN: atomicMin(&t.state[f.s0][s], v); break;
           case TG_AGG_MAX: atomicMax(&t.state[f.s0][s], v); break;
           default: break;
@@ -471,6 +523,15 @@ k_agg_finalize(AggTable t, AggSpec spec, int gk_kind, AggOut out, unsigned long 
     for (int k = 0; k < spec.n; k++) {
       const AggFuncDev& f = spec.f[k];
       unsigned long long nn = f.s1 >= 0 ? t.state[f.s1][(size_t)i * t.stride] : rows;   // non-NULL inputs seen
+      if (f.s2 >= 0) {   // DECIMAL SUM / AVG: a 40-byte MyDecimal cell, NULL without a non-NULL input (decimal.cuh)
+        uint8_t* cell = reinterpret_cast<uint8_t*>(out.data[k]) + (size_t)o * TG_DEC_CELL_BYTES;
+        const unsigned long long lo = t.state[f.s0][(size_t)i * t.stride], hi = t.state[f.s2][(size_t)i * t.stride];
+        if (nn == 0) dec_store_null(cell);
+        else if (f.name == TG_AGG_SUM) dec_sum_cell(cell, lo, hi);
+        else dec_avg_cell(cell, lo, hi, nn, f.dec_frac);
+        if (out.valid[k]) out.valid[k][o] = nn != 0 ? 1 : 0;
+        continue;
+      }
       bool valid = true;
       unsigned long long v = 0;
       switch (f.name) {
@@ -650,6 +711,7 @@ struct AggImpl {
   AggSpec spec{};
   int nstates = 0;
   std::vector<char> out_nullable;
+  std::vector<int> out_elem;   // bytes per result cell: 8, or 40 for a DECIMAL (MyDecimal) column
 
   // table
   DevBuf tbl_mem;
@@ -711,10 +773,25 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d) {
   a->spec.n = d->n_funcs;
   a->nstates = 0;
   a->out_nullable.assign(d->n_funcs, 0);
+  a->out_elem.assign(d->n_funcs, 8);
   for (int k = 0; k < d->n_funcs; k++) {
     const tg_agg_func& f = d->funcs[k];
     AggFuncDev& o = a->spec.f[k];
-    o = AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, 0, f.arg_const};
+    o = AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, -1, 0, 0, f.arg_const};
+    // DECIMAL SUM / AVG of an integer column (typeInfer4Sum / typeInfer4Avg, aggregation/base_func.go); any other ret_type
+    // keeps the result type each function has always had here
+    const bool dec = f.ret_type == TG_TYPE_NEWDECIMAL;
+    if (dec) {
+      if (f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG only");
+      if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG are offloaded in Complete mode only (no DECIMAL partial results)");
+      if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG take a plain column argument");
+      if (f.arg_col < 0 || f.arg_col >= a->ncols) return fail(TG_ERR_INVALID, "aggregate argument column out of range");
+      const int t = a->types[f.arg_col];
+      if (!is_int_family(t) || t == TG_TYPE_DURATION || a->elem[f.arg_col] != 8)
+        return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG are offloaded over 8-byte integer columns only");
+      if (f.name == TG_AGG_SUM && f.ret_frac != 0) return fail(TG_ERR_INVALID, "DECIMAL SUM of an integer column has scale 0");
+      if (f.name == TG_AGG_AVG && (f.ret_frac < 0 || f.ret_frac > 30)) return fail(TG_ERR_INVALID, "DECIMAL AVG scale must be 0..30");
+    }
     if (f.arg_expr != TG_ARGEXPR_COL) {
       if (f.arg_expr != TG_ARGEXPR_MUL && f.arg_expr != TG_ARGEXPR_MUL_CSUB) return fail(TG_ERR_INVALID, "unknown aggregate argument expression");
       if ((f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) || f.mode != TG_AGGMODE_COMPLETE)
@@ -738,13 +815,26 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d) {
         else if (f.arg_col >= 0 && arg_nullable) o.s0 = a->nstates++;   // NOT NULL COUNT(x) == COUNT(*) == rows[]
         break;
       case TG_AGG_SUM:
-        // SUM(int) yields DECIMAL in TiDB (aggregation/base_func.go:223-245): not offloaded
+        if (dec) {   // states: low word, high word, non-NULL count (a NOT NULL argument counts with rows[])
+          o.s0 = a->nstates++; o.s2 = a->nstates++;
+          if (arg_nullable) o.s1 = a->nstates++;
+          a->out_nullable[k] = 1; a->out_elem[k] = TG_DEC_CELL_BYTES;
+          break;
+        }
+        // SUM(int) yields DECIMAL in TiDB (aggregation/base_func.go:223-245): offloaded only when ret_type asks for it
         if (f.arg_col < 0 || atype != TG_TYPE_DOUBLE) return fail(TG_ERR_UNSUPPORTED, "SUM is offloaded for DOUBLE arguments only (SUM(int) is DECIMAL)");
         o.s0 = a->nstates++;
         if (arg_nullable) o.s1 = a->nstates++;
         a->out_nullable[k] = 1;
         break;
       case TG_AGG_AVG:
+        if (dec) {
+          o.s0 = a->nstates++; o.s2 = a->nstates++;
+          if (arg_nullable) o.s1 = a->nstates++;
+          o.dec_frac = f.ret_frac;
+          a->out_nullable[k] = 1; a->out_elem[k] = TG_DEC_CELL_BYTES;
+          break;
+        }
         if (o.final_mode) {
           if (f.arg_col < 0 || f.arg_col2 < 0 || a->types[f.arg_col2] != TG_TYPE_DOUBLE || !is_int_family(a->types[f.arg_col]))
             return fail(TG_ERR_UNSUPPORTED, "final AVG takes (count BIGINT, sum DOUBLE)");
@@ -774,6 +864,7 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d) {
       default: return fail(TG_ERR_UNSUPPORTED, "aggregate function is not offloaded");
     }
   }
+  if (a->nstates > 2 * TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "the aggregate list needs more than 24 state words (a DECIMAL SUM / AVG takes up to 3)");
   a->device = d->device;
   a->expected_groups = d->expected_groups;
   return TG_OK;
@@ -1239,7 +1330,7 @@ static int afinalize(AggImpl* a) {
   int64_t cap = (int64_t)fill + 2 + 1;
   AggOut ao{};
   for (int k = 0; k < nf; k++) {
-    TG_TRY(a->out_cols[k]->ensure(a->device, (size_t)cap * 8 + 16));
+    TG_TRY(a->out_cols[k]->ensure(a->device, (size_t)cap * a->out_elem[k] + 16));
     ao.data[k] = a->out_cols[k]->p;
     ao.valid[k] = nullptr;
     if (a->out_nullable[k] || default_row) { TG_TRY(a->out_valid[k]->ensure(a->device, (size_t)cap + 16)); ao.valid[k] = a->out_valid[k]->as<uint8_t>(); }
@@ -1254,8 +1345,8 @@ static int afinalize(AggImpl* a) {
   if (default_row && nrows == 0) {
     // write the default row on the host side: COUNT → 0, everything else NULL
     for (int k = 0; k < nf; k++) {
-      unsigned long long zero = 0; uint8_t v = a->spec.f[k].name == TG_AGG_COUNT ? 1 : 0;
-      TG_CUDA(cudaMemcpyAsync(a->out_cols[k]->p, &zero, 8, cudaMemcpyHostToDevice, a->stream));
+      uint8_t v = a->spec.f[k].name == TG_AGG_COUNT ? 1 : 0;
+      TG_CUDA(cudaMemsetAsync(a->out_cols[k]->p, 0, (size_t)a->out_elem[k], a->stream));
       TG_CUDA(cudaMemcpyAsync(a->out_valid[k]->p, &v, 1, cudaMemcpyHostToDevice, a->stream));
       TG_CUDA(cudaStreamSynchronize(a->stream));
     }
@@ -1362,9 +1453,13 @@ int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) 
   // any RequiredRows >= 1 is served: bitmaps that start inside a byte are fetched whole and shifted on the host
   const int shift = (int)(lo & 7);
   std::vector<std::vector<uint8_t>> shifted;
+  for (int k = 0; k < a->spec.n; k++)
+    if (a->out_elem[k] == TG_DEC_CELL_BYTES && out->cols[k].elem_len != TG_DEC_CELL_BYTES)
+      return fail(TG_ERR_INVALID, "a DECIMAL result column needs elem_len 40 (MyDecimal cells)");
   for (int k = 0; k < a->spec.n; k++) {
-    TG_CUDA(cudaMemcpyAsync(out->cols[k].data, a->out_cols[k]->as<uint8_t>() + (size_t)lo * 8, (size_t)want * 8, cudaMemcpyDeviceToHost, a->stream));
-    a->stats.d2h_bytes += want * 8;
+    const size_t el = (size_t)a->out_elem[k];
+    TG_CUDA(cudaMemcpyAsync(out->cols[k].data, a->out_cols[k]->as<uint8_t>() + (size_t)lo * el, (size_t)want * el, cudaMemcpyDeviceToHost, a->stream));
+    a->stats.d2h_bytes += want * (int64_t)el;
     size_t nb = (size_t)((want + 7) / 8);
     if (a->out_bitmaps[k]->p) {
       if (!out->cols[k].null_bitmap) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");

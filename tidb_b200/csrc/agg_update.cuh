@@ -36,6 +36,26 @@ __device__ __forceinline__ unsigned long long scas_u64(uint32_t a, unsigned long
   asm volatile("atom.shared.cas.b64 %0, [%1], %2, %3;" : "=l"(old) : "r"(a), "l"(cmp), "l"(v) : "memory");
   return old;
 }
+__device__ __forceinline__ unsigned long long satom_add_u64(uint32_t a, unsigned long long v) {
+  unsigned long long old;
+  asm volatile("atom.shared.add.u64 %0, [%1], %2;" : "=l"(old) : "r"(a), "l"(v) : "memory");
+  return old;
+}
+// dec_add (agg.cu) on the shared-memory table: the same carry rule
+__device__ __forceinline__ void sdec_add(uint32_t lo, uint32_t hi, unsigned long long v, unsigned long long ext) {
+  const unsigned long long old = satom_add_u64(lo, v);
+  const unsigned long long add = ext + (old + v < old ? 1ull : 0ull);
+  if (add) sred_add_u64(hi, add);
+}
+// one row of a DECIMAL SUM / AVG: the 128-bit add and the non-NULL count (count: nullptr / has_cnt false = NOT NULL argument)
+__device__ __noinline__ void dec_apply(unsigned long long* lo, unsigned long long* hi, unsigned long long* cnt, unsigned long long v, unsigned long long ext) {
+  dec_add(lo, hi, v, ext);
+  if (cnt) atomicAdd(cnt, 1ull);
+}
+__device__ __noinline__ void sdec_apply(uint32_t lo, uint32_t hi, bool has_cnt, uint32_t cnt, unsigned long long v, unsigned long long ext) {
+  sdec_add(lo, hi, v, ext);
+  if (has_cnt) sred_inc_lo32(cnt);
+}
 __device__ __forceinline__ unsigned long long sld_u64(uint32_t a) {
   unsigned long long v;
   asm volatile("ld.volatile.shared.u64 %0, [%1];" : "=l"(v) : "r"(a) : "memory");
@@ -73,6 +93,12 @@ __device__ __forceinline__ void agg_apply2(const AggTable& t, const LocalTable& 
         break;
       }
       case TG_AGG_SUM: case TG_AGG_AVG: {
+        if (f.s2 >= 0) {   // DECIMAL: exact 128-bit sum of the integer argument (out of line: keeps the DOUBLE path's registers)
+          const unsigned long long v = arg_raw(cols, f.arg_col, row), ext = dec_ext(f, v);
+          if (SH) sdec_apply(lt_state(lt, f.s0, (uint32_t)s), lt_state(lt, f.s2, (uint32_t)s), f.s1 >= 0, lt_state(lt, f.s1 >= 0 ? f.s1 : 0, (uint32_t)s), v, ext);
+          else dec_apply(&t.state[f.s0][s], &t.state[f.s2][s], f.s1 >= 0 ? &t.state[f.s1][s] : nullptr, v, ext);
+          break;
+        }
         unsigned long long cnt = 1ull;
         int vcol = f.arg_col;
         if (f.name == TG_AGG_AVG && f.final_mode) {   // args: count column, sum column (func_avg.go:405)
@@ -117,7 +143,10 @@ __device__ __forceinline__ void agg_merge_into(const AggTable& t, const AggSpec&
       unsigned long long v = st[f.s0];
       switch (f.name) {
         case TG_AGG_COUNT: atomicAdd(&t.state[f.s0][s], v); break;
-        case TG_AGG_SUM: case TG_AGG_AVG: atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v)); break;
+        case TG_AGG_SUM: case TG_AGG_AVG:
+          if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, st[f.s2]);
+          else atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v));
+          break;
         case TG_AGG_MIN: atomicMin(&t.state[f.s0][s], v); break;
         case TG_AGG_MAX: atomicMax(&t.state[f.s0][s], v); break;
         default: break;
@@ -175,6 +204,7 @@ k_agg_update2(Agg2Params p, DevCols cols, AggTable t, AggSpec spec) {
         const AggFuncDev& f = spec.f[k];
         if (f.s0 >= 0) w[(size_t)NT * (2 + f.s0) + i] = f.name == TG_AGG_MIN ? ~0ull : 0ull;
         if (f.s1 >= 0) w[(size_t)NT * (2 + f.s1) + i] = 0;
+        if (f.s2 >= 0) w[(size_t)NT * (2 + f.s2) + i] = 0;
       }
     }
     if (tid == 0) { s_fill = 0; s_seen = 0; s_hit = 0; s_use_local = 1; }

@@ -17,7 +17,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 from . import abi
-from .chunk import Chunk, Column, MutChunk
+from .chunk import DECIMAL_DTYPE, Chunk, Column, MutChunk
 from .plan import AggPlan, FieldType, JoinPlan
 
 MAX_CHUNK_SIZE = 1024  # tidb_max_chunk_size default (vardef/tidb_vars.go:1464)
@@ -28,6 +28,8 @@ def np_dtype_of(t: FieldType):
         return np.float64
     if t.tp == abi.TYPE_FLOAT:
         return np.float32
+    if t.tp == abi.TYPE_NEWDECIMAL:
+        return DECIMAL_DTYPE      # raw 40-byte MyDecimal cells, as a Go chunk column holds them
     return np.int64   # unsigned columns keep their bit pattern (chunk.Column stores raw 8 bytes)
 
 
@@ -166,7 +168,7 @@ class HashAggExec(Executor):
         if f.name == abi.AGG_COUNT:
             return FieldType(abi.TYPE_LONGLONG, abi.FLAG_NOT_NULL)
         if f.name in (abi.AGG_SUM, abi.AGG_AVG):
-            return FieldType(abi.TYPE_DOUBLE, 0)
+            return FieldType(abi.TYPE_NEWDECIMAL if f.ret_type == abi.TYPE_NEWDECIMAL else abi.TYPE_DOUBLE, 0)
         return FieldType(plan.col_types[f.arg_col].tp, plan.col_types[f.arg_col].flag & ~abi.FLAG_NOT_NULL)
 
     def open(self) -> None:

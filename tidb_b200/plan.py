@@ -163,6 +163,8 @@ class AggFunc:
     arg_col2: int = -1
     arg_expr: int = 0          # abi.ARGEXPR_*: the argument as arg_col * arg_col2 / arg_col * (arg_const - arg_col2)
     arg_const: float = 0.0
+    ret_type: int = 0          # AggFuncDesc.RetTp.GetType(): abi.TYPE_NEWDECIMAL = exact DECIMAL SUM / AVG of an integer column
+    ret_frac: int = 0          # AggFuncDesc.RetTp.GetDecimal()
 
 
 @dataclass
@@ -186,6 +188,7 @@ class AggPlan:
             fa[i].name, fa[i].mode, fa[i].arg_col = f.name, f.mode, f.arg_col
             fa[i].arg_type, fa[i].arg_flag, fa[i].arg_col2 = f.arg_type, f.arg_flag, f.arg_col2
             fa[i].arg_expr, fa[i].arg_const = f.arg_expr, f.arg_const
+            fa[i].ret_type, fa[i].ret_frac = f.ret_type, f.ret_frac
         keep.append(fa)
         d.funcs = fa
         d.n_funcs = len(self.funcs)
