@@ -438,8 +438,10 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk,
  * TopN                         replaces sortexec.TopNExec (pkg/executor/sortexec/topn.go:74, :230)
  * ORDER BY items over plain columns, LIMIT offset, count.  Rows [offset, offset + count) of the child's rows in item
  * order (NULL sorts before every value, DESC reverses: chunk.GetCompareFunc) are written to `out` (child schema, host
- * buffers, capacity >= count); ties are broken arbitrarily, as by the reference's heap.  `on_device` as in the VecEval
- * calls.  8-byte int-family / double / time columns.
+ * buffers, capacity >= min(count, rows - offset)); ties are broken arbitrarily, as by the reference's heap.
+ * `on_device` as in the VecEval calls.  8-byte int-family / double / time columns.  DOUBLE compares as Go cmp.Compare
+ * (NaN first, -0 == +0); DATE / DATETIME / TIMESTAMP compare by calendar value and microseconds, ignoring the fsp and
+ * type bits (types/core_time.go compareTime).  The output rows keep the input's bits.
  * ------------------------------------------------------------------------------------------- */
 typedef struct tg_sort_item { int32_t col; int32_t desc; } tg_sort_item;
 int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_types, const uint32_t* col_flags,

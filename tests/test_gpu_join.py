@@ -103,9 +103,13 @@ def test_gpu_filters(jt):
     rng = np.random.default_rng(77 + jt)
     ltypes, rtypes, l, r = make_case(rng, 2000, 3000, 0.1, True, False)
     semi = jt >= abi.JOIN_SEMI
-    lf = [FilterItem(abi.CMP_GT, 0, const_i64=0)]
-    rf = [FilterItem(abi.CMP_LT, 1, const_i64=1 << 39), FilterItem(abi.CMP_NE, 2, rhs_col=1)]
-    for build_is_right in (True, False):
+    signed = ([FilterItem(abi.CMP_GT, 0, const_i64=0)],
+              [FilterItem(abi.CMP_LT, 1, const_i64=1 << 39), FilterItem(abi.CMP_NE, 2, rhs_col=1)])
+    # UNSIGNED items over the same words: a negative word is a value of at least 2^63 (types.CompareInt)
+    unsigned = ([FilterItem(abi.CMP_LT, 0, const_i64=1 << 39, lhs_unsigned=True)],
+                [FilterItem(abi.CMP_GT, 1, rhs_col=2, lhs_unsigned=True), FilterItem(abi.CMP_LE, 2, rhs_col=1, rhs_unsigned=True),
+                 FilterItem(abi.CMP_LT, 0, const_i64=-20, lhs_unsigned=True, rhs_unsigned=True)])
+    for (lf, rf), build_is_right in ((f, b) for f in (signed, unsigned) for b in (True, False)):
         plan = JoinPlan(jt, ltypes, rtypes, [1], [0], build_is_right=build_is_right, lused=None, rused=[] if semi else None,
                         build_filter=rf if build_is_right else lf, probe_filter=lf if build_is_right else rf)
         if jt == abi.JOIN_LEFT_OUTER:

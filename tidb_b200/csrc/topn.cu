@@ -17,11 +17,19 @@
 
 namespace tg {
 
-__device__ __forceinline__ unsigned long long rank_of(unsigned long long raw, bool is_null, int kind /*0 signed, 1 unsigned, 2 real*/, bool desc) {
+// ORDER BY kinds: how a column's 8-byte value is compared
+enum { KIND_SIGNED = 0, KIND_UNSIGNED = 1, KIND_REAL = 2, KIND_TIME = 3 };
+// Packed CoreTime (types/time.go:235-251): year..microsecond from bit 63 down to bit 4, then 4 fspTt bits (fsp and
+// type).  compareTime (types/core_time.go:256) compares the calendar fields and the microseconds only, which is the
+// unsigned order of the word with the fspTt bits cleared.
+constexpr unsigned long long kTimeValueMask = ~0xFull;
+
+__device__ __forceinline__ unsigned long long rank_of(unsigned long long raw, bool is_null, int kind, bool desc) {
   unsigned long long o;
   if (is_null) o = 0ull;                         // NULL sorts before every value (chunk.GetCompareFunc -> cmpNull)
-  else if (kind == 2) { o = (raw >> 63) ? ~raw : (raw | 0x8000000000000000ull); }
-  else if (kind == 1) o = raw;
+  else if (kind == KIND_REAL) { o = (raw >> 63) ? ~raw : (raw | 0x8000000000000000ull); }
+  else if (kind == KIND_UNSIGNED) o = raw;
+  else if (kind == KIND_TIME) o = raw & kTimeValueMask;
   else o = raw ^ 0x8000000000000000ull;
   // NULL and the smallest value may share rank 0 (and, inverted, the largest): that only widens the candidate set; the
   // final order comes from the exact comparator on the host
@@ -36,7 +44,11 @@ k_topn_rank(const unsigned long long* __restrict__ data, const uint8_t* __restri
   for (; i < n; i += stride) {
     bool isn = nulls && !bit_not_null(nulls, i);
     unsigned long long raw = __ldcs(data + i);
-    if (kind == 2 && !isn) { double d = __longlong_as_double((long long)raw); if (d != d) raw = 0xFFF8000000000000ull; }   // NaN below everything (Go cmp.Compare)
+    if (kind == KIND_REAL && !isn) {
+      const double d = __longlong_as_double((long long)raw);
+      if (d != d) raw = 0xFFF8000000000000ull;   // every NaN below everything and equal (Go cmp.Compare)
+      else if (d == 0.0) raw = 0ull;             // -0 == +0: both zeros share one rank, so a tie on zero is collected whole
+    }
     rank[i] = rank_of(raw, isn, kind, desc != 0);
   }
 }
@@ -84,9 +96,9 @@ k_topn_gather(const unsigned long long* __restrict__ data, const uint8_t* __rest
 }
 
 static int kind_of(int tp, uint32_t flag) {
-  if (tp == TG_TYPE_DOUBLE) return 2;
-  if (is_int_family(tp)) return (flag & TG_FLAG_UNSIGNED) ? 1 : 0;
-  if (tp == TG_TYPE_DATE || tp == TG_TYPE_DATETIME || tp == TG_TYPE_TIMESTAMP) return 1;   // packed CoreTime compares as uint64 (types/time.go:646)
+  if (tp == TG_TYPE_DOUBLE) return KIND_REAL;
+  if (is_int_family(tp)) return (flag & TG_FLAG_UNSIGNED) ? KIND_UNSIGNED : KIND_SIGNED;
+  if (tp == TG_TYPE_DATE || tp == TG_TYPE_DATETIME || tp == TG_TYPE_TIMESTAMP) return KIND_TIME;
   return -1;
 }
 
@@ -120,8 +132,8 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
   if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t n = chk->cols[0].length;
-  const int64_t want = std::min<int64_t>(n, offset + count);
-  if (want <= offset || n == 0 || count == 0) return TG_OK;
+  if (n == 0 || count == 0 || offset >= n) return TG_OK;
+  const int64_t want = count >= n - offset ? n : offset + count;   // min(n, offset + count) without overflowing int64
   // device-resident columns
   std::vector<std::unique_ptr<DevBuf>> hold;
   std::vector<const unsigned long long*> dcol(nc);
@@ -197,12 +209,15 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
     if (an || bn) r = an == bn ? 0 : (an ? -1 : 1);
     else {
       const unsigned long long x = hv[c][(size_t)a], y = hv[c][(size_t)b];
-      if (kinds[c] == 2) {
+      if (kinds[c] == KIND_REAL) {
         double dx, dy; std::memcpy(&dx, &x, 8); std::memcpy(&dy, &y, 8);
         const bool xn = dx != dx, yn = dy != dy;
         r = xn ? (yn ? 0 : -1) : (yn ? 1 : (dx < dy ? -1 : (dx > dy ? 1 : 0)));
-      } else if (kinds[c] == 1) r = x < y ? -1 : (x > y ? 1 : 0);
-      else r = (long long)x < (long long)y ? -1 : ((long long)x > (long long)y ? 1 : 0);
+      } else if (kinds[c] == KIND_UNSIGNED) r = x < y ? -1 : (x > y ? 1 : 0);
+      else if (kinds[c] == KIND_TIME) {
+        const unsigned long long tx = x & kTimeValueMask, ty = y & kTimeValueMask;
+        r = tx < ty ? -1 : (tx > ty ? 1 : 0);
+      } else r = (long long)x < (long long)y ? -1 : ((long long)x > (long long)y ? 1 : 0);
     }
     return items[q].desc ? -r : r;
   };

@@ -394,7 +394,8 @@ class TopNExec(Executor):
             self._result = self.empty_chunk()
             return
         dense = _concat_chunks(chunks)
-        out = _out_chunk(self.schema, max(self.count, 8))
+        # at most the rows past the offset: a LIMIT far above the input size must not allocate `count` rows
+        out = _out_chunk(self.schema, max(min(self.count, max(dense.num_rows() - self.offset, 0)), 8))
         items = (abi.TgSortItem * len(self.by_items))(*[abi.TgSortItem(c, int(bool(d))) for c, d in self.by_items])
         tps = (C.c_int32 * len(self.schema))(*[t.tp for t in self.schema])
         fls = (C.c_uint32 * len(self.schema))(*[t.flag for t in self.schema])

@@ -237,6 +237,9 @@ class ScalarFunc(Expr):
     b_unsigned: bool = False
 
     def ret_type(self, schema):
-        if self.kind == "arith":
-            return FieldType(abi.TYPE_DOUBLE if self.is_real else abi.TYPE_LONGLONG, 0)
+        if self.kind == "arith" and self.is_real:
+            return FieldType(abi.TYPE_DOUBLE, 0)
+        if self.kind == "arith" and (self.a_unsigned or self.b_unsigned):
+            # integer +, - and * are UNSIGNED when either argument is (builtin_arithmetic.go:207, :378, :583)
+            return FieldType(abi.TYPE_LONGLONG, abi.FLAG_UNSIGNED)
         return FieldType(abi.TYPE_LONGLONG, 0)
