@@ -494,6 +494,55 @@ static int composite_key(JoinImpl* j, const Side& s, const DevCols& v, int64_t n
   return TG_OK;
 }
 
+// ---- fast-path launch tuning (env overrides are for A/B sweeps; the defaults are the production choice) ----
+struct ProbeTuning { int variant; int R; int evict_last; int ctas_per_sm; int partition; int subseg; int parts; int part_min_mb; int part_min_rows; int seg_vec; int seg_lean; int carveout; int tma; int stages; int tma_ctas; int cta_agg; };
+static ProbeTuning probe_tuning() {
+  ProbeTuning t;
+  t.variant = env_int("TG_PROBE_VARIANT", 1);      // 0: CTA-tile kernel (shared-memory offsets), 1: warp-autonomous kernel
+  t.R = env_int("TG_PROBE_R", 4);
+  t.evict_last = env_int("TG_PROBE_EVICT_LAST", 0);
+  t.ctas_per_sm = env_int("TG_PROBE_CTAS_PER_SM", 0);   // 0 = exactly the resident CTA count (occupancy query)
+  t.partition = env_int("TG_PROBE_PARTITION", 1);   // regroup big probes into L2-sized partitions first (0 = never, 2 = counted/dense variant)
+  t.subseg = env_int("TG_PROBE_SUBSEG", 0);         // 1 = CTA-private sub-segments in the L2 partition pass (no global cursor atomics): off, slower (thousands of write streams, and the interleaved empty tails let warps drift across partitions)
+  t.parts = env_int("TG_PROBE_PARTS", 0);           // 0 = auto (probe_slices), at most TG_MAX_PARTS
+  t.part_min_mb = env_int("TG_PROBE_PART_MIN_MB", 64);
+  t.part_min_rows = env_int("TG_PROBE_PART_MIN_ROWS", 1 << 22);
+  t.seg_vec = env_int("TG_PROBE_SEG_VEC", 1);            // 128-bit loads/stores in the segment probe
+  t.seg_lean = env_int("TG_PROBE_SEG_LEAN", 1);          // 1 = lean full-tile path (default), 0 = round-1 kernel, 2 = + register prefetch
+  t.carveout = env_int("TG_PROBE_CARVEOUT", -1);         // EXPERIMENTAL: preferred shared-memory carve-out (%) of the segment probe kernels, -1 = driver default
+  t.tma = 0;                                        // (the TMA-fed probe kernels were removed in round 2)
+  t.stages = env_int("TG_PROBE_STAGES", 4);
+  t.tma_ctas = env_int("TG_PROBE_TMA_CTAS", 3);
+  t.cta_agg = env_int("TG_PROBE_CTA_AGG", 1);        // one output-cursor atomic per CTA tile (TMA kernel)
+  return t;
+}
+
+// ---- L2 slices of the partitioned probe -------------------------------------------------------------------
+// The partition pass cuts the table into P contiguous slices and probes one at a time; a slice only stays L2 resident while
+// it is a fraction of L2, because the probe's input and output columns stream through the same cache.  On an H100 (50 MiB
+// L2) the segment probe's time per row stops falling at slices of about a quarter of L2: 100 M probe rows against a 109 MiB
+// table took 2.81 / 2.56 / 2.44 ms with slices of 27 / 13.6 / 6.8 MiB (tools/probe_slices.py --sweep slice, DESIGN.md §4.1).
+static size_t l2_slice_target(int device) {
+  static size_t cache[64];
+  if (device >= 0 && device < 64 && cache[device]) return cache[device];
+  int l2 = 0;
+  if (cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, device) != cudaSuccess || l2 <= 0) { cudaGetLastError(); l2 = 50 << 20; }
+  const size_t t = (size_t)l2 / 4;
+  if (device >= 0 && device < 64) cache[device] = t;
+  return t;
+}
+// P for a table of `table_bytes`: slices of at most l2_slice_target, at most TG_MAX_PARTS (TG_PROBE_PARTS > 0 overrides)
+static int probe_slices(size_t table_bytes, int device, int parts_override) {
+  if (parts_override > 0) return std::min(parts_override, TG_MAX_PARTS);
+  const size_t target = l2_slice_target(device);
+  return (int)std::min<size_t>((table_bytes + target - 1) / target, TG_MAX_PARTS);
+}
+// A U1 table the partitioned probe will slice is built dense enough for TG_MAX_PARTS slices of l2_slice_target, but no
+// denser than this: longer linear-probe runs cost more than the L2 hits gain.  10 M keys, 100 M probe rows, 16 slices, home
+// width 4 (tools/probe_slices.py --sweep shape, H100 at 400 W): load factor 0.5 4.30 ms (50 % match 4.51), 0.6 4.66 (5.57),
+// 0.7 5.47 (7.80), against 4.80 (4.40) for the 0.35 table the build used to keep
+static const double kMaxDenseLoad = 0.5;
+
 // ---- build --------------------------------------------------------------------------------------------
 static int build_table(JoinImpl* j) {
   const Side& b = j->build;
@@ -506,16 +555,19 @@ static int build_table(JoinImpl* j) {
     ks.data = j->bkey_syn.p; ks.nulls = j->bkey_syn_nn.as<uint8_t>();
   } else { ks.data = bview.data[b.key_col]; ks.nulls = bview.nulls[b.key_col]; }
   unsigned long long nslots = (unsigned long long)((double)(n > 0 ? n : 1) / j->load_factor) + 32;
-  // the L2 partition pass handles at most TG_MAX_PARTS slices of <= ~33 MB: with the DEFAULT load factor a table that would
-  // need more slices is made denser, down to load factor 0.5, instead of growing its slices.  (These sizes suit an L2
-  // larger than an H100's; see the partition pass in probe_device.)
+  // with the DEFAULT load factor a table bigger than TG_MAX_PARTS x 33 MB is made denser, down to load factor 0.5 (bounds the
+  // memory of big G tables; U1 tables are resized for the L2 slices below, once the build knows it is U1)
   if (j->default_load_factor) {
     const unsigned long long fit = ((unsigned long long)TG_MAX_PARTS * (33ull << 20)) / sizeof(Slot);
     const unsigned long long dense = (unsigned long long)((double)(n > 0 ? n : 1) / 0.5) + 32;
     if (nslots > fit) nslots = std::max(fit, dense);
   }
-  nslots &= ~1ull;   // even: slots are addressed as 32-byte pairs
-  const int pair_home = env_int("TG_PAIR_HOME", 1);
+  // TG_PAIR_HOME: home width in slots (0 = 1, a single slot; 1 or 2 = a 32-byte pair; 4 = a 64-byte half-line, the default:
+  // 2-6 % faster than pairs on the 100 % match step at load factors 0.5-0.8, same sweep as kMaxDenseLoad)
+  const int pair_home = env_int("TG_PAIR_HOME", 4);
+  const int home_width = pair_home >= 4 ? 4 : pair_home >= 1 ? 2 : 1;
+  const unsigned long long align = home_width > 2 ? home_width : 2;   // even in any case: runs continue by 32-byte pairs
+  nslots &= ~(align - 1);
   if (nslots + 1 >= 0xFFFFFFFFull) return fail(TG_ERR_UNSUPPORTED, "build side too large for 32-bit slot ids");
   TG_TRY(j->table.ensure(j->device, (size_t)(nslots + 1) * sizeof(Slot)));
   TG_TRY(j->row_slot.ensure(j->device, (size_t)(n + 1) * 4));
@@ -528,7 +580,7 @@ static int build_table(JoinImpl* j) {
   k_table_init<<<grid_for(j, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, nslots);
   j->stats.kernel_launches++;
   if (n > 0) {
-    k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots, pair_home,
+    k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots, home_width,
                                                                   j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>());
     j->stats.kernel_launches++;
   }
@@ -552,7 +604,25 @@ static int build_table(JoinImpl* j) {
     int pc = payload[0];
     if (b.elem[pc] != 8 || j->bcols.has_nulls[pc]) u1 = false;
   }
-  j->tv = TableView{slots, nslots, nullptr, 0, -1, TABLE_NONE, pair_home};
+  if (u1 && j->default_load_factor && n > 0) {
+    // the partitioned probe will slice this table: rebuild it dense enough for TG_MAX_PARTS L2-sized slices (probe_slices)
+    const ProbeTuning& tune = probe_tuning();
+    const size_t part_min = (size_t)tune.part_min_mb << 20;
+    const unsigned long long dense = std::max<unsigned long long>((unsigned long long)TG_MAX_PARTS * l2_slice_target(j->device) / sizeof(Slot),
+                                                                  (unsigned long long)((double)n / kMaxDenseLoad) + 32) & ~(align - 1);
+    if (tune.partition == 1 && nslots * sizeof(Slot) > part_min && dense < nslots && dense * sizeof(Slot) > part_min) {
+      nslots = dense;
+      j->table.release();
+      TG_TRY(j->table.ensure(j->device, (size_t)(nslots + 1) * sizeof(Slot)));
+      slots = j->table.as<Slot>();
+      k_table_init<<<grid_for(j, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, nslots);
+      k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots, home_width,
+                                                                    j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>());
+      j->stats.kernel_launches += 2;
+      j->stats.table_slots = (int64_t)nslots;
+    }
+  }
+  j->tv = TableView{slots, nslots, nullptr, 0, -1, TABLE_NONE, home_width};
   j->build_word_of_col.assign(b.ncols, -1);
   if (u1) {
     j->u1_payload_col = payload.empty() ? -1 : payload[0];
@@ -721,29 +791,6 @@ static bool uq_path_ok(const JoinImpl* j, const DevCols& pview) {
   return true;
 }
 
-// ---- fast-path launch tuning (env overrides are for A/B sweeps; the defaults are the production choice) ----
-struct ProbeTuning { int variant; int R; int evict_last; int ctas_per_sm; int partition; int subseg; int parts; int part_min_mb; int part_min_rows; int seg_vec; int seg_lean; int carveout; int tma; int stages; int tma_ctas; int cta_agg; };
-static ProbeTuning probe_tuning() {
-  ProbeTuning t;
-  t.variant = env_int("TG_PROBE_VARIANT", 1);      // 0: CTA-tile kernel (shared-memory offsets), 1: warp-autonomous kernel
-  t.R = env_int("TG_PROBE_R", 4);
-  t.evict_last = env_int("TG_PROBE_EVICT_LAST", 0);
-  t.ctas_per_sm = env_int("TG_PROBE_CTAS_PER_SM", 0);   // 0 = exactly the resident CTA count (occupancy query)
-  t.partition = env_int("TG_PROBE_PARTITION", 1);   // regroup big probes into L2-sized partitions first (0 = never, 2 = counted/dense variant)
-  t.subseg = env_int("TG_PROBE_SUBSEG", 0);         // 1 = CTA-private sub-segments in the L2 partition pass (no global cursor atomics): off, slower (thousands of write streams, and the interleaved empty tails let warps drift across partitions)
-  t.parts = env_int("TG_PROBE_PARTS", 0);           // 0 = auto: table slices of <= 32 MB, at most TG_MAX_PARTS
-  t.part_min_mb = env_int("TG_PROBE_PART_MIN_MB", 64);
-  t.part_min_rows = env_int("TG_PROBE_PART_MIN_ROWS", 1 << 22);
-  t.seg_vec = env_int("TG_PROBE_SEG_VEC", 1);            // 128-bit loads/stores in the segment probe
-  t.seg_lean = env_int("TG_PROBE_SEG_LEAN", 1);          // 1 = lean full-tile path (default), 0 = round-1 kernel, 2 = + register prefetch
-  t.carveout = env_int("TG_PROBE_CARVEOUT", -1);         // EXPERIMENTAL: preferred shared-memory carve-out (%) of the segment probe kernels, -1 = driver default
-  t.tma = 0;                                        // (the TMA-fed probe kernels were removed in round 2)
-  t.stages = env_int("TG_PROBE_STAGES", 4);
-  t.tma_ctas = env_int("TG_PROBE_TMA_CTAS", 3);
-  t.cta_agg = env_int("TG_PROBE_CTA_AGG", 1);        // one output-cursor atomic per CTA tile (TMA kernel)
-  return t;
-}
-
 // classify the output columns of the fused fast path by the register that feeds them; false = shape not covered by
 // the templated kernels (the CTA-tile kernel handles it)
 static bool build_fast_out(const JoinImpl* j, const OutCols& oc, const DevCols& pview, FastOut& fo) {
@@ -812,7 +859,7 @@ struct LaunchSeg {
     int64_t ctas = (n / 128 + 7) / 8;
     int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
     int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
-    if (t.seg_lean && j->tv.pair_home) {   // lean variants (see join_kernels.cuh); 3 CTAs per SM as well
+    if (t.seg_lean && j->tv.home_width > 1) {   // lean variants (see join_kernels.cuh); 3 CTAs per SM as well
       if (t.carveout >= 0) {
         cudaFuncSetAttribute(k_probe_inner_u1_seg_lean<NPC, NKD, NMD, false>, cudaFuncAttributePreferredSharedMemoryCarveout, t.carveout);
         cudaFuncSetAttribute(k_probe_inner_u1_seg_lean<NPC, NKD, NMD, true>, cudaFuncAttributePreferredSharedMemoryCarveout, t.carveout);
@@ -872,13 +919,10 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
           // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments.
           // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
           // [p/P, (p+1)/P) while the probe kernel sweeps the segment.  The pass trades 32 B/row of extra streaming traffic for
-          // random HBM traffic, which only pays while a slice stays L2 resident.  The ~32 MB slices below do not stay
-          // resident in the 50 MB L2 of an H100, where the pass measured no faster than the direct probe (DESIGN.md §4.1);
-          // it stays the default only until smaller slices, which need more than TG_MAX_PARTS partitions, are measured
-          // there.  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
+          // random HBM traffic, which only pays while a slice stays L2 resident (probe_slices; U1 tables are built dense
+          // enough for that, build_table).  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
           // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
-          int P = tune.parts > 0 ? tune.parts : (int)((table_bytes + (32u << 20) - 1) / (32u << 20));
-          if (P > TG_MAX_PARTS) P = TG_MAX_PARTS;
+          const int P = probe_slices(table_bytes, j->device, tune.parts);
           const int64_t n_main = n / PTILE * PTILE;
           const int nc = 1 + fo.n_pcols;
           // Segment layout.  Default: one segment per partition filled through global cursors.  TG_PROBE_SUBSEG=1 (experiment,
@@ -929,8 +973,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
         }
         if (!partitioned && !in_seg && tune.partition == 2 && n >= (1ll << 20) && table_bytes > ((size_t)tune.part_min_mb << 20)) {
           // counted variant (kept for A/B runs): histogram pass → exact offsets → dense partitions
-          int P = tune.parts > 0 ? tune.parts : (int)((table_bytes + (32u << 20) - 1) / (32u << 20));
-          if (P > TG_MAX_PARTS) P = TG_MAX_PARTS;
+          const int P = probe_slices(table_bytes, j->device, tune.parts);
           if (P >= 2) {
             int nc = 1 + fo.n_pcols;
             for (int c = 0; c < nc; c++) {

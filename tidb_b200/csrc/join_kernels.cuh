@@ -48,13 +48,15 @@ struct TableView {
   int32_t row_words;
   int32_t null_word;                // index of the per-row NULL mask word in the row store, -1 = none
   int32_t mode;
-  int32_t pair_home;                // 1: a key's home is the even slot of a 32-byte pair, so that a displacement by
-                                    // one slot stays inside the DRAM/L2 sector fetched by the first gather
+  int32_t home_width;               // 1, 2 or 4 slots (nslots is a multiple of it): a key's home is the first slot of an
+                                    // aligned group of that many slots.  2: the 32-byte pair one sector fetch brings in;
+                                    // 4: a key's first two pairs lie in one 64-byte half-line
 };
 
-// home slot of a hash value
-__device__ __forceinline__ unsigned long long home_slot(unsigned long long h, unsigned long long nslots, int pair_home) {
-  return pair_home ? ((unsigned long long)slot32(h, (uint32_t)(nslots >> 1)) << 1) : (unsigned long long)slot32(h, (uint32_t)nslots);
+// home slot of a hash value: slot32(h, nslots / w) * w.  Linear probing runs on from there one slot at a time, whatever w is.
+__device__ __forceinline__ unsigned long long home_slot(unsigned long long h, unsigned long long nslots, int home_width) {
+  const int sh = home_width >> 1;   // log2 of 1, 2, 4
+  return (unsigned long long)slot32(h, (uint32_t)(nslots >> sh)) << sh;
 }
 
 #define TG_MAX_OUT 24
@@ -142,6 +144,29 @@ __device__ __forceinline__ void load_pair(const Slot* p, Slot& a, Slot& b) {
   a.key = (int64_t)x0; a.meta = x1; b.key = (int64_t)x2; b.meta = x3;
 }
 
+// continue the linear probe for key k (not the sentinel) at slot s: one slot if s is odd, then by aligned 32-byte pairs
+// (nslots is even, so pairs wrap exactly at the end), until the slot holding k or the first empty slot.  true iff found.
+__device__ __forceinline__ bool probe_run(const Slot* __restrict__ slots, unsigned long long nslots, int64_t k, unsigned long long s,
+                                       unsigned long long& meta) {
+  if (s >= nslots) s = 0;
+  if (s & 1) {
+    const Slot x = load_slot(slots + s);
+    if (x.key == k) { meta = x.meta; return true; }
+    if (x.key == kEmptyKey) return false;
+    if (++s == nslots) s = 0;
+  }
+  for (;;) {
+    Slot a, b;
+    load_pair(slots + s, a, b);
+    if (a.key == k) { meta = a.meta; return true; }
+    if (a.key == kEmptyKey) return false;
+    if (b.key == k) { meta = b.meta; return true; }
+    if (b.key == kEmptyKey) return false;
+    s += 2;
+    if (s == nslots) s = 0;
+  }
+}
+
 // lookup without insertion: returns slot index or kInvalidSlot; meta of the found slot in *meta
 __device__ __forceinline__ uint32_t table_find(const TableView& t, int64_t k, unsigned long long* meta) {
   if (k == kEmptyKey) {
@@ -150,7 +175,7 @@ __device__ __forceinline__ uint32_t table_find(const TableView& t, int64_t k, un
     // the side slot is "occupied" iff a build row carried this key: mode U1 marks that in key
     return s.key == 0 ? kInvalidSlot : (uint32_t)t.nslots;
   }
-  unsigned long long s = home_slot(hash64((uint64_t)k), t.nslots, t.pair_home);
+  unsigned long long s = home_slot(hash64((uint64_t)k), t.nslots, t.home_width);
   for (;;) {
     Slot v = load_slot(t.slots + s);
     if (v.key == k) { *meta = v.meta; return (uint32_t)s; }
@@ -219,7 +244,7 @@ __global__ void k_table_init(Slot* slots, unsigned long long n_total, unsigned l
 
 // pass 1: claim one slot per distinct key, count multiplicities, remember (slot, rank) per build row
 __global__ void __launch_bounds__(256)
-k_build_insert(KeySpec key, DevCols cols, DevFilter filt, int64_t n, Slot* slots, unsigned long long nslots, int pair_home,
+k_build_insert(KeySpec key, DevCols cols, DevFilter filt, int64_t n, Slot* slots, unsigned long long nslots, int home_width,
                uint32_t* __restrict__ row_slot, uint32_t* __restrict__ row_rank) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -233,7 +258,7 @@ k_build_insert(KeySpec key, DevCols cols, DevFilter filt, int64_t n, Slot* slots
       s = nslots;
       slots[s].key = 1;   // occupied flag (benign race: every writer stores 1)
     } else {
-      s = home_slot(hash64((uint64_t)k), nslots, pair_home);
+      s = home_slot(hash64((uint64_t)k), nslots, home_width);
       for (;;) {
         int64_t cur = *reinterpret_cast<volatile int64_t*>(&slots[s].key);
         if (cur == k) break;
@@ -360,7 +385,7 @@ k_probe_inner_u1(const int64_t* __restrict__ pkey, DevCols pcols, int64_t n, Tab
     unsigned long long s[R];
 #pragma unroll
     for (int j = 0; j < R; j++) {
-      s[j] = (k[j] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[j]), t.nslots, t.pair_home);
+      s[j] = (k[j] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[j]), t.nslots, t.home_width);
       v[j] = load_slot(t.slots + s[j]);
     }
 #pragma unroll
@@ -450,17 +475,16 @@ __device__ __forceinline__ void probe_rows_u1(const int64_t (&k)[R], const unsig
                                               const unsigned long long (&sl0)[R], const bool (&in)[R], const TableView& t,
                                               const FastOut& out, unsigned long long* __restrict__ out_cursor, int lane) {
   Slot v[R], w[R];
-  unsigned long long sl[R];
-  if (t.pair_home) {
+  const bool pair = t.home_width > 1;   // the home is the first slot of an aligned pair: load both
+  if (pair) {
 #pragma unroll
     for (int j = 0; j < R; j++) {
-      sl[j] = sl0[j];
-      if (k[j] == kEmptyKey) { v[j] = load_slot(t.slots + sl[j]); w[j].key = kEmptyKey; w[j].meta = 0; }
-      else load_pair(t.slots + sl[j], v[j], w[j]);
+      if (k[j] == kEmptyKey) { v[j] = load_slot(t.slots + sl0[j]); w[j].key = kEmptyKey; w[j].meta = 0; }
+      else load_pair(t.slots + sl0[j], v[j], w[j]);
     }
   } else {
 #pragma unroll
-    for (int j = 0; j < R; j++) { sl[j] = sl0[j]; v[j] = load_slot(t.slots + sl[j]); w[j].key = kEmptyKey; w[j].meta = 0; }
+    for (int j = 0; j < R; j++) { v[j] = load_slot(t.slots + sl0[j]); w[j].key = kEmptyKey; w[j].meta = 0; }
   }
   unsigned bal[R];
   uint32_t total = 0;
@@ -469,19 +493,9 @@ __device__ __forceinline__ void probe_rows_u1(const int64_t (&k)[R], const unsig
     bool m;
     if (k[j] == kEmptyKey) m = in[j] && v[j].key != 0;
     else if (v[j].key == k[j]) m = true;
-    else if (t.pair_home && w[j].key == k[j]) { v[j] = w[j]; m = true; }
-    else if (v[j].key == kEmptyKey || (t.pair_home && w[j].key == kEmptyKey)) m = false;
-    else {
-      // the home slots hold other keys: continue the linear probe behind them (rare at the configured load factor)
-      sl[j] += t.pair_home ? 2 : 1;
-      if (sl[j] >= t.nslots) sl[j] = 0;
-      v[j] = load_slot(t.slots + sl[j]);
-      while (v[j].key != k[j] && v[j].key != kEmptyKey) {
-        if (++sl[j] == t.nslots) sl[j] = 0;
-        v[j] = load_slot(t.slots + sl[j]);
-      }
-      m = v[j].key == k[j];
-    }
+    else if (pair && w[j].key == k[j]) { v[j] = w[j]; m = true; }
+    else if (v[j].key == kEmptyKey || (pair && w[j].key == kEmptyKey)) m = false;
+    else m = probe_run(t.slots, t.nslots, k[j], sl0[j] + (pair ? 2 : 1), v[j].meta);   // the home slots hold other keys
     bal[j] = __ballot_sync(0xffffffffu, m);
     total += __popc(bal[j]);
   }
@@ -592,7 +606,7 @@ k_probe_inner_u1_w(const int64_t* __restrict__ pkey, int64_t n, TableView t, Fas
 #pragma unroll
     for (int j = 0; j < R; j++) {
       int64_t i = base + j * 32 + lane;
-      sl[j] = (k[j] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[j]), t.nslots, t.pair_home);
+      sl[j] = (k[j] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[j]), t.nslots, t.home_width);
 #pragma unroll
       for (int c = 0; c < NPC; c++) pv[j][c] = in[j] ? __ldcs(out.psrc[c] + i) : 0ull;
     }
@@ -648,8 +662,8 @@ k_probe_inner_u1_seg(const int64_t* __restrict__ pkey, int64_t n, TableView t, F
 #pragma unroll
     for (int g = 0; g < R / 2; g++) {
       const int64_t i = base + g * 64 + 2 * lane;
-      sl[2 * g] = (k[2 * g] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g]), t.nslots, t.pair_home);
-      sl[2 * g + 1] = (k[2 * g + 1] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g + 1]), t.nslots, t.pair_home);
+      sl[2 * g] = (k[2 * g] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g]), t.nslots, t.home_width);
+      sl[2 * g + 1] = (k[2 * g + 1] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g + 1]), t.nslots, t.home_width);
 #pragma unroll
       for (int cc = 0; cc < NPC; cc++) {
         const ulonglong2 pp = __ldcs(reinterpret_cast<const ulonglong2*>(out.psrc[cc] + i));
@@ -685,8 +699,8 @@ __device__ __forceinline__ void probe_tile_generic(const int64_t* __restrict__ p
 #pragma unroll
   for (int g = 0; g < R / 2; g++) {
     const int64_t i = base + g * 64 + 2 * lane;
-    sl[2 * g] = (k[2 * g] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g]), t.nslots, t.pair_home);
-    sl[2 * g + 1] = (k[2 * g + 1] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g + 1]), t.nslots, t.pair_home);
+    sl[2 * g] = (k[2 * g] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g]), t.nslots, t.home_width);
+    sl[2 * g + 1] = (k[2 * g + 1] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g + 1]), t.nslots, t.home_width);
 #pragma unroll
     for (int cc = 0; cc < NPC; cc++) {
       const ulonglong2 pp = __ldcs(reinterpret_cast<const ulonglong2*>(out.psrc[cc] + i));
@@ -742,25 +756,45 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
     }
     Slot v[R], w[R];
 #pragma unroll
-    for (int j = 0; j < R; j++) load_pair(t.slots + home_slot(hash64((uint64_t)k[j]), t.nslots, 1), v[j], w[j]);
+    for (int j = 0; j < R; j++) load_pair(t.slots + home_slot(hash64((uint64_t)k[j]), t.nslots, t.home_width), v[j], w[j]);
     unsigned long long meta[R];
+    unsigned hit = 0, run = 0;   // bit j: row j matched / row j's home pair holds two other keys
+#pragma unroll
+    for (int j = 0; j < R; j++) {
+      meta[j] = 0;
+      if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; }
+      else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; }
+      else if (v[j].key != kEmptyKey && w[j].key != kEmptyKey) run |= 1u << j;
+    }
+    if (run) {
+      // continue the linear probe of every such row behind its home pair, one aligned pair per row and step: the rows of a
+      // lane walk their runs side by side, so a step costs one L2 round trip however many rows are still walking (dense
+      // tables: one of the 128 rows of a tile nearly always has a run)
+      uint32_t sl[R];
+#pragma unroll
+      for (int j = 0; j < R; j++) {
+        const unsigned long long s = home_slot(hash64((uint64_t)k[j]), t.nslots, t.home_width) + 2;
+        sl[j] = s == t.nslots ? 0u : (uint32_t)s;
+      }
+      do {
+#pragma unroll
+        for (int j = 0; j < R; j++) if ((run >> j) & 1u) load_pair(t.slots + sl[j], v[j], w[j]);
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+          if (!((run >> j) & 1u)) continue;
+          if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; run &= ~(1u << j); }
+          else if (v[j].key == kEmptyKey) run &= ~(1u << j);
+          else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; run &= ~(1u << j); }
+          else if (w[j].key == kEmptyKey) run &= ~(1u << j);
+          else { sl[j] += 2; if (sl[j] == t.nslots) sl[j] = 0; }
+        }
+      } while (run);
+    }
     unsigned bal[R];
     uint32_t total = 0;
 #pragma unroll
     for (int j = 0; j < R; j++) {
-      bool m;
-      if (v[j].key == k[j]) { m = true; meta[j] = v[j].meta; }
-      else if (w[j].key == k[j]) { m = true; meta[j] = w[j].meta; }
-      else if (v[j].key == kEmptyKey || w[j].key == kEmptyKey) { m = false; meta[j] = 0; }
-      else {
-        // both home slots hold other keys: continue the linear probe behind the pair (rare at the configured load factor)
-        unsigned long long sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1) + 2;
-        if (sl >= t.nslots) sl = 0;
-        Slot x = load_slot(t.slots + sl);
-        while (x.key != k[j] && x.key != kEmptyKey) { if (++sl == t.nslots) sl = 0; x = load_slot(t.slots + sl); }
-        m = x.key == k[j]; meta[j] = x.meta;
-      }
-      bal[j] = __ballot_sync(0xffffffffu, m);
+      bal[j] = __ballot_sync(0xffffffffu, (hit >> j) & 1u);
       total += __popc(bal[j]);
     }
     unsigned long long wbase = 0;
@@ -1055,7 +1089,7 @@ k_probe_inner_uq(KeySpec key, DevCols pcols, DevFilter filt, int64_t n, TableVie
     for (int r = 0; r < UQ_R; r++) {
       sl[r] = t.nslots; v[r].key = kEmptyKey; v[r].meta = 0;
       if (valid[r]) {
-        if (k[r] != kEmptyKey) sl[r] = home_slot(hash64((uint64_t)k[r]), t.nslots, t.pair_home);
+        if (k[r] != kEmptyKey) sl[r] = home_slot(hash64((uint64_t)k[r]), t.nslots, t.home_width);
         v[r] = load_slot(t.slots + sl[r]);
       }
     }
@@ -1065,10 +1099,8 @@ k_probe_inner_uq(KeySpec key, DevCols pcols, DevFilter filt, int64_t n, TableVie
       bool m = false;
       if (valid[r]) {
         if (k[r] == kEmptyKey) m = v[r].key != 0;                       // the side slot is occupied iff a build row carried this key
-        else {
-          while (v[r].key != k[r] && v[r].key != kEmptyKey) { if (++sl[r] == t.nslots) sl[r] = 0; v[r] = load_slot(t.slots + sl[r]); }
-          m = v[r].key == k[r];
-        }
+        else if (v[r].key == k[r]) m = true;
+        else if (v[r].key != kEmptyKey) m = probe_run(t.slots, t.nslots, k[r], sl[r] + 1, v[r].meta);   // run on behind the home slot
       }
       bal[r] = __ballot_sync(0xffffffffu, m);
       if (lane == 0) s_cnt[par][r][warp] = __popc(bal[r]);

@@ -36,11 +36,11 @@ __global__ void k_lab_init(Slot* s, u64 n) {
   u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x;
   if (i < n) { s[i].key = kEmptyKey; s[i].meta = 0; }
 }
-__global__ void k_lab_insert(const int64_t* bk, const u64* bp, int64_t nb, Slot* slots, u64 nslots, int pair_home = 1) {
+__global__ void k_lab_insert(const int64_t* bk, const u64* bp, int64_t nb, Slot* slots, u64 nslots, int home_width = 2) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= nb) return;
   int64_t k = bk[i];
-  u64 s = home_slot(hash64((uint64_t)k), nslots, pair_home);
+  u64 s = home_slot(hash64((uint64_t)k), nslots, home_width);
   for (;;) {
     unsigned long long prev = atomicCAS(reinterpret_cast<unsigned long long*>(&slots[s].key), (unsigned long long)kEmptyKey, (unsigned long long)k);
     if (prev == (unsigned long long)kEmptyKey) { slots[s].meta = bp[i]; return; }
@@ -169,7 +169,7 @@ __device__ __forceinline__ uint32_t gather_match(const int64_t (&k)[R], const Ta
   Slot v[R], w[R];
 #pragma unroll
   for (int j = 0; j < R; j++) {
-    u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1);
+    u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 2);
     load_pair(t.slots + sl, v[j], w[j]);
   }
   uint32_t total = 0;
@@ -180,7 +180,7 @@ __device__ __forceinline__ uint32_t gather_match(const int64_t (&k)[R], const Ta
     else if (w[j].key == k[j]) { m = true; meta[j] = w[j].meta; }
     else if (v[j].key == kEmptyKey || w[j].key == kEmptyKey) { m = false; meta[j] = 0; }
     else {
-      u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1) + 2;
+      u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 2) + 2;
       if (sl >= t.nslots) sl = 0;
       Slot x = load_slot(t.slots + sl);
       while (x.key != k[j] && x.key != kEmptyKey) { if (++sl == t.nslots) sl = 0; x = load_slot(t.slots + sl); }
@@ -478,8 +478,8 @@ __global__ void __launch_bounds__(256, MINB) k_probe_vec2_tpf(const int64_t* __r
     if (nt < ntiles) {
 #pragma unroll
       for (int g = 0; g < G; g++) {
-        const Slot* a0 = t.slots + home_slot(hash64(kn[g].x), t.nslots, 1);
-        const Slot* a1 = t.slots + home_slot(hash64(kn[g].y), t.nslots, 1);
+        const Slot* a0 = t.slots + home_slot(hash64(kn[g].x), t.nslots, 2);
+        const Slot* a1 = t.slots + home_slot(hash64(kn[g].y), t.nslots, 2);
         if (PF == 1) { asm volatile("prefetch.global.L1 [%0];" ::"l"(a0)); asm volatile("prefetch.global.L1 [%0];" ::"l"(a1)); }
         else { asm volatile("prefetch.global.L2 [%0];" ::"l"(a0)); asm volatile("prefetch.global.L2 [%0];" ::"l"(a1)); }
       }
@@ -640,7 +640,7 @@ __global__ void __launch_bounds__(256, MINB) k_probe_v3(const int64_t* __restric
 #pragma unroll
     for (int g = 0; g < G; g++) {
       const ulonglong2 kk = lds128(st + g * 32 + lane);
-      sl[2 * g] = home_slot(hash64(kk.x), t.nslots, 0); sl[2 * g + 1] = home_slot(hash64(kk.y), t.nslots, 0);
+      sl[2 * g] = home_slot(hash64(kk.x), t.nslots, 1); sl[2 * g + 1] = home_slot(hash64(kk.y), t.nslots, 1);
       v[2 * g] = load_slot(t.slots + sl[2 * g]); v[2 * g + 1] = load_slot(t.slots + sl[2 * g + 1]);
     }
     unsigned bal[R];
@@ -739,7 +739,7 @@ __global__ void __launch_bounds__(256, MINB) k_probe_pol(const int64_t* __restri
     Slot v[R], w[R];
 #pragma unroll
     for (int j = 0; j < R; j++) {
-      const u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1);
+      const u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 2);
       if (POL & 1) load_pair_pol(t.slots + sl, v[j], w[j], pol_last); else load_pair(t.slots + sl, v[j], w[j]);
     }
     uint32_t total = 0;
@@ -750,7 +750,7 @@ __global__ void __launch_bounds__(256, MINB) k_probe_pol(const int64_t* __restri
       else if (w[j].key == k[j]) { m = true; meta[j] = w[j].meta; }
       else if (v[j].key == kEmptyKey || w[j].key == kEmptyKey) { m = false; meta[j] = 0; }
       else {
-        u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1) + 2;
+        u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 2) + 2;
         if (sl >= t.nslots) sl = 0;
         Slot x = load_slot(t.slots + sl);
         while (x.key != k[j] && x.key != kEmptyKey) { if (++sl == t.nslots) sl = 0; x = load_slot(t.slots + sl); }
@@ -935,7 +935,7 @@ __global__ void __launch_bounds__(256, MINB) k_probe_seg(const int64_t* __restri
     // rows of this lane inside the tile: g*64 + 2*lane + {0,1}
     Slot v[R], w[R];
 #pragma unroll
-    for (int j = 0; j < R; j++) { const u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1); load_pair(t.slots + sl, v[j], w[j]); }
+    for (int j = 0; j < R; j++) { const u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 2); load_pair(t.slots + sl, v[j], w[j]); }
     uint32_t total = 0;
     const bool full_tile = left >= 128;
 #pragma unroll
@@ -948,7 +948,7 @@ __global__ void __launch_bounds__(256, MINB) k_probe_seg(const int64_t* __restri
       else {
         m = false; meta[j] = 0;
         if (valid) {
-          u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1) + 2;
+          u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 2) + 2;
           if (sl >= t.nslots) sl = 0;
           Slot x = load_slot(t.slots + sl);
           while (x.key != k[j] && x.key != kEmptyKey) { if (++sl == t.nslots) sl = 0; x = load_slot(t.slots + sl); }
@@ -1041,7 +1041,7 @@ __global__ void __launch_bounds__(256, MINB) k_probe_seg_dyn(const int64_t* __re
     // rows of this lane inside the tile: g*64 + 2*lane + {0,1}
     Slot v[R], w[R];
 #pragma unroll
-    for (int j = 0; j < R; j++) { const u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1); load_pair(t.slots + sl, v[j], w[j]); }
+    for (int j = 0; j < R; j++) { const u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 2); load_pair(t.slots + sl, v[j], w[j]); }
     uint32_t total = 0;
     const bool full_tile = left >= 128;
 #pragma unroll
@@ -1054,7 +1054,7 @@ __global__ void __launch_bounds__(256, MINB) k_probe_seg_dyn(const int64_t* __re
       else {
         m = false; meta[j] = 0;
         if (valid) {
-          u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 1) + 2;
+          u64 sl = home_slot(hash64((uint64_t)k[j]), t.nslots, 2) + 2;
           if (sl >= t.nslots) sl = 0;
           Slot x = load_slot(t.slots + sl);
           while (x.key != k[j] && x.key != kEmptyKey) { if (++sl == t.nslots) sl = 0; x = load_slot(t.slots + sl); }
