@@ -344,6 +344,7 @@ typedef struct tg_agg_func {
    *     digitsInt = 9 * the number of integer words (at least one word, as FromUint makes it), digitsFrac = resultFrac =
    *     ret_frac.  tg_agg_next fails with TG_ERR_INVALID unless the caller's tg_mut_column.elem_len for that column is 40;
    *     tg_agg_result_dev returns a device column of 40-byte cells.
+   *   - SUM / AVG / MIN / MAX over a DECIMAL column follow the same rules at the column's scale: see tg_agg_desc_ex.
    * The table keeps such a function in three 8-byte words (128-bit sum lo / hi, non-NULL count), so a plan needs at most
    * 24 state words in all; more is TG_ERR_UNSUPPORTED.                                                                     */
   int16_t ret_type;
@@ -364,9 +365,41 @@ typedef struct tg_agg_desc {
   int64_t expected_groups;        /* hint (planner NDV estimate); 0 = grow on demand            */
 } tg_agg_desc;
 
+/* tg_agg_desc plus the precision and scale of the child columns, for aggregates over DECIMAL(p <= 18) columns.
+ * tg_agg_supported / tg_agg_open are tg_agg_supported_ex / tg_agg_open_ex with both arrays NULL.
+ *   col_flen[c]    = FieldType.GetFlen() of child column c, col_decimal[c] = FieldType.GetDecimal(); NULL or -1 = not given.
+ * A function whose argument column is TG_TYPE_NEWDECIMAL is offloaded when the mode is Complete, arg_expr is
+ * TG_ARGEXPR_COL, 1 <= flen <= 18 and 0 <= decimal <= flen, and (s = the column's decimal):
+ *   SUM    ret_type TG_TYPE_NEWDECIMAL, ret_frac = s: the exact sum at scale s (typeInfer4Sum, aggregation/base_func.go;
+ *          sum4Decimal, func_sum.go)
+ *   AVG    ret_type TG_TYPE_NEWDECIMAL, s <= ret_frac <= 30: DecimalDiv(sum, count) rounded to ret_frac digits with
+ *          ModeHalfUp, by the truncate-then-round rule of tg_agg_func.ret_type (typeInfer4Avg; avgOriginal4Decimal /
+ *          baseAvgDecimal, func_avg.go)
+ *   MIN / MAX  ret_type TG_TYPE_NEWDECIMAL, ret_frac = s: the smallest / largest value, at scale s (typeInfer4MaxMin;
+ *          max4Decimal / min4Decimal, func_max_min.go:906)
+ *   COUNT  its usual BIGINT result (only the null bitmap is read)
+ * A scale rule not met or decimal > flen is TG_ERR_INVALID.  flen > 18, flen / decimal not given, Final / Partial2 mode
+ * (a partial DECIMAL sum has p + 22 digits), a fused argument expression, FIRSTROW, a DECIMAL GROUP BY column or a
+ * non-DECIMAL ret_type over a DECIMAL argument is TG_ERR_UNSUPPORTED.  SUM / AVG keep the 128-bit sum of
+ * tg_agg_func.ret_type (2-3 state words), MIN / MAX 1-2 words, under the same 24-word limit.
+ * Input columns hold 40-byte MyDecimal cells (elem_len 40, host or device memory; device columns need only 8-byte
+ * alignment).  A non-NULL cell must be in the column's stored form, as MyDecimal.FromBin (types/mydecimal.go:1465) makes
+ * it: digitsFrac = decimal, ceil(digitsInt / 9) integer words (digitsInt may be 0, leading words may be 0), then
+ * ceil(decimal / 9) fraction words, left-aligned (0.5 at decimal 1 is the word 500000000), at most flen significant
+ * digits; resultFrac is ignored and a negative zero is 0.  A push with any other non-NULL cell fails with TG_ERR_INVALID
+ * and leaves the groups unchanged.  Cells under NULL are not looked at.  Results are cells in the canonical form of
+ * tg_agg_func.ret_type, with digitsFrac = resultFrac = ret_frac.                                                      */
+typedef struct tg_agg_desc_ex {
+  tg_agg_desc base;               /* first member: everything tg_agg_desc says, unchanged       */
+  const int32_t* col_flen;        /* FieldType.GetFlen() per child column; NULL = not given      */
+  const int32_t* col_decimal;     /* FieldType.GetDecimal() per child column; NULL = not given   */
+} tg_agg_desc_ex;
+
 int tg_agg_supported(const tg_agg_desc* desc);
+int tg_agg_supported_ex(const tg_agg_desc_ex* desc);
 /* HashAggExec.Open (agg_hash_executor.go:237) */
 int tg_agg_open(const tg_agg_desc* desc, tg_agg** out);
+int tg_agg_open_ex(const tg_agg_desc_ex* desc, tg_agg** out);
 /* fetchChildData + HashAggPartialWorker.updatePartialResult (agg_hash_executor.go:449,
  * agg_hash_partial_worker.go:256): one child chunk (host / device-resident)                    */
 int tg_agg_push(tg_agg* a, const tg_chunk* chk);

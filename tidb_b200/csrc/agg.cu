@@ -33,9 +33,10 @@ struct AggFuncDev {
   int32_t final_mode;   // TG_AGGMODE_FINAL: inputs are partial results
   int32_t arg_col2;
   int32_t arg_expr;     // TG_ARGEXPR_*
-  int32_t s2;           // >= 0: DECIMAL SUM / AVG of an integer column, an exact 128-bit sum: s0 its low word, s2 its high word
+  int32_t s2;           // >= 0: DECIMAL SUM / AVG, an exact 128-bit sum of the integer (or scaled DECIMAL) argument: s0 its low word, s2 its high word
   int32_t dec_frac;     // DECIMAL AVG: result scale (AggFuncDesc.RetTp decimal)
-  int32_t pad;
+  int32_t dec_scale;    // >= 0: the result is a DECIMAL cell and the argument's values are integers * 10^-dec_scale (0 for an
+                        // integer column); -1: an 8-byte result
   double arg_const;
 };
 struct AggSpec { int32_t n; int32_t pad; unsigned long long* err; AggFuncDev f[TG_MAX_AGG]; };
@@ -523,12 +524,14 @@ k_agg_finalize(AggTable t, AggSpec spec, int gk_kind, AggOut out, unsigned long 
     for (int k = 0; k < spec.n; k++) {
       const AggFuncDev& f = spec.f[k];
       unsigned long long nn = f.s1 >= 0 ? t.state[f.s1][(size_t)i * t.stride] : rows;   // non-NULL inputs seen
-      if (f.s2 >= 0) {   // DECIMAL SUM / AVG: a 40-byte MyDecimal cell, NULL without a non-NULL input (decimal.cuh)
+      if (f.dec_scale >= 0) {   // DECIMAL SUM / AVG / MIN / MAX: a 40-byte MyDecimal cell, NULL without a non-NULL input (decimal.cuh)
         uint8_t* cell = reinterpret_cast<uint8_t*>(out.data[k]) + (size_t)o * TG_DEC_CELL_BYTES;
-        const unsigned long long lo = t.state[f.s0][(size_t)i * t.stride], hi = t.state[f.s2][(size_t)i * t.stride];
+        // SUM / AVG: the 128-bit sum; MIN / MAX: the int64 of the ordered domain (i64_to_ordered), sign-extended
+        unsigned long long lo = t.state[f.s0][(size_t)i * t.stride], hi;
+        if (f.s2 >= 0) hi = t.state[f.s2][(size_t)i * t.stride];
+        else { lo ^= 0x8000000000000000ull; hi = (unsigned long long)((long long)lo >> 63); }
         if (nn == 0) dec_store_null(cell);
-        else if (f.name == TG_AGG_SUM) dec_sum_cell(cell, lo, hi);
-        else dec_avg_cell(cell, lo, hi, nn, f.dec_frac);
+        else dec_result_cell(cell, f.name == TG_AGG_AVG, lo, hi, nn, f.dec_scale, f.dec_frac);
         if (out.valid[k]) out.valid[k][o] = nn != 0 ? 1 : 0;
         continue;
       }
@@ -670,6 +673,49 @@ __global__ void k_agg_rehash_mk(AggTable oldt, AggTable newt, int nstates) {
   }
 }
 
+// A DECIMAL(flen <= 18, scale) argument column of 40-byte cells -> value * 10^scale as int64 (dec_parse_cell), once per batch
+// and column, so that every update kernel sees an 8-byte integer column (40 bytes read + 8 written per row).  A thread owns
+// two adjacent rows: 80 bytes, five 16-byte loads when the column is 16-byte aligned (V16; then so is every pair), else ten
+// 8-byte loads (a caller's device column is only guaranteed 8-byte alignment).  A cell under NULL is not parsed and its
+// loads are skipped (the 16-byte load in the middle of a pair may still fetch 8 of its bytes); its output is 0.  A
+// non-NULL cell not in the column's stored form raises *err to `tag` (atomicMax: the host names the column).
+template <bool V16>
+__global__ void __launch_bounds__(256)
+k_dec_to_scaled(const uint8_t* __restrict__ cells, const uint8_t* __restrict__ nulls, int64_t n, int flen, int scale,
+                long long* __restrict__ out, unsigned long long* err, unsigned long long tag) {
+  const int64_t npair = (n + 1) >> 1;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < npair; p += stride) {
+    const int64_t r0 = 2 * p;
+    const bool two = r0 + 1 < n;
+    const bool nn0 = !nulls || bit_not_null(nulls, r0), nn1 = two && (!nulls || bit_not_null(nulls, r0 + 1));
+    uint32_t c0[10], c1[10];
+#pragma unroll
+    for (int j = 0; j < 10; j++) { c0[j] = 0; c1[j] = 0; }
+    if (V16 && two) {
+      const uint4* q = reinterpret_cast<const uint4*>(cells + (size_t)r0 * TG_DEC_CELL_BYTES);
+      const uint4 z = make_uint4(0, 0, 0, 0);
+      const uint4 a = nn0 ? __ldcs(q) : z, b = nn0 ? __ldcs(q + 1) : z, m = (nn0 || nn1) ? __ldcs(q + 2) : z;
+      const uint4 d = nn1 ? __ldcs(q + 3) : z, e = nn1 ? __ldcs(q + 4) : z;
+      c0[0] = a.x; c0[1] = a.y; c0[2] = a.z; c0[3] = a.w; c0[4] = b.x; c0[5] = b.y; c0[6] = b.z; c0[7] = b.w; c0[8] = m.x; c0[9] = m.y;
+      c1[0] = m.z; c1[1] = m.w; c1[2] = d.x; c1[3] = d.y; c1[4] = d.z; c1[5] = d.w; c1[6] = e.x; c1[7] = e.y; c1[8] = e.z; c1[9] = e.w;
+    } else {
+      const unsigned long long* q = reinterpret_cast<const unsigned long long*>(cells + (size_t)r0 * TG_DEC_CELL_BYTES);
+#pragma unroll
+      for (int j = 0; j < 5; j++) {
+        if (nn0) { const unsigned long long w = __ldcs(q + j); c0[2 * j] = (uint32_t)w; c0[2 * j + 1] = (uint32_t)(w >> 32); }
+        if (nn1) { const unsigned long long w = __ldcs(q + 5 + j); c1[2 * j] = (uint32_t)w; c1[2 * j + 1] = (uint32_t)(w >> 32); }
+      }
+    }
+    long long v0 = 0, v1 = 0;
+    bool bad = nn0 && !dec_parse_cell(c0, flen, scale, &v0);
+    bad |= nn1 && !dec_parse_cell(c1, flen, scale, &v1);
+    if (bad) atomicMax(err, tag);
+    if (two) __stcs(reinterpret_cast<longlong2*>(out) + p, make_longlong2(v0, v1));   // `out` is a 256-byte aligned scratch column
+    else out[r0] = v0;
+  }
+}
+
 }  // namespace tg
 #include "agg_update.cuh"
 namespace tg {
@@ -712,6 +758,9 @@ struct AggImpl {
   int nstates = 0;
   std::vector<char> out_nullable;
   std::vector<int> out_elem;   // bytes per result cell: 8, or 40 for a DECIMAL (MyDecimal) column
+  std::vector<int> col_flen, col_dec;   // tg_agg_desc_ex: precision / scale per child column, -1 = not given
+  std::vector<char> dec_decode;         // DECIMAL argument column of SUM / AVG / MIN / MAX: k_dec_to_scaled runs on every batch
+  std::vector<std::unique_ptr<DevBuf>> dscaled;   // its int64 value * 10^scale, one pooled scratch column per such column
 
   // table
   DevBuf tbl_mem;
@@ -741,7 +790,28 @@ static int agrid(const AggImpl* a, int64_t n, int block = 256, int per_sm = 8) {
   return (int)(need < cap ? need : cap);
 }
 
-static int agg_setup(AggImpl* a, const tg_agg_desc* d) {
+// A function over a DECIMAL column (tg_agg_desc_ex): TG_OK when it is offloaded, else the status and message
+static int dec_arg_rules(const AggImpl* a, const tg_agg_func& f) {
+  const int c = f.arg_col, p = a->col_flen[c], s = a->col_dec[c];
+  if (p < 0 || s < 0) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL argument column needs its precision and scale (tg_agg_desc_ex col_flen / col_decimal)");
+  if (p > 18) return fail(TG_ERR_UNSUPPORTED, "DECIMAL arguments are offloaded up to precision 18 (one int64 at the column's scale)");
+  if (p < 1 || s > p) return fail(TG_ERR_INVALID, "a DECIMAL column needs 1 <= flen and 0 <= decimal <= flen");
+  if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "aggregates over DECIMAL columns are offloaded in Complete mode only (no DECIMAL partial results)");
+  if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL column is not offloaded in a fused argument expression");
+  switch (f.name) {
+    case TG_AGG_COUNT:   // reads the null bitmap only
+      return f.ret_type == TG_TYPE_NEWDECIMAL ? fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG / MIN / MAX only") : TG_OK;
+    case TG_AGG_SUM: case TG_AGG_AVG: case TG_AGG_MIN: case TG_AGG_MAX:
+      if (f.ret_type != TG_TYPE_NEWDECIMAL) return fail(TG_ERR_UNSUPPORTED, "SUM / AVG / MIN / MAX over a DECIMAL column need a DECIMAL ret_type");
+      if (f.name == TG_AGG_AVG ? (f.ret_frac < s || f.ret_frac > 30) : f.ret_frac != s)
+        return fail(TG_ERR_INVALID, f.name == TG_AGG_AVG ? "DECIMAL AVG scale must be the column's scale .. 30"
+                                                        : "DECIMAL SUM / MIN / MAX of a DECIMAL column have the column's scale");
+      return TG_OK;
+    default: return fail(TG_ERR_UNSUPPORTED, "this aggregate function is not offloaded over a DECIMAL column");
+  }
+}
+
+static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, const int32_t* col_dec) {
   if (!d) return fail(TG_ERR_INVALID, "desc is NULL");
   if (d->n_cols <= 0 || d->n_cols > TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "child schema must have 1..16 columns");
   a->ncols = d->n_cols;
@@ -750,6 +820,12 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d) {
   for (int i = 0; i < d->n_cols; i++) a->flags[i] = d->col_flags ? d->col_flags[i] : 0;
   a->elem.resize(d->n_cols);
   for (int i = 0; i < d->n_cols; i++) a->elem[i] = fixed_len(a->types[i]);
+  a->col_flen.assign(d->n_cols, -1); a->col_dec.assign(d->n_cols, -1);
+  for (int i = 0; i < d->n_cols; i++) {
+    if (col_flen) a->col_flen[i] = col_flen[i];
+    if (col_dec) a->col_dec[i] = col_dec[i];
+  }
+  a->dec_decode.assign(d->n_cols, 0);
   a->needed.assign(d->n_cols, 0);
   if (d->n_group_by > TG_MAX_GROUP_COLS) return fail(TG_ERR_UNSUPPORTED, "GPU hash aggregation handles up to 4 GROUP BY columns");
   a->group_col = -1; a->gk_kind = GK_NONE; a->nkw = 0;
@@ -777,11 +853,15 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d) {
   for (int k = 0; k < d->n_funcs; k++) {
     const tg_agg_func& f = d->funcs[k];
     AggFuncDev& o = a->spec.f[k];
-    o = AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, -1, 0, 0, f.arg_const};
+    o = AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, -1, 0, -1, f.arg_const};
+    // a DECIMAL(p <= 18, s) argument column (tg_agg_desc_ex): decoded to int64 value * 10^s on every batch, then the integer
+    // update paths run unchanged
+    const bool dec_arg = f.arg_col >= 0 && f.arg_col < a->ncols && a->types[f.arg_col] == TG_TYPE_NEWDECIMAL;
+    if (dec_arg) TG_TRY(dec_arg_rules(a, f));
     // DECIMAL SUM / AVG of an integer column (typeInfer4Sum / typeInfer4Avg, aggregation/base_func.go); any other ret_type
     // keeps the result type each function has always had here
     const bool dec = f.ret_type == TG_TYPE_NEWDECIMAL;
-    if (dec) {
+    if (dec && !dec_arg) {
       if (f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG only");
       if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG are offloaded in Complete mode only (no DECIMAL partial results)");
       if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG take a plain column argument");
@@ -805,10 +885,12 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d) {
     if (f.arg_col >= a->ncols || f.arg_col2 >= a->ncols) return fail(TG_ERR_INVALID, "aggregate argument column out of range");
     bool arg_nullable = f.arg_col >= 0 && !(a->flags[f.arg_col] & TG_FLAG_NOT_NULL);
     if (f.arg_expr != TG_ARGEXPR_COL && f.arg_col2 >= 0 && f.arg_col2 < d->n_cols && !(a->flags[f.arg_col2] & TG_FLAG_NOT_NULL)) arg_nullable = true;
-    if (f.arg_col >= 0) { if (a->elem[f.arg_col] != 8) return fail(TG_ERR_UNSUPPORTED, "aggregate arguments must be 8-byte columns"); a->needed[f.arg_col] = 1; }
+    if (f.arg_col >= 0) { if (a->elem[f.arg_col] != 8 && !dec_arg) return fail(TG_ERR_UNSUPPORTED, "aggregate arguments must be 8-byte columns"); a->needed[f.arg_col] = 1; }
     int atype = f.arg_col >= 0 ? a->types[f.arg_col] : TG_TYPE_LONGLONG;
     o.is_real = atype == TG_TYPE_DOUBLE;
-    o.is_unsigned = f.arg_col >= 0 && (a->flags[f.arg_col] & TG_FLAG_UNSIGNED) != 0;
+    o.is_unsigned = f.arg_col >= 0 && !dec_arg && (a->flags[f.arg_col] & TG_FLAG_UNSIGNED) != 0;   // a decoded DECIMAL is a signed int64
+    if (dec_arg && f.name != TG_AGG_COUNT) { o.dec_scale = a->col_dec[f.arg_col]; a->dec_decode[f.arg_col] = 1; }
+    else if (dec) o.dec_scale = 0;
     switch (f.name) {
       case TG_AGG_COUNT:
         if (o.final_mode) { if (f.arg_col < 0) return fail(TG_ERR_INVALID, "final COUNT needs the partial count column"); o.s0 = a->nstates++; }
@@ -848,10 +930,11 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d) {
         a->out_nullable[k] = 1;
         break;
       case TG_AGG_MIN: case TG_AGG_MAX:
-        if (f.arg_col < 0 || !(is_int_family(atype) || atype == TG_TYPE_DOUBLE)) return fail(TG_ERR_UNSUPPORTED, "MIN/MAX are offloaded for int family / DOUBLE");
+        if (f.arg_col < 0 || !(dec_arg || is_int_family(atype) || atype == TG_TYPE_DOUBLE)) return fail(TG_ERR_UNSUPPORTED, "MIN/MAX are offloaded for int family / DOUBLE / DECIMAL");
         o.s0 = a->nstates++;
         if (arg_nullable) o.s1 = a->nstates++;
         a->out_nullable[k] = 1;
+        if (dec_arg) a->out_elem[k] = TG_DEC_CELL_BYTES;   // the signed int64 MIN / MAX at the column's scale
         break;
       case TG_AGG_FIRSTROW: {
         int gi = -1;
@@ -1221,8 +1304,44 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
   return TG_OK;
 }
 
+// DECIMAL argument columns of the batch -> int64 scratch columns (k_dec_to_scaled), checked before any update kernel runs:
+// a cell not in its column's stored form fails the push with the group table untouched.  One 8-byte read-back and one
+// synchronisation per batch; the error word is scalars[8], next to the overflow word of spec.err.
+static int decode_decimal_args(AggImpl* a, DevCols& cols, int64_t n) {
+  if (n == 0 || std::find(a->dec_decode.begin(), a->dec_decode.end(), 1) == a->dec_decode.end()) return TG_OK;
+  TG_TRY(a->scalars.ensure(a->device, 72));
+  unsigned long long* err = a->scalars.as<unsigned long long>() + 8;
+  TG_CUDA(cudaMemsetAsync(err, 0, 8, a->stream));
+  for (int c = 0; c < a->ncols; c++) {
+    if (!a->dec_decode[c]) continue;
+    TG_TRY(a->dscaled[c]->ensure(a->device, (size_t)n * 8 + 16));
+    const uint8_t* cells = static_cast<const uint8_t*>(cols.data[c]);
+    long long* out = a->dscaled[c]->as<long long>();
+    const int grid = agrid(a, (n + 1) / 2);
+    if ((reinterpret_cast<uintptr_t>(cells) & 15) == 0)
+      k_dec_to_scaled<true><<<grid, 256, 0, a->stream>>>(cells, cols.nulls[c], n, a->col_flen[c], a->col_dec[c], out, err, (unsigned long long)c + 1);
+    else
+      k_dec_to_scaled<false><<<grid, 256, 0, a->stream>>>(cells, cols.nulls[c], n, a->col_flen[c], a->col_dec[c], out, err, (unsigned long long)c + 1);
+    a->stats.kernel_launches++;
+    cols.data[c] = out;
+    cols.elem_len[c] = 8;
+  }
+  unsigned long long e = 0;
+  TG_CUDA(cudaMemcpyAsync(&e, err, 8, cudaMemcpyDeviceToHost, a->stream));
+  TG_CUDA(cudaStreamSynchronize(a->stream));
+  TG_CUDA(cudaGetLastError());
+  if (e) {
+    const int c = (int)e - 1;
+    return fail(TG_ERR_INVALID, "DECIMAL(" + std::to_string(a->col_flen[c]) + ", " + std::to_string(a->col_dec[c]) + ") column " + std::to_string(c) +
+                                ": a non-NULL cell is not in the column's stored form (digitsFrac must equal the scale, at most flen digits)");
+  }
+  return TG_OK;
+}
+
 // aggregate n device-resident rows; a fused argument expression that overflowed fails the call (types.ErrOverflow)
-static int update_device(AggImpl* a, const DevCols& cols, int64_t n) {
+static int update_device(AggImpl* a, const DevCols& in, int64_t n) {
+  DevCols cols = in;
+  TG_TRY(decode_decimal_args(a, cols, n));
   TG_TRY(update_device_impl(a, cols, n));
   bool has_expr = false;
   for (int k = 0; k < a->spec.n; k++) has_expr |= a->spec.f[k].arg_expr != TG_ARGEXPR_COL;
@@ -1255,12 +1374,16 @@ static int astage_append(AggImpl* a, const tg_chunk* chk) {
     if (!a->needed[c]) continue;
     const tg_column& col = chk->cols[c];
     PinBuf& d = *st.data[c];
-    TG_TRY(d.reserve((size_t)(st.rows + n) * 8));
-    uint64_t* dst = reinterpret_cast<uint64_t*>(d.p) + st.rows;
-    const uint64_t* src = reinterpret_cast<const uint64_t*>(col.data);
-    if (!chk->sel) std::memcpy(dst, src, (size_t)n * 8);
-    else for (int64_t i = 0; i < n; i++) dst[i] = src[chk->sel[i]];
-    d.used = (size_t)(st.rows + n) * 8;
+    const size_t el = (size_t)a->elem[c];   // 8, or 40 for a DECIMAL column
+    TG_TRY(d.reserve((size_t)(st.rows + n) * el));
+    uint8_t* dst = d.p + (size_t)st.rows * el;
+    if (!chk->sel) std::memcpy(dst, col.data, (size_t)n * el);
+    else if (el == 8) {
+      uint64_t* dst8 = reinterpret_cast<uint64_t*>(dst);
+      const uint64_t* src8 = reinterpret_cast<const uint64_t*>(col.data);
+      for (int64_t i = 0; i < n; i++) dst8[i] = src8[chk->sel[i]];
+    } else for (int64_t i = 0; i < n; i++) std::memcpy(dst + (size_t)i * el, col.data + (size_t)chk->sel[i] * el, el);
+    d.used = (size_t)(st.rows + n) * el;
     bool bring = col.null_bitmap != nullptr;
     if (bring || st.has_nulls[c]) {
       PinBuf& nb = *st.nulls[c];
@@ -1287,7 +1410,7 @@ static int aflush(AggImpl* a) {
   for (int c = 0; c < a->ncols; c++) {
     v.elem_len[c] = a->elem[c];
     if (!a->needed[c]) continue;
-    size_t bytes = (size_t)st.rows * 8;
+    size_t bytes = (size_t)st.rows * a->elem[c];
     TG_TRY(a->dcols[c]->ensure(a->device, bytes + 16));
     TG_CUDA(cudaMemcpyAsync(a->dcols[c]->p, st.data[c]->p, bytes, cudaMemcpyHostToDevice, a->stream));
     a->stats.h2d_bytes += bytes;
@@ -1380,14 +1503,19 @@ static int afinalize(AggImpl* a) {
 
 extern "C" {
 
-int tg_agg_supported(const tg_agg_desc* desc) { AggImpl tmp; return agg_setup(&tmp, desc); }
+int tg_agg_supported(const tg_agg_desc* desc) { AggImpl tmp; return agg_setup(&tmp, desc, nullptr, nullptr); }
 
-int tg_agg_open(const tg_agg_desc* desc, tg_agg** out) {
+int tg_agg_supported_ex(const tg_agg_desc_ex* desc) {
+  AggImpl tmp;
+  return agg_setup(&tmp, desc ? &desc->base : nullptr, desc ? desc->col_flen : nullptr, desc ? desc->col_decimal : nullptr);
+}
+
+static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int32_t* col_dec, tg_agg** out) {
   if (!out) return fail(TG_ERR_INVALID, "out is NULL");
   *out = nullptr;
   std::unique_ptr<tg_agg> shell(new tg_agg());
   std::unique_ptr<AggImpl> a(new AggImpl());
-  TG_TRY(agg_setup(a.get(), desc));
+  TG_TRY(agg_setup(a.get(), desc, col_flen, col_dec));
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(TG_ERR_CUDA, "no CUDA device: the GPU hash aggregation has no CPU fallback"); }
   if (a->device < 0 || a->device >= ndev) return fail(TG_ERR_INVALID, "device ordinal out of range");
@@ -1400,12 +1528,18 @@ int tg_agg_open(const tg_agg_desc* desc, tg_agg** out) {
   a->nsm = device_sm_count(a->device);
   for (int c = 0; c < a->ncols; c++) {
     a->stage.data.emplace_back(new PinBuf()); a->stage.nulls.emplace_back(new PinBuf());
-    a->dcols.emplace_back(new DevBuf()); a->dnulls.emplace_back(new DevBuf());
+    a->dcols.emplace_back(new DevBuf()); a->dnulls.emplace_back(new DevBuf()); a->dscaled.emplace_back(new DevBuf());
   }
   a->stage.has_nulls.assign(a->ncols, 0);
   shell->impl = a.release();
   *out = shell.release();
   return TG_OK;
+}
+
+int tg_agg_open(const tg_agg_desc* desc, tg_agg** out) { return agg_open(desc, nullptr, nullptr, out); }
+
+int tg_agg_open_ex(const tg_agg_desc_ex* desc, tg_agg** out) {
+  return agg_open(desc ? &desc->base : nullptr, desc ? desc->col_flen : nullptr, desc ? desc->col_decimal : nullptr, out);
 }
 
 int tg_agg_push(tg_agg* h, const tg_chunk* chk) {

@@ -1,11 +1,13 @@
-// decimal.cuh — the MyDecimal cell of an exact DECIMAL aggregate result (included by agg.cu; only k_agg_finalize uses it).
+// decimal.cuh — the MyDecimal cell of an exact DECIMAL aggregate result and of a DECIMAL argument column (included by agg.cu:
+// k_agg_finalize writes cells, k_dec_to_scaled parses them).
 //
 // A cell is the 40-byte types.MyDecimal (types/mydecimal.go:236-248) that chunk.Column copies whole (util/chunk/column.go:41):
 //   byte 0 digitsInt (int8), byte 1 digitsFrac (int8), byte 2 resultFrac (int8), byte 3 negative (bool),
 //   then int32 wordBuf[9] in base 10^9, most significant word first: integer words, then fraction words, the rest 0.
 // The library writes one canonical form: digitsInt = 9 * the number of integer words, at least one word (FromUint,
 // mydecimal.go:1069), digitsFrac = resultFrac = the result scale, and a zero result is never negative.  The update
-// kernels only see the 128-bit sum in two state words; this header is the one place that knows the layout.
+// kernels only see the 128-bit sum in two state words, or the int64 value * 10^scale of a DECIMAL argument; this header
+// is the one place that knows the layout.
 #pragma once
 
 namespace tg {
@@ -42,19 +44,80 @@ __device__ __forceinline__ __int128 dec_sum_of(unsigned long long lo, unsigned l
   return (__int128)(((unsigned __int128)hi << 64) | lo);
 }
 
-// SUM: the exact sum at scale 0 (sum4Decimal, func_sum.go:207-253; its final Round to 0 digits leaves an integer alone)
-__device__ __noinline__ void dec_sum_cell(uint8_t* cell, unsigned long long lo, unsigned long long hi) {
-  const __int128 s = dec_sum_of(lo, hi);
-  const bool neg = s < 0;
-  dec_store(cell, neg, neg ? (unsigned __int128)(-s) : (unsigned __int128)s, nullptr, 0, 0);
+__device__ __forceinline__ unsigned long long dec_pow10_u64(int k) {
+  unsigned long long p = 1;
+  for (int j = 0; j < k; j++) p *= 10ull;
+  return p;
 }
 
-// AVG: DecimalDiv(sum, count, frac) then Round(frac, ModeHalfUp) (baseAvgDecimal.AppendFinalResult2Chunk, func_avg.go:84-109).
-// doDivMod (mydecimal.go:2203) truncates the quotient at 9 * ceil(frac / 9) fraction digits; Round then looks only at the
-// first digit after the scale and rounds the magnitude.  With frac a multiple of 9 there is no such digit in the quotient,
-// so the result is the truncated quotient.  A quotient or rounded result of zero loses its sign (doDivMod and Round both
-// clear `negative` on zero).  `n` < 2^63, so r * 10^9 fits 128 bits.
-__device__ __noinline__ void dec_avg_cell(uint8_t* cell, unsigned long long lo, unsigned long long hi, unsigned long long n, int frac) {
+// ---- input cells of a DECIMAL(flen, scale) argument column, flen <= 18 --------------------------------------------------
+// A stored cell (MyDecimal.FromBin, mydecimal.go:1465) has digitsFrac == scale, ceil(digitsInt / 9) integer words (digitsInt
+// may be 0, and leading integer words may be 0), then ceil(scale / 9) fraction words, left-aligned: 0.5 at scale 1 is the
+// word 500000000.  resultFrac is not looked at, nor are the words after the fraction words.  Returns false for a cell in
+// any other form (digitsFrac != scale, a word >= 10^9, digits after the scale, more than flen significant digits); else
+// *v = value * 10^scale, |*v| < 10^flen <= 10^18, and a negative zero is 0.  c[0] is the header word (bytes digitsInt,
+// digitsFrac, resultFrac, negative), c[1..9] the words; every index is a constant, so c stays in registers.
+__device__ __forceinline__ bool dec_parse_cell(const uint32_t (&c)[10], int flen, int scale, long long* v) {
+  const int di = (int)(int8_t)(c[0] & 0xffu), df = (int)(int8_t)((c[0] >> 8) & 0xffu);
+  const bool neg = (c[0] >> 24) != 0;
+  if (df != scale || di < 0) return false;
+  const int wi = (di + 8) / 9, wf = (scale + 8) / 9;   // wf <= 2
+  if (wi + wf > 9) return false;
+  unsigned long long ip = 0, fr = 0;
+  bool ok = true;
+#pragma unroll
+  for (int j = 0; j < 9; j++) {
+    const uint32_t w = c[1 + j];
+    if (j < wi) {
+      // 1844674407 * 10^9 > 10^18 >= the bound checked below: a larger prefix is too many digits, and this keeps ip in 64 bits
+      if (w >= TG_DEC_WORD_BASE || ip >= 1844674407ull) ok = false;
+      else ip = ip * TG_DEC_WORD_BASE + w;
+    } else if (j < wi + wf) {
+      if (w >= TG_DEC_WORD_BASE) ok = false;
+      fr = fr * TG_DEC_WORD_BASE + w;
+    }
+  }
+  const unsigned long long pad = dec_pow10_u64(9 * wf - scale);
+  if (!ok || fr % pad != 0 || ip >= dec_pow10_u64(flen - scale)) return false;
+  const unsigned long long m = ip * dec_pow10_u64(scale) + fr / pad;
+  *v = neg ? -(long long)m : (long long)m;
+  return true;
+}
+
+// SUM: the exact sum at the argument's scale (sum4Decimal, func_sum.go:207-253; its final Round to the scale leaves the sum
+// alone).  The integer part is |sum| / 10^scale; the remainder, left-aligned, gives the ceil(scale / 9) fraction words.  A
+// DECIMAL MIN / MAX writes its int64 here too (hi = the sign extension).
+__device__ __noinline__ void dec_sum_cell(uint8_t* cell, unsigned long long lo, unsigned long long hi, int scale) {
+  const __int128 s = dec_sum_of(lo, hi);
+  const bool neg = s < 0;
+  unsigned __int128 m = neg ? (unsigned __int128)(-s) : (unsigned __int128)s;
+  const int nfw = (scale + 8) / 9;   // scale <= 18
+  uint32_t fw[2] = {0, 0};
+  if (scale) {
+    const unsigned long long p = dec_pow10_u64(scale);
+    const unsigned long long r = (unsigned long long)(m % p) * dec_pow10_u64(9 * nfw - scale);   // < 10^(9 nfw) <= 10^18
+    m /= p;
+    if (nfw == 2) { fw[0] = (uint32_t)(r / TG_DEC_WORD_BASE); fw[1] = (uint32_t)(r % TG_DEC_WORD_BASE); }
+    else fw[0] = (uint32_t)r;
+  }
+  dec_store(cell, neg, m, fw, nfw, scale);
+}
+
+// AVG: DecimalDiv(sum, count, incr) then Round(frac, ModeHalfUp) (baseAvgDecimal.AppendFinalResult2Chunk, func_avg.go:84-109),
+// for a sum of `scale` fraction digits and frac = min(scale + incr, 30) (typeInfer4Avg, base_func.go:274).
+// Why the quotient is truncated at 9 * ceil(frac / 9) fraction digits for every div_precision_increment `incr`: every input
+// cell has digitsFrac == scale, so the sum does too (DecimalAdd keeps the larger digitsFrac), and the count has 0.  doDivMod
+// (mydecimal.go:2203) then computes ceil((9 * ceil(scale / 9) + max(0, incr - (9 * ceil(scale / 9) - scale))) / 9) =
+// ceil((scale + incr) / 9) fraction words of the quotient, truncated, i.e. T = 9 * ceil((scale + incr) / 9) digits.  When
+// scale + incr <= 30, frac = scale + incr and T = 9 * ceil(frac / 9).  When it is capped (frac = 30), T >= 36 > 31 digits:
+// the first 31 digits are those of the exact quotient either way, and Round looks only at the first digit after the scale,
+// so truncating at 36 = 9 * ceil(30 / 9) gives the same result.  Round rounds the magnitude half up on digit frac + 1; with
+// frac a multiple of 9 (uncapped) there is no such digit in the quotient, so the result is the truncated quotient.  A
+// quotient or rounded result of zero loses its sign (doDivMod and Round both clear `negative` on zero).
+// The value is sum / (count * 10^scale), and count * 10^scale can pass 64 bits: the digits are those of m / n (m = |sum|),
+// with the point moved `scale` places, so the integer part is q / 10^scale (q = m / n), the fraction digits are the low
+// `scale` digits of q, then the digits of r / n (r = m % n).  `n` < 2^63, so r * 10^9 fits 128 bits.  frac >= scale.
+__device__ __noinline__ void dec_avg_cell(uint8_t* cell, unsigned long long lo, unsigned long long hi, unsigned long long n, int scale, int frac) {
   const __int128 s = dec_sum_of(lo, hi);
   const bool neg = s < 0;
   const unsigned __int128 m = neg ? (unsigned __int128)(-s) : (unsigned __int128)s;
@@ -62,10 +125,25 @@ __device__ __noinline__ void dec_avg_cell(uint8_t* cell, unsigned long long lo, 
   unsigned long long r = (unsigned long long)(m % n);
   const int nfw = (frac + 8) / 9;
   uint32_t fw[4];   // frac <= 30
+  // the low `scale` digits of q: its first 9 * (scale / 9) digits as whole words (`top`), then the last scale % 9 digits
+  // (`carry`), which shift the words of r / n right by scale % 9 digits (scale 0: top = carry = 0, the words of r / n as they are)
+  const int aw = scale / 9;
+  const unsigned long long pb = dec_pow10(scale % 9), lift = TG_DEC_WORD_BASE / pb;
+  unsigned long long low = 0;
+  if (scale) {   // a DECIMAL(p <= 18) argument: |sum| < n * 10^18, so q < 10^18 fits 64 bits
+    const unsigned long long q64 = (unsigned long long)q, p = dec_pow10_u64(scale);
+    low = q64 % p;
+    q = q64 / p;
+  }
+  const unsigned long long top = low / pb;
+  unsigned long long carry = low % pb;
   for (int j = 0; j < nfw; j++) {
+    if (j < aw) { fw[j] = (uint32_t)(aw == 2 && j == 0 ? top / TG_DEC_WORD_BASE : top % TG_DEC_WORD_BASE); continue; }
     const unsigned __int128 x = (unsigned __int128)r * TG_DEC_WORD_BASE;
-    fw[j] = (uint32_t)(x / n);
+    const unsigned long long e = (unsigned long long)(x / n);
     r = (unsigned long long)(x % n);
+    fw[j] = (uint32_t)(carry * lift + e / pb);
+    carry = e % pb;
   }
   if (frac % 9) {   // Round, mydecimal.go:892-898: keep the word's first frac % 9 digits, half up on the next one
     const uint32_t p = dec_pow10(9 - frac % 9 - 1);
@@ -84,6 +162,13 @@ __device__ __noinline__ void dec_avg_cell(uint8_t* cell, unsigned long long lo, 
   bool zero = q == 0;
   for (int j = 0; j < nfw; j++) zero &= fw[j] == 0;
   dec_store(cell, neg && !zero, q, fw, nfw, frac);
+}
+
+// the one call k_agg_finalize makes for a non-NULL DECIMAL result: AVG, or SUM / MIN / MAX (one call site instead of two
+// keeps the kernel at 64 registers)
+__device__ __noinline__ void dec_result_cell(uint8_t* cell, bool avg, unsigned long long lo, unsigned long long hi, unsigned long long n, int scale, int frac) {
+  if (avg) dec_avg_cell(cell, lo, hi, n, scale, frac);
+  else dec_sum_cell(cell, lo, hi, scale);
 }
 
 }  // namespace tg

@@ -14,14 +14,16 @@ from .plan import AggPlan, JoinPlan
 
 
 def dev_chunk(cols: Sequence[torch.Tensor], nulls: Optional[Sequence[Optional[torch.Tensor]]] = None):
-    """tg_chunk whose pointers are device addresses of 1-D int64/float64/float32 CUDA tensors."""
+    """tg_chunk whose pointers are device addresses of 1-D int64/float64/float32 CUDA tensors, or (n, 40) uint8 tensors of
+    MyDecimal cells (a DECIMAL column)."""
     n = len(cols)
     arr = (abi.TgColumn * max(n, 1))()
     for i, t in enumerate(cols):
-        assert t.is_cuda and t.dim() == 1 and t.is_contiguous()
-        arr[i].length = t.numel()
+        dec = t.dim() == 2 and t.dtype == torch.uint8 and t.shape[1] == 40
+        assert t.is_cuda and (t.dim() == 1 or dec) and t.is_contiguous()
+        arr[i].length = t.shape[0]
         arr[i].data = t.data_ptr()
-        arr[i].elem_len = t.element_size()
+        arr[i].elem_len = 40 if dec else t.element_size()
         arr[i].offsets = None
         nb = nulls[i] if nulls is not None else None
         arr[i].null_bitmap = nb.data_ptr() if nb is not None else None
@@ -91,9 +93,9 @@ class DeviceAgg:
     def __init__(self, plan: AggPlan):
         self.lib = abi.load_lib()
         self.plan = plan
-        desc, self._keep = plan.to_struct()
+        desc, self._keep = plan.to_struct_ex()
         self.h = C.c_void_p()
-        abi.check(self.lib.tg_agg_open(C.byref(desc), C.byref(self.h)))
+        abi.check(self.lib.tg_agg_open_ex(C.byref(desc), C.byref(self.h)))
         self.n_out = len(plan.funcs)
 
     def push(self, cols: Sequence[torch.Tensor], nulls=None) -> None:

@@ -167,16 +167,24 @@ class HashAggExec(Executor):
     def _ret_type(plan: AggPlan, f) -> FieldType:
         if f.name == abi.AGG_COUNT:
             return FieldType(abi.TYPE_LONGLONG, abi.FLAG_NOT_NULL)
+        arg = plan.col_types[f.arg_col] if f.arg_col >= 0 else None
         if f.name in (abi.AGG_SUM, abi.AGG_AVG):
+            if arg is not None and arg.tp == abi.TYPE_NEWDECIMAL and f.ret_type == abi.TYPE_NEWDECIMAL:
+                # typeInfer4Sum / typeInfer4Avg over DECIMAL(p, s) (aggregation/base_func.go:223, :274): SUM (p + 22, s),
+                # AVG (p + the scale increment, ret_frac), both at most 65 digits
+                if f.name == abi.AGG_SUM:
+                    return FieldType(abi.TYPE_NEWDECIMAL, 0, min(arg.flen + 22, 65), arg.decimal)
+                return FieldType(abi.TYPE_NEWDECIMAL, 0, min(arg.flen + f.ret_frac - arg.decimal, 65), f.ret_frac)
             return FieldType(abi.TYPE_NEWDECIMAL if f.ret_type == abi.TYPE_NEWDECIMAL else abi.TYPE_DOUBLE, 0)
-        return FieldType(plan.col_types[f.arg_col].tp, plan.col_types[f.arg_col].flag & ~abi.FLAG_NOT_NULL)
+        # MIN / MAX / FIRSTROW: the argument's type without NOT NULL (typeInfer4MaxMin), DECIMAL(p, s) included
+        return FieldType(arg.tp, arg.flag & ~abi.FLAG_NOT_NULL, arg.flen, arg.decimal)
 
     def open(self) -> None:
         super().open()
         self._lib = abi.load_lib()
-        desc, self._keep = self.plan.to_struct()
+        desc, self._keep = self.plan.to_struct_ex()
         self._h = C.c_void_p()
-        abi.check(self._lib.tg_agg_open(C.byref(desc), C.byref(self._h)))
+        abi.check(self._lib.tg_agg_open_ex(C.byref(desc), C.byref(self._h)))
         self._prepared = False
 
     def next(self, required_rows: int = MAX_CHUNK_SIZE) -> Chunk:

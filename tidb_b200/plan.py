@@ -15,11 +15,17 @@ from typing import List, Optional, Sequence, Tuple
 from . import abi
 
 
+UNSPECIFIED_LENGTH = -1   # types.UnspecifiedLength
+
+
 @dataclass
 class FieldType:
-    """types.FieldType reduced to what the path needs: MySQL type code + flag bits."""
+    """types.FieldType reduced to what the path needs: MySQL type code + flag bits, and GetFlen() / GetDecimal() (the
+    precision and scale of a DECIMAL column; -1 = not given)."""
     tp: int = abi.TYPE_LONGLONG
     flag: int = 0
+    flen: int = UNSPECIFIED_LENGTH
+    decimal: int = UNSPECIFIED_LENGTH
 
     @property
     def not_null(self) -> bool:
@@ -163,7 +169,8 @@ class AggFunc:
     arg_col2: int = -1
     arg_expr: int = 0          # abi.ARGEXPR_*: the argument as arg_col * arg_col2 / arg_col * (arg_const - arg_col2)
     arg_const: float = 0.0
-    ret_type: int = 0          # AggFuncDesc.RetTp.GetType(): abi.TYPE_NEWDECIMAL = exact DECIMAL SUM / AVG of an integer column
+    ret_type: int = 0          # AggFuncDesc.RetTp.GetType(): abi.TYPE_NEWDECIMAL = exact DECIMAL SUM / AVG of an integer
+                               # column, or SUM / AVG / MIN / MAX of a DECIMAL column
     ret_frac: int = 0          # AggFuncDesc.RetTp.GetDecimal()
 
 
@@ -196,6 +203,15 @@ class AggPlan:
         d.stream = self.stream or None
         d.expected_groups = self.expected_groups
         return d, keep
+
+    def to_struct_ex(self) -> Tuple[abi.TgAggDescEx, list]:
+        """tg_agg_desc_ex: to_struct() plus the precision and scale of every child column"""
+        d, keep = self.to_struct()
+        ex = abi.TgAggDescEx()
+        ex.base = d
+        a = _i32([t.flen for t in self.col_types]); keep.append(a); ex.col_flen = a
+        a = _i32([t.decimal for t in self.col_types]); keep.append(a); ex.col_decimal = a
+        return ex, keep
 
 
 # ---------------------------------------------------------------------------------------------------------------
