@@ -299,10 +299,10 @@ enum {
   TG_JOIN_PATH_PROBE_UQ = 1 << 0,       /* single-pass unique-key probe (k_probe_inner_uq)                       */
   TG_JOIN_PATH_PROBE_GENERAL = 1 << 1,  /* general count -> scan -> write probe                                  */
   TG_JOIN_PATH_PROBE_DIRECT = 1 << 2,   /* fused warp probe (k_probe_inner_u1_w), also the gated fallback launch  */
-  TG_JOIN_PATH_PROBE_SEG = 1 << 3,      /* segment probe over L2-partitioned rows (k_probe_inner_u1_seg*)        */
-  TG_JOIN_PATH_PROBE_TILE = 1 << 4,     /* fused CTA-tile probe (k_probe_inner_u1)                               */
+  TG_JOIN_PATH_PROBE_SEG = 1 << 3,      /* segment probe over L2-partitioned rows (k_probe_inner_u1_seg_lean)    */
+  /* 1 << 4 is unassigned: older headers name a removed kernel with it, so a new path must not reuse it              */
   TG_JOIN_PATH_SCATTER_BULK = 1 << 5,   /* bulk partition scatter (k_partition_scatter_bulk)                     */
-  TG_JOIN_PATH_SCATTER = 1 << 6         /* any other partition scatter kernel                                    */
+  TG_JOIN_PATH_SCATTER = 1 << 6         /* LSU partition scatter over the whole input (k_partition_scatter)      */
 };
 int tg_join_get_stats(tg_join* j, tg_join_stats* out);
 

@@ -40,9 +40,10 @@ def test_stats_struct_layout_and_path_bits():
     assert abi.TgAggStats.paths.offset == 9 * 8
     hdr = open(os.path.join(ROOT, "include", "tidbgpu.h")).read()
     bits = dict((m.group(1), 1 << int(m.group(2))) for m in re.finditer(r"\bTG_((?:JOIN|AGG)_PATH_[A-Z0-9_]+) = 1 << (\d+)", hdr))
-    assert len(bits) == 14
+    assert len(bits) == 13
     for name, v in bits.items():
         assert getattr(abi, name) == v, name
+    assert 1 << 4 not in [v for name, v in bits.items() if name.startswith("JOIN")]   # unassigned, never reused
 
 
 def test_fixed_len_matches_reference(lib):

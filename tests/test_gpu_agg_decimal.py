@@ -406,6 +406,7 @@ def test_full_scale_100m_rows_1m_groups():
     gen = torch.Generator(device="cuda").manual_seed(21)
     keys = torch.randint(0, G, (n,), device="cuda", dtype=torch.int64, generator=gen)
     vals = torch.randint(-(1 << 31), 1 << 31, (n,), device="cuda", dtype=torch.int64, generator=gen)
+    torch.cuda.synchronize()   # the aggregation reads its input on a stream of its own: it must be written first
     plan = AggPlan([INT_NN, INT_NN], [0], [AggFunc(P.AGG_FIRSTROW, 0), sum_(1), AggFunc(P.AGG_COUNT, -1)], expected_groups=G)
     agg = DeviceAgg(plan)
     try:

@@ -598,6 +598,7 @@ def test_full_scale_100m_rows_1m_groups():
     w[:, 3] = ((m % 100) * 10 ** 7).to(torch.int32)
     del m, ip
     cells = w.view(torch.uint8).view(n, 40)
+    torch.cuda.synchronize()   # the aggregation reads its input on a stream of its own: it must be written first
     plan = AggPlan([INT_NN, FieldType(DEC, abi.FLAG_NOT_NULL, 15, 2)], [0], [AggFunc(P.AGG_FIRSTROW, 0), dsum(1, 2), AggFunc(P.AGG_COUNT, -1)],
                    expected_groups=G)
     agg = DeviceAgg(plan)

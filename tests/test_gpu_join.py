@@ -417,34 +417,19 @@ def test_partial_match_and_stats():
 def _fused_variant_paths(env):
     """(bits that must be set, bits that must be clear) in tg_join_stats.paths for a test_fused_probe_variants_forced env"""
     J = abi
-    seg, bulk, other, direct, tile = J.JOIN_PATH_PROBE_SEG, J.JOIN_PATH_SCATTER_BULK, J.JOIN_PATH_SCATTER, J.JOIN_PATH_PROBE_DIRECT, J.JOIN_PATH_PROBE_TILE
-    never = J.JOIN_PATH_PROBE_UQ | J.JOIN_PATH_PROBE_GENERAL
-    if env.get("TG_PROBE_VARIANT") == "0":           # CTA-tile kernel; the partition pass needs the warp kernels
-        return tile, never | direct | seg | bulk | other
-    part = env.get("TG_PROBE_PARTITION", "1")
-    if part == "0":
-        return direct, never | tile | seg | bulk | other
-    if part == "1":                                  # count-free pass: bulk scatter, segment probe (8-byte warp kernel without SEG_VEC)
-        if env.get("TG_PROBE_SEG_VEC") == "0":
-            return direct | bulk, never | tile | seg | other
-        return direct | bulk | seg, never | tile | other
-    scatter, no_scatter = (other, bulk) if env.get("TG_SCATTER_BULK") == "0" else (bulk, other)
-    return direct | scatter, never | tile | seg | no_scatter   # counted pass, then the warp kernel over dense partitions
+    seg, bulk, other, direct = J.JOIN_PATH_PROBE_SEG, J.JOIN_PATH_SCATTER_BULK, J.JOIN_PATH_SCATTER, J.JOIN_PATH_PROBE_DIRECT
+    never = J.JOIN_PATH_PROBE_UQ | J.JOIN_PATH_PROBE_GENERAL | 1 << 4   # bit 4 is unassigned
+    if env.get("TG_PROBE_PARTITION", "1") == "0":
+        return direct, never | seg | bulk | other
+    return direct | bulk | seg, never | other   # count-free pass: bulk scatter, segment probe, gated fallback + tail
 
 
-@pytest.mark.parametrize("env", [dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="5"), dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="16"),
-                                 dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="7", TG_PROBE_SEG_VEC="0"),
-                                 dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="5", TG_PROBE_SEG_LEAN="0"), dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="6", TG_PROBE_SEG_LEAN="2"),
-                                 dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="4", TG_PROBE_SEG_LEAN="1", TG_PROBE_CARVEOUT="0"),
-                                 dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="5", TG_PROBE_SUBSEG="0"), dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="2", TG_PROBE_SUBSEG="1"),
-                                 dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="9", TG_PROBE_SUBSEG="0", TG_PROBE_SEG_LEAN="0"),
-                                 dict(TG_PROBE_PARTITION="2", TG_PROBE_PARTS="5"), dict(TG_PROBE_PARTITION="2", TG_PROBE_PARTS="3", TG_SCATTER_BULK="0"),
-                                 dict(TG_PROBE_PARTITION="0"), dict(TG_PROBE_VARIANT="0")])
+@pytest.mark.parametrize("env", [dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS=p) for p in ("2", "4", "5", "6", "7", "9", "16")]
+                         + [dict(TG_PROBE_PARTITION="0")])
 def test_fused_probe_variants_forced(env, monkeypatch):
-    # every launch variant of the fused fast path (L2 partition pass in both layouts, segment kernels, warp kernel, CTA-tile kernel) must
-    # give the same multiset; odd sizes exercise the tail tiles; PART_MIN_MB=0 forces the partition pass on a small table
-    for k in ("TG_PROBE_VARIANT", "TG_PROBE_SEG_VEC", "TG_SCATTER_BULK", "TG_PROBE_UQ"):
-        monkeypatch.delenv(k, raising=False)
+    # the fused fast path with the L2 partition pass at several slice counts, and without the pass, must give the same
+    # multiset; odd sizes exercise the tail tiles; PART_MIN_MB=0 forces the partition pass on a small table
+    monkeypatch.delenv("TG_PROBE_UQ", raising=False)
     for k, v in dict(env, TG_PROBE_PART_MIN_MB="0", TG_PROBE_PART_MIN_ROWS="0").items():
         monkeypatch.setenv(k, v)
     rng = np.random.default_rng(17)
@@ -478,6 +463,43 @@ def test_fused_probe_variants_forced(env, monkeypatch):
     assert np.array_equal(got[0], pk[got[1]]) and np.array_equal(got[2], got[0])     # keys travel with their row
     exp_pay = (order[pos] * 3)[got[1]]
     assert np.array_equal(got[3], exp_pay)                                           # and with the right build payload
+
+
+@pytest.mark.parametrize("lused,rused", [([0, 1, 2, 3, 4], [0, 1]),   # four probe payload columns
+                                         ([0, 1, 1], [1]),             # one probe column output twice
+                                         ([0, 0, 1], [0, 1])])         # three outputs carry the join key
+def test_unique_key_shapes_the_warp_kernels_do_not_cover(lused, rused):
+    # a U1 table (unique keys, one 8-byte payload) and an output shape the fused warp kernels are not instantiated for:
+    # the single-pass unique-key kernel takes the batch
+    rng = np.random.default_rng(31)
+    nb, npr = 60_000, 400_001
+    bk = rng.permutation(nb).astype(np.int64) * 2654435761 - (1 << 40)
+    bv = np.arange(nb, dtype=np.int64) * 3 + 1
+    pk = np.where(rng.random(npr) < 0.7, bk[rng.integers(0, nb, npr)], rng.integers(1 << 50, 1 << 51, npr))
+    pcols = [pk] + [np.arange(npr, dtype=np.int64) * m + a for m, a in ((1, 0), (5, 2), (-7, 1), (11, -3))]
+    plan = JoinPlan(abi.JOIN_INNER, [INT_NN] * 5, [INT_NN, INT_NN], [0], [0], lused=lused, rused=rused)
+    e = HashJoinExec(plan, MockDataSource(plan.left_types, [Chunk([Column(c) for c in pcols])]),
+                     MockDataSource(plan.right_types, [Chunk([Column(bk), Column(bv)])]))
+    e.open()
+    chunks = []
+    while True:
+        c = e.next(1 << 20)
+        if c.num_rows() == 0:
+            break
+        chunks.append(c)
+    st = e.stats()
+    e.close()
+    assert st.table_mode == 1
+    assert st.paths & abi.JOIN_PATH_PROBE_UQ, hex(st.paths)
+    assert not st.paths & (abi.JOIN_PATH_PROBE_DIRECT | abi.JOIN_PATH_PROBE_SEG | abi.JOIN_PATH_PROBE_GENERAL | 1 << 4), hex(st.paths)
+    got = [np.concatenate([c.columns[i].data for c in chunks]) for i in range(len(lused) + len(rused))]
+    order = np.argsort(bk)
+    pos = np.minimum(np.searchsorted(bk[order], pk), nb - 1)
+    rows = np.nonzero(bk[order][pos] == pk)[0]                     # matching probe rows, ascending
+    want = [pcols[c][rows] for c in lused] + [(bk, bv)[c][order[pos[rows]]] for c in rused]
+    by_row = np.argsort(got[lused.index(1)])                       # probe column 1 is the probe row index
+    for g, w in zip(got, want):
+        assert np.array_equal(g[by_row], w)
 
 
 def test_partitioned_probe_overflow_falls_back(monkeypatch):
@@ -650,9 +672,7 @@ def test_probe_device_segments_matches_dense_probe(monkeypatch):
         pk_all.append(k); pv_all.append(v)
     pk, pv = np.concatenate(pk_all), np.concatenate(pv_all)
     t = lambda a: torch.from_numpy(a).to(dev)
-    for env in (dict(TG_PROBE_PARTITION="0"), dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="6", TG_PROBE_PART_MIN_MB="0", TG_PROBE_PART_MIN_ROWS="0"),
-                dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="6", TG_PROBE_PART_MIN_MB="0", TG_PROBE_PART_MIN_ROWS="0", TG_PROBE_SEG_LEAN="0"),
-                dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="6", TG_PROBE_PART_MIN_MB="0", TG_PROBE_PART_MIN_ROWS="0", TG_PROBE_SUBSEG="0")):
+    for env in (dict(TG_PROBE_PARTITION="0"), dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="6", TG_PROBE_PART_MIN_MB="0", TG_PROBE_PART_MIN_ROWS="0")):
         for k_, v_ in env.items():
             monkeypatch.setenv(k_, v_)
         plan = JoinPlan(abi.JOIN_INNER, [INT_NN, INT_NN], [INT_NN, INT_NN], [0], [0], device=0)

@@ -1,6 +1,6 @@
-"""Unique-key join tables at high load factors and every home width: long linear-probe runs (probed by 32-byte pairs),
-runs that wrap past the last slot, the sentinel key, every probe path, and the densified default table.  Every output row
-is compared with a numpy reference."""
+"""Unique-key join tables at high load factors: long linear-probe runs (probed by 32-byte pairs), runs that wrap past the
+last slot, the sentinel key, every probe path, and the densified default table.  Every output row is compared with a numpy
+reference."""
 import numpy as np
 import pytest
 
@@ -75,36 +75,32 @@ def run_host(bk, bv, pk, lf, filt=None):
 
 
 def setenv(monkeypatch, env):
-    for k in ("TG_PROBE_PARTITION", "TG_PROBE_PARTS", "TG_PROBE_SEG_VEC", "TG_PROBE_VARIANT", "TG_PROBE_UQ", "TG_PAIR_HOME"):
+    for k in ("TG_PROBE_PARTITION", "TG_PROBE_PARTS", "TG_PROBE_UQ"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)
 
 
-@pytest.mark.parametrize("width", [1, 2, 4])
 @pytest.mark.parametrize("lf", [0.35, 0.8, 0.95])
 @pytest.mark.parametrize("match", [1.0, 0.5, 0.0])
-def test_dense_table_segment_probe(width, lf, match, monkeypatch):
-    setenv(monkeypatch, dict(PART, TG_PAIR_HOME={1: "0", 2: "2", 4: "4"}[width]))
+def test_dense_table_segment_probe(lf, match, monkeypatch):
+    setenv(monkeypatch, PART)
     nb, npr = 100_003, 700_001
-    bk, bv, pk = make_sides(nb, npr, match, seed=int(lf * 100) + width)
+    bk, bv, pk = make_sides(nb, npr, match, seed=int(lf * 100))
     got, st = run_host(bk, bv, pk, lf)
     check(got, bk, bv, pk)
-    assert st.table_slots == table_slots(nb, 50 << 20, load_factor=lf, home_width=width)
-    want = abi.JOIN_PATH_PROBE_SEG if width > 1 else abi.JOIN_PATH_PROBE_SEG | abi.JOIN_PATH_PROBE_DIRECT
-    assert st.paths & want == want, hex(st.paths)
+    assert st.table_slots == table_slots(nb, 50 << 20, load_factor=lf)
+    assert st.paths & abi.JOIN_PATH_PROBE_SEG, hex(st.paths)
 
 
 @pytest.mark.parametrize("path,env,filt,bit", [
     ("direct", dict(TG_PROBE_PARTITION="0"), None, abi.JOIN_PATH_PROBE_DIRECT),
     ("segment", PART, None, abi.JOIN_PATH_PROBE_SEG),
-    ("segment, 8-byte stores", dict(PART, TG_PROBE_SEG_VEC="0"), None, abi.JOIN_PATH_PROBE_DIRECT | abi.JOIN_PATH_SCATTER_BULK),
     ("unique key", {}, [FilterItem(abi.CMP_GE, 1, const_i64=0)], abi.JOIN_PATH_PROBE_UQ),
     ("general", dict(TG_PROBE_UQ="0"), [FilterItem(abi.CMP_GE, 1, const_i64=0)], abi.JOIN_PATH_PROBE_GENERAL),
 ])
-@pytest.mark.parametrize("width", [1, 2, 4])
-def test_dense_table_every_probe_path(path, env, filt, bit, width, monkeypatch):
-    setenv(monkeypatch, dict(env, TG_PAIR_HOME={1: "0", 2: "2", 4: "4"}[width]))
+def test_dense_table_every_probe_path(path, env, filt, bit, monkeypatch):
+    setenv(monkeypatch, env)
     bk, bv, pk = make_sides(60_001, 500_001, 0.5, seed=7)
     got, st = run_host(bk, bv, pk, 0.9, filt)
     check(got, bk, bv, pk)
@@ -113,7 +109,7 @@ def test_dense_table_every_probe_path(path, env, filt, bit, width, monkeypatch):
 
 def test_dense_table_skewed_probe_takes_the_fallback(monkeypatch):
     # 70 % of the probe rows carry one key: a segment overflows and the gated direct launch probes the dense table
-    setenv(monkeypatch, dict(PART, TG_PAIR_HOME="4"))
+    setenv(monkeypatch, PART)
     bk, bv, pk = make_sides(80_001, 1_000_000, 1.0, seed=5)
     pk[np.random.default_rng(1).random(len(pk)) < 0.7] = bk[0]
     got, st = run_host(bk, bv, pk, 0.9)
@@ -134,6 +130,7 @@ def _device_join(nb, npr, lf, dup=False):
     pk = torch.where(torch.rand(npr, device=dev, generator=g) < 0.5, bk[torch.randint(0, nb, (npr,), device=dev, generator=g)],
                      torch.randint(0, 1 << 60, (npr,), device=dev, generator=g) * 2)   # misses: even, build keys are odd
     pv = torch.arange(npr, device=dev, dtype=torch.int64)
+    torch.cuda.synchronize(dev)   # the join reads its inputs on a stream of its own: they must be written first
     INT = FieldType(abi.TYPE_LONGLONG, abi.FLAG_NOT_NULL)
     plan = JoinPlan(abi.JOIN_INNER, [INT, INT], [INT, INT], [0], [0], build_is_right=True, device=0, load_factor=lf)
     j = DeviceJoin(plan)
@@ -155,9 +152,9 @@ def test_densified_default_table_device_input(monkeypatch):
 
 
 def test_dense_table_explicit_load_factor_device_input(monkeypatch):
-    setenv(monkeypatch, dict(TG_PAIR_HOME="4"))
+    setenv(monkeypatch, {})
     (bk, bv, pk), got, st, l2 = _device_join(6_000_000, 20_000_000, 0.9)
-    assert st.table_slots == table_slots(6_000_000, l2, load_factor=0.9, home_width=4)
+    assert st.table_slots == table_slots(6_000_000, l2, load_factor=0.9)
     check(got, bk, bv, pk)
 
 

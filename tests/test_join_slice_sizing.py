@@ -7,6 +7,7 @@ SLOT = 16                  # bytes per table slot {int64 key, u64 meta}
 MAX_PARTS = 16             # TG_MAX_PARTS
 MAX_DENSE_LOAD = 0.5       # kMaxDenseLoad
 PART_MIN_MB = 64           # TG_PROBE_PART_MIN_MB default
+HOME_WIDTH = 4             # kHomeWidth: the slot count is a multiple of it
 H100_L2 = 50 << 20         # cudaDevAttrL2CacheSize of an H100 SXM
 
 
@@ -18,16 +19,15 @@ def probe_slices(table_bytes, l2_bytes):
     return min(-(-table_bytes // slice_target(l2_bytes)), MAX_PARTS)
 
 
-def table_slots(n, l2_bytes, load_factor=None, u1=True, home_width=4):
+def table_slots(n, l2_bytes, load_factor=None, u1=True):
     """slots of the table a build of n rows gets (load_factor None = the default)"""
     default = load_factor is None
     nslots = int(max(n, 1) / (0.35 if default else load_factor)) + 32
     if default and nslots > MAX_PARTS * (33 << 20) // SLOT:
         nslots = max(MAX_PARTS * (33 << 20) // SLOT, int(max(n, 1) / 0.5) + 32)
-    align = max(home_width, 2)
-    nslots &= ~(align - 1)
+    nslots &= ~(HOME_WIDTH - 1)
     if u1 and default and n > 0:
-        dense = max(MAX_PARTS * slice_target(l2_bytes) // SLOT, int(n / MAX_DENSE_LOAD) + 32) & ~(align - 1)
+        dense = max(MAX_PARTS * slice_target(l2_bytes) // SLOT, int(n / MAX_DENSE_LOAD) + 32) & ~(HOME_WIDTH - 1)
         part_min = PART_MIN_MB << 20
         if nslots * SLOT > part_min and dense < nslots and dense * SLOT > part_min:
             nslots = dense
@@ -58,9 +58,9 @@ def test_tables_that_stay_as_they_are():
     # small tables (no partition pass), tables already within 16 target slices, explicit load factors, G tables
     assert table_slots(1_000_000, H100_L2) == int(1_000_000 / 0.35) + 32 & ~3
     assert table_slots(4_000_000, H100_L2) == int(4_000_000 / 0.35) + 32 & ~3          # 183 MB <= 16 x 12.5 MiB
-    assert table_slots(10_000_000, H100_L2, load_factor=0.35) == 28_571_460 == table_slots(10_000_000, H100_L2, load_factor=0.35, home_width=2)
+    assert table_slots(10_000_000, H100_L2, load_factor=0.35) == 28_571_460
     assert table_slots(10_000_000, H100_L2, u1=False) == 28_571_460
-    assert table_slots(101, H100_L2) % 4 == 0 and table_slots(101, H100_L2, home_width=2) % 2 == 0
+    assert table_slots(101, H100_L2) % 4 == 0
 
 
 def test_slices_follow_l2():

@@ -494,26 +494,16 @@ static int composite_key(JoinImpl* j, const Side& s, const DevCols& v, int64_t n
   return TG_OK;
 }
 
-// ---- fast-path launch tuning (env overrides are for A/B sweeps; the defaults are the production choice) ----
-struct ProbeTuning { int variant; int R; int evict_last; int ctas_per_sm; int partition; int subseg; int parts; int part_min_mb; int part_min_rows; int seg_vec; int seg_lean; int carveout; int tma; int stages; int tma_ctas; int cta_agg; };
+// ---- fast-path launch tuning (the defaults are the production choice; the overrides let tests and tools force the
+// partition pass, or no pass, on any input) ----
+struct ProbeTuning { int ctas_per_sm; bool partition; int parts; int part_min_mb; int part_min_rows; };
 static ProbeTuning probe_tuning() {
   ProbeTuning t;
-  t.variant = env_int("TG_PROBE_VARIANT", 1);      // 0: CTA-tile kernel (shared-memory offsets), 1: warp-autonomous kernel
-  t.R = env_int("TG_PROBE_R", 4);
-  t.evict_last = env_int("TG_PROBE_EVICT_LAST", 0);
   t.ctas_per_sm = env_int("TG_PROBE_CTAS_PER_SM", 0);   // 0 = exactly the resident CTA count (occupancy query)
-  t.partition = env_int("TG_PROBE_PARTITION", 1);   // regroup big probes into L2-sized partitions first (0 = never, 2 = counted/dense variant)
-  t.subseg = env_int("TG_PROBE_SUBSEG", 0);         // 1 = CTA-private sub-segments in the L2 partition pass (no global cursor atomics): off, slower (thousands of write streams, and the interleaved empty tails let warps drift across partitions)
+  t.partition = env_int("TG_PROBE_PARTITION", 1) != 0;   // regroup big probes into L2-sized partitions first (0 = never)
   t.parts = env_int("TG_PROBE_PARTS", 0);           // 0 = auto (probe_slices), at most TG_MAX_PARTS
   t.part_min_mb = env_int("TG_PROBE_PART_MIN_MB", 64);
   t.part_min_rows = env_int("TG_PROBE_PART_MIN_ROWS", 1 << 22);
-  t.seg_vec = env_int("TG_PROBE_SEG_VEC", 1);            // 128-bit loads/stores in the segment probe
-  t.seg_lean = env_int("TG_PROBE_SEG_LEAN", 1);          // 1 = lean full-tile path (default), 0 = round-1 kernel, 2 = + register prefetch
-  t.carveout = env_int("TG_PROBE_CARVEOUT", -1);         // EXPERIMENTAL: preferred shared-memory carve-out (%) of the segment probe kernels, -1 = driver default
-  t.tma = 0;                                        // (the TMA-fed probe kernels were removed in round 2)
-  t.stages = env_int("TG_PROBE_STAGES", 4);
-  t.tma_ctas = env_int("TG_PROBE_TMA_CTAS", 3);
-  t.cta_agg = env_int("TG_PROBE_CTA_AGG", 1);        // one output-cursor atomic per CTA tile (TMA kernel)
   return t;
 }
 
@@ -562,14 +552,10 @@ static int build_table(JoinImpl* j) {
     const unsigned long long dense = (unsigned long long)((double)(n > 0 ? n : 1) / 0.5) + 32;
     if (nslots > fit) nslots = std::max(fit, dense);
   }
-  // TG_PAIR_HOME: home width in slots (0 = 1, a single slot; 1 or 2 = a 32-byte pair; 4 = a 64-byte half-line, the default:
-  // 2-6 % faster than pairs on the 100 % match step at load factors 0.5-0.8, same sweep as kMaxDenseLoad)
-  const int pair_home = env_int("TG_PAIR_HOME", 4);
-  const int home_width = pair_home >= 4 ? 4 : pair_home >= 1 ? 2 : 1;
-  const unsigned long long align = home_width > 2 ? home_width : 2;   // even in any case: runs continue by 32-byte pairs
+  const unsigned long long align = kHomeWidth;   // whole homes; even, as runs continue by 32-byte pairs
   nslots &= ~(align - 1);
   if (nslots + 1 >= 0xFFFFFFFFull) return fail(TG_ERR_UNSUPPORTED, "build side too large for 32-bit slot ids");
-  TG_TRY(j->table.ensure(j->device, (size_t)(nslots + 1) * sizeof(Slot)));
+  TG_TRY(j->table.ensure(j->device, (size_t)(nslots + 2) * sizeof(Slot)));   // + the side slot and a spare (probe_rows_u1)
   TG_TRY(j->row_slot.ensure(j->device, (size_t)(n + 1) * 4));
   TG_TRY(j->row_rank.ensure(j->device, (size_t)(n + 1) * 4));
   TG_TRY(j->scalars.ensure(j->device, 64));
@@ -580,7 +566,7 @@ static int build_table(JoinImpl* j) {
   k_table_init<<<grid_for(j, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, nslots);
   j->stats.kernel_launches++;
   if (n > 0) {
-    k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots, home_width,
+    k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots,
                                                                   j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>());
     j->stats.kernel_launches++;
   }
@@ -610,19 +596,19 @@ static int build_table(JoinImpl* j) {
     const size_t part_min = (size_t)tune.part_min_mb << 20;
     const unsigned long long dense = std::max<unsigned long long>((unsigned long long)TG_MAX_PARTS * l2_slice_target(j->device) / sizeof(Slot),
                                                                   (unsigned long long)((double)n / kMaxDenseLoad) + 32) & ~(align - 1);
-    if (tune.partition == 1 && nslots * sizeof(Slot) > part_min && dense < nslots && dense * sizeof(Slot) > part_min) {
+    if (tune.partition && nslots * sizeof(Slot) > part_min && dense < nslots && dense * sizeof(Slot) > part_min) {
       nslots = dense;
       j->table.release();
-      TG_TRY(j->table.ensure(j->device, (size_t)(nslots + 1) * sizeof(Slot)));
+      TG_TRY(j->table.ensure(j->device, (size_t)(nslots + 2) * sizeof(Slot)));   // + the side slot and a spare (probe_rows_u1)
       slots = j->table.as<Slot>();
       k_table_init<<<grid_for(j, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, nslots);
-      k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots, home_width,
+      k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots,
                                                                     j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>());
       j->stats.kernel_launches += 2;
       j->stats.table_slots = (int64_t)nslots;
     }
   }
-  j->tv = TableView{slots, nslots, nullptr, 0, -1, TABLE_NONE, home_width};
+  j->tv = TableView{slots, nslots, nullptr, 0, -1, TABLE_NONE};
   j->build_word_of_col.assign(b.ncols, -1);
   if (u1) {
     j->u1_payload_col = payload.empty() ? -1 : payload[0];
@@ -791,8 +777,8 @@ static bool uq_path_ok(const JoinImpl* j, const DevCols& pview) {
   return true;
 }
 
-// classify the output columns of the fused fast path by the register that feeds them; false = shape not covered by
-// the templated kernels (the CTA-tile kernel handles it)
+// classify the output columns of the fused fast path by the register that feeds them, with the destinations oc.data
+// holds; false = shape not covered by the warp kernels (k_probe_inner_uq or the general path takes it)
 static bool build_fast_out(const JoinImpl* j, const OutCols& oc, const DevCols& pview, FastOut& fo) {
   std::memset(&fo, 0, sizeof(fo));
   int pcol_of[TG_FAST_MAX_PCOLS];
@@ -853,23 +839,13 @@ struct LaunchSeg {
     static int resident = 0;
     if (!resident) {
       int nb = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_probe_inner_u1_seg<NPC, NKD, NMD>, 256, 0) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 3; }
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_probe_inner_u1_seg_lean<NPC, NKD, NMD>, 256, 0) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 3; }
       resident = nb;
     }
     int64_t ctas = (n / 128 + 7) / 8;
     int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
     int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
-    if (t.seg_lean && j->tv.home_width > 1) {   // lean variants (see join_kernels.cuh); 3 CTAs per SM as well
-      if (t.carveout >= 0) {
-        cudaFuncSetAttribute(k_probe_inner_u1_seg_lean<NPC, NKD, NMD, false>, cudaFuncAttributePreferredSharedMemoryCarveout, t.carveout);
-        cudaFuncSetAttribute(k_probe_inner_u1_seg_lean<NPC, NKD, NMD, true>, cudaFuncAttributePreferredSharedMemoryCarveout, t.carveout);
-      }
-      if (t.seg_lean >= 2) k_probe_inner_u1_seg_lean<NPC, NKD, NMD, true><<<grid, 256, 0, j->stream>>>(pkey, n, j->tv, fo, cur, seg);
-      else k_probe_inner_u1_seg_lean<NPC, NKD, NMD, false><<<grid, 256, 0, j->stream>>>(pkey, n, j->tv, fo, cur, seg);
-      return TG_OK;
-    }
-    if (t.carveout >= 0) cudaFuncSetAttribute(k_probe_inner_u1_seg<NPC, NKD, NMD>, cudaFuncAttributePreferredSharedMemoryCarveout, t.carveout);
-    k_probe_inner_u1_seg<NPC, NKD, NMD><<<grid, 256, 0, j->stream>>>(pkey, n, j->tv, fo, cur, seg);
+    k_probe_inner_u1_seg_lean<NPC, NKD, NMD><<<grid, 256, 0, j->stream>>>(pkey, n, j->tv, fo, cur, seg);
     return TG_OK;
   }
 };
@@ -895,126 +871,75 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
     ks.data = j->pkey_syn.p; ks.nulls = j->pkey_syn_nn.as<uint8_t>();
   } else { ks.data = pview.data[p.key_col]; ks.nulls = pview.nulls[p.key_col]; }
   TG_TRY(j->out_cursor.ensure(j->device, 64));
-  if (in_seg && !fast_path_ok(j, pview)) return fail(TG_ERR_UNSUPPORTED, "segmented device chunks are only accepted by the fused fast path (unique build keys, <= 1 payload, no filters)");
-  if (fast_path_ok(j, pview)) {
+  OutCols oc{};
+  fill_outspec_probe(j, oc);
+  FastOut fo{};
+  // the output shape decides the path before any output is allocated: the fused warp kernels, else the single-pass
+  // unique-key kernel, else the general path.  build_fast_out runs again once the output pointers are known.
+  const bool fast = fast_path_ok(j, pview) && build_fast_out(j, oc, pview, fo);
+  if (in_seg && !fast) return fail(TG_ERR_UNSUPPORTED, "segmented device chunks are only accepted by the fused fast path (unique build keys, <= 1 payload, no filters, an output shape the warp kernels cover)");
+  if (fast) {
     TG_TRY(ensure_result(j, rb, rb.rows + n, rb.rows > 0, rb.rows));
-    OutCols oc{};
-    fill_outspec_probe(j, oc);
     for (int c = 0; c < j->n_out; c++) { oc.data[c] = rb.cols[c]->as<uint8_t>() + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
+    build_fast_out(j, oc, pview, fo);
     unsigned long long* cur = j->out_cursor.as<unsigned long long>();
     TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
     if (n > 0) {
       const ProbeTuning& tune = probe_tuning();
-      FastOut fo{};
-      bool warp_ok = (tune.variant != 0 || in_seg) && build_fast_out(j, oc, pview, fo);
-      if (in_seg && !warp_ok) return fail(TG_ERR_UNSUPPORTED, "segmented device chunks: output shape not covered by the warp kernels");
-      if (warp_ok) {
-        const int64_t* pkey = reinterpret_cast<const int64_t*>(ks.data);
-        size_t table_bytes = (size_t)j->tv.nslots * sizeof(Slot);
-        bool partitioned = false;   // the L2 partition pass + segment probe took the whole call
-        bool src16 = aligned16(pkey);
-        for (int c = 0; c < fo.n_pcols; c++) src16 = src16 && aligned16(fo.psrc[c]);
-        const int64_t PTILE = 1024;   // rows per scatter tile (k_partition_scatter_bulk<.., 4>)
-        if (tune.partition == 1 && src16 && scatter_bulk_enabled() && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
-          // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments.
-          // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
-          // [p/P, (p+1)/P) while the probe kernel sweeps the segment.  The pass trades 32 B/row of extra streaming traffic for
-          // random HBM traffic, which only pays while a slice stays L2 resident (probe_slices; U1 tables are built dense
-          // enough for that, build_table).  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
-          // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
-          const int P = probe_slices(table_bytes, j->device, tune.parts);
-          const int64_t n_main = n / PTILE * PTILE;
-          const int nc = 1 + fo.n_pcols;
-          // Segment layout.  Default: one segment per partition filled through global cursors.  TG_PROBE_SUBSEG=1 (experiment,
-          // slower): every scatter CTA owns a private sub-segment of each partition —
-          // G = grid, sub-segment (p, b) = rows [(p*G + b) * C, ...) — placed with a shared-memory cursor, no global atomics.
-          const int G = tune.subseg ? scatter_bulk_grid_nc(j->device, n_main, nc) : 1;
-          const int64_t nsegs = (int64_t)P * G;
-          const int64_t C = tune.subseg ? ((int64_t)((double)n_main / nsegs * 1.06) + PTILE / P + 256 + 127) / 128 * 128   // + one tile's share: CTAs differ by a tile
-                                        : ((int64_t)((double)n_main / P * 1.05) + 16384 + 127) / 128 * 128;
-          if (P >= 2 && G >= 1 && nsegs * C / 128 < (1ll << 31)) {
-            for (int c = 0; c < nc; c++) {
-              if (!j->part_cols[c]) j->part_cols[c].reset(new DevBuf());
-              TG_TRY(j->part_cols[c]->ensure(j->device, (size_t)nsegs * C * 8 + 64));
-            }
-            const int64_t ncur = std::max<int64_t>(nsegs, TG_MAX_PARTS);                 // k_segment_bases zeroes TG_MAX_PARTS cursors
-            TG_TRY(j->part_scratch.ensure(j->device, (size_t)(ncur + 2 * TG_MAX_PARTS) * 8 + 64));
-            unsigned long long* cursors = j->part_scratch.as<unsigned long long>();     // fill count per segment
-            long long* bases = reinterpret_cast<long long*>(cursors + ncur);             // first row of each segment (one per partition)
-            unsigned long long* flag = cursors + ncur + TG_MAX_PARTS;                    // overflow
-            PartDst d{};
-            d.nparts = P; d.ncols = nc;
-            d.src[0] = pkey;
-            for (int c = 0; c < fo.n_pcols; c++) d.src[1 + c] = fo.psrc[c];
-            for (int c = 0; c < nc; c++) for (int q = 0; q < P; q++) d.dst[q][c] = j->part_cols[c]->p;
-            if (tune.subseg) {
-              TG_CUDA(cudaMemsetAsync(flag, 0, 8, j->stream));
-              d.dst_base = nullptr; d.base_const = 0; d.capacity = C; d.overflow = flag; d.sub_cap = C; d.sub_grid = (uint32_t)G;
-            } else {
-              k_segment_bases<<<1, 32, 0, j->stream>>>(cursors, bases, flag, P, C);
-              d.dst_base = bases; d.capacity = C; d.overflow = flag;
-            }
-            if (in_seg) { d.in_cnt = in_seg->cnt; d.in_cap = in_seg->cap; d.in_tiles_per_seg = (uint32_t)(in_seg->cap / PTILE); }
-            TG_TRY(launch_partition_scatter<true>(j->device, j->stream, reinterpret_cast<const long long*>(pkey), nullptr, n_main, d, cursors,
-                                                  &j->stats.kernel_launches, 0, &j->stats.paths));
-            FastOut pf = fo;
-            for (int c = 0; c < fo.n_pcols; c++) pf.psrc[c] = j->part_cols[1 + c]->as<unsigned long long>();
-            // the 128-bit stores of the segment kernel need 16-byte aligned output columns: results appended behind an odd
-            // number of rows fall back to the 8-byte kernel
-            if (tune.seg_vec && (rb.rows & 1) == 0) TG_TRY(launch_probe_seg(j, j->part_cols[0]->as<int64_t>(), nsegs * C, pf, cur, tune, SegSpec{cursors, (uint32_t)(C / 128), 0, C, flag}));
-            else TG_TRY(launch_probe_warp(j, j->part_cols[0]->as<int64_t>(), nsegs * C, pf, cur, tune, SegSpec{cursors, (uint32_t)(C / 128), 0, C, flag}));
-            // gated fallback: probes the ORIGINAL input only after an overflow; the < 1024-row tail the scatter left behind
-            // (dense input only) rides on the same launch — it is probed whatever the flag says
-            if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n_main, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 1, in_seg->cap, flag, 0}));
-            else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{nullptr, 0, 1, 0, flag, n_main < n ? n_main : 0}));
-            j->stats.kernel_launches += 3;
-            partitioned = true;
+      const int64_t* pkey = reinterpret_cast<const int64_t*>(ks.data);
+      size_t table_bytes = (size_t)j->tv.nslots * sizeof(Slot);
+      bool partitioned = false;   // the L2 partition pass + segment probe took the whole call
+      bool src16 = aligned16(pkey);
+      for (int c = 0; c < fo.n_pcols; c++) src16 = src16 && aligned16(fo.psrc[c]);
+      const int64_t PTILE = 1024;   // rows per scatter tile (k_partition_scatter_bulk<.., 4>)
+      if (tune.partition && src16 && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
+        // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments.
+        // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
+        // [p/P, (p+1)/P) while the probe kernel sweeps the segment.  The pass trades 32 B/row of extra streaming traffic for
+        // random HBM traffic, which only pays while a slice stays L2 resident (probe_slices; U1 tables are built dense
+        // enough for that, build_table).  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
+        // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
+        const int P = probe_slices(table_bytes, j->device, tune.parts);
+        const int64_t n_main = n / PTILE * PTILE;
+        const int nc = 1 + fo.n_pcols;
+        // one segment of C rows per partition, filled through global cursors
+        const int64_t C = ((int64_t)((double)n_main / P * 1.05) + 16384 + 127) / 128 * 128;
+        if (P >= 2 && (int64_t)P * C / 128 < (1ll << 31)) {
+          for (int c = 0; c < nc; c++) {
+            if (!j->part_cols[c]) j->part_cols[c].reset(new DevBuf());
+            TG_TRY(j->part_cols[c]->ensure(j->device, (size_t)P * C * 8 + 64));
           }
+          TG_TRY(j->part_scratch.ensure(j->device, (size_t)3 * TG_MAX_PARTS * 8 + 64));
+          unsigned long long* cursors = j->part_scratch.as<unsigned long long>();     // fill count per segment
+          long long* bases = reinterpret_cast<long long*>(cursors + TG_MAX_PARTS);   // first row of each segment
+          unsigned long long* flag = cursors + 2 * TG_MAX_PARTS;                      // overflow
+          PartDst d{};
+          d.nparts = P; d.ncols = nc;
+          d.src[0] = pkey;
+          for (int c = 0; c < fo.n_pcols; c++) d.src[1 + c] = fo.psrc[c];
+          for (int c = 0; c < nc; c++) for (int q = 0; q < P; q++) d.dst[q][c] = j->part_cols[c]->p;
+          k_segment_bases<<<1, 32, 0, j->stream>>>(cursors, bases, flag, P, C);
+          d.dst_base = bases; d.capacity = C; d.overflow = flag;
+          if (in_seg) { d.in_cnt = in_seg->cnt; d.in_cap = in_seg->cap; d.in_tiles_per_seg = (uint32_t)(in_seg->cap / PTILE); }
+          TG_TRY(launch_partition_scatter<true>(j->device, j->stream, reinterpret_cast<const long long*>(pkey), nullptr, n_main, d, cursors,
+                                                &j->stats.kernel_launches, 0, &j->stats.paths));
+          FastOut pf = fo;
+          for (int c = 0; c < fo.n_pcols; c++) pf.psrc[c] = j->part_cols[1 + c]->as<unsigned long long>();
+          // the 128-bit stores of the segment kernel need 16-byte aligned output columns: every caller passes a fresh
+          // batch (rb.rows == 0), so the columns start at the allocation
+          TG_TRY(launch_probe_seg(j, j->part_cols[0]->as<int64_t>(), (int64_t)P * C, pf, cur, tune, SegSpec{cursors, (uint32_t)(C / 128), 0, C, flag}));
+          // gated fallback: probes the ORIGINAL input only after an overflow; the < 1024-row tail the scatter left behind
+          // (dense input only) rides on the same launch — it is probed whatever the flag says
+          if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n_main, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 1, in_seg->cap, flag, 0}));
+          else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{nullptr, 0, 1, 0, flag, n_main < n ? n_main : 0}));
+          j->stats.kernel_launches += 3;
+          partitioned = true;
         }
-        if (!partitioned && !in_seg && tune.partition == 2 && n >= (1ll << 20) && table_bytes > ((size_t)tune.part_min_mb << 20)) {
-          // counted variant (kept for A/B runs): histogram pass → exact offsets → dense partitions
-          const int P = probe_slices(table_bytes, j->device, tune.parts);
-          if (P >= 2) {
-            int nc = 1 + fo.n_pcols;
-            for (int c = 0; c < nc; c++) {
-              if (!j->part_cols[c]) j->part_cols[c].reset(new DevBuf());
-              TG_TRY(j->part_cols[c]->ensure(j->device, (size_t)n * 8 + 64));
-            }
-            TG_TRY(j->part_scratch.ensure(j->device, (size_t)TG_MAX_PARTS * 8 * 3 + 64));
-            unsigned long long* counts = j->part_scratch.as<unsigned long long>();
-            unsigned long long* cursors = counts + TG_MAX_PARTS;
-            long long* offs = reinterpret_cast<long long*>(cursors + TG_MAX_PARTS);
-            TG_CUDA(cudaMemsetAsync(counts, 0, (size_t)TG_MAX_PARTS * 8 * 3 + 8, j->stream));
-            const long long* k64 = reinterpret_cast<const long long*>(pkey);
-            TG_TRY(launch_partition_count<true>(j->device, j->stream, k64, nullptr, n, (uint32_t)P, counts, &j->stats.kernel_launches));
-            k_partition_offsets<<<1, 32, 0, j->stream>>>(counts, (uint32_t)P, offs, cursors);
-            j->stats.kernel_launches++;
-            PartDst d{};
-            d.nparts = P; d.ncols = nc;
-            d.src[0] = pkey;
-            for (int c = 0; c < fo.n_pcols; c++) d.src[1 + c] = fo.psrc[c];
-            for (int c = 0; c < nc; c++) for (int q = 0; q < P; q++) d.dst[q][c] = j->part_cols[c]->p;
-            d.dst_base = offs;
-            TG_TRY(launch_partition_scatter<true>(j->device, j->stream, k64, nullptr, n, d, cursors, &j->stats.kernel_launches, 0, &j->stats.paths));
-            pkey = j->part_cols[0]->as<int64_t>();
-            for (int c = 0; c < fo.n_pcols; c++) fo.psrc[c] = j->part_cols[1 + c]->as<unsigned long long>();
-          }
-        }
-        int64_t done = partitioned ? n : 0;
-        if (done < n) {
-          FastOut tail = fo;
-          for (int c = 0; c < fo.n_pcols; c++) tail.psrc[c] = fo.psrc[c] + done;
-          if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 0, in_seg->cap, nullptr}));
-          else TG_TRY(launch_probe_warp(j, pkey + done, n - done, tail, cur, tune));
-          j->stats.kernel_launches++;
-        }
-      } else {
-        constexpr int R = 4;
-        int64_t tiles = (n + 256 * R - 1) / (256 * R);
-        int grid = (int)std::min<int64_t>(tiles, (int64_t)j->nsm * (tune.ctas_per_sm > 0 ? tune.ctas_per_sm : 8));
-        k_probe_inner_u1<R><<<grid, 256, 0, j->stream>>>(reinterpret_cast<const int64_t*>(ks.data), pview, n, j->tv, oc, cur);
+      }
+      if (!partitioned) {
+        if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 0, in_seg->cap, nullptr}));
+        else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune));
         j->stats.kernel_launches++;
-        j->stats.paths |= TG_JOIN_PATH_PROBE_TILE;
       }
     }
     if (sync_count) {
@@ -1027,10 +952,8 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
     return TG_OK;
   }
   // single-pass path: inner join on unique build keys with filters / several payload columns (k_probe_inner_uq)
-  if (uq_path_ok(j, pview) && !in_seg) {
+  if (uq_path_ok(j, pview)) {
     TG_TRY(ensure_result(j, rb, rb.rows + n, rb.rows > 0, rb.rows));
-    OutCols oc{};
-    fill_outspec_probe(j, oc);
     for (int c = 0; c < j->n_out; c++) { oc.data[c] = rb.cols[c]->as<uint8_t>() + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
     unsigned long long* cur = j->out_cursor.as<unsigned long long>();
     TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
@@ -1220,13 +1143,6 @@ int tg_join_open(const tg_join_desc* desc, tg_join** out) {
   TG_CUDA(cudaEventCreate(&j->ev1));
   TG_CUDA(cudaStreamCreateWithFlags(&j->d2h_stream, cudaStreamNonBlocking));
   j->nsm = device_sm_count(j->device);
-  {
-    // L2 fetch granularity (cudaLimitMaxL2FetchGranularity): left at the device default.  Capping it at 32 B cuts the HBM
-    // bytes of the random gathers, but they are bound by DRAM access rate, not bytes; TG_L2_FETCH={32,64,128} overrides
-    // for experiments (tools/sweep_probe.py).
-    int gran = env_int("TG_L2_FETCH", 0);
-    if (gran == 32 || gran == 64 || gran == 128) { if (cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)gran) != cudaSuccess) cudaGetLastError(); }
-  }
   j->bstage.init(j->build.ncols); j->bcols.init(j->build.ncols);
   j->pstage.init(j->probe.ncols); j->pcols_dev.init(j->probe.ncols);
   shell->impl = j.release();

@@ -7,8 +7,9 @@
 //                                                                      k_build_scatter_u1 / _rows
 //   probe : baseJoinProbe.SetChunkForProbe (base_join_probe.go:179) + innerJoinProbe.Probe
 //           (inner_join_probe.go:27) + append{Build,Probe}RowToChunkInternal (:589/:677)
-//                                                                    → k_probe_inner_u1 (fused fast path)
-//                                                                      k_probe_count / k_probe_write
+//                                                                    → k_probe_inner_u1_seg_lean / k_probe_inner_u1_w
+//                                                                      (fused fast path), k_probe_inner_uq (unique
+//                                                                      keys, one pass), k_probe_count / k_probe_write
 //
 // Data layout in HBM (GPU-first, not the reference's chained row pointers):
 //   * open-addressing table of 16-byte slots {int64 key, u64 meta}, linear probing, one slot per
@@ -48,15 +49,17 @@ struct TableView {
   int32_t row_words;
   int32_t null_word;                // index of the per-row NULL mask word in the row store, -1 = none
   int32_t mode;
-  int32_t home_width;               // 1, 2 or 4 slots (nslots is a multiple of it): a key's home is the first slot of an
-                                    // aligned group of that many slots.  2: the 32-byte pair one sector fetch brings in;
-                                    // 4: a key's first two pairs lie in one 64-byte half-line
+  int32_t pad;
 };
 
-// home slot of a hash value: slot32(h, nslots / w) * w.  Linear probing runs on from there one slot at a time, whatever w is.
-__device__ __forceinline__ unsigned long long home_slot(unsigned long long h, unsigned long long nslots, int home_width) {
-  const int sh = home_width >> 1;   // log2 of 1, 2, 4
-  return (unsigned long long)slot32(h, (uint32_t)(nslots >> sh)) << sh;
+// A key's home is the first slot of an aligned group of kHomeWidth slots (nslots is a multiple of it), so its first two
+// 32-byte pairs lie in one 64-byte half-line.  4 beat homes of one 32-byte pair at every load factor measured (DESIGN.md §4.1).
+static constexpr int kHomeWidth = 4;
+
+// home slot of a hash value: slot32(h, nslots / w) * w, which equals slot32(h, nslots) rounded down to a multiple of w
+// because nslots is one.  Linear probing runs on from there one slot at a time.
+__device__ __forceinline__ uint32_t home_slot(unsigned long long h, unsigned long long nslots) {
+  return slot32(h, (uint32_t)nslots) & ~(uint32_t)(kHomeWidth - 1);
 }
 
 #define TG_MAX_OUT 24
@@ -175,7 +178,7 @@ __device__ __forceinline__ uint32_t table_find(const TableView& t, int64_t k, un
     // the side slot is "occupied" iff a build row carried this key: mode U1 marks that in key
     return s.key == 0 ? kInvalidSlot : (uint32_t)t.nslots;
   }
-  unsigned long long s = home_slot(hash64((uint64_t)k), t.nslots, t.home_width);
+  unsigned long long s = home_slot(hash64((uint64_t)k), t.nslots);
   for (;;) {
     Slot v = load_slot(t.slots + s);
     if (v.key == k) { *meta = v.meta; return (uint32_t)s; }
@@ -244,7 +247,7 @@ __global__ void k_table_init(Slot* slots, unsigned long long n_total, unsigned l
 
 // pass 1: claim one slot per distinct key, count multiplicities, remember (slot, rank) per build row
 __global__ void __launch_bounds__(256)
-k_build_insert(KeySpec key, DevCols cols, DevFilter filt, int64_t n, Slot* slots, unsigned long long nslots, int home_width,
+k_build_insert(KeySpec key, DevCols cols, DevFilter filt, int64_t n, Slot* slots, unsigned long long nslots,
                uint32_t* __restrict__ row_slot, uint32_t* __restrict__ row_rank) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -258,7 +261,7 @@ k_build_insert(KeySpec key, DevCols cols, DevFilter filt, int64_t n, Slot* slots
       s = nslots;
       slots[s].key = 1;   // occupied flag (benign race: every writer stores 1)
     } else {
-      s = home_slot(hash64((uint64_t)k), nslots, home_width);
+      s = home_slot(hash64((uint64_t)k), nslots);
       for (;;) {
         int64_t cur = *reinterpret_cast<volatile int64_t*>(&slots[s].key);
         if (cur == k) break;
@@ -357,90 +360,8 @@ __global__ void k_build_scatter_rows(const uint32_t* __restrict__ row_slot, cons
 
 // ---------------------------------------------------------------------------------------------
 // probe — fused fast path: unique build keys (mode U1), inner join, NOT NULL 8-byte columns.
-// One pass: stream probe key (+ payload columns) with coalesced loads, one 16-byte gather per row,
-// warp-ballot compaction, one atomicAdd per CTA tile for the output cursor, coalesced column stores.
-// ---------------------------------------------------------------------------------------------
-template <int R>
-__global__ void __launch_bounds__(256)
-k_probe_inner_u1(const int64_t* __restrict__ pkey, DevCols pcols, int64_t n, TableView t, OutCols out,
-                 unsigned long long* __restrict__ out_cursor) {
-  constexpr int BLOCK = 256;
-  constexpr int WARPS = BLOCK / 32;
-  __shared__ uint32_t s_warp_cnt[R][WARPS];
-  __shared__ unsigned long long s_base;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t tile_rows = (int64_t)BLOCK * R;
-  const int64_t ntiles = (n + tile_rows - 1) / tile_rows;
-  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int64_t base = tile * tile_rows;
-    int64_t k[R];
-    Slot v[R];
-    bool m[R];
-    // issue all R independent key loads, then all R independent gathers (memory-level parallelism)
-#pragma unroll
-    for (int j = 0; j < R; j++) {
-      int64_t i = base + (int64_t)j * BLOCK + threadIdx.x;
-      k[j] = i < n ? __ldcs(pkey + i) : kEmptyKey;
-    }
-    unsigned long long s[R];
-#pragma unroll
-    for (int j = 0; j < R; j++) {
-      s[j] = (k[j] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[j]), t.nslots, t.home_width);
-      v[j] = load_slot(t.slots + s[j]);
-    }
-#pragma unroll
-    for (int j = 0; j < R; j++) {
-      int64_t i = base + (int64_t)j * BLOCK + threadIdx.x;
-      bool in = i < n;
-      if (k[j] == kEmptyKey) {
-        m[j] = in && v[j].key != 0;
-      } else {
-        // linear probing tail: rare at the configured load factor
-        while (v[j].key != k[j] && v[j].key != kEmptyKey) {
-          if (++s[j] == t.nslots) s[j] = 0;
-          v[j] = load_slot(t.slots + s[j]);
-        }
-        m[j] = v[j].key == k[j];
-      }
-    }
-    // compaction: position of each match inside the tile
-    uint32_t pre[R];
-#pragma unroll
-    for (int j = 0; j < R; j++) {
-      unsigned b = __ballot_sync(0xffffffffu, m[j]);
-      pre[j] = __popc(b & ((1u << lane) - 1));
-      if (lane == 0) s_warp_cnt[j][warp] = __popc(b);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      uint32_t run = 0;
-#pragma unroll
-      for (int j = 0; j < R; j++)
-        for (int w = 0; w < WARPS; w++) { uint32_t c = s_warp_cnt[j][w]; s_warp_cnt[j][w] = run; run += c; }
-      s_base = run ? atomicAdd(out_cursor, (unsigned long long)run) : 0ull;
-    }
-    __syncthreads();
-    const unsigned long long obase = s_base;
-#pragma unroll
-    for (int j = 0; j < R; j++) {
-      if (!m[j]) continue;
-      int64_t i = base + (int64_t)j * BLOCK + threadIdx.x;
-      unsigned long long o = obase + s_warp_cnt[j][warp] + pre[j];
-      for (int c = 0; c < out.n; c++) {
-        const OutSpec sp = out.spec[c];
-        unsigned long long val;
-        if (sp.src == SRC_PROBE_COL) val = __ldcs(reinterpret_cast<const unsigned long long*>(pcols.data[sp.idx]) + i);
-        else if (sp.src == SRC_BUILD_KEY) val = (unsigned long long)k[j];
-        else val = v[j].meta;
-        __stcs(reinterpret_cast<unsigned long long*>(out.data[c]) + o, val);
-      }
-    }
-    __syncthreads();   // s_warp_cnt / s_base are reused by the next tile
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// probe — fused fast path, warp-autonomous and TMA-fed variants.
+// One pass: stream probe key (+ payload columns) with coalesced loads, one gather of the home slot pair per row,
+// warp-ballot compaction, one output-cursor atomic per warp tile, coalesced column stores.
 // The output shape is a template parameter (NPC probe payload columns, NKD outputs fed by the join key, NMD outputs
 // fed by the build payload): with run-time destination counts ptxas unrolled the store loops into ~360 predicated
 // STG + 350 LDC per kernel.
@@ -456,36 +377,17 @@ struct FastOut {
   unsigned long long* meta_dst[TG_FAST_MAX_METADST]; // output that carries the build payload
 };
 
-__device__ __forceinline__ unsigned long long policy_evict_last() {
-  unsigned long long p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ Slot load_slot_policy(const Slot* p, unsigned long long pol) {
-  unsigned long long x, y;
-  asm volatile("ld.global.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(x), "=l"(y) : "l"(p), "l"(pol));
-  Slot s; s.key = (int64_t)x; s.meta = y;
-  return s;
-}
-
-// R rows per lane, keys (and prefetched payload) already in registers: gather, resolve, compact, store.
+// R rows per lane, keys and payloads already in registers: gather, resolve, compact, store.
 // `in[j]` = row j of this lane exists (tail tiles).
-template <int R, int NPC, int NKD, int NMD, bool CTA_AGG, bool PAIRED = false>
+template <int R, int NPC, int NKD, int NMD, bool PAIRED = false>
 __device__ __forceinline__ void probe_rows_u1(const int64_t (&k)[R], const unsigned long long (&pv)[R][NPC > 0 ? NPC : 1],
                                               const unsigned long long (&sl0)[R], const bool (&in)[R], const TableView& t,
                                               const FastOut& out, unsigned long long* __restrict__ out_cursor, int lane) {
   Slot v[R], w[R];
-  const bool pair = t.home_width > 1;   // the home is the first slot of an aligned pair: load both
-  if (pair) {
+  // the home is the first slot of an aligned pair: load both.  The side slot of the sentinel key is loaded as a pair too
+  // (the table holds one spare slot behind it); only its first slot counts.
 #pragma unroll
-    for (int j = 0; j < R; j++) {
-      if (k[j] == kEmptyKey) { v[j] = load_slot(t.slots + sl0[j]); w[j].key = kEmptyKey; w[j].meta = 0; }
-      else load_pair(t.slots + sl0[j], v[j], w[j]);
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < R; j++) { v[j] = load_slot(t.slots + sl0[j]); w[j].key = kEmptyKey; w[j].meta = 0; }
-  }
+  for (int j = 0; j < R; j++) load_pair(t.slots + sl0[j], v[j], w[j]);
   unsigned bal[R];
   uint32_t total = 0;
 #pragma unroll
@@ -493,34 +395,15 @@ __device__ __forceinline__ void probe_rows_u1(const int64_t (&k)[R], const unsig
     bool m;
     if (k[j] == kEmptyKey) m = in[j] && v[j].key != 0;
     else if (v[j].key == k[j]) m = true;
-    else if (pair && w[j].key == k[j]) { v[j] = w[j]; m = true; }
-    else if (v[j].key == kEmptyKey || (pair && w[j].key == kEmptyKey)) m = false;
-    else m = probe_run(t.slots, t.nslots, k[j], sl0[j] + (pair ? 2 : 1), v[j].meta);   // the home slots hold other keys
+    else if (w[j].key == k[j]) { v[j] = w[j]; m = true; }
+    else if (v[j].key == kEmptyKey || w[j].key == kEmptyKey) m = false;
+    else m = probe_run(t.slots, t.nslots, k[j], sl0[j] + 2, v[j].meta);   // the home slots hold other keys
     bal[j] = __ballot_sync(0xffffffffu, m);
     total += __popc(bal[j]);
   }
   unsigned long long wbase = 0;
-  if (CTA_AGG) {
-    // one atomic per CTA tile instead of one per warp: every atomic of a launch hits the SAME address and the L2
-    // serialises them (781 K per 100 M rows with per-warp reservation)
-    __shared__ uint32_t s_wtot[8];
-    __shared__ unsigned long long s_cta_base;
-    const int warp = threadIdx.x >> 5;
-    if (lane == 0) s_wtot[warp] = total;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      uint32_t sum = 0;
-#pragma unroll
-      for (int q = 0; q < 8; q++) sum += s_wtot[q];
-      s_cta_base = sum ? atomicAdd(out_cursor, (unsigned long long)sum) : 0ull;
-    }
-    __syncthreads();
-    wbase = s_cta_base;
-    for (int q = 0; q < warp; q++) wbase += s_wtot[q];
-  } else {
-    if (lane == 0 && total) wbase = atomicAdd(out_cursor, (unsigned long long)total);
-    wbase = __shfl_sync(0xffffffffu, wbase, 0);
-  }
+  if (lane == 0 && total) wbase = atomicAdd(out_cursor, (unsigned long long)total);
+  wbase = __shfl_sync(0xffffffffu, wbase, 0);
   if (PAIRED && total == 32u * R && (wbase & 1ull) == 0) {
     // rows 2g, 2g+1 of a lane are adjacent input rows and the whole warp tile matched: keep the input order and write
     // 16 bytes per lane and column (half the store instructions of the compacting path below)
@@ -606,79 +489,20 @@ k_probe_inner_u1_w(const int64_t* __restrict__ pkey, int64_t n, TableView t, Fas
 #pragma unroll
     for (int j = 0; j < R; j++) {
       int64_t i = base + j * 32 + lane;
-      sl[j] = (k[j] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[j]), t.nslots, t.home_width);
+      sl[j] = (k[j] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[j]), t.nslots);
 #pragma unroll
       for (int c = 0; c < NPC; c++) pv[j][c] = in[j] ? __ldcs(out.psrc[c] + i) : 0ull;
     }
-    probe_rows_u1<R, NPC, NKD, NMD, false>(k, pv, sl, in, t, out, out_cursor, lane);
-  }
-}
-
-// Segment-ordered input (SegSpec.cnt != nullptr), 128-bit accesses: a lane owns 2 ADJACENT rows of each 64-row group, so
-// keys and payloads are read with LDG.128 and — when the whole tile matched — written with STG.128.  Segment bases are
-// 1 KB aligned and the capacity is allocated in full, so a tile is always loaded whole; rows past the fill count are
-// masked.  3 CTAs per SM (80 registers): launch exactly 3 x SMs CTAs.
-template <int NPC, int NKD, int NMD>
-__global__ void __launch_bounds__(256, 3)
-k_probe_inner_u1_seg(const int64_t* __restrict__ pkey, int64_t n, TableView t, FastOut out,
-                     unsigned long long* __restrict__ out_cursor, SegSpec seg) {
-  constexpr int R = 4;
-  if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) return;
-  const int lane = threadIdx.x & 31;
-  const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
-  const int64_t warp_id = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t ntiles = n / 128;
-  const int64_t nseg = ntiles / seg.tiles_per_seg;
-  // Pass 1 sweeps the FULL tiles, pass 2 the (at most one per segment) partial tile at the end of each segment: a partial
-  // tile adds an odd row count to the output cursor about half the time, and from then on every 128-row reservation
-  // would start at an odd row — misaligned for the 128-bit stores of the all-matched path.
-  for (int64_t it = warp_id; it < ntiles + nseg; it += warps_total) {
-    int64_t tile = it;
-    if (it >= ntiles) {
-      const int64_t sp = it - ntiles;
-      const unsigned long long cc = seg.cnt[sp];
-      const int64_t fill = (int64_t)(cc < (unsigned long long)seg.cap ? cc : (unsigned long long)seg.cap);
-      if ((fill & 127) == 0) continue;
-      tile = sp * seg.tiles_per_seg + fill / 128;
-    }
-    const int64_t base = tile * 128;
-    const uint32_t p = (uint32_t)tile / seg.tiles_per_seg;
-    const unsigned long long c = seg.cnt[p];
-    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
-    if (base >= limit) continue;
-    if (it < ntiles && limit - base < 128) continue;   // partial tile: pass 2
-    int64_t k[R];
-    unsigned long long pv[R][NPC > 0 ? NPC : 1];
-    unsigned long long sl[R];
-    bool in[R];
-#pragma unroll
-    for (int g = 0; g < R / 2; g++) {
-      const int64_t i = base + g * 64 + 2 * lane;
-      const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + i));
-      in[2 * g] = i < limit; in[2 * g + 1] = i + 1 < limit;
-      k[2 * g] = in[2 * g] ? (int64_t)kk.x : kEmptyKey;
-      k[2 * g + 1] = in[2 * g + 1] ? (int64_t)kk.y : kEmptyKey;
-    }
-#pragma unroll
-    for (int g = 0; g < R / 2; g++) {
-      const int64_t i = base + g * 64 + 2 * lane;
-      sl[2 * g] = (k[2 * g] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g]), t.nslots, t.home_width);
-      sl[2 * g + 1] = (k[2 * g + 1] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g + 1]), t.nslots, t.home_width);
-#pragma unroll
-      for (int cc = 0; cc < NPC; cc++) {
-        const ulonglong2 pp = __ldcs(reinterpret_cast<const ulonglong2*>(out.psrc[cc] + i));
-        pv[2 * g][cc] = pp.x; pv[2 * g + 1][cc] = pp.y;
-      }
-    }
-    probe_rows_u1<R, NPC, NKD, NMD, false, true>(k, pv, sl, in, t, out, out_cursor, lane);
+    probe_rows_u1<R, NPC, NKD, NMD>(k, pv, sl, in, t, out, out_cursor, lane);
   }
 }
 
 // ---------------------------------------------------------------------------------------------
-// DEFAULT (TG_PROBE_SEG_LEAN=1; 0 = the kernel above, 2 = + register prefetch): the same segment probe with a lean
-// full-tile path — no per-row `in` flags, no slot array, sentinel-valued
-// keys detected once per tile (then the tile takes the generic path) — and, with PREFETCH, the next tile's keys/payloads
-// requested before the current tile's gathers are issued.
+// Segment-ordered input (SegSpec.cnt != nullptr), 128-bit accesses: a lane owns 2 ADJACENT rows of each 64-row group, so
+// keys and payloads are read with LDG.128 and — when the whole tile matched — written with STG.128.  Segment bases are
+// 1 KB aligned and the capacity is allocated in full, so a tile is always loaded whole; rows past the fill count are
+// masked.  A full tile takes a lean path — no per-row `in` flags, no slot array, sentinel-valued keys detected once per
+// tile (then the tile takes the generic path).  3 CTAs per SM (80 registers): launch exactly the resident CTA count.
 // ---------------------------------------------------------------------------------------------
 template <int NPC, int NKD, int NMD>
 __device__ __forceinline__ void probe_tile_generic(const int64_t* __restrict__ pkey, int64_t base, int64_t limit, const TableView& t,
@@ -699,18 +523,18 @@ __device__ __forceinline__ void probe_tile_generic(const int64_t* __restrict__ p
 #pragma unroll
   for (int g = 0; g < R / 2; g++) {
     const int64_t i = base + g * 64 + 2 * lane;
-    sl[2 * g] = (k[2 * g] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g]), t.nslots, t.home_width);
-    sl[2 * g + 1] = (k[2 * g + 1] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g + 1]), t.nslots, t.home_width);
+    sl[2 * g] = (k[2 * g] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g]), t.nslots);
+    sl[2 * g + 1] = (k[2 * g + 1] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[2 * g + 1]), t.nslots);
 #pragma unroll
     for (int cc = 0; cc < NPC; cc++) {
       const ulonglong2 pp = __ldcs(reinterpret_cast<const ulonglong2*>(out.psrc[cc] + i));
       pv[2 * g][cc] = pp.x; pv[2 * g + 1][cc] = pp.y;
     }
   }
-  probe_rows_u1<R, NPC, NKD, NMD, false, true>(k, pv, sl, in, t, out, out_cursor, lane);
+  probe_rows_u1<R, NPC, NKD, NMD, true>(k, pv, sl, in, t, out, out_cursor, lane);
 }
 
-template <int NPC, int NKD, int NMD, bool PREFETCH>
+template <int NPC, int NKD, int NMD>
 __global__ void __launch_bounds__(256, 3)
 k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView t, FastOut out,
                           unsigned long long* __restrict__ out_cursor, SegSpec seg) {
@@ -720,30 +544,24 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
   const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
   const int64_t warp_id = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t ntiles = n / 128;
-  const int64_t nseg = ntiles / seg.tiles_per_seg;
-  ulonglong2 kn[G], pn[G][NP];
-  auto fetch = [&](int64_t tile) {
-#pragma unroll
-    for (int g = 0; g < G; g++) {
-      const int64_t i = tile * 128 + g * 64 + 2 * lane;
-      kn[g] = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + i));
-#pragma unroll
-      for (int c = 0; c < NPC; c++) pn[g][c] = __ldcs(reinterpret_cast<const ulonglong2*>(out.psrc[c] + i));
-    }
-  };
-  // pass 1: full tiles (tile == it); the capacity of every segment is allocated in full, so a tile can always be loaded
-  if (PREFETCH && warp_id < ntiles) fetch(warp_id);
+  // Pass 1 sweeps the FULL tiles, pass 2 the (at most one per segment) partial tile at the end of each segment: a partial
+  // tile adds an odd row count to the output cursor about half the time, and from then on every 128-row reservation
+  // would start at an odd row — misaligned for the 128-bit stores of the all-matched path.
+  // Pass 1: the capacity of every segment is allocated in full, so a tile can always be loaded
   for (int64_t tile = warp_id; tile < ntiles; tile += warps_total) {
-    if (!PREFETCH) fetch(tile);
     int64_t k[R];
     unsigned long long pv[R][NP];
 #pragma unroll
     for (int g = 0; g < G; g++) {
-      k[2 * g] = (int64_t)kn[g].x; k[2 * g + 1] = (int64_t)kn[g].y;
+      const int64_t i = tile * 128 + g * 64 + 2 * lane;
+      const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + i));
+      k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
 #pragma unroll
-      for (int c = 0; c < NPC; c++) { pv[2 * g][c] = pn[g][c].x; pv[2 * g + 1][c] = pn[g][c].y; }
+      for (int c = 0; c < NPC; c++) {
+        const ulonglong2 pp = __ldcs(reinterpret_cast<const ulonglong2*>(out.psrc[c] + i));
+        pv[2 * g][c] = pp.x; pv[2 * g + 1][c] = pp.y;
+      }
     }
-    if (PREFETCH && tile + warps_total < ntiles) fetch(tile + warps_total);
     const int64_t base = tile * 128;
     const uint32_t p = (uint32_t)tile / seg.tiles_per_seg;
     const unsigned long long c = seg.cnt[p];
@@ -756,7 +574,7 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
     }
     Slot v[R], w[R];
 #pragma unroll
-    for (int j = 0; j < R; j++) load_pair(t.slots + home_slot(hash64((uint64_t)k[j]), t.nslots, t.home_width), v[j], w[j]);
+    for (int j = 0; j < R; j++) load_pair(t.slots + home_slot(hash64((uint64_t)k[j]), t.nslots), v[j], w[j]);
     unsigned long long meta[R];
     unsigned hit = 0, run = 0;   // bit j: row j matched / row j's home pair holds two other keys
 #pragma unroll
@@ -773,7 +591,7 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
       uint32_t sl[R];
 #pragma unroll
       for (int j = 0; j < R; j++) {
-        const unsigned long long s = home_slot(hash64((uint64_t)k[j]), t.nslots, t.home_width) + 2;
+        const unsigned long long s = home_slot(hash64((uint64_t)k[j]), t.nslots) + 2;
         sl[j] = s == t.nslots ? 0u : (uint32_t)s;
       }
       do {
@@ -828,7 +646,8 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
       }
     }
   }
-  // pass 2: the partial tile of each segment (see k_probe_inner_u1_seg)
+  // pass 2: the partial tile of each segment
+  const int64_t nseg = ntiles / seg.tiles_per_seg;
   for (int64_t sp = warp_id; sp < nseg; sp += warps_total) {
     const unsigned long long cc = seg.cnt[sp];
     const int64_t fill = (int64_t)(cc < (unsigned long long)seg.cap ? cc : (unsigned long long)seg.cap);
@@ -1089,7 +908,7 @@ k_probe_inner_uq(KeySpec key, DevCols pcols, DevFilter filt, int64_t n, TableVie
     for (int r = 0; r < UQ_R; r++) {
       sl[r] = t.nslots; v[r].key = kEmptyKey; v[r].meta = 0;
       if (valid[r]) {
-        if (k[r] != kEmptyKey) sl[r] = home_slot(hash64((uint64_t)k[r]), t.nslots, t.home_width);
+        if (k[r] != kEmptyKey) sl[r] = home_slot(hash64((uint64_t)k[r]), t.nslots);
         v[r] = load_slot(t.slots + sl[r]);
       }
     }

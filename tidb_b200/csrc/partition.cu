@@ -116,7 +116,6 @@ static int exchange_cf_impl(int device, const int64_t* key_dev, int64_t rows, in
   TG_TRY(check_parts(nparts, ncols));
   if (spill_cursor_dev && (!spill_cols_dev || spill_cap <= 0)) return fail(TG_ERR_INVALID, "a spill cursor needs spill columns and a positive spill_cap");
   if (ncols > 4) return fail(TG_ERR_UNSUPPORTED, "count-free exchange moves at most 4 columns per call");
-  if (!scatter_bulk_enabled()) return fail(TG_ERR_UNSUPPORTED, "count-free exchange needs the bulk-store scatter kernel (TG_SCATTER_BULK=0 disables it)");
   if (!sent_rows_dev || !overflow_dev || region_cap <= 0) return fail(TG_ERR_INVALID, "sent_rows_dev / overflow_dev / region_cap are required");
   if (src_cols_dev[0] != (const void*)key_dev) return fail(TG_ERR_INVALID, "src_cols_dev[0] must be the key column");
   for (int c = 0; c < ncols; c++) if (!ptr_aligned16(src_cols_dev[c])) return fail(TG_ERR_UNSUPPORTED, "source columns must be 16-byte aligned");

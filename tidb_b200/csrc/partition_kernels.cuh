@@ -30,13 +30,8 @@ struct PartDst {
   // in_cap a multiple of the scatter tile; nullptr = dense input
   const unsigned long long* in_cnt;
   long long in_cap;
-  uint32_t in_tiles_per_seg, sub_grid;   // sub_grid: the grid the sub-segment layout was sized for (checked at launch)
-  // sub_cap > 0 (k_partition_scatter_bulk only): CTA-PRIVATE sub-segments.  Destination p is split into gridDim.x
-  // sub-segments of sub_cap rows, sub-segment (p, b) at rows [(p * gridDim.x + b) * sub_cap, ...) belongs to CTA b alone,
-  // so a tile is placed with a shared-memory cursor — no global atomic (and its ~1 us round trip between two CTA
-  // barriers) per (tile, destination).  At the end CTA b stores its fill counts to cursors[p * gridDim.x + b].
-  long long sub_cap;
-  // spill_cursor != nullptr (count-free mode, no sub-segments): rows that do not fit their destination's capacity are not
+  uint32_t in_tiles_per_seg;
+  // spill_cursor != nullptr (count-free mode): rows that do not fit their destination's capacity are not
   // dropped but appended to a LOCAL spill area (column c at spill[c], at most spill_cap rows, one global cursor); the host
   // drains it afterwards through a counted exchange.  *overflow is then raised only when the spill area itself is full.
   // A skewed key distribution makes the exchange slower, never wrong (the reference's exchange queues are unbounded).
@@ -179,97 +174,6 @@ k_partition_scatter(const long long* __restrict__ key, const uint8_t* __restrict
 }
 
 
-// TMA-fed scatter for 8-byte columns, no NULL keys: the source tiles (key = column 0 plus NC-1 more columns) arrive in
-// shared memory through a 2-stage cp.async.bulk ring.  Each row's destination (partition, global position) is computed
-// ONCE, parked next to its tile slot, and reused for every column; columns are regrouped through one 16 KB buffer and
-// written as coalesced runs.  Full 2048-row tiles only; the tail goes through k_partition_scatter.
-template <bool HIGH, int NC>
-__global__ void __launch_bounds__(PT_BLOCK)
-k_partition_scatter_tma(int64_t ntiles, PartDst d, unsigned long long* __restrict__ cursors) {
-  constexpr int STAGES = 2;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  unsigned long long* ring = reinterpret_cast<unsigned long long*>(smem_raw);                  // [STAGES][NC][PT_TILE]
-  unsigned long long* s_val = ring + (size_t)STAGES * NC * PT_TILE;                            // [PT_TILE] regrouped values
-  unsigned long long* s_pos = s_val + PT_TILE;                                                 // [PT_TILE] part<<58 | global row
-  uint64_t* full = reinterpret_cast<uint64_t*>(s_pos + PT_TILE);
-  __shared__ uint32_t s_cnt[TG_MAX_PARTS], s_off[TG_MAX_PARTS];
-  __shared__ unsigned long long s_gbase[TG_MAX_PARTS];
-  const int tid = threadIdx.x, lane = tid & 31;
-  const uint32_t P = (uint32_t)d.nparts;
-  const unsigned long long pol = l2_policy_evict_first();
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; s++) mbar_init(&full[s], 1);
-    mbar_fence_init();
-  }
-  __syncthreads();
-  auto issue = [&](int64_t it) {
-    int64_t tile = (int64_t)blockIdx.x + it * gridDim.x;
-    if (tile >= ntiles) return;
-    int s = (int)(it % STAGES);
-    mbar_arrive_expect_tx(&full[s], (uint32_t)(NC * PT_TILE * 8));
-#pragma unroll
-    for (int c = 0; c < NC; c++)
-      bulk_g2s(ring + ((size_t)s * NC + c) * PT_TILE, reinterpret_cast<const unsigned long long*>(d.src[c]) + tile * PT_TILE,
-               PT_TILE * 8, &full[s], pol);
-  };
-  if (tid == 0) for (int it = 0; it < STAGES; it++) issue(it);
-  for (int64_t it = 0;; it++) {
-    const int64_t tile = (int64_t)blockIdx.x + it * gridDim.x;
-    if (tile >= ntiles) break;
-    const int s = (int)(it % STAGES);
-    if (tid < TG_MAX_PARTS) s_cnt[tid] = 0;
-    mbar_wait(&full[s], (uint32_t)((it / STAGES) & 1));
-    __syncthreads();
-    const unsigned long long* in = ring + (size_t)s * NC * PT_TILE;
-    unsigned long long key[PT_ITEMS];
-    uint32_t pr[PT_ITEMS];   // part << 16 | rank inside (tile, part)
-#pragma unroll
-    for (int j = 0; j < PT_ITEMS; j++) {
-      key[j] = in[j * PT_BLOCK + tid];
-      uint64_t h = hash64(key[j]);
-      uint32_t p = HIGH ? mulhi32((uint32_t)(h >> 32), P) : part_of(h, P);
-      // rank inside (tile, destination): one shared-memory atomic per row.  Warp-aggregating it (match_any + leader
-      // election) costs more instructions than the contention it saves (tools/scratch/probe_lab.cu compares both).
-      pr[j] = (p << 16) | atomicAdd(&s_cnt[p], 1u);
-    }
-    __syncthreads();
-    if (tid < 32) {   // exclusive scan of the P counts by one warp + one global reservation per destination
-      uint32_t c = tid < (int)P ? s_cnt[tid] : 0, incl = c;
-      for (int o = 1; o < 32; o <<= 1) { uint32_t u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
-      if (tid < (int)P) {
-        s_off[tid] = incl - c;
-        s_gbase[tid] = (c ? atomicAdd(&cursors[tid], (unsigned long long)c) : 0ull) + (unsigned long long)(d.dst_base ? d.dst_base[tid] : d.base_const);
-      }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < PT_ITEMS; j++) {
-      uint32_t p = pr[j] >> 16, r = pr[j] & 0xffffu;
-      uint32_t slot = s_off[p] + r;
-      pr[j] = slot;
-      s_pos[slot] = ((unsigned long long)p << 58) | (s_gbase[p] + r);
-      s_val[slot] = key[j];
-    }
-    __syncthreads();
-#pragma unroll
-    for (int c = 0; c < NC; c++) {
-      if (c > 0) {
-#pragma unroll
-        for (int j = 0; j < PT_ITEMS; j++) s_val[pr[j]] = in[(size_t)c * PT_TILE + j * PT_BLOCK + tid];
-        __syncthreads();
-      }
-      if (c == NC - 1 && tid == 0) issue(it + STAGES);   // every column of stage s has been drained (values consumed by STS)
-#pragma unroll
-      for (int j = 0; j < PT_ITEMS; j++) {
-        uint32_t sidx = j * PT_BLOCK + tid;
-        unsigned long long pos = s_pos[sidx];
-        reinterpret_cast<unsigned long long*>(d.dst[pos >> 58][c])[pos & ((1ull << 58) - 1)] = s_val[sidx];
-      }
-      __syncthreads();
-    }
-  }
-}
-
 // shared → global bulk store (cp.async.bulk, bulk_group completion) and its fences
 __device__ __forceinline__ void bulk_s2g(void* dst_gmem, const void* src_smem, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(smem_u32(src_smem)), "r"(bytes) : "memory");
@@ -295,12 +199,11 @@ k_partition_scatter_bulk(int64_t ntiles, PartDst d, unsigned long long* __restri
   unsigned long long* stage = ring + (size_t)STAGES * NC * TILE;                   // [NC][SROWS]
   uint64_t* full = reinterpret_cast<uint64_t*>(stage + (size_t)NC * SROWS);
   __shared__ uint32_t s_cnt[TG_MAX_PARTS], s_off[TG_MAX_PARTS], s_len[TG_MAX_PARTS];
-  __shared__ unsigned long long s_gbase[TG_MAX_PARTS], s_cur[TG_MAX_PARTS], s_spg[TG_MAX_PARTS];
+  __shared__ unsigned long long s_gbase[TG_MAX_PARTS], s_spg[TG_MAX_PARTS];
   __shared__ uint32_t s_spn[TG_MAX_PARTS];    // rows of this tile's run that go to the spill area, starting at spill row s_spg
   const int tid = threadIdx.x, lane = tid & 31;
   const uint32_t P = (uint32_t)d.nparts;
   const unsigned long long pol = l2_policy_evict_first();
-  if (tid < TG_MAX_PARTS) s_cur[tid] = 0;
   if (tid == 0) {
     for (int s = 0; s < STAGES; s++) mbar_init(&full[s], 1);
     mbar_fence_init();
@@ -345,27 +248,19 @@ k_partition_scatter_bulk(int64_t ntiles, PartDst d, unsigned long long* __restri
       uint32_t c = tid < (int)P ? s_cnt[tid] : 0, len = c, spn = 0;
       unsigned long long g = 0, spg = 0;
       if (tid < (int)P) {
-        if (d.sub_cap > 0) {   // CTA-private sub-segment: the cursor lives in shared memory
-          const unsigned long long old = s_cur[tid];
-          s_cur[tid] = old + c;
-          const unsigned long long avail = old < (unsigned long long)d.sub_cap ? (unsigned long long)d.sub_cap - old : 0ull;
-          if ((unsigned long long)c > avail) { len = (uint32_t)avail; *d.overflow = 1ull; }
-          g = ((unsigned long long)tid * gridDim.x + blockIdx.x) * (unsigned long long)d.sub_cap + old;
-        } else {
-          unsigned long long old = c ? atomicAdd(&cursors[tid], (unsigned long long)c) : 0ull;
-          if (d.capacity > 0) {
-            unsigned long long avail = old < (unsigned long long)d.capacity ? (unsigned long long)d.capacity - old : 0ull;
-            if ((unsigned long long)c > avail) {
-              len = (uint32_t)avail;
-              if (d.spill_cursor) {   // skewed destination: the rest of the run goes to the local spill area
-                spn = c - len;
-                spg = atomicAdd(d.spill_cursor, (unsigned long long)spn);
-                if (spg + spn > (unsigned long long)d.spill_cap) { spn = 0; *d.overflow = 1ull; }
-              } else *d.overflow = 1ull;
-            }
+        unsigned long long old = c ? atomicAdd(&cursors[tid], (unsigned long long)c) : 0ull;
+        if (d.capacity > 0) {
+          unsigned long long avail = old < (unsigned long long)d.capacity ? (unsigned long long)d.capacity - old : 0ull;
+          if ((unsigned long long)c > avail) {
+            len = (uint32_t)avail;
+            if (d.spill_cursor) {   // skewed destination: the rest of the run goes to the local spill area
+              spn = c - len;
+              spg = atomicAdd(d.spill_cursor, (unsigned long long)spn);
+              if (spg + spn > (unsigned long long)d.spill_cap) { spn = 0; *d.overflow = 1ull; }
+            } else *d.overflow = 1ull;
           }
-          g = old + (unsigned long long)(d.dst_base ? d.dst_base[tid] : d.base_const);
         }
+        g = old + (unsigned long long)(d.dst_base ? d.dst_base[tid] : d.base_const);
       }
       uint32_t w = tid < (int)P ? (((uint32_t)(g & 1) + c + 1) & ~1u) : 0, incl = w;
       for (int o = 1; o < 32; o <<= 1) { uint32_t u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
@@ -402,10 +297,6 @@ k_partition_scatter_bulk(int64_t ntiles, PartDst d, unsigned long long* __restri
     }
   }
   if (tid < (int)P * NC) bulk_wait_read_all();
-  if (d.sub_cap > 0 && tid < (int)P) {   // fill counts of this CTA's sub-segments (s_cur was last written by this very thread)
-    const unsigned long long c = s_cur[tid];
-    cursors[(size_t)tid * gridDim.x + blockIdx.x] = c < (unsigned long long)d.sub_cap ? c : (unsigned long long)d.sub_cap;
-  }
 }
 
 // histogram of destinations: 128-bit loads, 4 in flight per thread, counts packed 8 x 8 bit in two 64-bit registers
@@ -484,64 +375,30 @@ inline int launch_partition_count(int device, cudaStream_t st, const long long* 
   return TG_OK;
 }
 
-inline int scatter_bulk_enabled() { return env_int("TG_SCATTER_BULK", 1); }
-
-// grid the bulk scatter will use for n rows of NC columns (the CTA-private sub-segment layout depends on it)
-template <int NC>
-inline int scatter_bulk_grid(int device, int64_t n) {
-  constexpr int TILE = PT_BLOCK * 4;
-  size_t smem = (size_t)2 * NC * TILE * 8 + (size_t)NC * (TILE + 2 * TG_MAX_PARTS) * 8 + 2 * 8 + 16;
-  int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (smem + 1024)));
-  return (int)std::min<int64_t>(n / TILE, (int64_t)device_sm_count(device) * per_sm);
-}
-inline int scatter_bulk_grid_nc(int device, int64_t n, int nc) {
-  switch (nc) { case 1: return scatter_bulk_grid<1>(device, n); case 2: return scatter_bulk_grid<2>(device, n); case 3: return scatter_bulk_grid<3>(device, n); default: return scatter_bulk_grid<4>(device, n); }
-}
-
 template <bool HIGH, int NC>
 inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d, unsigned long long* cursors, int64_t* launches, int ctas_per_sm,
                              int32_t* paths) {
   int nsm = device_sm_count(device);
-  if (scatter_bulk_enabled()) {
-    // 1024-row tiles: 4 CTAs per SM for NC <= 2
-    constexpr int ITEMS = 4, TILE = PT_BLOCK * ITEMS;
-    int64_t ntiles = n / TILE;
-    if (ntiles > 0) {
-      size_t smem = (size_t)2 * NC * TILE * 8 + (size_t)NC * (TILE + 2 * TG_MAX_PARTS) * 8 + 2 * 8 + 16;
-      TG_CUDA(cudaFuncSetAttribute(k_partition_scatter_bulk<HIGH, NC, ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (smem + 1024)));
-      // a scatter that runs NEXT TO a probe kernel (exchange of step k+1 under the probe of step k) should leave the SMs'
-      // L1 to the probe: TG_SCATTER_CTAS_PER_SM caps the CTAs (and with them the shared-memory carve-out) per SM
-      const int cap_env = env_int("TG_SCATTER_CTAS_PER_SM", 0);
-      if (!HIGH && cap_env > 0 && per_sm > cap_env) per_sm = cap_env;
-      if (ctas_per_sm > 0 && per_sm > ctas_per_sm) per_sm = ctas_per_sm;
-      int grid = (int)std::min<int64_t>(ntiles, (int64_t)nsm * per_sm);
-      if (d.sub_cap > 0 && (uint32_t)grid != d.sub_grid) return fail(TG_ERR_CUDA, "internal: sub-segment layout sized for another grid");
-      k_partition_scatter_bulk<HIGH, NC, ITEMS><<<grid, PT_BLOCK, smem, st>>>(ntiles, d, cursors);
-      if (launches) (*launches)++;
-      if (paths) *paths |= TG_JOIN_PATH_SCATTER_BULK;
-    }
-    int64_t done = ntiles * TILE;
-    if (done < n) {
-      if (d.capacity > 0) return fail(TG_ERR_CUDA, "internal: capacity-bounded scatter needs a whole number of tiles");
-      PartDst tail = d;
-      for (int c = 0; c < NC; c++) tail.src[c] = reinterpret_cast<const unsigned long long*>(d.src[c]) + done;
-      k_partition_scatter<HIGH><<<1, PT_BLOCK, 0, st>>>(reinterpret_cast<const long long*>(tail.src[0]), nullptr, n - done, tail, cursors);
-      if (launches) (*launches)++;
-    }
-    return TG_OK;
-  }
-  int64_t ntiles = n / PT_TILE;
+  // 1024-row tiles: 4 CTAs per SM for NC <= 2
+  constexpr int ITEMS = 4, TILE = PT_BLOCK * ITEMS;
+  int64_t ntiles = n / TILE;
   if (ntiles > 0) {
-    size_t smem = (size_t)2 * NC * PT_TILE * 8 + 2 * PT_TILE * 8 + 2 * 8 + 16;
-    TG_CUDA(cudaFuncSetAttribute(k_partition_scatter_tma<HIGH, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int grid = (int)std::min<int64_t>(ntiles, (int64_t)nsm * 2);
-    k_partition_scatter_tma<HIGH, NC><<<grid, PT_BLOCK, smem, st>>>(ntiles, d, cursors);
+    size_t smem = (size_t)2 * NC * TILE * 8 + (size_t)NC * (TILE + 2 * TG_MAX_PARTS) * 8 + 2 * 8 + 16;
+    TG_CUDA(cudaFuncSetAttribute(k_partition_scatter_bulk<HIGH, NC, ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (smem + 1024)));
+    // a scatter that runs NEXT TO a probe kernel (exchange of step k+1 under the probe of step k) should leave the SMs'
+    // L1 to the probe: TG_SCATTER_CTAS_PER_SM caps the CTAs (and with them the shared-memory carve-out) per SM
+    const int cap_env = env_int("TG_SCATTER_CTAS_PER_SM", 0);
+    if (!HIGH && cap_env > 0 && per_sm > cap_env) per_sm = cap_env;
+    if (ctas_per_sm > 0 && per_sm > ctas_per_sm) per_sm = ctas_per_sm;
+    int grid = (int)std::min<int64_t>(ntiles, (int64_t)nsm * per_sm);
+    k_partition_scatter_bulk<HIGH, NC, ITEMS><<<grid, PT_BLOCK, smem, st>>>(ntiles, d, cursors);
     if (launches) (*launches)++;
-    if (paths) *paths |= TG_JOIN_PATH_SCATTER;
+    if (paths) *paths |= TG_JOIN_PATH_SCATTER_BULK;
   }
-  int64_t done = ntiles * PT_TILE;
+  int64_t done = ntiles * TILE;
   if (done < n) {
+    if (d.capacity > 0) return fail(TG_ERR_CUDA, "internal: capacity-bounded scatter needs a whole number of tiles");
     PartDst tail = d;
     for (int c = 0; c < NC; c++) tail.src[c] = reinterpret_cast<const unsigned long long*>(d.src[c]) + done;
     k_partition_scatter<HIGH><<<1, PT_BLOCK, 0, st>>>(reinterpret_cast<const long long*>(tail.src[0]), nullptr, n - done, tail, cursors);
@@ -551,8 +408,8 @@ inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d,
 }
 
 // d.src[0] must be the key column; falls back to the LSU kernel for NULL-able keys, unaligned sources or > 4 columns.
-// `paths` (optional) gains TG_JOIN_PATH_SCATTER_BULK when the bulk kernel ran, TG_JOIN_PATH_SCATTER for the other
-// full-tile kernels (the < 1-tile remainder kernel is not counted)
+// `paths` (optional) gains TG_JOIN_PATH_SCATTER_BULK when the bulk kernel ran, TG_JOIN_PATH_SCATTER when the LSU kernel
+// scattered the whole input (the < 1-tile remainder behind the bulk kernel is not counted)
 template <bool HIGH>
 inline int launch_partition_scatter(int device, cudaStream_t st, const long long* key, const uint8_t* nulls, int64_t n, PartDst& d,
                                     unsigned long long* cursors, int64_t* launches, int ctas_per_sm = 0, int32_t* paths = nullptr) {

@@ -10,9 +10,9 @@ factors can be read off one run.
   --profile DIR                                            one more pass per point under torch.profiler: time per kernel
 
 Every point prints one JSON line: step time at 100 % match and at 50 % match (the keys of bench.py's side line), table
-slots, P and slice size, plus the card name and power limit read in the same run.  The switches are the production ones
-(TG_PROBE_SUBSEG=0, TG_PROBE_SEG_LEAN=1) unless given.  Not a bench: bench.py gives the reported numbers."""
-import argparse, itertools, json, os, subprocess, sys
+slots, P and slice size, plus the card name and power limit read in the same run.  Not a bench: bench.py gives the
+reported numbers."""
+import argparse, json, os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
@@ -77,7 +77,6 @@ def main():
     ap.add_argument("--probe-rows", type=int, default=100_000_000)
     ap.add_argument("--lf", default=None, help="load factors; 0 = the library default")
     ap.add_argument("--parts", default=None, help="TG_PROBE_PARTS; 0 = the library's choice, -1 = TG_PROBE_PARTITION=0")
-    ap.add_argument("--home-width", default="0", help="TG_PAIR_HOME values (slots per home; 0 = the library default)")
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--profile", default=None, metavar="DIR", help="also write DIR/profile.jsonl: ms per step of every kernel")
     ap.add_argument("--out", default=None, metavar="DIR", help="also append the JSON lines to DIR/probe_slices.jsonl")
@@ -86,8 +85,6 @@ def main():
     nb = a.build_rows or nb
     lfs, parts = a.lf or lfs, a.parts or parts
     L = lambda s, f: [f(x) for x in s.split(",")]
-    os.environ.setdefault("TG_PROBE_SUBSEG", "0")
-    os.environ.setdefault("TG_PROBE_SEG_LEAN", "1")
     info = card()
     dev = torch.device("cuda", 0)
     stream = torch.cuda.Stream(device=dev)
@@ -105,11 +102,7 @@ def main():
         if d:
             os.makedirs(d, exist_ok=True)
         sinks.append(open(os.path.join(d, name), "a") if d else None)
-    for lf, hw in itertools.product(L(lfs, float), L(a.home_width, int)):
-        if hw:
-            os.environ["TG_PAIR_HOME"] = str(hw)
-        else:
-            os.environ.pop("TG_PAIR_HOME", None)
+    for lf in L(lfs, float):
         plan = make_plan(0, stream.cuda_stream)
         if lf:
             plan.load_factor = lf
@@ -128,7 +121,7 @@ def main():
             paths = j.stats().paths   # accumulated over the handle's probes
             assert p < 0 or paths & abi.JOIN_PATH_PROBE_SEG, paths
             nparts = max(p, 0) or min(MAX_PARTS, -(-int(bs.table_slots * SLOT_BYTES) // (l2 // 4)))   # join.cu: probe_slices
-            rec = dict(build_rows=nb, probe_rows=a.probe_rows, lf=lf or None, home_width=hw or None, table_slots=bs.table_slots,
+            rec = dict(build_rows=nb, probe_rows=a.probe_rows, lf=lf or None, table_slots=bs.table_slots,
                        table_mb=round(table_mb, 1), parts=nparts if p >= 0 else 1, slice_mb=round(table_mb / nparts, 2) if p >= 0 else None,
                        partition=p >= 0, paths=paths, build_ms=round(bs.build_ms, 2),
                        ms=round(timed(j, stream, [pk, pv], a.steps), 3), ms_match50=round(timed(j, stream, [pk2, pv], a.steps), 3), **info)
@@ -136,7 +129,7 @@ def main():
             if sinks[0]:
                 sinks[0].write(json.dumps(rec) + "\n"); sinks[0].flush()
             if a.profile:
-                prof = dict(lf=rec["lf"], home_width=rec["home_width"], parts=rec["parts"], partition=rec["partition"],
+                prof = dict(lf=rec["lf"], parts=rec["parts"], partition=rec["partition"],
                             kernels_ms=profile(j, stream, [pk, pv], a.steps), kernels_ms_match50=profile(j, stream, [pk2, pv], a.steps))
                 sinks[1].write(json.dumps(prof) + "\n"); sinks[1].flush()
         j.close()
