@@ -379,9 +379,17 @@ typedef struct tg_agg_desc {
  *          max4Decimal / min4Decimal, func_max_min.go:906)
  *   COUNT  its usual BIGINT result (only the null bitmap is read)
  * A scale rule not met or decimal > flen is TG_ERR_INVALID.  flen > 18, flen / decimal not given, Final / Partial2 mode
- * (a partial DECIMAL sum has p + 22 digits), a fused argument expression, FIRSTROW, a DECIMAL GROUP BY column or a
- * non-DECIMAL ret_type over a DECIMAL argument is TG_ERR_UNSUPPORTED.  SUM / AVG keep the 128-bit sum of
- * tg_agg_func.ret_type (2-3 state words), MIN / MAX 1-2 words, under the same 24-word limit.
+ * (a partial DECIMAL sum has p + 22 digits), FIRSTROW, a DECIMAL GROUP BY column or a non-DECIMAL ret_type over a
+ * DECIMAL argument is TG_ERR_UNSUPPORTED.  SUM / AVG keep the 128-bit sum of tg_agg_func.ret_type (2-3 state words),
+ * MIN / MAX 1-2 words, under the same 24-word limit.
+ * SUM / AVG of a product, arg_expr TG_ARGEXPR_MUL (arg_col * arg_col2) or TG_ARGEXPR_MUL_CSUB (arg_col * (c - arg_col2),
+ * c = arg_const), are offloaded when both columns are DECIMAL with 1 <= flen <= 18 and 0 <= decimal <= flen (the same
+ * column may be both), the mode is Complete, ret_type is TG_TYPE_NEWDECIMAL and s = s_a + s_b <= 30; for MUL_CSUB c must be
+ * a finite integer with |c| * 10^s_b <= 10^18.  The value is the exact product (DecimalMul; c - b is exact at scale s_b)
+ * at scale s.  SUM needs ret_frac = s, AVG s <= ret_frac <= 30 (TG_ERR_INVALID otherwise); results follow the column rules
+ * above at scale s.  s > 30, a constant that is not such an integer, a DECIMAL operand paired with a DOUBLE or integer one,
+ * flen > 18, MIN / MAX / COUNT of an expression and Final / Partial modes are TG_ERR_UNSUPPORTED.  The state is an exact
+ * 192-bit sum (3 words, 4 with a nullable operand), under the same 24-word limit.
  * Input columns hold 40-byte MyDecimal cells (elem_len 40, host or device memory; device columns need only 8-byte
  * alignment).  A non-NULL cell must be in the column's stored form, as MyDecimal.FromBin (types/mydecimal.go:1465) makes
  * it: digitsFrac = decimal, ceil(digitsInt / 9) integer words (digitsInt may be 0, leading words may be 0), then

@@ -15,6 +15,7 @@
 // (NULL group keys DO form a group: codec.go:1766), slot S+1 the group whose key equals the sentinel.
 #include <memory>
 #include <algorithm>
+#include <cmath>
 #include "common.cuh"
 #include "tma.cuh"
 #include "decimal.cuh"
@@ -36,8 +37,11 @@ struct AggFuncDev {
   int32_t s2;           // >= 0: DECIMAL SUM / AVG, an exact 128-bit sum of the integer (or scaled DECIMAL) argument: s0 its low word, s2 its high word
   int32_t dec_frac;     // DECIMAL AVG: result scale (AggFuncDesc.RetTp decimal)
   int32_t dec_scale;    // >= 0: the result is a DECIMAL cell and the argument's values are integers * 10^-dec_scale (0 for an
-                        // integer column); -1: an 8-byte result
+                        // integer column, s_a + s_b for a product); -1: an 8-byte result
+  int32_t s3;           // >= 0: DECIMAL SUM / AVG of a product of two DECIMAL columns (arg_expr), an exact 192-bit sum: s0, s2, s3
+                        // its low, middle and top words
   double arg_const;
+  long long dec_c;      // DECIMAL MUL_CSUB: the integer constant c * 10^(s_b), |dec_c| <= 10^18
 };
 struct AggSpec { int32_t n; int32_t pad; unsigned long long* err; AggFuncDev f[TG_MAX_AGG]; };
 
@@ -98,6 +102,43 @@ __device__ __forceinline__ void dec_add(unsigned long long* lo, unsigned long lo
   const unsigned long long add = ext + (old + v < old ? 1ull : 0ull);
   if (add) atomicAdd(hi, add);
 }
+// DECIMAL SUM / AVG of a product: adds the 192-bit value (v2:v1:v0) to the 192-bit sum (*w2:*w1:*w0) with dec_add's carry
+// rule, one word after the other: the middle word only when v1 plus the low word's carry is not 0, the top word only on a
+// middle carry or a negative value.  A non-negative product below 2^64 costs one atomic, like an integer row.  Products
+// are below 2 * 10^36 < 2^121 in magnitude, so fewer than 2^63 rows keep |sum| < 2^184: exact in any order of the additions.
+__device__ __forceinline__ void dec3_add(unsigned long long* w0, unsigned long long* w1, unsigned long long* w2, unsigned long long v0,
+                                         unsigned long long v1, unsigned long long v2) {
+  const unsigned long long old0 = atomicAdd(w0, v0);
+  const unsigned long long x1 = v1 + (old0 + v0 < old0 ? 1ull : 0ull);
+  unsigned long long x2 = v2 + (x1 < v1 ? 1ull : 0ull);   // v1 = 2^64 - 1 plus a carry wraps to 0
+  if (x1) { const unsigned long long old1 = atomicAdd(w1, x1); x2 += old1 + x1 < old1 ? 1ull : 0ull; }
+  if (x2) atomicAdd(w2, x2);
+}
+// the exact signed product a * t as (top:mid:lo): one 64x64 multiply for the low word, its signed high half, the sign
+__device__ __forceinline__ void dec_mul(long long a, long long t, unsigned long long& lo, unsigned long long& mid, unsigned long long& top) {
+  lo = (unsigned long long)a * (unsigned long long)t;
+  mid = (unsigned long long)__mul64hi(a, t);
+  top = (unsigned long long)((long long)mid >> 63);
+}
+// one row of a DECIMAL SUM / AVG of a product: the 192-bit add of a * t and the non-NULL count (nullptr: NOT NULL operands).
+// The three words are the consecutive states s0, s2 = s0 + 1, s3 = s0 + 2, so they sit at w0, w0 + step, w0 + 2 * step in
+// every table layout.  Out of line, like dec_apply, and with few arguments: a kernel's register count includes its callees'.
+__device__ __noinline__ void dec3_apply(unsigned long long* w0, int64_t step, unsigned long long* cnt, long long a, long long t) {
+  unsigned long long lo, mid, top;
+  dec_mul(a, t, lo, mid, top);
+  dec3_add(w0, w0 + step, w0 + 2 * step, lo, mid, top);
+  if (cnt) atomicAdd(cnt, 1ull);
+}
+// the operands of a DECIMAL product row (k_dec_to_scaled has turned both columns into int64 value * 10^scale): a, and
+// t = b (MUL) or c * 10^(s_b) - b (MUL_CSUB, |t| < 2 * 10^18); false when b is NULL (the caller has checked a)
+__device__ __forceinline__ bool dec_expr_operands(const AggFuncDev& f, const DevCols& cols, int64_t row, long long& a, long long& t) {
+  const uint8_t* nb2 = cols.nulls[f.arg_col2];
+  if (nb2 && !bit_not_null(nb2, row)) return false;
+  a = __ldcs(reinterpret_cast<const long long*>(cols.data[f.arg_col]) + row);
+  const long long b = __ldcs(reinterpret_cast<const long long*>(cols.data[f.arg_col2]) + row);
+  t = f.arg_expr == TG_ARGEXPR_MUL_CSUB ? f.dec_c - b : b;
+  return true;
+}
 // high word of an integer argument as a 128-bit value
 __device__ __forceinline__ unsigned long long dec_ext(const AggFuncDev& f, unsigned long long v) {
   return f.is_unsigned ? 0ull : (unsigned long long)((long long)v >> 63);
@@ -125,10 +166,15 @@ __global__ void k_agg_init(AggTable t, AggSpec spec, unsigned long long n_total)
       }
       if (f.s1 >= 0) t.state[f.s1][(size_t)i * t.stride] = 0;
       if (f.s2 >= 0) t.state[f.s2][(size_t)i * t.stride] = 0;
+      if (f.s3 >= 0) t.state[f.s3][(size_t)i * t.stride] = 0;
     }
   }
 }
 
+// WIDE: the plan has a DECIMAL SUM / AVG of a product (AggFuncDev::s3).  Only the WIDE instantiations of the update, merge
+// and finalize kernels carry the 192-bit code: a kernel's register count includes its out-of-line callees', and every other
+// plan keeps the kernels it had.
+template <bool WIDE>
 __device__ __forceinline__ void agg_apply(const AggTable& t, const AggSpec& spec, const DevCols& cols, int64_t row,
                                           unsigned long long s) {
   atomicAdd(&t.rows[(size_t)s * t.stride], 1ull);
@@ -137,6 +183,12 @@ __device__ __forceinline__ void agg_apply(const AggTable& t, const AggSpec& spec
     if (f.arg_col < 0 || f.s0 < 0) continue;   // COUNT(*) and NOT NULL COUNT(x) read rows[]; FIRSTROW reads the key
     const uint8_t* nb = cols.nulls[f.arg_col];
     if (nb && !bit_not_null(nb, row)) continue;
+    if (WIDE && f.s3 >= 0) {   // DECIMAL SUM / AVG of a product
+      long long x, y;
+      if (dec_expr_operands(f, cols, row, x, y))
+        dec3_apply(&t.state[f.s0][(size_t)s * t.stride], t.state[f.s2] - t.state[f.s0], f.s1 >= 0 ? &t.state[f.s1][(size_t)s * t.stride] : nullptr, x, y);
+      continue;
+    }
     switch (f.name) {
       case TG_AGG_COUNT:
         if (f.final_mode) atomicAdd(&t.state[f.s0][(size_t)s * t.stride], reinterpret_cast<const unsigned long long*>(cols.data[f.arg_col])[row]);
@@ -189,6 +241,7 @@ __device__ __forceinline__ void agg_apply(const AggTable& t, const AggSpec& spec
 // One thread per row: find-or-insert the group slot, then atomics.  Rows whose NEW key would push the
 // table past max_fill are deferred (bit set in `deferred`) so the host can grow the table and re-run
 // them; `only` restricts a re-run to those rows.
+template <bool WIDE>
 __global__ void __launch_bounds__(256)
 k_agg_update(GroupKey gk, DevCols cols, int64_t n, AggTable t, AggSpec spec, unsigned long long max_fill,
              unsigned long long* fill, uint32_t* deferred, const uint32_t* only, unsigned long long* n_deferred) {
@@ -233,11 +286,40 @@ k_agg_update(GroupKey gk, DevCols cols, int64_t n, AggTable t, AggSpec spec, uns
         }
       }
     }
-    agg_apply(t, spec, cols, i, s);
+    agg_apply<WIDE>(t, spec, cols, i, s);
+  }
+}
+
+// no GROUP BY, DECIMAL SUM / AVG of a product: a 192-bit sum per thread, a warp reduction, one dec3_add per warp (out of
+// line: the 192-bit accumulator stays out of k_agg_update_nogroup's other paths)
+__device__ __forceinline__ void add192(unsigned long long& s0, unsigned long long& s1, unsigned long long& s2, unsigned long long v0,
+                                       unsigned long long v1, unsigned long long v2) {
+  asm("add.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u64 %2, %2, %5;" : "+l"(s0), "+l"(s1), "+l"(s2) : "l"(v0), "l"(v1), "l"(v2));
+}
+__device__ __noinline__ void dec3_nogroup(const long long* a, const uint8_t* na, const long long* b, const uint8_t* nb, bool csub, long long c,
+                                          int64_t i0, int64_t n, int64_t stride, unsigned long long* w0, unsigned long long* w1,
+                                          unsigned long long* w2, unsigned long long* cnt_out) {
+  unsigned long long s0 = 0, s1 = 0, s2 = 0, cnt = 0;
+  for (int64_t i = i0; i < n; i += stride) {
+    if ((na && !bit_not_null(na, i)) || (nb && !bit_not_null(nb, i))) continue;
+    unsigned long long lo, mid, top;
+    dec_mul(a[i], csub ? c - b[i] : b[i], lo, mid, top);
+    add192(s0, s1, s2, lo, mid, top);
+    cnt++;
+  }
+  for (int o = 16; o; o >>= 1) {
+    const unsigned long long t0 = __shfl_xor_sync(0xffffffffu, s0, o), t1 = __shfl_xor_sync(0xffffffffu, s1, o), t2 = __shfl_xor_sync(0xffffffffu, s2, o);
+    add192(s0, s1, s2, t0, t1, t2);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if ((threadIdx.x & 31) == 0 && cnt) {
+    dec3_add(w0, w1, w2, s0, s1, s2);
+    if (cnt_out) atomicAdd(cnt_out, cnt);
   }
 }
 
 // no GROUP BY: one group.  Warp-shuffle partial reduction, then one atomic per warp and aggregate.
+template <bool WIDE>
 __global__ void __launch_bounds__(256)
 k_agg_update_nogroup(DevCols cols, int64_t n, AggTable t, AggSpec spec) {
   int64_t i0 = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -251,6 +333,12 @@ k_agg_update_nogroup(DevCols cols, int64_t n, AggTable t, AggSpec spec) {
     const AggFuncDev& f = spec.f[k];
     if (f.arg_col < 0 || f.s0 < 0) continue;
     const uint8_t* nb = cols.nulls[f.arg_col];
+    if (WIDE && f.s3 >= 0) {
+      dec3_nogroup(reinterpret_cast<const long long*>(cols.data[f.arg_col]), nb, reinterpret_cast<const long long*>(cols.data[f.arg_col2]),
+                   cols.nulls[f.arg_col2], f.arg_expr == TG_ARGEXPR_MUL_CSUB, f.dec_c, i0, n, stride, &t.state[f.s0][t.nslots],
+                   &t.state[f.s2][t.nslots], &t.state[f.s3][t.nslots], f.s1 >= 0 ? &t.state[f.s1][t.nslots] : nullptr);
+      continue;
+    }
     double fs = 0; unsigned long long cnt = 0, ext = f.name == TG_AGG_MIN ? ~0ull : 0ull, isum = 0;
     __int128 dsum = 0;   // DECIMAL SUM / AVG: exact
     for (int64_t i = i0; i < n; i += stride) {
@@ -334,6 +422,7 @@ struct AggPartials {   // columnar partial results, capacity = gridDim.x * (loca
   unsigned long long* count;           // number of tuples emitted
 };
 
+template <bool WIDE>
 __global__ void __launch_bounds__(256)
 k_agg_update_local(GroupKey gk, DevCols cols, int64_t row_lo, int64_t row_hi, AggSpec spec, int nstates, int local_slots,
                    AggPartials out, uint32_t* deferred, unsigned long long* n_deferred) {
@@ -354,6 +443,7 @@ k_agg_update_local(GroupKey gk, DevCols cols, int64_t row_lo, int64_t row_hi, Ag
       if (f.s0 >= 0) lt.state[f.s0][i] = f.name == TG_AGG_MIN ? ~0ull : 0ull;
       if (f.s1 >= 0) lt.state[f.s1][i] = 0;
       if (f.s2 >= 0) lt.state[f.s2][i] = 0;
+      if (f.s3 >= 0) lt.state[f.s3][i] = 0;
     }
   }
   if (threadIdx.x == 0) s_fill = 0;
@@ -387,7 +477,7 @@ k_agg_update_local(GroupKey gk, DevCols cols, int64_t row_lo, int64_t row_hi, Ag
       }
     }
     if (defer) { atomicOr(&deferred[i >> 5], 1u << (i & 31)); my_deferred++; continue; }
-    agg_apply(lt, spec, cols, i, s);
+    agg_apply<WIDE>(lt, spec, cols, i, s);
   }
   for (int o = 16; o; o >>= 1) my_deferred += __shfl_xor_sync(0xffffffffu, my_deferred, o);
   if ((threadIdx.x & 31) == 0 && my_deferred) atomicAdd(n_deferred, my_deferred);
@@ -405,6 +495,7 @@ k_agg_update_local(GroupKey gk, DevCols cols, int64_t row_lo, int64_t row_hi, Ag
 }
 
 // fold partial results into the global table; same deferral protocol as k_agg_update
+template <bool WIDE>
 __global__ void __launch_bounds__(256)
 k_agg_merge(AggPartials in, int64_t m, AggTable t, AggSpec spec, unsigned long long max_fill, unsigned long long* fill,
             uint32_t* deferred, const uint32_t* only, unsigned long long* n_deferred) {
@@ -440,7 +531,8 @@ k_agg_merge(AggPartials in, int64_t m, AggTable t, AggSpec spec, unsigned long l
         switch (f.name) {
           case TG_AGG_COUNT: atomicAdd(&t.state[f.s0][s], v); break;                                                  // countPartial merge func_count.go:481
           case TG_AGG_SUM: case TG_AGG_AVG:   // func_sum.go:106, func_avg.go:444
-            if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, in.state[f.s2][i]);
+            if (WIDE && f.s3 >= 0) dec3_add(&t.state[f.s0][s], &t.state[f.s2][s], &t.state[f.s3][s], v, in.state[f.s2][i], in.state[f.s3][i]);
+            else if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, in.state[f.s2][i]);
             else atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v));
             break;
           case TG_AGG_MIN: atomicMin(&t.state[f.s0][s], v); break;
@@ -490,6 +582,9 @@ struct AggOut { void* data[TG_MAX_AGG]; uint8_t* valid[TG_MAX_AGG]; };
 
 // compact the occupied slots into the result columns (Go-map iteration order is unspecified in the
 // reference too; here it is slot order within warps, warp order by the atomic cursor)
+// DEC: the plan has a DECIMAL result column (the cell writers of decimal.cuh); WIDE: one of them is a SUM / AVG of a
+// product (the 192-bit writers, which take more registers)
+template <bool DEC, bool WIDE>
 __global__ void __launch_bounds__(256)
 k_agg_finalize(AggTable t, AggSpec spec, int gk_kind, AggOut out, unsigned long long* cursor) {
   unsigned long long n_total = t.nslots + 2;
@@ -524,13 +619,16 @@ k_agg_finalize(AggTable t, AggSpec spec, int gk_kind, AggOut out, unsigned long 
     for (int k = 0; k < spec.n; k++) {
       const AggFuncDev& f = spec.f[k];
       unsigned long long nn = f.s1 >= 0 ? t.state[f.s1][(size_t)i * t.stride] : rows;   // non-NULL inputs seen
-      if (f.dec_scale >= 0) {   // DECIMAL SUM / AVG / MIN / MAX: a 40-byte MyDecimal cell, NULL without a non-NULL input (decimal.cuh)
+      if (DEC && f.dec_scale >= 0) {   // DECIMAL SUM / AVG / MIN / MAX: a 40-byte MyDecimal cell, NULL without a non-NULL input (decimal.cuh)
         uint8_t* cell = reinterpret_cast<uint8_t*>(out.data[k]) + (size_t)o * TG_DEC_CELL_BYTES;
-        // SUM / AVG: the 128-bit sum; MIN / MAX: the int64 of the ordered domain (i64_to_ordered), sign-extended
+        // SUM / AVG: the 128-bit sum (192-bit over a product); MIN / MAX: the int64 of the ordered domain (i64_to_ordered),
+        // sign-extended
         unsigned long long lo = t.state[f.s0][(size_t)i * t.stride], hi;
         if (f.s2 >= 0) hi = t.state[f.s2][(size_t)i * t.stride];
         else { lo ^= 0x8000000000000000ull; hi = (unsigned long long)((long long)lo >> 63); }
         if (nn == 0) dec_store_null(cell);
+        else if (WIDE && f.s3 >= 0)
+          dec3_result_cell(cell, lo, hi, t.state[f.s3][(size_t)i * t.stride], nn, f.dec_scale | (f.dec_frac << 8) | (f.name == TG_AGG_AVG ? 1 << 16 : 0));
         else dec_result_cell(cell, f.name == TG_AGG_AVG, lo, hi, nn, f.dec_scale, f.dec_frac);
         if (out.valid[k]) out.valid[k][o] = nn != 0 ? 1 : 0;
         continue;
@@ -637,6 +735,7 @@ __device__ __forceinline__ unsigned long long mk_find_or_insert(const AggTable& 
   }
 }
 
+template <bool WIDE>
 __global__ void __launch_bounds__(256)
 k_agg_update_mk(GroupKeys gk, DevCols cols, int64_t n, AggTable t, AggSpec spec, uint32_t max_probe,
                 uint32_t* deferred, const uint32_t* only, unsigned long long* n_deferred) {
@@ -649,7 +748,7 @@ k_agg_update_mk(GroupKeys gk, DevCols cols, int64_t n, AggTable t, AggSpec spec,
     load_key_words(gk, i, k);
     const unsigned long long s = mk_find_or_insert(t, k, hash_words(k, t.nkw), max_probe);
     if (s == ~0ull) { atomicOr(&deferred[i >> 5], 1u << (i & 31)); my_deferred++; continue; }
-    agg_apply(t, spec, cols, i, s);
+    agg_apply<WIDE>(t, spec, cols, i, s);
   }
   for (int o = 16; o; o >>= 1) my_deferred += __shfl_xor_sync(0xffffffffu, my_deferred, o);
   if ((threadIdx.x & 31) == 0 && my_deferred) atomicAdd(n_deferred, my_deferred);
@@ -761,6 +860,8 @@ struct AggImpl {
   std::vector<int> col_flen, col_dec;   // tg_agg_desc_ex: precision / scale per child column, -1 = not given
   std::vector<char> dec_decode;         // DECIMAL argument column of SUM / AVG / MIN / MAX: k_dec_to_scaled runs on every batch
   std::vector<std::unique_ptr<DevBuf>> dscaled;   // its int64 value * 10^scale, one pooled scratch column per such column
+  bool wide = false;        // a DECIMAL SUM / AVG of a product: the WIDE kernel instantiations
+  bool dec_out = false;     // a DECIMAL result column: k_agg_finalize<true, wide>
 
   // table
   DevBuf tbl_mem;
@@ -790,6 +891,9 @@ static int agrid(const AggImpl* a, int64_t n, int block = 256, int per_sm = 8) {
   return (int)(need < cap ? need : cap);
 }
 
+static int dec_expr_rules(const AggImpl* a, const tg_agg_func& f);
+static long long pow10_i64(int k) { long long p = 1; while (k-- > 0) p *= 10; return p; }
+
 // A function over a DECIMAL column (tg_agg_desc_ex): TG_OK when it is offloaded, else the status and message
 static int dec_arg_rules(const AggImpl* a, const tg_agg_func& f) {
   const int c = f.arg_col, p = a->col_flen[c], s = a->col_dec[c];
@@ -797,7 +901,8 @@ static int dec_arg_rules(const AggImpl* a, const tg_agg_func& f) {
   if (p > 18) return fail(TG_ERR_UNSUPPORTED, "DECIMAL arguments are offloaded up to precision 18 (one int64 at the column's scale)");
   if (p < 1 || s > p) return fail(TG_ERR_INVALID, "a DECIMAL column needs 1 <= flen and 0 <= decimal <= flen");
   if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "aggregates over DECIMAL columns are offloaded in Complete mode only (no DECIMAL partial results)");
-  if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL column is not offloaded in a fused argument expression");
+  if (f.arg_expr == TG_ARGEXPR_MUL || f.arg_expr == TG_ARGEXPR_MUL_CSUB) return dec_expr_rules(a, f);
+  if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL column is not offloaded in this argument expression");
   switch (f.name) {
     case TG_AGG_COUNT:   // reads the null bitmap only
       return f.ret_type == TG_TYPE_NEWDECIMAL ? fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG / MIN / MAX only") : TG_OK;
@@ -809,6 +914,33 @@ static int dec_arg_rules(const AggImpl* a, const tg_agg_func& f) {
       return TG_OK;
     default: return fail(TG_ERR_UNSUPPORTED, "this aggregate function is not offloaded over a DECIMAL column");
   }
+}
+
+// SUM / AVG of a * b or a * (c - b) over two DECIMAL(p <= 18) columns (dec_arg_rules has checked a and the mode): the exact
+// product (DecimalMul, mydecimal.go:2041) has scale s = s_a + s_b, and c - b (DecimalSub) is exact at scale s_b
+static int dec_expr_rules(const AggImpl* a, const tg_agg_func& f) {
+  const int c2 = f.arg_col2;
+  if (c2 < 0 || c2 >= a->ncols || a->types[c2] != TG_TYPE_NEWDECIMAL)
+    return fail(TG_ERR_UNSUPPORTED, "a DECIMAL argument expression takes two DECIMAL columns");
+  const int p2 = a->col_flen[c2], s2 = a->col_dec[c2];
+  if (p2 < 0 || s2 < 0) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL argument column needs its precision and scale (tg_agg_desc_ex col_flen / col_decimal)");
+  if (p2 > 18) return fail(TG_ERR_UNSUPPORTED, "DECIMAL arguments are offloaded up to precision 18 (one int64 at the column's scale)");
+  if (p2 < 1 || s2 > p2) return fail(TG_ERR_INVALID, "a DECIMAL column needs 1 <= flen and 0 <= decimal <= flen");
+  if (f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) return fail(TG_ERR_UNSUPPORTED, "argument expressions are fused for SUM / AVG only");
+  if (f.ret_type != TG_TYPE_NEWDECIMAL) return fail(TG_ERR_UNSUPPORTED, "SUM / AVG of a DECIMAL product need a DECIMAL ret_type");
+  const int s = a->col_dec[f.arg_col] + s2;
+  // TiDB types the product with frac min(s, 30) but keeps digitsFrac min(s, 31) in the value: past 30 the two disagree
+  if (s > 30) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL product is offloaded up to scale 30 (s_a + s_b)");
+  if (f.arg_expr == TG_ARGEXPR_MUL_CSUB) {   // c * 10^s_b - b must fit int64: |c| * 10^s_b <= 10^18 keeps it below 2 * 10^18
+    const double c = f.arg_const;
+    const double lim = 1e18 / (double)pow10_i64(s2);   // 10^(18 - s_b), exact in a double
+    if (!std::isfinite(c) || c != std::trunc(c) || std::fabs(c) > lim)
+      return fail(TG_ERR_UNSUPPORTED, "a DECIMAL c - b takes an integer constant c with |c| * 10^scale(b) <= 10^18");
+  }
+  if (f.name == TG_AGG_AVG ? (f.ret_frac < s || f.ret_frac > 30) : f.ret_frac != s)
+    return fail(TG_ERR_INVALID, f.name == TG_AGG_AVG ? "DECIMAL AVG of a product: scale must be s_a + s_b .. 30"
+                                                    : "DECIMAL SUM of a product has the scale s_a + s_b");
+  return TG_OK;
 }
 
 static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, const int32_t* col_dec) {
@@ -853,7 +985,7 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
   for (int k = 0; k < d->n_funcs; k++) {
     const tg_agg_func& f = d->funcs[k];
     AggFuncDev& o = a->spec.f[k];
-    o = AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, -1, 0, -1, f.arg_const};
+    o = AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, -1, 0, -1, -1, f.arg_const, 0};
     // a DECIMAL(p <= 18, s) argument column (tg_agg_desc_ex): decoded to int64 value * 10^s on every batch, then the integer
     // update paths run unchanged
     const bool dec_arg = f.arg_col >= 0 && f.arg_col < a->ncols && a->types[f.arg_col] == TG_TYPE_NEWDECIMAL;
@@ -876,7 +1008,7 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
       if (f.arg_expr != TG_ARGEXPR_MUL && f.arg_expr != TG_ARGEXPR_MUL_CSUB) return fail(TG_ERR_INVALID, "unknown aggregate argument expression");
       if ((f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) || f.mode != TG_AGGMODE_COMPLETE)
         return fail(TG_ERR_UNSUPPORTED, "argument expressions are fused for SUM / AVG in Complete mode only");
-      if (f.arg_col < 0 || f.arg_col2 < 0 || f.arg_col2 >= d->n_cols || a->types[f.arg_col] != TG_TYPE_DOUBLE || a->types[f.arg_col2] != TG_TYPE_DOUBLE)
+      if (!dec_arg && (f.arg_col < 0 || f.arg_col2 < 0 || f.arg_col2 >= d->n_cols || a->types[f.arg_col] != TG_TYPE_DOUBLE || a->types[f.arg_col2] != TG_TYPE_DOUBLE))
         return fail(TG_ERR_UNSUPPORTED, "argument expressions take two DOUBLE columns");
       a->needed[f.arg_col2] = 1;
     }
@@ -891,14 +1023,22 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
     o.is_unsigned = f.arg_col >= 0 && !dec_arg && (a->flags[f.arg_col] & TG_FLAG_UNSIGNED) != 0;   // a decoded DECIMAL is a signed int64
     if (dec_arg && f.name != TG_AGG_COUNT) { o.dec_scale = a->col_dec[f.arg_col]; a->dec_decode[f.arg_col] = 1; }
     else if (dec) o.dec_scale = 0;
+    const bool dec_expr = dec_arg && f.arg_expr != TG_ARGEXPR_COL;   // SUM / AVG of a DECIMAL product (dec_expr_rules)
+    if (dec_expr) {
+      const int sb = a->col_dec[f.arg_col2];
+      o.dec_scale += sb;
+      a->dec_decode[f.arg_col2] = 1;
+      if (f.arg_expr == TG_ARGEXPR_MUL_CSUB) o.dec_c = (long long)f.arg_const * pow10_i64(sb);
+    }
     switch (f.name) {
       case TG_AGG_COUNT:
         if (o.final_mode) { if (f.arg_col < 0) return fail(TG_ERR_INVALID, "final COUNT needs the partial count column"); o.s0 = a->nstates++; }
         else if (f.arg_col >= 0 && arg_nullable) o.s0 = a->nstates++;   // NOT NULL COUNT(x) == COUNT(*) == rows[]
         break;
       case TG_AGG_SUM:
-        if (dec) {   // states: low word, high word, non-NULL count (a NOT NULL argument counts with rows[])
+        if (dec) {   // states: low word, high word (a product: middle and top word), non-NULL count (NOT NULL arguments count with rows[])
           o.s0 = a->nstates++; o.s2 = a->nstates++;
+          if (dec_expr) o.s3 = a->nstates++;
           if (arg_nullable) o.s1 = a->nstates++;
           a->out_nullable[k] = 1; a->out_elem[k] = TG_DEC_CELL_BYTES;
           break;
@@ -912,6 +1052,7 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
       case TG_AGG_AVG:
         if (dec) {
           o.s0 = a->nstates++; o.s2 = a->nstates++;
+          if (dec_expr) o.s3 = a->nstates++;
           if (arg_nullable) o.s1 = a->nstates++;
           o.dec_frac = f.ret_frac;
           a->out_nullable[k] = 1; a->out_elem[k] = TG_DEC_CELL_BYTES;
@@ -947,7 +1088,15 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
       default: return fail(TG_ERR_UNSUPPORTED, "aggregate function is not offloaded");
     }
   }
-  if (a->nstates > 2 * TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "the aggregate list needs more than 24 state words (a DECIMAL SUM / AVG takes up to 3)");
+  a->wide = a->dec_out = false;
+  for (int k = 0; k < d->n_funcs; k++) {
+    const AggFuncDev& o = a->spec.f[k];
+    // dec3_apply / sdec3_apply find the middle and top words one and two state strides after the low word
+    if (o.s3 >= 0 && (o.s2 != o.s0 + 1 || o.s3 != o.s0 + 2)) return fail(TG_ERR_CUDA, "internal: the 192-bit sum's state words are not consecutive");
+    a->wide |= o.s3 >= 0;
+    a->dec_out |= o.dec_scale >= 0;
+  }
+  if (a->nstates > 2 * TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "the aggregate list needs more than 24 state words (a DECIMAL SUM / AVG takes up to 3, up to 4 over a product)");
   a->device = d->device;
   a->expected_groups = d->expected_groups;
   return TG_OK;
@@ -1028,7 +1177,7 @@ static int merge_partials(AggImpl* a, const AggPartials& pp, unsigned long long 
   const uint32_t* only = nullptr;
   for (int round = 0; round < 40; round++) {
     unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
-    k_agg_merge<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->tbl, a->spec, max_fill, sc, mdef.as<uint32_t>(), only, sc + 4);
+    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->tbl, a->spec, max_fill, sc, mdef.as<uint32_t>(), only, sc + 4);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_MERGE;
     unsigned long long nd = 0;
@@ -1067,7 +1216,7 @@ static int update_grouped_mk(AggImpl* a, const DevCols& cols, int64_t n, unsigne
   const uint32_t* only = nullptr;
   for (int round = 0; round < 40; round++) {
     TG_CUDA(cudaMemsetAsync(sc + 1, 0, 8, a->stream));
-    k_agg_update_mk<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, 48u, a->deferred.as<uint32_t>(), only, sc + 1);
+    (a->wide ? k_agg_update_mk<true> : k_agg_update_mk<false>)<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, 48u, a->deferred.as<uint32_t>(), only, sc + 1);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_MULTI_KEY;
     unsigned long long nd = 0;
@@ -1109,14 +1258,14 @@ static int update_grouped_v2(AggImpl* a, const GroupKey& gk, const DevCols& cols
     size_t per = 8 + 8 + 8 * (size_t)a->nstates + 1;
     TG_TRY(a->partials_mem.ensure(a->device, (size_t)p.spill_cap * per + 256));
     layout_partials(a->partials_mem.as<uint8_t>(), (size_t)p.spill_cap, a->nstates, sc + 5, p.spill);
-    TG_CUDA(cudaFuncSetAttribute(k_agg_update2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    TG_CUDA(cudaFuncSetAttribute(a->wide ? k_agg_update2<true, true> : k_agg_update2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
   DevBuf prev_deferred;
   for (int round = 0; round < 40; round++) {
     TG_CUDA(cudaMemsetAsync(sc + 1, 0, 8, a->stream));
     TG_CUDA(cudaMemsetAsync(sc + 5, 0, 8, a->stream));
-    if (local && round == 0) k_agg_update2<true><<<grid, AGG2_BLOCK, smem, a->stream>>>(p, cols, a->tbl, a->spec);
-    else k_agg_update2<false><<<grid, AGG2_BLOCK, 0, a->stream>>>(p, cols, a->tbl, a->spec);
+    if (local && round == 0) (a->wide ? k_agg_update2<true, true> : k_agg_update2<true, false>)<<<grid, AGG2_BLOCK, smem, a->stream>>>(p, cols, a->tbl, a->spec);
+    else (a->wide ? k_agg_update2<false, true> : k_agg_update2<false, false>)<<<grid, AGG2_BLOCK, 0, a->stream>>>(p, cols, a->tbl, a->spec);
     a->stats.kernel_launches++;
     a->stats.paths |= (local && round == 0) ? TG_AGG_PATH_V2_LOCAL : TG_AGG_PATH_V2_GLOBAL;
     unsigned long long back[8] = {0};
@@ -1160,8 +1309,8 @@ static int local_partial_pass(AggImpl* a, const GroupKey& gk, const DevCols& col
   pp.count = sc + 3;
   TG_CUDA(cudaMemsetAsync(sc + 3, 0, 8, a->stream));
   size_t smem = (size_t)(local_slots + 2) * 8 * (2 + a->nstates);
-  TG_CUDA(cudaFuncSetAttribute(k_agg_update_local, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_agg_update_local<<<grid, 256, smem, a->stream>>>(gk, cols, lo, hi, a->spec, a->nstates, local_slots, pp, a->deferred.as<uint32_t>(), sc + 1);
+  TG_CUDA(cudaFuncSetAttribute(a->wide ? k_agg_update_local<true> : k_agg_update_local<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  (a->wide ? k_agg_update_local<true> : k_agg_update_local<false>)<<<grid, 256, smem, a->stream>>>(gk, cols, lo, hi, a->spec, a->nstates, local_slots, pp, a->deferred.as<uint32_t>(), sc + 1);
   a->stats.kernel_launches++;
   a->stats.paths |= TG_AGG_PATH_V1_LOCAL;
   unsigned long long m = 0;
@@ -1177,7 +1326,7 @@ static int local_partial_pass(AggImpl* a, const GroupKey& gk, const DevCols& col
   const uint32_t* only = nullptr;
   for (int round = 0; round < 40; round++) {
     unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
-    k_agg_merge<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->tbl, a->spec, max_fill, sc, mdef.as<uint32_t>(), only, sc + 4);
+    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->tbl, a->spec, max_fill, sc, mdef.as<uint32_t>(), only, sc + 4);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_MERGE;
     unsigned long long nd = 0;
@@ -1215,7 +1364,7 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
   }
   TG_CUDA(cudaEventRecord(a->ev0, a->stream));
   if (a->group_col < 0) {
-    k_agg_update_nogroup<<<agrid(a, n, 256, 4), 256, 0, a->stream>>>(cols, n, a->tbl, a->spec);
+    (a->wide ? k_agg_update_nogroup<true> : k_agg_update_nogroup<false>)<<<agrid(a, n, 256, 4), 256, 0, a->stream>>>(cols, n, a->tbl, a->spec);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_NOGROUP;
   } else {
@@ -1278,7 +1427,7 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
       }
       for (int round = 0; round < 40; round++) {
         unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
-        k_agg_update<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, max_fill, sc, a->deferred.as<uint32_t>(), only, sc + 1);
+        (a->wide ? k_agg_update<true> : k_agg_update<false>)<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, max_fill, sc, a->deferred.as<uint32_t>(), only, sc + 1);
         a->stats.kernel_launches++;
         a->stats.paths |= TG_AGG_PATH_V1_GLOBAL;
         unsigned long long nd = 0;
@@ -1460,7 +1609,7 @@ static int afinalize(AggImpl* a) {
   }
   TG_CUDA(cudaEventRecord(a->ev0, a->stream));
   TG_CUDA(cudaMemsetAsync(sc + 2, 0, 8, a->stream));
-  k_agg_finalize<<<agrid(a, (int64_t)a->nslots + 2), 256, 0, a->stream>>>(a->tbl, a->spec, a->gk_kind, ao, sc + 2);
+  (a->wide ? k_agg_finalize<true, true> : a->dec_out ? k_agg_finalize<true, false> : k_agg_finalize<false, false>)<<<agrid(a, (int64_t)a->nslots + 2), 256, 0, a->stream>>>(a->tbl, a->spec, a->gk_kind, ao, sc + 2);
   a->stats.kernel_launches++;
   unsigned long long nrows = 0;
   TG_CUDA(cudaMemcpyAsync(&nrows, sc + 2, 8, cudaMemcpyDeviceToHost, a->stream));

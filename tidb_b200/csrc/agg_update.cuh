@@ -56,6 +56,20 @@ __device__ __noinline__ void sdec_apply(uint32_t lo, uint32_t hi, bool has_cnt, 
   sdec_add(lo, hi, v, ext);
   if (has_cnt) sred_inc_lo32(cnt);
 }
+// dec3_add / dec3_apply (agg.cu) on the shared-memory table: the same carry rule
+__device__ __forceinline__ void sdec3_add(uint32_t w0, uint32_t w1, uint32_t w2, unsigned long long v0, unsigned long long v1, unsigned long long v2) {
+  const unsigned long long old0 = satom_add_u64(w0, v0);
+  const unsigned long long x1 = v1 + (old0 + v0 < old0 ? 1ull : 0ull);
+  unsigned long long x2 = v2 + (x1 < v1 ? 1ull : 0ull);
+  if (x1) { const unsigned long long old1 = satom_add_u64(w1, x1); x2 += old1 + x1 < old1 ? 1ull : 0ull; }
+  if (x2) sred_add_u64(w2, x2);
+}
+__device__ __noinline__ void sdec3_apply(uint32_t w0, uint32_t step, bool has_cnt, uint32_t cnt, long long a, long long t) {
+  unsigned long long lo, mid, top;
+  dec_mul(a, t, lo, mid, top);
+  sdec3_add(w0, w0 + step, w0 + 2 * step, lo, mid, top);
+  if (has_cnt) sred_inc_lo32(cnt);
+}
 __device__ __forceinline__ unsigned long long sld_u64(uint32_t a) {
   unsigned long long v;
   asm volatile("ld.volatile.shared.u64 %0, [%1];" : "=l"(v) : "r"(a) : "memory");
@@ -75,7 +89,7 @@ __device__ __forceinline__ unsigned long long arg_raw(const DevCols& cols, int c
 }
 
 // per-row update of one group's states; SH = shared-memory table at 32-bit addresses, else the global table
-template <bool SH>
+template <bool SH, bool WIDE>
 __device__ __forceinline__ void agg_apply2(const AggTable& t, const LocalTable& lt, const AggSpec& spec, const DevCols& cols, int64_t row, unsigned long long s) {
   if (SH) sred_inc_lo32(lt_rows(lt, (uint32_t)s)); else atomicAdd(&t.rows[s], 1ull);
 #pragma unroll 1
@@ -84,6 +98,13 @@ __device__ __forceinline__ void agg_apply2(const AggTable& t, const LocalTable& 
     if (f.arg_col < 0 || f.s0 < 0) continue;   // COUNT(*) and NOT NULL COUNT(x) read rows[]; FIRSTROW reads the key
     const uint8_t* nb = cols.nulls[f.arg_col];
     if (nb && !bit_not_null(nb, row)) continue;
+    if (WIDE && f.s3 >= 0) {   // DECIMAL SUM / AVG of a product: exact 192-bit sum (out of line, like dec_apply)
+      long long x, y;
+      if (!dec_expr_operands(f, cols, row, x, y)) continue;
+      if (SH) sdec3_apply(lt_state(lt, f.s0, (uint32_t)s), lt.stride_bytes, f.s1 >= 0, lt_state(lt, f.s1 >= 0 ? f.s1 : 0, (uint32_t)s), x, y);
+      else dec3_apply(&t.state[f.s0][s], t.state[f.s2] - t.state[f.s0], f.s1 >= 0 ? &t.state[f.s1][s] : nullptr, x, y);
+      continue;
+    }
     switch (f.name) {
       case TG_AGG_COUNT: {
         unsigned long long v = f.final_mode ? arg_raw(cols, f.arg_col, row) : 1ull;
@@ -135,6 +156,7 @@ __device__ __forceinline__ void agg_apply2(const AggTable& t, const LocalTable& 
 
 // fold one partial group (rows + states) into global slot s: MergePartialResult (func_sum.go:106, func_count.go:481,
 // func_avg.go:444, func_max_min.go merge)
+template <bool WIDE>
 __device__ __forceinline__ void agg_merge_into(const AggTable& t, const AggSpec& spec, unsigned long long s, unsigned long long rows, const unsigned long long* st) {
   atomicAdd(&t.rows[s], rows);
   for (int k = 0; k < spec.n; k++) {
@@ -144,7 +166,8 @@ __device__ __forceinline__ void agg_merge_into(const AggTable& t, const AggSpec&
       switch (f.name) {
         case TG_AGG_COUNT: atomicAdd(&t.state[f.s0][s], v); break;
         case TG_AGG_SUM: case TG_AGG_AVG:
-          if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, st[f.s2]);
+          if (WIDE && f.s3 >= 0) dec3_add(&t.state[f.s0][s], &t.state[f.s2][s], &t.state[f.s3][s], v, st[f.s2], st[f.s3]);
+          else if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, st[f.s2]);
           else atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v));
           break;
         case TG_AGG_MIN: atomicMin(&t.state[f.s0][s], v); break;
@@ -187,7 +210,7 @@ struct Agg2Params {
   unsigned long long spill_cap;
 };
 
-template <bool LOCAL>
+template <bool LOCAL, bool WIDE>
 __global__ void __launch_bounds__(AGG2_BLOCK)
 k_agg_update2(Agg2Params p, DevCols cols, AggTable t, AggSpec spec) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -205,6 +228,7 @@ k_agg_update2(Agg2Params p, DevCols cols, AggTable t, AggSpec spec) {
         if (f.s0 >= 0) w[(size_t)NT * (2 + f.s0) + i] = f.name == TG_AGG_MIN ? ~0ull : 0ull;
         if (f.s1 >= 0) w[(size_t)NT * (2 + f.s1) + i] = 0;
         if (f.s2 >= 0) w[(size_t)NT * (2 + f.s2) + i] = 0;
+        if (f.s3 >= 0) w[(size_t)NT * (2 + f.s3) + i] = 0;
       }
     }
     if (tid == 0) { s_fill = 0; s_seen = 0; s_hit = 0; s_use_local = 1; }
@@ -258,7 +282,7 @@ k_agg_update2(Agg2Params p, DevCols cols, AggTable t, AggSpec spec) {
             if (++ls == lt.ls) ls = 0;
           }
         }
-        if (ok) { agg_apply2<true>(t, lt, spec, cols, i, ls); kind[r] = 4; hit++; }
+        if (ok) { agg_apply2<true, WIDE>(t, lt, spec, cols, i, ls); kind[r] = 4; hit++; }
       }
       my_local += hit;
       // hit-rate statistics of the CTA's first tiles decide whether the local level stays on
@@ -291,7 +315,7 @@ k_agg_update2(Agg2Params p, DevCols cols, AggTable t, AggSpec spec) {
         }
         s = sl;
       }
-      agg_apply2<false>(t, lt, spec, cols, i, s);
+      agg_apply2<false, WIDE>(t, lt, spec, cols, i, s);
     }
   }
   for (int o = 16; o; o >>= 1) { my_deferred += __shfl_xor_sync(0xffffffffu, my_deferred, o); my_local += __shfl_xor_sync(0xffffffffu, my_local, o); }
@@ -318,7 +342,7 @@ k_agg_update2(Agg2Params p, DevCols cols, AggTable t, AggSpec spec) {
       ok = global_find_or_insert(t, k, sl, c0, p.max_probe);
       s = sl;
     }
-    if (ok) { agg_merge_into(t, spec, s, rows, st); continue; }
+    if (ok) { agg_merge_into<WIDE>(t, spec, s, rows, st); continue; }
     unsigned long long o = atomicAdd(p.spill.count, 1ull);   // overfull table: hand the group to the host's grow-and-merge loop
     if (o < p.spill_cap) {
       p.spill.keys[o] = k; p.spill.kind[o] = 0; p.spill.rows[o] = rows;

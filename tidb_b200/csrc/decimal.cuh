@@ -6,8 +6,8 @@
 //   then int32 wordBuf[9] in base 10^9, most significant word first: integer words, then fraction words, the rest 0.
 // The library writes one canonical form: digitsInt = 9 * the number of integer words, at least one word (FromUint,
 // mydecimal.go:1069), digitsFrac = resultFrac = the result scale, and a zero result is never negative.  The update
-// kernels only see the 128-bit sum in two state words, or the int64 value * 10^scale of a DECIMAL argument; this header
-// is the one place that knows the layout.
+// kernels only see the 128-bit sum in two state words (192 bits in three for a product of DECIMAL columns), or the int64
+// value * 10^scale of a DECIMAL argument; this header is the one place that knows the layout.
 #pragma once
 
 namespace tg {
@@ -169,6 +169,123 @@ __device__ __noinline__ void dec_avg_cell(uint8_t* cell, unsigned long long lo, 
 __device__ __noinline__ void dec_result_cell(uint8_t* cell, bool avg, unsigned long long lo, unsigned long long hi, unsigned long long n, int scale, int frac) {
   if (avg) dec_avg_cell(cell, lo, hi, n, scale, frac);
   else dec_sum_cell(cell, lo, hi, scale);
+}
+
+// 192-bit magnitudes, least significant word first: m /= d, returns m % d (d < 2^64; each step's quotient fits 64 bits
+// because the running remainder is below d)
+__device__ __forceinline__ unsigned long long dec_divmod192(unsigned long long (&m)[3], unsigned long long d) {
+  unsigned long long r = 0;
+#pragma unroll
+  for (int j = 2; j >= 0; j--) {
+    const unsigned __int128 x = ((unsigned __int128)r << 64) | m[j];
+    m[j] = (unsigned long long)(x / d);
+    r = (unsigned long long)(x % d);
+  }
+  return r;
+}
+
+// the two's-complement 192-bit sum (top:mid:lo) -> its magnitude in m; returns the sign
+__device__ __forceinline__ bool dec_magnitude(unsigned long long (&m)[3], unsigned long long lo, unsigned long long mid, unsigned long long top) {
+  const bool neg = (long long)top < 0;
+  m[0] = lo; m[1] = mid; m[2] = top;
+  if (neg) {
+    m[0] = ~m[0] + 1ull;
+    unsigned long long c = m[0] == 0 ? 1ull : 0ull;
+    m[1] = ~m[1] + c;
+    c = (c && m[1] == 0) ? 1ull : 0ull;
+    m[2] = ~m[2] + c;
+  }
+  return neg;
+}
+
+// dec_store for a 192-bit integer part `ip` (magnitude, consumed).  ip < 2^184 has at most 56 digits, 7 words;
+// the callers' bounds keep ni + nfw <= 9 (dec3_sum_cell, dec3_avg_cell)
+__device__ __forceinline__ void dec3_store(uint8_t* cell, bool neg, unsigned long long (&ip)[3], const uint32_t* fw, int nfw, int frac) {
+  uint32_t iw[7];
+  int ni = 0;
+  do { iw[ni++] = (uint32_t)dec_divmod192(ip, TG_DEC_WORD_BASE); } while ((ip[0] | ip[1] | ip[2]) != 0 && ni < 7);
+  uint32_t c[10];
+  for (int j = 0; j < 10; j++) c[j] = 0;
+  c[0] = (uint32_t)(9 * ni) | ((uint32_t)frac << 8) | ((uint32_t)frac << 16) | ((neg ? 1u : 0u) << 24);
+  for (int j = 0; j < ni; j++) c[1 + j] = iw[ni - 1 - j];
+  for (int j = 0; j < nfw; j++) c[1 + ni + j] = fw[j];
+  unsigned long long* o = reinterpret_cast<unsigned long long*>(cell);   // cells are 8-byte aligned (40-byte stride)
+  for (int j = 0; j < 5; j++) o[j] = (unsigned long long)c[2 * j] | ((unsigned long long)c[2 * j + 1] << 32);
+}
+
+// ---- cells of a DECIMAL SUM / AVG of a product (k_agg_finalize<true, true>) ------------------------------------------
+// The same rules as dec_sum_cell / dec_avg_cell above, for the exact 192-bit two's-complement sum (top:mid:lo) of DECIMAL
+// products a * b / a * (c - b) at scale s = s_a + s_b <= 30.  They stay beside the 128-bit writers, which every other plan
+// keeps: the long division of three words costs registers (a kernel's count includes its callees').  Why every accepted
+// result fits MyDecimal's 9 words, so that fixWordCntError (mydecimal.go) never truncates a fraction word:
+//   SUM: |sum| < 2^184 has at most 56 digits.  Its integer part has at most 56 - scale of them, so
+//        ceil((56 - scale) / 9) + ceil(scale / 9) <= 8 words at any scale.
+//   AVG: |avg| = |sum| / n < 2 * 10^(36 - scale) (|a * t| < 10^18 * 2 * 10^18, in units of 10^-scale): at most 37 - scale
+//        integer digits, ceil((37 - scale) / 9) <= 5 words, and frac <= 30 gives at most 4 fraction words; 5 + 4 = 9 only
+//        at scale 0.
+
+// SUM: the integer part is |sum| / 10^scale; the remainder, left-aligned, gives the ceil(scale / 9) fraction words: the
+// last scale % 9 digits first (padded to a whole word), then whole words towards the point.
+__device__ __noinline__ void dec3_sum_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, int scale) {
+  unsigned long long m[3];
+  const bool neg = dec_magnitude(m, lo, mid, top);
+  const int aw = scale / 9, nfw = (scale + 8) / 9;   // scale <= 30
+  uint32_t fw[4] = {0, 0, 0, 0};
+  if (scale % 9) {
+    const uint32_t pb = dec_pow10(scale % 9);
+    fw[aw] = (uint32_t)dec_divmod192(m, pb) * (TG_DEC_WORD_BASE / pb);
+  }
+  for (int j = aw - 1; j >= 0; j--) fw[j] = (uint32_t)dec_divmod192(m, TG_DEC_WORD_BASE);
+  dec3_store(cell, neg, m, fw, nfw, scale);
+}
+
+// AVG: dec_avg_cell's rule (the truncation at 9 * ceil(frac / 9) digits derived there holds for any scale <= 30: a product
+// has digitsFrac s_a + s_b, so the sum does too).  q = m / n by 192-bit long division (n < 2^63); the integer part is
+// q / 10^scale, the fraction digits are the low `scale` digits of q, then the digits of r / n (r * 10^9 fits 128 bits).
+__device__ __noinline__ void dec3_avg_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, unsigned long long n, int scale, int frac) {
+  unsigned long long q[3];
+  const bool neg = dec_magnitude(q, lo, mid, top);
+  unsigned long long r = dec_divmod192(q, n);
+  const int nfw = (frac + 8) / 9;
+  uint32_t fw[4];   // frac <= 30
+  // the low `scale` digits of q: the last scale % 9 of them (`carry`) shift the words of r / n right by scale % 9 digits;
+  // the 9 * (scale / 9) before them are whole words (scale 0: no words, carry 0, the words of r / n as they are)
+  const int aw = scale / 9;
+  const unsigned long long pb = dec_pow10(scale % 9), lift = TG_DEC_WORD_BASE / pb;
+  unsigned long long carry = scale % 9 ? dec_divmod192(q, pb) : 0ull;
+  for (int j = aw - 1; j >= 0; j--) fw[j] = (uint32_t)dec_divmod192(q, TG_DEC_WORD_BASE);
+  for (int j = aw; j < nfw; j++) {
+    const unsigned __int128 x = (unsigned __int128)r * TG_DEC_WORD_BASE;
+    const unsigned long long e = (unsigned long long)(x / n);
+    r = (unsigned long long)(x % n);
+    fw[j] = (uint32_t)(carry * lift + e / pb);
+    carry = e % pb;
+  }
+  if (frac % 9) {   // Round, mydecimal.go:892-898: keep the word's first frac % 9 digits, half up on the next one
+    const uint32_t p = dec_pow10(9 - frac % 9 - 1);
+    unsigned long long sh = fw[nfw - 1] / p;
+    const unsigned long long dig = sh % 10;
+    if (dig >= 5) sh += 10;
+    unsigned long long w = (unsigned long long)p * (sh - dig);
+    int j = nfw - 1;
+    for (;;) {   // carry into the words before it and the integer part (999.99995 -> 1000.0000)
+      if (w < TG_DEC_WORD_BASE) { fw[j] = (uint32_t)w; break; }
+      fw[j] = (uint32_t)(w - TG_DEC_WORD_BASE);
+      if (--j < 0) { if (++q[0] == 0 && ++q[1] == 0) ++q[2]; break; }
+      w = (unsigned long long)fw[j] + 1;
+    }
+  }
+  bool zero = (q[0] | q[1] | q[2]) == 0;
+  for (int j = 0; j < nfw; j++) zero &= fw[j] == 0;
+  dec3_store(cell, neg && !zero, q, fw, nfw, frac);
+}
+
+// the one call k_agg_finalize<true, true> makes for a non-NULL product result (the scale, AVG's scale and the AVG flag in
+// one word `how` = scale | frac << 8 | avg << 16: fewer argument registers)
+__device__ __noinline__ void dec3_result_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, unsigned long long n, int how) {
+  const int scale = how & 0xff, frac = (how >> 8) & 0xff;
+  if (how >> 16) dec3_avg_cell(cell, lo, mid, top, n, scale, frac);
+  else dec3_sum_cell(cell, lo, mid, top, scale);
 }
 
 }  // namespace tg

@@ -164,11 +164,28 @@ class HashAggExec(Executor):
         self._out: Optional[MutChunk] = None
 
     @staticmethod
+    def _product_type(a: FieldType, b: FieldType, f) -> FieldType:
+        """DECIMAL(P, s) of a * b, or of a * (c - b) with the integer literal c (its flen = its digit count, scale 0):
+        minus has frac s_b and precision max(integer digits) + frac + 1; multiply has frac s_a + s_t and precision
+        (p_a - s_a) + (p_t - s_t) + frac; both capped at 65 digits / 30 fraction digits"""
+        t_flen, t_dec = b.flen, b.decimal
+        if f.arg_expr == abi.ARGEXPR_MUL_CSUB:
+            c_digits = len(str(abs(int(f.arg_const))))
+            t_dec = min(b.decimal, 30)
+            t_flen = min(max(c_digits, b.flen - b.decimal) + t_dec + 1, 65)
+        frac = min(a.decimal + t_dec, 30)
+        return FieldType(abi.TYPE_NEWDECIMAL, 0, min((a.flen - a.decimal) + (t_flen - t_dec) + frac, 65), frac)
+
+    @staticmethod
     def _ret_type(plan: AggPlan, f) -> FieldType:
         if f.name == abi.AGG_COUNT:
             return FieldType(abi.TYPE_LONGLONG, abi.FLAG_NOT_NULL)
         arg = plan.col_types[f.arg_col] if f.arg_col >= 0 else None
         if f.name in (abi.AGG_SUM, abi.AGG_AVG):
+            if arg is not None and arg.tp == abi.TYPE_NEWDECIMAL and f.ret_type == abi.TYPE_NEWDECIMAL and f.arg_expr != abi.ARGEXPR_COL:
+                # a * b or a * (c - b) over DECIMAL columns: the product's type (setFlenDecimal4RealOrDecimal,
+                # expression/builtin_arithmetic.go:106), then SUM / AVG over it as over a DECIMAL(P, s) column
+                arg = HashAggExec._product_type(arg, plan.col_types[f.arg_col2], f)
             if arg is not None and arg.tp == abi.TYPE_NEWDECIMAL and f.ret_type == abi.TYPE_NEWDECIMAL:
                 # typeInfer4Sum / typeInfer4Avg over DECIMAL(p, s) (aggregation/base_func.go:223, :274): SUM (p + 22, s),
                 # AVG (p + the scale increment, ret_frac), both at most 65 digits
