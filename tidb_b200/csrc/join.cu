@@ -135,6 +135,8 @@ struct JoinImpl {
   ColStore pcols_dev;
   DevBuf tmp_cnt, tmp_slot, tmp_off, tmp_sums, out_cursor;
   DevBuf part_scratch;                               // counts | cursors | offsets of the L2 partition pass
+  DevBuf tile_cnt;                                   // rows each 128-row tile keeps in the in-place segment probe
+  double seg_match = 1.0;                            // output / input rows of the last partitioned probe whose count the host read
   std::unique_ptr<DevBuf> part_cols[1 + TG_FAST_MAX_PCOLS];   // partitioned copies of the probe key and payload columns
   std::vector<std::unique_ptr<DevBuf>> tmp_valid;
   std::deque<std::unique_ptr<ResultBatch>> results;
@@ -496,7 +498,7 @@ static int composite_key(JoinImpl* j, const Side& s, const DevCols& v, int64_t n
 
 // ---- fast-path launch tuning (the defaults are the production choice; the overrides let tests and tools force the
 // partition pass, or no pass, on any input) ----
-struct ProbeTuning { int ctas_per_sm; bool partition; int parts; int part_min_mb; int part_min_rows; };
+struct ProbeTuning { int ctas_per_sm; bool partition; int parts; int part_min_mb; int part_min_rows; int inplace; };
 static ProbeTuning probe_tuning() {
   ProbeTuning t;
   t.ctas_per_sm = env_int("TG_PROBE_CTAS_PER_SM", 0);   // 0 = exactly the resident CTA count (occupancy query)
@@ -504,6 +506,7 @@ static ProbeTuning probe_tuning() {
   t.parts = env_int("TG_PROBE_PARTS", 0);           // 0 = auto (probe_slices), at most TG_MAX_PARTS
   t.part_min_mb = env_int("TG_PROBE_PART_MIN_MB", 64);
   t.part_min_rows = env_int("TG_PROBE_PART_MIN_ROWS", 1 << 22);
+  t.inplace = env_int("TG_PROBE_INPLACE", -1);      // -1 = by the last match fraction (kInplaceMinMatch), 0 / 1 = never / always
   return t;
 }
 
@@ -532,6 +535,11 @@ static int probe_slices(size_t table_bytes, int device, int parts_override) {
 // width 4 (tools/probe_slices.py --sweep shape, H100 at 400 W): load factor 0.5 4.30 ms (50 % match 4.51), 0.6 4.66 (5.57),
 // 0.7 5.47 (7.80), against 4.80 (4.40) for the 0.35 table the build used to keep
 static const double kMaxDenseLoad = 0.5;
+// The in-place segment probe (probe_device) is taken while the last partitioned call of the handle matched at least this
+// fraction of its rows: below it, tiles with misses are compacted and the hole fill moves more rows.  bench.py's join
+// forced in place / not (tools/probe_slices.py --sweep match, H100 SXM at 700 W): 100 % match 3.63 / 4.25 ms, 99.9 % 3.79 /
+// 4.34, 99 % 4.63 / 4.35, 50 % 5.63 / 4.33.
+static const double kInplaceMinMatch = 0.995;
 
 // ---- build --------------------------------------------------------------------------------------------
 static int build_table(JoinImpl* j) {
@@ -730,7 +738,8 @@ static void fill_outspec_probe(const JoinImpl* j, OutCols& oc) {
   }
 }
 
-static int scan_counts(JoinImpl* j, int64_t n, unsigned long long* total_out) {
+// exclusive scan of the n counts in tmp_cnt into tmp_off (n + 1 entries), enqueued only; returns the block count
+static int enqueue_scan(JoinImpl* j, int64_t n, int64_t* nblocks_out) {
   int64_t nblocks = (n + TG_SCAN_BLOCK * TG_SCAN_ITEMS - 1) / (TG_SCAN_BLOCK * TG_SCAN_ITEMS);
   TG_TRY(j->tmp_sums.ensure(j->device, (size_t)(nblocks + 2) * 8));
   TG_TRY(j->tmp_off.ensure(j->device, (size_t)(n + 2) * 8));
@@ -739,6 +748,13 @@ static int scan_counts(JoinImpl* j, int64_t n, unsigned long long* total_out) {
   k_scan_write<<<(unsigned)nblocks, TG_SCAN_BLOCK, 0, j->stream>>>(j->tmp_cnt.as<uint32_t>(), n, j->tmp_sums.as<unsigned long long>(),
                                                                   j->tmp_off.as<unsigned long long>());
   j->stats.kernel_launches += 3;
+  *nblocks_out = nblocks;
+  return TG_OK;
+}
+
+static int scan_counts(JoinImpl* j, int64_t n, unsigned long long* total_out) {
+  int64_t nblocks = 0;
+  TG_TRY(enqueue_scan(j, n, &nblocks));
   TG_CUDA(cudaMemcpyAsync(total_out, j->tmp_sums.as<unsigned long long>() + nblocks, 8, cudaMemcpyDeviceToHost, j->stream));
   TG_CUDA(cudaStreamSynchronize(j->stream));
   return TG_OK;
@@ -849,6 +865,26 @@ struct LaunchSeg {
     return TG_OK;
   }
 };
+template <int NPC, int NKD, int NMD>
+struct LaunchInplace {
+  static int run(JoinImpl* j, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t, const SegSpec& seg, uint32_t* tile_cnt) {
+    if constexpr (NKD == 0) {
+      return fail(TG_ERR_CUDA, "internal: the in-place segment probe needs an output fed by the join key");
+    } else {
+      static int resident = 0;
+      if (!resident) {
+        int nb = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_probe_inner_u1_seg_inplace<NPC, NKD, NMD>, 256, 0) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 3; }
+        resident = nb;
+      }
+      int64_t ctas = (n / 128 + 7) / 8;
+      int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
+      int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
+      k_probe_inner_u1_seg_inplace<NPC, NKD, NMD><<<grid, 256, 0, j->stream>>>(n, j->tv, fo, cur, seg, tile_cnt);
+      return TG_OK;
+    }
+  }
+};
 static int launch_probe_warp(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t,
                              const SegSpec& seg = SegSpec{nullptr, 0, 0, 0, nullptr}) {
   j->stats.paths |= TG_JOIN_PATH_PROBE_DIRECT;
@@ -879,64 +915,89 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
   const bool fast = fast_path_ok(j, pview) && build_fast_out(j, oc, pview, fo);
   if (in_seg && !fast) return fail(TG_ERR_UNSUPPORTED, "segmented device chunks are only accepted by the fused fast path (unique build keys, <= 1 payload, no filters, an output shape the warp kernels cover)");
   if (fast) {
-    TG_TRY(ensure_result(j, rb, rb.rows + n, rb.rows > 0, rb.rows));
+    const ProbeTuning& tune = probe_tuning();
+    const int64_t* pkey = reinterpret_cast<const int64_t*>(ks.data);
+    const size_t table_bytes = (size_t)j->tv.nslots * sizeof(Slot);
+    bool src16 = aligned16(pkey);
+    for (int c = 0; c < fo.n_pcols; c++) src16 = src16 && aligned16(fo.psrc[c]);
+    const int64_t PTILE = 1024;   // rows per scatter tile (k_partition_scatter_bulk<.., 4>)
+    const int64_t n_main = n / PTILE * PTILE;
+    // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments of C rows.
+    // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
+    // [p/P, (p+1)/P) while the probe kernel sweeps the segment.  The pass trades 32 B/row of extra streaming traffic for
+    // random HBM traffic, which only pays while a slice stays L2 resident (probe_slices; U1 tables are built dense
+    // enough for that, build_table).  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
+    // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
+    int P = 0;
+    int64_t C = 0;
+    if (n > 0 && tune.partition && src16 && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
+      P = probe_slices(table_bytes, j->device, tune.parts);
+      C = ((int64_t)((double)n_main / P * 1.05) + 16384 + 127) / 128 * 128;
+      if (!(P >= 2 && (int64_t)P * C / 128 < (1ll << 31))) P = 0;
+    }
+    // In place (k_probe_inner_u1_seg_inplace): the scatter writes the probe columns straight into the output columns, which
+    // then take the segment layout, P·C rows.  It moves fewer bytes than the lean segment probe only when nearly every
+    // 128-row tile matches in full, so it follows the match fraction of the last partitioned call whose count the host read
+    // (the first call takes it); a mispredicted call is slower, never wrong.  Dense input and a fresh batch only: the
+    // segment layout starts at the allocation.
+    const bool inplace = P && !in_seg && rb.rows == 0 && fo.n_key_dst >= 1 &&
+                         (tune.inplace >= 0 ? tune.inplace != 0 : j->seg_match >= kInplaceMinMatch);
+    TG_TRY(ensure_result(j, rb, inplace ? std::max<int64_t>(n, (int64_t)P * C) : rb.rows + n, rb.rows > 0, rb.rows));
     for (int c = 0; c < j->n_out; c++) { oc.data[c] = rb.cols[c]->as<uint8_t>() + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
     build_fast_out(j, oc, pview, fo);
     unsigned long long* cur = j->out_cursor.as<unsigned long long>();
     TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
     if (n > 0) {
-      const ProbeTuning& tune = probe_tuning();
-      const int64_t* pkey = reinterpret_cast<const int64_t*>(ks.data);
-      size_t table_bytes = (size_t)j->tv.nslots * sizeof(Slot);
-      bool partitioned = false;   // the L2 partition pass + segment probe took the whole call
-      bool src16 = aligned16(pkey);
-      for (int c = 0; c < fo.n_pcols; c++) src16 = src16 && aligned16(fo.psrc[c]);
-      const int64_t PTILE = 1024;   // rows per scatter tile (k_partition_scatter_bulk<.., 4>)
-      if (tune.partition && src16 && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
-        // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments.
-        // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
-        // [p/P, (p+1)/P) while the probe kernel sweeps the segment.  The pass trades 32 B/row of extra streaming traffic for
-        // random HBM traffic, which only pays while a slice stays L2 resident (probe_slices; U1 tables are built dense
-        // enough for that, build_table).  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
-        // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
-        const int P = probe_slices(table_bytes, j->device, tune.parts);
-        const int64_t n_main = n / PTILE * PTILE;
+      if (P) {
         const int nc = 1 + fo.n_pcols;
-        // one segment of C rows per partition, filled through global cursors
-        const int64_t C = ((int64_t)((double)n_main / P * 1.05) + 16384 + 127) / 128 * 128;
-        if (P >= 2 && (int64_t)P * C / 128 < (1ll << 31)) {
+        if (!inplace) {
           for (int c = 0; c < nc; c++) {
             if (!j->part_cols[c]) j->part_cols[c].reset(new DevBuf());
             TG_TRY(j->part_cols[c]->ensure(j->device, (size_t)P * C * 8 + 64));
           }
-          TG_TRY(j->part_scratch.ensure(j->device, (size_t)3 * TG_MAX_PARTS * 8 + 64));
-          unsigned long long* cursors = j->part_scratch.as<unsigned long long>();     // fill count per segment
-          long long* bases = reinterpret_cast<long long*>(cursors + TG_MAX_PARTS);   // first row of each segment
-          unsigned long long* flag = cursors + 2 * TG_MAX_PARTS;                      // overflow
-          PartDst d{};
-          d.nparts = P; d.ncols = nc;
-          d.src[0] = pkey;
-          for (int c = 0; c < fo.n_pcols; c++) d.src[1 + c] = fo.psrc[c];
-          for (int c = 0; c < nc; c++) for (int q = 0; q < P; q++) d.dst[q][c] = j->part_cols[c]->p;
-          k_segment_bases<<<1, 32, 0, j->stream>>>(cursors, bases, flag, P, C);
-          d.dst_base = bases; d.capacity = C; d.overflow = flag;
-          if (in_seg) { d.in_cnt = in_seg->cnt; d.in_cap = in_seg->cap; d.in_tiles_per_seg = (uint32_t)(in_seg->cap / PTILE); }
-          TG_TRY(launch_partition_scatter<true>(j->device, j->stream, reinterpret_cast<const long long*>(pkey), nullptr, n_main, d, cursors,
-                                                &j->stats.kernel_launches, 0, &j->stats.paths));
+        }
+        TG_TRY(j->part_scratch.ensure(j->device, (size_t)3 * TG_MAX_PARTS * 8 + 64));
+        unsigned long long* cursors = j->part_scratch.as<unsigned long long>();     // fill count per segment
+        long long* bases = reinterpret_cast<long long*>(cursors + TG_MAX_PARTS);   // first row of each segment
+        unsigned long long* flag = cursors + 2 * TG_MAX_PARTS;                      // overflow
+        PartDst d{};
+        d.nparts = P; d.ncols = nc;
+        d.src[0] = pkey;
+        for (int c = 0; c < fo.n_pcols; c++) d.src[1 + c] = fo.psrc[c];
+        for (int c = 0; c < nc; c++)
+          for (int q = 0; q < P; q++) d.dst[q][c] = inplace ? (c == 0 ? (void*)fo.key_dst[0] : (void*)fo.pdst[c - 1]) : j->part_cols[c]->p;
+        k_segment_bases<<<1, 32, 0, j->stream>>>(cursors, bases, flag, P, C);
+        d.dst_base = bases; d.capacity = C; d.overflow = flag;
+        if (in_seg) { d.in_cnt = in_seg->cnt; d.in_cap = in_seg->cap; d.in_tiles_per_seg = (uint32_t)(in_seg->cap / PTILE); }
+        TG_TRY(launch_partition_scatter<true>(j->device, j->stream, reinterpret_cast<const long long*>(pkey), nullptr, n_main, d, cursors,
+                                              &j->stats.kernel_launches, 0, &j->stats.paths));
+        const SegSpec seg{cursors, (uint32_t)(C / 128), 0, C, flag};
+        if (inplace) {
+          // probe in place, then make the output dense: the rows at or beyond R = *cur fill the holes below R
+          const int64_t ntiles = (int64_t)P * C / 128;
+          TG_TRY(j->tile_cnt.ensure(j->device, (size_t)ntiles * 4 + 16));
+          TG_TRY(j->tmp_cnt.ensure(j->device, (size_t)(2 * ntiles + 1) * 4));
+          j->stats.paths |= TG_JOIN_PATH_PROBE_SEG;
+          TG_TRY(dispatch_shape<LaunchInplace>(fo, j, (int64_t)P * C, fo, cur, tune, seg, j->tile_cnt.as<uint32_t>()));
+          k_inplace_holes<<<grid_for(j, ntiles, 256, 4), 256, 0, j->stream>>>(j->tile_cnt.as<uint32_t>(), ntiles, cur, flag, j->tmp_cnt.as<uint32_t>());
+          int64_t nblocks = 0;
+          TG_TRY(enqueue_scan(j, 2 * ntiles, &nblocks));
+          k_inplace_fill<<<j->nsm * 8, 256, 0, j->stream>>>(j->tile_cnt.as<uint32_t>(), ntiles, j->tmp_off.as<unsigned long long>(), cur, flag, fo);
+          j->stats.kernel_launches += 3;
+        } else {
           FastOut pf = fo;
           for (int c = 0; c < fo.n_pcols; c++) pf.psrc[c] = j->part_cols[1 + c]->as<unsigned long long>();
           // the 128-bit stores of the segment kernel need 16-byte aligned output columns: every caller passes a fresh
           // batch (rb.rows == 0), so the columns start at the allocation
-          TG_TRY(launch_probe_seg(j, j->part_cols[0]->as<int64_t>(), (int64_t)P * C, pf, cur, tune, SegSpec{cursors, (uint32_t)(C / 128), 0, C, flag}));
-          // gated fallback: probes the ORIGINAL input only after an overflow; the < 1024-row tail the scatter left behind
-          // (dense input only) rides on the same launch — it is probed whatever the flag says
-          if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n_main, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 1, in_seg->cap, flag, 0}));
-          else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{nullptr, 0, 1, 0, flag, n_main < n ? n_main : 0}));
-          j->stats.kernel_launches += 3;
-          partitioned = true;
+          TG_TRY(launch_probe_seg(j, j->part_cols[0]->as<int64_t>(), (int64_t)P * C, pf, cur, tune, seg));
+          j->stats.kernel_launches++;
         }
-      }
-      if (!partitioned) {
+        // gated fallback: probes the ORIGINAL input only after an overflow; the < 1024-row tail the scatter left behind
+        // (dense input only) rides on the same launch — it is probed whatever the flag says, and appended at R
+        if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n_main, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 1, in_seg->cap, flag, 0}));
+        else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{nullptr, 0, 1, 0, flag, n_main < n ? n_main : 0}));
+        j->stats.kernel_launches += 2;
+      } else {
         if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 0, in_seg->cap, nullptr}));
         else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune));
         j->stats.kernel_launches++;
@@ -948,6 +1009,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
       TG_CUDA(cudaStreamSynchronize(j->stream));
       rb.rows += (int64_t)got;
       j->stats.output_rows += (int64_t)got;
+      if (P && n > 0) j->seg_match = (double)got / (double)n;
     }
     return TG_OK;
   }

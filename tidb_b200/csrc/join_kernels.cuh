@@ -661,6 +661,237 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
 // L1 gather issue, every KB of shared memory such a ring holds costs L1, and it would add 96 instantiations to the library.
 // tools/scratch/probe_lab.cu keeps the experiment.)
 
+// ---------------------------------------------------------------------------------------------
+// In-place segment probe (dense input, fresh output batch, at least one output fed by the join key): the partition pass
+// has scattered the probe key into out.key_dst[0] and the probe payloads into out.pdst[c], in segment layout.  A warp owns
+// 128-row tiles, as in k_probe_inner_u1_seg_lean.  A tile whose 128 rows all match stays where it is: the kernel reads its
+// keys and writes only key_dst[1..NKD) and the build payload, 8 + 8·(NKD-1+NMD) bytes per row instead of the lean kernel's
+// 8·(1+NPC) read and 8·(NKD+NMD+NPC) written.  Any other tile (misses, a segment's partial last tile, sentinel-valued
+// keys) is compacted to its front; the warp holds the whole tile in registers before the __syncwarp that precedes its
+// stores, so it may overwrite its own rows.  tile_cnt[t] = rows tile t keeps (every tile is written); the warp adds its
+// total to the output cursor once.  The output is dense in [0, *out_cursor) after k_inplace_holes + scan + k_inplace_fill.
+// ---------------------------------------------------------------------------------------------
+template <int NPC, int NKD, int NMD>
+__device__ __forceinline__ void inplace_store(int64_t base, const int64_t (&k)[4], const unsigned long long (&meta)[4],
+                                              const unsigned long long (&pv)[4][NPC > 0 ? NPC : 1], const unsigned (&bal)[4],
+                                              const FastOut& out, int lane) {
+  __syncwarp();   // every lane's loads of this tile precede any store into it
+  int64_t o = base;
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    if ((bal[j] >> lane) & 1u) {
+      const int64_t r = o + __popc(bal[j] & ((1u << lane) - 1));
+#pragma unroll
+      for (int d = 0; d < NKD; d++) __stcs(out.key_dst[d] + r, (unsigned long long)k[j]);
+#pragma unroll
+      for (int d = 0; d < NMD; d++) __stcs(out.meta_dst[d] + r, meta[j]);
+#pragma unroll
+      for (int c = 0; c < NPC; c++) __stcs(out.pdst[c] + r, pv[j][c]);
+    }
+    o += __popc(bal[j]);
+  }
+}
+
+// the probe payloads of a tile's rows (lane owns rows 2·lane, 2·lane+1 of each 64-row group)
+template <int NPC>
+__device__ __forceinline__ void inplace_load_pv(int64_t base, const FastOut& out, unsigned long long (&pv)[4][NPC > 0 ? NPC : 1], int lane) {
+#pragma unroll
+  for (int g = 0; g < 2; g++) {
+    const int64_t i = base + g * 64 + 2 * lane;
+#pragma unroll
+    for (int c = 0; c < NPC; c++) {
+      const ulonglong2 pp = __ldcs(reinterpret_cast<const ulonglong2*>(out.pdst[c] + i));
+      pv[2 * g][c] = pp.x; pv[2 * g + 1][c] = pp.y;
+    }
+  }
+}
+
+// a tile with rows past the segment's fill count or sentinel-valued keys: per-row `in` flags, side slot, compaction
+template <int NPC, int NKD, int NMD>
+__device__ __forceinline__ uint32_t inplace_tile_generic(int64_t base, int64_t limit, const TableView& t, const FastOut& out, int lane) {
+  constexpr int R = 4;
+  int64_t k[R];
+  unsigned long long pv[R][NPC > 0 ? NPC : 1], meta[R];
+  bool in[R];
+#pragma unroll
+  for (int g = 0; g < R / 2; g++) {
+    const int64_t i = base + g * 64 + 2 * lane;
+    const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(out.key_dst[0] + i));
+    in[2 * g] = i < limit; in[2 * g + 1] = i + 1 < limit;
+    k[2 * g] = in[2 * g] ? (int64_t)kk.x : kEmptyKey;
+    k[2 * g + 1] = in[2 * g + 1] ? (int64_t)kk.y : kEmptyKey;
+  }
+  inplace_load_pv<NPC>(base, out, pv, lane);
+  unsigned bal[R];
+  uint32_t total = 0;
+#pragma unroll
+  for (int j = 0; j < R; j++) {
+    const unsigned long long sl = (k[j] == kEmptyKey) ? t.nslots : home_slot(hash64((uint64_t)k[j]), t.nslots);
+    Slot v, w;
+    load_pair(t.slots + sl, v, w);
+    bool m;
+    meta[j] = v.meta;
+    if (k[j] == kEmptyKey) m = in[j] && v.key != 0;
+    else if (v.key == k[j]) m = true;
+    else if (w.key == k[j]) { meta[j] = w.meta; m = true; }
+    else if (v.key == kEmptyKey || w.key == kEmptyKey) m = false;
+    else m = probe_run(t.slots, t.nslots, k[j], sl + 2, meta[j]);
+    bal[j] = __ballot_sync(0xffffffffu, m);
+    total += __popc(bal[j]);
+  }
+  inplace_store<NPC, NKD, NMD>(base, k, meta, pv, bal, out, lane);
+  return total;
+}
+
+template <int NPC, int NKD, int NMD>
+__global__ void __launch_bounds__(256, 3)
+k_probe_inner_u1_seg_inplace(int64_t n, TableView t, FastOut out, unsigned long long* __restrict__ out_cursor, SegSpec seg,
+                             uint32_t* __restrict__ tile_cnt) {
+  static_assert(NKD >= 1, "the probe key is read from the first key destination");
+  constexpr int R = 4, G = 2, NP = NPC > 0 ? NPC : 1;
+  if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) return;
+  const int lane = threadIdx.x & 31;
+  const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const int64_t warp_id = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t ntiles = n / 128;
+  const int64_t* __restrict__ pkey = reinterpret_cast<const int64_t*>(out.key_dst[0]);
+  unsigned long long kept = 0;
+  for (int64_t tile = warp_id; tile < ntiles; tile += warps_total) {
+    const int64_t base = tile * 128;
+    const uint32_t p = (uint32_t)tile / seg.tiles_per_seg;
+    const unsigned long long c = seg.cnt[p];
+    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+    uint32_t m = 0;
+    if (limit - base >= 128) {
+      int64_t k[R];
+#pragma unroll
+      for (int g = 0; g < G; g++) {
+        const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + base + g * 64 + 2 * lane));
+        k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
+      }
+      const bool sentinel = (k[0] == kEmptyKey) | (k[1] == kEmptyKey) | (k[2] == kEmptyKey) | (k[3] == kEmptyKey);
+      if (__any_sync(0xffffffffu, sentinel)) {
+        m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
+      } else {
+        // gather and run walk exactly as k_probe_inner_u1_seg_lean
+        Slot v[R], w[R];
+#pragma unroll
+        for (int j = 0; j < R; j++) load_pair(t.slots + home_slot(hash64((uint64_t)k[j]), t.nslots), v[j], w[j]);
+        unsigned long long meta[R];
+        unsigned hit = 0, run = 0;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+          meta[j] = 0;
+          if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; }
+          else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; }
+          else if (v[j].key != kEmptyKey && w[j].key != kEmptyKey) run |= 1u << j;
+        }
+        if (run) {
+          uint32_t sl[R];
+#pragma unroll
+          for (int j = 0; j < R; j++) {
+            const unsigned long long s = home_slot(hash64((uint64_t)k[j]), t.nslots) + 2;
+            sl[j] = s == t.nslots ? 0u : (uint32_t)s;
+          }
+          do {
+#pragma unroll
+            for (int j = 0; j < R; j++) if ((run >> j) & 1u) load_pair(t.slots + sl[j], v[j], w[j]);
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+              if (!((run >> j) & 1u)) continue;
+              if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; run &= ~(1u << j); }
+              else if (v[j].key == kEmptyKey) run &= ~(1u << j);
+              else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; run &= ~(1u << j); }
+              else if (w[j].key == kEmptyKey) run &= ~(1u << j);
+              else { sl[j] += 2; if (sl[j] == t.nslots) sl[j] = 0; }
+            }
+          } while (run);
+        }
+        if (__all_sync(0xffffffffu, hit == 0xFu)) {
+          // every row matched: the probe columns are already in place
+          m = 128;
+#pragma unroll
+          for (int g = 0; g < G; g++) {
+            const int64_t o = base + g * 64 + 2 * lane;
+            const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
+#pragma unroll
+            for (int d = 1; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
+#pragma unroll
+            for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
+          }
+        } else {
+          unsigned long long pv[R][NP];
+          inplace_load_pv<NPC>(base, out, pv, lane);
+          unsigned bal[R];
+#pragma unroll
+          for (int j = 0; j < R; j++) {
+            bal[j] = __ballot_sync(0xffffffffu, (hit >> j) & 1u);
+            m += __popc(bal[j]);
+          }
+          inplace_store<NPC, NKD, NMD>(base, k, meta, pv, bal, out, lane);
+        }
+      }
+    } else if (limit > base) {
+      m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
+    }
+    if (lane == 0) tile_cnt[tile] = m;
+    kept += m;
+  }
+  if (lane == 0 && kept) atomicAdd(out_cursor, kept);
+}
+
+// Hole fill behind k_probe_inner_u1_seg_inplace, R = *out_cursor: tile t keeps rows [128t, 128t + m_t).  cnt[t] = its holes
+// below R, [128t + m_t, min(128t + 128, R)); cnt[ntiles + t] = its kept rows at or beyond R.  Both sum to the same total;
+// one exclusive scan over the 2·ntiles counts numbers the holes and the rows that fill them.
+__global__ void __launch_bounds__(256)
+k_inplace_holes(const uint32_t* __restrict__ tile_cnt, int64_t ntiles, const unsigned long long* out_cursor,
+                const unsigned long long* gate, uint32_t* __restrict__ cnt) {
+  if (*gate) return;
+  const int64_t R = (int64_t)*out_cursor;
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < ntiles; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t s = t * 128, e = s + tile_cnt[t];
+    cnt[t] = e < R ? (uint32_t)((s + 128 < R ? s + 128 : R) - e) : 0u;
+    cnt[ntiles + t] = e > R ? (uint32_t)(e - (s > R ? s : R)) : 0u;
+  }
+}
+
+// largest u in [lo, hi] with off[u] <= k (off non-decreasing, off[lo] <= k)
+__device__ __forceinline__ int64_t last_le(const unsigned long long* __restrict__ off, int64_t lo, int64_t hi, unsigned long long k) {
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if (off[mid] <= k) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// the k-th kept row at or beyond R moves into the k-th hole below R, every output column; a warp takes one tile's rows
+__global__ void __launch_bounds__(256)
+k_inplace_fill(const uint32_t* __restrict__ tile_cnt, int64_t ntiles, const unsigned long long* __restrict__ off,
+               const unsigned long long* out_cursor, const unsigned long long* gate, FastOut out) {
+  if (*gate) return;
+  const int lane = threadIdx.x & 31;
+  const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const int64_t warp_id = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t R = (int64_t)*out_cursor;
+  const unsigned long long holes = off[ntiles];
+  if (!holes) return;
+  for (int64_t t = R / 128 + warp_id; t < ntiles; t += warps_total) {
+    const uint32_t c = (uint32_t)(off[ntiles + t + 1] - off[ntiles + t]);
+    if (!c) continue;
+    const unsigned long long k0 = off[ntiles + t] - holes;
+    const int64_t first = t * 128 > R ? t * 128 : R;
+    const int64_t lo = last_le(off, 0, ntiles - 1, k0), hi = last_le(off, lo, ntiles - 1, k0 + c - 1);
+    for (uint32_t r = lane; r < c; r += 32) {
+      const unsigned long long k = k0 + r;
+      const int64_t u = last_le(off, lo, hi, k);
+      const int64_t dst = u * 128 + tile_cnt[u] + (int64_t)(k - off[u]), src = first + r;
+      for (int d = 0; d < out.n_key_dst; d++) out.key_dst[d][dst] = out.key_dst[d][src];
+      for (int d = 0; d < out.n_meta_dst; d++) out.meta_dst[d][dst] = out.meta_dst[d][src];
+      for (int c2 = 0; c2 < out.n_pcols; c2++) out.pdst[c2][dst] = out.pdst[c2][src];
+    }
+  }
+}
+
 // OtherCondition on ONE candidate pair (probe row i, build row `brow` of the row store): true iff every CNF item is
 // non-NULL true (expression.VectorizedFilter over the joined chunk, inner_join_probe.go:72-79)
 __device__ __forceinline__ bool other_operand(const OtherItemDev& it, bool lhs, const DevCols& pcols, int64_t i, const unsigned long long* brow,

@@ -7,6 +7,9 @@ factors can be read off one run.
   python tools/probe_slices.py --sweep slice --out DIR     2.5 M build rows at load factor 0.35, P = 4, 8, 16
   python tools/probe_slices.py --sweep shape --out DIR     10 M build rows at load factors 0.35 .. 0.8, P = 16 and no pass
   python tools/probe_slices.py --lf 0.7 --parts 16 ...     one point (any axis takes a comma-separated list)
+  python tools/probe_slices.py --sweep match --profile DIR  the bench shape at 100 .. 50 % match, in-place segment probe
+                                                           forced on and off (TG_PROBE_INPLACE): where the automatic
+                                                           choice should switch (join.cu: kInplaceMinMatch)
   --profile DIR                                            one more pass per point under torch.profiler: time per kernel
 
 Every point prints one JSON line: step time at 100 % match and at 50 % match (the keys of bench.py's side line), table
@@ -27,6 +30,7 @@ SWEEPS = {   # (build rows, load factors, parts; 0 = the library's own choice, -
     "slice": (2_500_000, "0.35", "4,8,16"),
     "shape": (10_000_000, "0.35,0.5,0.7,0.8", "16,-1"),
 }
+MATCHES = (1.0, 0.999, 0.99, 0.98, 0.95, 0.5)
 
 
 def card():
@@ -70,9 +74,44 @@ def profile(j, stream, cols, steps):
     return dict(sorted(out.items(), key=lambda kv: -kv[1]))
 
 
+def sweep_match(a, info, sinks):
+    """bench.py's join at several match fractions, in-place segment probe forced on (1) and off (0): step time and, with
+    --profile, ms per kernel"""
+    nb = a.build_rows or 10_000_000
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    with torch.cuda.stream(stream):
+        bk, bv, _, pv = gen_local(torch, dev, 0, 1, nb, a.probe_rows)
+    j = DeviceJoin(make_plan(0, stream.cuda_stream))
+    with torch.cuda.stream(stream):
+        j.build([bk, bv])
+    for m in MATCHES:
+        with torch.cuda.stream(stream):
+            g = torch.Generator(device=dev); g.manual_seed(4343)
+            ids = torch.randint(0, nb, (a.probe_rows,), device=dev, generator=g, dtype=torch.int64)
+            ids = torch.where(torch.rand(a.probe_rows, device=dev, generator=g) < m, ids, ids + nb)   # id >= nb: a miss
+            want = int((ids < nb).sum().item())
+            pk = ids * ODD
+            del ids
+        for mode in ("1", "0"):
+            os.environ["TG_PROBE_INPLACE"] = mode
+            with torch.cuda.stream(stream):
+                rows, _, _ = j.probe([pk, pv], sync=True)
+            assert rows == want, (m, mode, rows, want)
+            rec = dict(match=m, inplace=mode == "1", probe_rows=a.probe_rows, build_rows=nb, ms=round(timed(j, stream, [pk, pv], a.steps), 3), **info)
+            print(json.dumps(rec), flush=True)
+            if sinks[0]:
+                sinks[0].write(json.dumps(rec) + "\n"); sinks[0].flush()
+            if a.profile:
+                sinks[1].write(json.dumps(dict(match=m, inplace=mode == "1", kernels_ms=profile(j, stream, [pk, pv], a.steps))) + "\n"); sinks[1].flush()
+        del pk
+    j.close()
+    os.environ.pop("TG_PROBE_INPLACE", None)
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--sweep", choices=sorted(SWEEPS), default=None)
+    ap.add_argument("--sweep", choices=sorted(SWEEPS) + ["match"], default=None)
     ap.add_argument("--build-rows", type=int, default=None)
     ap.add_argument("--probe-rows", type=int, default=100_000_000)
     ap.add_argument("--lf", default=None, help="load factors; 0 = the library default")
@@ -81,11 +120,18 @@ def main():
     ap.add_argument("--profile", default=None, metavar="DIR", help="also write DIR/profile.jsonl: ms per step of every kernel")
     ap.add_argument("--out", default=None, metavar="DIR", help="also append the JSON lines to DIR/probe_slices.jsonl")
     a = ap.parse_args()
+    info = card()
+    sinks = []
+    for d, name in ((a.out, "probe_slices.jsonl"), (a.profile, "profile.jsonl")):
+        if d:
+            os.makedirs(d, exist_ok=True)
+        sinks.append(open(os.path.join(d, name), "a") if d else None)
+    if a.sweep == "match":
+        return sweep_match(a, info, sinks)
     nb, lfs, parts = SWEEPS[a.sweep] if a.sweep else (10_000_000, "0", "0")
     nb = a.build_rows or nb
     lfs, parts = a.lf or lfs, a.parts or parts
     L = lambda s, f: [f(x) for x in s.split(",")]
-    info = card()
     dev = torch.device("cuda", 0)
     stream = torch.cuda.Stream(device=dev)
     l2 = torch.cuda.get_device_properties(dev).L2_cache_size
@@ -97,11 +143,6 @@ def main():
         rows50 = int((ids2 < nb).sum().item())
         del ids2
     stream.synchronize()
-    sinks = []
-    for d, name in ((a.out, "probe_slices.jsonl"), (a.profile, "profile.jsonl")):
-        if d:
-            os.makedirs(d, exist_ok=True)
-        sinks.append(open(os.path.join(d, name), "a") if d else None)
     for lf in L(lfs, float):
         plan = make_plan(0, stream.cuda_stream)
         if lf:
