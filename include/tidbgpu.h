@@ -495,7 +495,9 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
  * in-process analogue: partitionHashSplitter.split, pkg/executor/shuffle.go:450).
  * Device-resident: scatter `ncols` 8-byte columns of `rows` rows into `nparts` contiguous
  * regions by hash(key) (bits disjoint from the local table slot bits).  part_offsets receives
- * nparts+1 row offsets (device int64).  dst columns have capacity `rows`.
+ * nparts+1 row offsets (device int64).  dst columns have capacity `rows`.  key_nulls_dev (bit 1 =
+ * NOT NULL, LSB first; NULL = no NULL keys) only routes rows: a NULL key at row i goes to the
+ * partition of hash(i).  No null bitmap is moved.
  * ------------------------------------------------------------------------------------------- */
 int tg_partition_by_key(int device, const int64_t* key_dev, const uint8_t* key_nulls_dev,
                         int64_t rows, int32_t nparts, int32_t ncols,
@@ -515,7 +517,8 @@ int tg_partition_exchange(int device, const int64_t* key_dev, int64_t rows, int3
 /* Count-free variant (no histogram pass, no host round trip): every destination p owns, inside each receiver's
  * buffers, the fixed-capacity region [region_base, region_base + region_cap) reserved for THIS sender; rows are
  * appended there in arrival order and sent_rows_dev[p] (device, zeroed by the call) ends up holding how many rows went
- * to p.  A destination that would overflow raises *overflow_dev (device u64, sticky: the caller zeroes it once) and drops the excess —
+ * to p.  sent_rows_dev[p] counts the rows destined to p, which can exceed region_cap; it is not the number of rows stored
+ * there (receivers clamp it to region_cap).  A destination that would overflow raises *overflow_dev (device u64, sticky: the caller zeroes it once) and drops the excess —
  * the caller re-runs that step through tg_partition_count + tg_partition_exchange.  Returns after ENQUEUEING on `stream`.
  * The MPP analogue is still ExchangeSender/HashPartition (physical_exchange_sender.go:115); the reference sizes
  * its per-partition chunks dynamically on the host (shuffle.go:450), which a single GPU kernel cannot.            */

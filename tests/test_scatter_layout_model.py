@@ -4,7 +4,8 @@ The kernel parks the run of destination p at a shared-memory offset whose parity
 row, so that the 16-byte aligned middle of the run can leave as one cp.async.bulk store (both addresses 16-byte aligned, size
 a multiple of 16) and at most one head and one tail element go out as scalar stores.  This test restates the index arithmetic
 (same expressions, same names) and checks the invariants for random cursor positions and counts; it documents the layout
-and catches an edit that breaks it — the kernel itself is exercised by the -m gpu parity tests."""
+and catches an edit that breaks it — the kernel itself, with its head / tail stores, truncated runs and spill area, is
+exercised on one GPU by tests/test_gpu_partition_exchange.py."""
 import numpy as np
 
 
