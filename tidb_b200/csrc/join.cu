@@ -4,6 +4,7 @@
 #include <memory>
 #include <deque>
 #include <algorithm>
+#include <cmath>
 #include <condition_variable>
 #include "join_kernels.cuh"
 #include "partition_kernels.cuh"
@@ -137,6 +138,10 @@ struct JoinImpl {
   DevBuf part_scratch;                               // counts | cursors | offsets of the L2 partition pass
   DevBuf tile_cnt;                                   // rows each 128-row tile keeps in the in-place segment probe
   double seg_match = 1.0;                            // output / input rows of the last partitioned probe whose count the host read
+  // the fills of that probe's segments, for the in-place segment capacity (inplace_seg_cap): its P (0 = nothing learned:
+  // no such call yet, or it overflowed a segment), the rows it scattered and its largest segment fill
+  int seg_parts = 0;
+  int64_t seg_rows = 0, seg_fill_max = 0;
   std::unique_ptr<DevBuf> part_cols[1 + TG_FAST_MAX_PCOLS];   // partitioned copies of the probe key and payload columns
   std::vector<std::unique_ptr<DevBuf>> tmp_valid;
   std::deque<std::unique_ptr<ResultBatch>> results;
@@ -541,6 +546,23 @@ static const double kMaxDenseLoad = 0.5;
 // 4.34, 99 % 4.63 / 4.35, 50 % 5.63 / 4.33.
 static const double kInplaceMinMatch = 0.995;
 
+// Segment capacity of the in-place segment probe.  The fallback C0 = 1.05·n/P + 16 K leaves ≈ 330 K rows of slack per segment
+// at 100 M rows and P = 16, about 130 σ of a uniform multinomial fill (σ ≈ sqrt(n/P) ≈ 2.5 K), and every unused row below the
+// output count costs the hole fill a move of the whole output row.  So once the host has read the fills of a partitioned
+// call of the handle that overflowed no segment, a call with the same P sizes its segments from that call's largest fill,
+// scaled to its own rows: f = max_p fill_p · n / n_learned, C = f + 8·sqrt(f) + 4 K, never above C0.  The largest fill
+// carries any systematic skew of the key distribution; a fresh batch from the same distribution moves each fill by about
+// σ = sqrt(f), and the largest of P fills sits a few σ above the mean at most, so 8 σ overflows with a probability far
+// below 1e-9 per call; the 4 K is a floor for small fills, where 8 σ is a few hundred rows.  A batch that overflows all the
+// same is probed from its original input by the gated fallback (slower, never wrong), and a synced overflow drops the
+// learned fills.  The lean segment probe keeps C0: it has no hole fill, so a tighter capacity saves it only memory.
+static int64_t inplace_seg_cap(const JoinImpl* j, int P, int64_t n_main, int64_t C0) {
+  if (j->seg_parts != P || j->seg_rows <= 0) return C0;
+  const double f = (double)j->seg_fill_max * (double)n_main / (double)j->seg_rows;
+  const int64_t C = ((int64_t)(f + 8.0 * std::sqrt(f)) + 4096 + 127) / 128 * 128;
+  return std::min(C, C0);
+}
+
 // ---- build --------------------------------------------------------------------------------------------
 static int build_table(JoinImpl* j) {
   const Side& b = j->build;
@@ -942,6 +964,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
     // segment layout starts at the allocation.
     const bool inplace = P && !in_seg && rb.rows == 0 && fo.n_key_dst >= 1 &&
                          (tune.inplace >= 0 ? tune.inplace != 0 : j->seg_match >= kInplaceMinMatch);
+    if (inplace) C = inplace_seg_cap(j, P, n_main, C);
     TG_TRY(ensure_result(j, rb, inplace ? std::max<int64_t>(n, (int64_t)P * C) : rb.rows + n, rb.rows > 0, rb.rows));
     for (int c = 0; c < j->n_out; c++) { oc.data[c] = rb.cols[c]->as<uint8_t>() + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
     build_fast_out(j, oc, pview, fo);
@@ -1004,12 +1027,19 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
       }
     }
     if (sync_count) {
-      unsigned long long got = 0;
+      unsigned long long got = 0, part[2 * TG_MAX_PARTS + 1];   // fill counts | segment bases | overflow flag
+      const bool learn = P && !in_seg;
+      if (learn) TG_CUDA(cudaMemcpyAsync(part, j->part_scratch.p, sizeof(part), cudaMemcpyDeviceToHost, j->stream));
       TG_CUDA(cudaMemcpyAsync(&got, cur, 8, cudaMemcpyDeviceToHost, j->stream));
       TG_CUDA(cudaStreamSynchronize(j->stream));
       rb.rows += (int64_t)got;
       j->stats.output_rows += (int64_t)got;
       if (P && n > 0) j->seg_match = (double)got / (double)n;
+      if (learn) {
+        j->seg_parts = part[2 * TG_MAX_PARTS] ? 0 : P;
+        j->seg_rows = n_main;
+        j->seg_fill_max = (int64_t)*std::max_element(part, part + P);
+      }
     }
     return TG_OK;
   }
