@@ -403,11 +403,44 @@ typedef struct tg_agg_desc_ex {
   const int32_t* col_decimal;     /* FieldType.GetDecimal() per child column; NULL = not given   */
 } tg_agg_desc_ex;
 
+/* tg_agg_desc_ex plus AggFuncDesc.HasDistinct per function, for COUNT, SUM and AVG with DISTINCT in Complete mode
+ * (aggfuncs/builder.go: countOriginalWithDistinct*, sum4Distinct*, avgOriginal4Distinct*).  has_distinct NULL or all 0:
+ * tg_agg_supported_ex2 / tg_agg_open_ex2 answer exactly like tg_agg_supported_ex / tg_agg_open_ex.
+ * A DISTINCT function aggregates each distinct non-NULL value of its argument once per group.  Groups are formed as
+ * without DISTINCT (NULL keys make one group, a DOUBLE key -0 is +0), and a value seen in an earlier push of the handle
+ * stays seen.  Values are distinct by:
+ *   integer family (signed, TG_FLAG_UNSIGNED, YEAR, DURATION)   the 64 bits (Int64Set)
+ *   DOUBLE                                                      -0 and +0 are one value; every NaN row is a new value
+ *                                                               (Go map[float64]: NaN != NaN)
+ *   DECIMAL(flen <= 18, decimal)                                the value at the column's scale (MyDecimal.ToHashKey:
+ *                                                               1.50 = 1.5)
+ *   COUNT(DISTINCT x)   BIGINT, the number of distinct values; 0 for a group without one
+ *   SUM(DISTINCT x)     the sum of the distinct values, NULL without one
+ *   AVG(DISTINCT x)     that sum divided by the number of distinct values; a DECIMAL result is rounded by the rule of
+ *                       tg_agg_func.ret_type
+ *   MIN / MAX           HasDistinct changes nothing (buildMaxMin ignores it)
+ * Without GROUP BY, empty input gives the usual default row (COUNT 0, SUM and AVG NULL).  A DISTINCT function is
+ * accepted when the same function without DISTINCT is (same argument types, ret_type / ret_frac rules and 24-word
+ * limit; COUNT over a DECIMAL(flen <= 18) column included), and it needs a free column slot: child columns plus distinct
+ * DISTINCT argument columns <= 16.  TG_ERR_UNSUPPORTED: DISTINCT in Final / Partial modes, an argument expression
+ * (arg_expr != TG_ARGEXPR_COL), a date-time, string, FLOAT or DECIMAL(flen > 18) argument, COUNT(DISTINCT a, b)
+ * (arg_col2 >= 0: arg_col2 must be -1) and FIRSTROW.  DISTINCT with arg_col < 0 is TG_ERR_INVALID.
+ * The library keeps one dedup set per DISTINCT argument column, in device memory, for the life of the handle; COUNT,
+ * SUM and AVG with DISTINCT over one column share it.  It grows on demand; a push whose growth cannot be allocated fails
+ * with TG_ERR_OOM, and every later push and finish of that handle fails with TG_ERR_STATE (the set already holds
+ * values of rows that were not aggregated).  A push that fails on a bad DECIMAL cell leaves groups and sets unchanged. */
+typedef struct tg_agg_desc_ex2 {
+  tg_agg_desc_ex ex;              /* everything tg_agg_desc_ex says, unchanged                  */
+  const uint8_t* has_distinct;    /* AggFuncDesc.HasDistinct per function (n_funcs); NULL = none */
+} tg_agg_desc_ex2;
+
 int tg_agg_supported(const tg_agg_desc* desc);
 int tg_agg_supported_ex(const tg_agg_desc_ex* desc);
+int tg_agg_supported_ex2(const tg_agg_desc_ex2* desc);
 /* HashAggExec.Open (agg_hash_executor.go:237) */
 int tg_agg_open(const tg_agg_desc* desc, tg_agg** out);
 int tg_agg_open_ex(const tg_agg_desc_ex* desc, tg_agg** out);
+int tg_agg_open_ex2(const tg_agg_desc_ex2* desc, tg_agg** out);
 /* fetchChildData + HashAggPartialWorker.updatePartialResult (agg_hash_executor.go:449,
  * agg_hash_partial_worker.go:256): one child chunk (host / device-resident)                    */
 int tg_agg_push(tg_agg* a, const tg_chunk* chk);
@@ -440,6 +473,14 @@ enum {
   TG_AGG_PATH_MERGE = 1 << 6        /* partial results folded into the global table (k_agg_merge)                */
 };
 int tg_agg_get_stats(tg_agg* a, tg_agg_stats* out);
+/* the dedup pass of the DISTINCT functions (k_agg_distinct_mark), cumulative over the handle's pushes: (group, value)
+ * pairs in the sets (NaN rows never enter one), slots of all sets, set growths, mark kernel launches, and the device time
+ * of the pass including its growth (CUDA events).  All 0 for a plan without DISTINCT. */
+typedef struct tg_agg_distinct_stats {
+  int64_t pairs, set_slots, set_grows, launches;
+  double mark_ms;
+} tg_agg_distinct_stats;
+int tg_agg_get_distinct_stats(tg_agg* a, tg_agg_distinct_stats* out);
 
 /* ---------------------------------------------------------------------------------------------
  * VecEval* kernels             replace pkg/expression builtin_*_vec.go signatures

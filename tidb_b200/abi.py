@@ -119,6 +119,17 @@ class TgAggDescEx(C.Structure):
     _fields_ = [("base", TgAggDesc), ("col_flen", C.POINTER(C.c_int32)), ("col_decimal", C.POINTER(C.c_int32))]
 
 
+class TgAggDescEx2(C.Structure):
+    """tg_agg_desc_ex2: tg_agg_desc_ex plus AggFuncDesc.HasDistinct per function (NULL = none)"""
+    _fields_ = [("ex", TgAggDescEx), ("has_distinct", C.POINTER(C.c_uint8))]
+
+
+class TgAggDistinctStats(C.Structure):
+    """tg_agg_distinct_stats: the dedup pass of the DISTINCT functions, cumulative over the handle's pushes"""
+    _fields_ = [("pairs", C.c_int64), ("set_slots", C.c_int64), ("set_grows", C.c_int64), ("launches", C.c_int64),
+                ("mark_ms", C.c_double)]
+
+
 class TgAggStats(C.Structure):
     _fields_ = [("input_rows", C.c_int64), ("groups", C.c_int64), ("table_slots", C.c_int64),
                 ("kernel_launches", C.c_int64), ("update_ms", C.c_double),
@@ -142,8 +153,8 @@ EXPORTED_SYMBOLS = [
     "tg_join_supported", "tg_join_open", "tg_join_build_push", "tg_join_build_push_dev",
     "tg_join_build_finish", "tg_join_probe_push", "tg_join_probe_finish", "tg_join_next", "tg_join_next_wait", "tg_join_probe_rewind",
     "tg_join_close", "tg_join_probe_dev", "tg_join_probe_dev_seg", "tg_join_get_stats",
-    "tg_agg_supported", "tg_agg_supported_ex", "tg_agg_open", "tg_agg_open_ex", "tg_agg_push", "tg_agg_push_dev", "tg_agg_finish",
-    "tg_agg_next", "tg_agg_close", "tg_agg_result_dev", "tg_agg_get_stats",
+    "tg_agg_supported", "tg_agg_supported_ex", "tg_agg_supported_ex2", "tg_agg_open", "tg_agg_open_ex", "tg_agg_open_ex2", "tg_agg_push",
+    "tg_agg_push_dev", "tg_agg_finish", "tg_agg_next", "tg_agg_close", "tg_agg_result_dev", "tg_agg_get_stats", "tg_agg_get_distinct_stats",
     "tg_vec_compare_int", "tg_vec_compare_real", "tg_vec_arith_int", "tg_vec_arith_real",
     "tg_vec_filter", "tg_topn",
     "tg_partition_by_key", "tg_partition_of_key", "tg_partition_exchange", "tg_partition_exchange_cf", "tg_partition_exchange_cf_ex", "tg_partition_exchange_cf_spill", "tg_partition_count",

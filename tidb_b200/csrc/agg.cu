@@ -681,13 +681,17 @@ __global__ void k_pack_bitmap_agg(const uint8_t* __restrict__ valid, int64_t n, 
 
 
 // ---- several GROUP BY columns: tag-claimed slots, global table only -------------------------------------------------
-struct KeyWords { long long w[TG_MAX_GROUP_COLS + 1]; };
-__device__ __forceinline__ unsigned long long hash_words(const KeyWords& k, int nkw) {
+// N key words: the group table's keys (the GROUP BY words and the NULL word), or a DISTINCT set's (those plus the value)
+template <int N> struct KeyWordsN { long long w[N]; };
+typedef KeyWordsN<TG_MAX_GROUP_COLS + 1> KeyWords;
+template <class K>
+__device__ __forceinline__ unsigned long long hash_words(const K& k, int nkw) {
   unsigned long long h = hash64((unsigned long long)k.w[0]);
   for (int j = 1; j < nkw; j++) h = hash64(h ^ ((unsigned long long)k.w[j] * 0xD6E8FEB86659FD93ull + (unsigned long long)j));
   return h;
 }
-__device__ __forceinline__ void load_key_words(const GroupKeys& gk, int64_t i, KeyWords& k) {
+template <class K>
+__device__ __forceinline__ void load_key_words(const GroupKeys& gk, int64_t i, K& k) {
   unsigned long long nullbits = 0;
   for (int j = 0; j < gk.n; j++) {
     long long v = 0;
@@ -700,8 +704,12 @@ __device__ __forceinline__ void load_key_words(const GroupKeys& gk, int64_t i, K
   }
   if (gk.nkw > gk.n) k.w[gk.n] = (long long)nullbits;
 }
-// find-or-insert; returns the slot or ~0 when the probe sequence is longer than max_probe (overfull: defer)
-__device__ __forceinline__ unsigned long long mk_find_or_insert(const AggTable& t, const KeyWords& k, unsigned long long h, uint32_t max_probe) {
+// find-or-insert; returns the slot or ~0 when the probe sequence is longer than max_probe (overfull: defer).  *inserted (when
+// given) is set when this call claimed the slot: of all the threads that look up one new key, exactly one sees it set.  T is
+// the group table (AggTable) or a DISTINCT set (DistinctSet): both have tags, keyw, nslots, nkw and stride.
+template <class T, class K>
+__device__ __forceinline__ unsigned long long mk_find_or_insert(const T& t, const K& k, unsigned long long h, uint32_t max_probe,
+                                                                bool* inserted = nullptr) {
   const unsigned long long ready = h | 3ull, busy = (h & ~3ull) | 1ull;
   uint32_t s = slot32(h, (uint32_t)t.nslots), steps = 0;
   for (;;) {
@@ -717,12 +725,22 @@ __device__ __forceinline__ unsigned long long mk_find_or_insert(const AggTable& 
         for (int j = 0; j < t.nkw; j++) t.keyw[j][(size_t)s * t.stride] = k.w[j];
         __threadfence();
         *reinterpret_cast<volatile unsigned long long*>(&t.tags[(size_t)s * t.stride]) = ready;   // publish
+        if (inserted) *inserted = true;
         return s;
       }
     }
     if ((cur | 2ull) == ready) {
       bool eq = cur == ready && (unsigned long long)k.w[0] == k0 && (t.nkw < 2 || (unsigned long long)k.w[1] == k1) && (t.nkw < 3 || (unsigned long long)k.w[2] == k2);
       if (eq && t.nkw > 3) eq = *reinterpret_cast<volatile long long*>(&t.keyw[3][(size_t)s * t.stride]) == k.w[3];
+      // a DISTINCT set compares its words past the fourth too (up to four group words, the NULL word and the value).  The
+      // group table keeps its four-word check here: its fifth word, the NULL word of four GROUP BY columns, is left to
+      // the tag as before, which keeps k_agg_update_mk at its register count.
+      constexpr int NW = (int)(sizeof(k.w) / sizeof(k.w[0]));
+      if (NW > TG_MAX_GROUP_COLS + 1) {
+#pragma unroll
+        for (int j = 4; j < NW; j++)
+          if (eq && t.nkw > j) eq = *reinterpret_cast<volatile long long*>(&t.keyw[j][(size_t)s * t.stride]) == k.w[j];
+      }
       if (!eq) {   // still being written, or the vector load raced with the writer, or a different key with the same hash: settle it with ordered loads
         while (cur != ready) cur = *reinterpret_cast<volatile unsigned long long*>(&t.tags[(size_t)s * t.stride]);
         eq = true;
@@ -769,6 +787,78 @@ __global__ void k_agg_rehash_mk(AggTable oldt, AggTable newt, int nstates) {
     for (int j = 0; j < oldt.nkw; j++) newt.keyw[j][(size_t)s * newt.stride] = oldt.keyw[j][(size_t)i * oldt.stride];
     newt.rows[(size_t)s * newt.stride] = oldt.rows[(size_t)i * oldt.stride];
     for (int a = 0; a < nstates; a++) newt.state[a][(size_t)s * newt.stride] = oldt.state[a][(size_t)i * oldt.stride];
+  }
+}
+
+// ---- DISTINCT arguments: one dedup set per argument column ----------------------------------------------------------
+// A set holds the (group key words, value word) pairs seen so far, in HBM, for the life of the handle.  Its records are
+// [tag | key words], claimed like the multi-key table's (mk_find_or_insert) and carrying no states; the key words are the
+// group table's (load_key_words: NULL group keys as 0 plus the NULL word, a DOUBLE -0 as +0) followed by the value.
+#define TG_SET_MAX_WORDS (TG_MAX_GROUP_COLS + 2)
+struct DistinctSet {
+  unsigned long long* tags;
+  long long* keyw[TG_SET_MAX_WORDS];
+  unsigned long long nslots;
+  int32_t nkw;
+  uint32_t stride;     // 8-byte words per record: 2 for a value alone, else a multiple of 4 (32-byte records)
+};
+typedef KeyWordsN<TG_SET_MAX_WORDS> SetKey;
+
+// One thread per row: bit i of `mark` = row i's argument is not NULL and row i claimed a new (group, value) pair — exactly
+// one row per pair, the one whose CAS claimed the slot.  The update kernels then read the argument column with `mark` as
+// its null bitmap, so COUNT / SUM / AVG(DISTINCT x) are the plain functions over it.  A DOUBLE value is keyed with -0 as
+// +0, and a NaN row is always new (Go map[float64]: NaN != NaN) without entering the set.  A row whose probe runs past
+// max_probe is deferred like the group table's; `only` restricts a re-run to those rows, whose bits are then ORed in.
+// Warps run whole 32-row words: lane 0 stores the ballot.  counters[0] = rows deferred, counters[1] = pairs inserted.
+__global__ void __launch_bounds__(256)
+k_agg_distinct_mark(GroupKeys gk, const long long* __restrict__ vals, const uint8_t* __restrict__ vnulls, int is_real, int64_t n,
+                    DistinctSet t, uint32_t max_probe, uint32_t* mark, uint32_t* deferred, const uint32_t* only,
+                    unsigned long long* counters) {
+  const int lane = threadIdx.x & 31;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  unsigned long long my_deferred = 0, my_new = 0;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i - lane < n; i += stride) {
+    bool win = false;
+    if (i < n && (!only || ((only[i >> 5] >> (i & 31)) & 1u)) && (!vnulls || bit_not_null(vnulls, i))) {
+      long long v = __ldcs(vals + i);
+      bool nan = false;
+      if (is_real) { double d = __longlong_as_double(v); if (d == 0) d = 0; nan = d != d; v = __double_as_longlong(d); }
+      if (nan) win = true;
+      else {
+        SetKey k;
+        load_key_words(gk, i, k);
+#pragma unroll
+        for (int j = 0; j < TG_SET_MAX_WORDS; j++) if (j == gk.nkw) k.w[j] = v;   // the value follows the group words
+        bool ins = false;
+        const unsigned long long s = mk_find_or_insert(t, k, hash_words(k, t.nkw), max_probe, &ins);
+        if (s == ~0ull) { atomicOr(&deferred[i >> 5], 1u << (i & 31)); my_deferred++; }
+        else if (ins) { win = true; my_new++; }
+      }
+    }
+    const uint32_t b = __ballot_sync(0xffffffffu, win);
+    if (lane == 0) { if (only) mark[i >> 5] |= b; else mark[i >> 5] = b; }
+  }
+  for (int o = 16; o; o >>= 1) {
+    my_deferred += __shfl_xor_sync(0xffffffffu, my_deferred, o);
+    my_new += __shfl_xor_sync(0xffffffffu, my_new, o);
+  }
+  if (lane == 0 && my_deferred) atomicAdd(&counters[0], my_deferred);
+  if (lane == 0 && my_new) atomicAdd(&counters[1], my_new);
+}
+
+// re-insert every pair of an old set into a bigger one (pairs are distinct: claim with the published tag)
+__global__ void k_agg_distinct_rehash(DistinctSet oldt, DistinctSet newt) {
+  unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  for (; i < oldt.nslots; i += stride) {
+    const unsigned long long tag = oldt.tags[(size_t)i * oldt.stride];
+    if (tag == 0) continue;
+    uint32_t s = slot32(tag, (uint32_t)newt.nslots);
+    for (;;) {
+      if (atomicCAS(&newt.tags[(size_t)s * newt.stride], 0ull, tag) == 0ull) break;
+      if (++s == (uint32_t)newt.nslots) s = 0;
+    }
+    for (int j = 0; j < oldt.nkw; j++) newt.keyw[j][(size_t)s * newt.stride] = oldt.keyw[j][(size_t)i * oldt.stride];
   }
 }
 
@@ -863,6 +953,17 @@ struct AggImpl {
   bool wide = false;        // a DECIMAL SUM / AVG of a product: the WIDE kernel instantiations
   bool dec_out = false;     // a DECIMAL result column: k_agg_finalize<true, wide>
 
+  // DISTINCT arguments (tg_agg_desc_ex2): set j dedups child column dist_cols[j] and feeds the virtual column ncols + j
+  // (the column's values, null bitmap = the set's mark bits), which the DISTINCT functions read as their argument
+  std::vector<char> fdistinct;          // per function: COUNT / SUM / AVG with HasDistinct
+  std::vector<int> dist_cols;
+  int dist_gkw = 0;                     // group key words of a set record (the value word follows)
+  struct SetMem { DevBuf mem, mark; DistinctSet t{}; };
+  std::vector<std::unique_ptr<SetMem>> dsets;
+  DevBuf dcounters;                     // k_agg_distinct_mark: [0] rows deferred [1] pairs inserted
+  bool broken = false;                  // a push failed after a set was touched: every later push / finish fails
+  tg_agg_distinct_stats dstats{};
+
   // table
   DevBuf tbl_mem;
   AggTable tbl{};
@@ -943,7 +1044,21 @@ static int dec_expr_rules(const AggImpl* a, const tg_agg_func& f) {
   return TG_OK;
 }
 
-static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, const int32_t* col_dec) {
+// COUNT / SUM / AVG with HasDistinct (tg_agg_desc_ex2), checked before the rules of the same function without it, which
+// must accept it too: TG_OK when its dedup pass is offloaded, else the status and message
+static int distinct_rules(const AggImpl* a, const tg_agg_func& f) {
+  if (f.arg_col < 0 || f.arg_col >= a->ncols) return fail(TG_ERR_INVALID, "a DISTINCT aggregate needs an argument column");
+  if (f.name == TG_AGG_FIRSTROW) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW with DISTINCT is not offloaded");
+  if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates are offloaded in Complete mode only");
+  if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates take a plain column argument");
+  if (f.name == TG_AGG_COUNT && f.arg_col2 >= 0) return fail(TG_ERR_UNSUPPORTED, "COUNT(DISTINCT a, b) over several arguments is not offloaded");
+  const int t = a->types[f.arg_col];
+  if (!((is_int_family(t) && a->elem[f.arg_col] == 8) || t == TG_TYPE_DOUBLE || t == TG_TYPE_NEWDECIMAL))
+    return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates are offloaded over integer-family, DOUBLE and DECIMAL(p <= 18) columns");
+  return TG_OK;
+}
+
+static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, const int32_t* col_dec, const uint8_t* has_distinct = nullptr) {
   if (!d) return fail(TG_ERR_INVALID, "desc is NULL");
   if (d->n_cols <= 0 || d->n_cols > TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "child schema must have 1..16 columns");
   a->ncols = d->n_cols;
@@ -982,10 +1097,17 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
   a->nstates = 0;
   a->out_nullable.assign(d->n_funcs, 0);
   a->out_elem.assign(d->n_funcs, 8);
+  a->fdistinct.assign(d->n_funcs, 0);
   for (int k = 0; k < d->n_funcs; k++) {
     const tg_agg_func& f = d->funcs[k];
     AggFuncDev& o = a->spec.f[k];
     o = AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, -1, 0, -1, -1, f.arg_const, 0};
+    if (has_distinct && has_distinct[k]) {
+      if (f.arg_col < 0) return fail(TG_ERR_INVALID, "a DISTINCT aggregate needs an argument column");
+      // MIN / MAX: DISTINCT changes nothing (buildMaxMin ignores HasDistinct)
+      if (f.name != TG_AGG_MIN && f.name != TG_AGG_MAX) { TG_TRY(distinct_rules(a, f)); a->fdistinct[k] = 1; }
+    }
+    const bool distinct = a->fdistinct[k] != 0;
     // a DECIMAL(p <= 18, s) argument column (tg_agg_desc_ex): decoded to int64 value * 10^s on every batch, then the integer
     // update paths run unchanged
     const bool dec_arg = f.arg_col >= 0 && f.arg_col < a->ncols && a->types[f.arg_col] == TG_TYPE_NEWDECIMAL;
@@ -1017,12 +1139,15 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
     if (f.arg_col >= a->ncols || f.arg_col2 >= a->ncols) return fail(TG_ERR_INVALID, "aggregate argument column out of range");
     bool arg_nullable = f.arg_col >= 0 && !(a->flags[f.arg_col] & TG_FLAG_NOT_NULL);
     if (f.arg_expr != TG_ARGEXPR_COL && f.arg_col2 >= 0 && f.arg_col2 < d->n_cols && !(a->flags[f.arg_col2] & TG_FLAG_NOT_NULL)) arg_nullable = true;
+    // a DISTINCT argument is NULL on every row that brought no new value: COUNT needs its own count, AVG its divisor
+    if (distinct) arg_nullable = true;
     if (f.arg_col >= 0) { if (a->elem[f.arg_col] != 8 && !dec_arg) return fail(TG_ERR_UNSUPPORTED, "aggregate arguments must be 8-byte columns"); a->needed[f.arg_col] = 1; }
     int atype = f.arg_col >= 0 ? a->types[f.arg_col] : TG_TYPE_LONGLONG;
     o.is_real = atype == TG_TYPE_DOUBLE;
     o.is_unsigned = f.arg_col >= 0 && !dec_arg && (a->flags[f.arg_col] & TG_FLAG_UNSIGNED) != 0;   // a decoded DECIMAL is a signed int64
     if (dec_arg && f.name != TG_AGG_COUNT) { o.dec_scale = a->col_dec[f.arg_col]; a->dec_decode[f.arg_col] = 1; }
     else if (dec) o.dec_scale = 0;
+    if (distinct && dec_arg) a->dec_decode[f.arg_col] = 1;   // COUNT(DISTINCT dec) too: the set is keyed on the value
     const bool dec_expr = dec_arg && f.arg_expr != TG_ARGEXPR_COL;   // SUM / AVG of a DECIMAL product (dec_expr_rules)
     if (dec_expr) {
       const int sb = a->col_dec[f.arg_col2];
@@ -1097,6 +1222,18 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
     a->dec_out |= o.dec_scale >= 0;
   }
   if (a->nstates > 2 * TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "the aggregate list needs more than 24 state words (a DECIMAL SUM / AVG takes up to 3, up to 4 over a product)");
+  // one dedup set per DISTINCT argument column; its functions read the virtual column ncols + j (free DevCols slots)
+  a->dist_cols.clear();
+  for (int k = 0; k < d->n_funcs; k++) {
+    if (!a->fdistinct[k]) continue;
+    const int c = d->funcs[k].arg_col;
+    const size_t j = std::find(a->dist_cols.begin(), a->dist_cols.end(), c) - a->dist_cols.begin();
+    if (j == a->dist_cols.size()) a->dist_cols.push_back(c);
+    a->spec.f[k].arg_col = a->ncols + (int)j;
+  }
+  if (a->ncols + (int)a->dist_cols.size() > TG_MAX_COLS)
+    return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates need one free column slot per argument column (child columns + DISTINCT columns <= 16)");
+  a->dist_gkw = d->n_group_by + (any_nullable ? 1 : 0);
   a->device = d->device;
   a->expected_groups = d->expected_groups;
   return TG_OK;
@@ -1487,10 +1624,88 @@ static int decode_decimal_args(AggImpl* a, DevCols& cols, int64_t n) {
   return TG_OK;
 }
 
-// aggregate n device-resident rows; a fused argument expression that overflowed fails the call (types.ErrOverflow)
-static int update_device(AggImpl* a, const DevCols& in, int64_t n) {
-  DevCols cols = in;
-  TG_TRY(decode_decimal_args(a, cols, n));
+// ---- DISTINCT sets ------------------------------------------------------------------------------------------------
+// records of 2 words (tag, value) without GROUP BY, else padded to 32-byte multiples like the multi-key table's
+static int set_record_words(int nkw) { return nkw == 1 ? 2 : ((1 + nkw + 3) / 4) * 4; }
+static int alloc_set(AggImpl* a, unsigned long long nslots, DevBuf& mem, DistinctSet& t) {
+  if (nslots >= (1ull << 32)) return fail(TG_ERR_OOM, "a DISTINCT set would need 2^32 slots or more");
+  const int nkw = a->dist_gkw + 1, w = set_record_words(nkw);
+  const size_t bytes = (size_t)nslots * w * 8 + 64;   // mk_find_or_insert reads 32 bytes from a 16-byte record's start
+  TG_TRY(mem.ensure(a->device, bytes));
+  TG_CUDA(cudaMemsetAsync(mem.p, 0, bytes, a->stream));   // tag 0 = empty
+  unsigned long long* base = mem.as<unsigned long long>();
+  t = DistinctSet{};
+  t.tags = base;
+  for (int j = 0; j < nkw; j++) t.keyw[j] = reinterpret_cast<long long*>(base + 1 + j);
+  t.nslots = nslots; t.nkw = nkw; t.stride = (uint32_t)w;
+  return TG_OK;
+}
+static int grow_set(AggImpl* a, AggImpl::SetMem& m, unsigned long long want) {
+  DevBuf nm;
+  DistinctSet nt{};
+  TG_TRY(alloc_set(a, want, nm, nt));
+  k_agg_distinct_rehash<<<agrid(a, (int64_t)m.t.nslots), 256, 0, a->stream>>>(m.t, nt);
+  a->stats.kernel_launches++;
+  TG_CUDA(cudaStreamSynchronize(a->stream));
+  std::swap(m.mem.p, nm.p); std::swap(m.mem.cap, nm.cap); std::swap(m.mem.device, nm.device);
+  m.t = nt;
+  a->dstats.set_grows++;
+  return TG_OK;
+}
+
+// k_agg_distinct_mark for every DISTINCT argument column of the batch (after decode_decimal_args: a DECIMAL value is its
+// int64 at the column's scale), then the virtual columns ncols + j point at the values and the mark bits.  A set is sized
+// from its first batch like the group table and grows x4 with the same defer / rehash / re-run loop.
+static int distinct_mark(AggImpl* a, DevCols& cols, int64_t n) {
+  if (a->dist_cols.empty() || n == 0) return TG_OK;
+  TG_TRY(a->dcounters.ensure(a->device, 16));
+  unsigned long long* cnt = a->dcounters.as<unsigned long long>();
+  GroupKeys gk{};
+  gk.n = (int)a->group_cols.size(); gk.nkw = a->dist_gkw;
+  for (int q = 0; q < gk.n; q++) { gk.data[q] = cols.data[a->group_cols[q]]; gk.nulls[q] = cols.nulls[a->group_cols[q]]; gk.kind[q] = a->group_kinds[q]; }
+  const size_t dwords = (size_t)((n + 31) / 32);
+  TG_TRY(a->deferred.ensure(a->device, dwords * 4 + 16));
+  TG_CUDA(cudaEventRecord(a->ev0, a->stream));
+  for (size_t j = 0; j < a->dist_cols.size(); j++) {
+    AggImpl::SetMem& m = *a->dsets[j];
+    const int c = a->dist_cols[j];
+    if (m.t.nslots == 0) TG_TRY(alloc_set(a, std::max<unsigned long long>(1024, (unsigned long long)std::min<int64_t>(n, 1ll << 22) * 2), m.mem, m.t));
+    TG_TRY(m.mark.ensure(a->device, dwords * 4 + 16));
+    TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
+    DevBuf prev_deferred;
+    const uint32_t* only = nullptr;
+    for (int round = 0; round < 40; round++) {
+      TG_CUDA(cudaMemsetAsync(cnt, 0, 16, a->stream));
+      k_agg_distinct_mark<<<agrid(a, n), 256, 0, a->stream>>>(gk, static_cast<const long long*>(cols.data[c]), cols.nulls[c],
+                                                               a->types[c] == TG_TYPE_DOUBLE, n, m.t, 48u, m.mark.as<uint32_t>(),
+                                                               a->deferred.as<uint32_t>(), only, cnt);
+      a->stats.kernel_launches++;
+      a->dstats.launches++;
+      unsigned long long back[2] = {0, 0};
+      TG_CUDA(cudaMemcpyAsync(back, cnt, 16, cudaMemcpyDeviceToHost, a->stream));
+      TG_CUDA(cudaStreamSynchronize(a->stream));
+      a->dstats.pairs += (int64_t)back[1];
+      if (back[0] == 0) break;
+      if (round == 39) return fail(TG_ERR_CUDA, "internal: DISTINCT set failed to converge");
+      TG_TRY(grow_set(a, m, std::max<unsigned long long>(m.t.nslots * 4, (unsigned long long)((m.t.nslots * 0.6 + (double)back[0]) * 2))));
+      TG_TRY(prev_deferred.ensure(a->device, dwords * 4 + 16));
+      TG_CUDA(cudaMemcpyAsync(prev_deferred.p, a->deferred.p, dwords * 4, cudaMemcpyDeviceToDevice, a->stream));
+      TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
+      only = prev_deferred.as<uint32_t>();
+    }
+    cols.data[a->ncols + j] = cols.data[c];
+    cols.nulls[a->ncols + j] = m.mark.as<uint8_t>();
+    cols.elem_len[a->ncols + j] = 8;
+  }
+  TG_CUDA(cudaEventRecord(a->ev1, a->stream));
+  TG_CUDA(cudaStreamSynchronize(a->stream));
+  TG_CUDA(cudaGetLastError());
+  float ms = 0; cudaEventElapsedTime(&ms, a->ev0, a->ev1); a->dstats.mark_ms += ms;
+  return TG_OK;
+}
+
+static int update_after_decode(AggImpl* a, DevCols& cols, int64_t n) {
+  TG_TRY(distinct_mark(a, cols, n));
   TG_TRY(update_device_impl(a, cols, n));
   bool has_expr = false;
   for (int k = 0; k < a->spec.n; k++) has_expr |= a->spec.f[k].arg_expr != TG_ARGEXPR_COL;
@@ -1500,6 +1715,22 @@ static int update_device(AggImpl* a, const DevCols& in, int64_t n) {
   TG_CUDA(cudaStreamSynchronize(a->stream));
   if (e) return fail(TG_ERR_OVERFLOW, "ErrOverflow: DOUBLE value is out of range in an aggregate argument expression");
   return TG_OK;
+}
+
+static int broken_fail() {
+  return fail(TG_ERR_STATE, "an earlier push failed after the DISTINCT sets had taken its values: this handle's results are lost");
+}
+
+// aggregate n device-resident rows; a fused argument expression that overflowed fails the call (types.ErrOverflow).  A bad
+// DECIMAL cell fails the push before the DISTINCT sets see it; any later failure leaves a set holding values whose rows
+// were not aggregated, so the handle refuses every later push and finish instead of counting them twice or never.
+static int update_device(AggImpl* a, const DevCols& in, int64_t n) {
+  if (a->broken) return broken_fail();
+  DevCols cols = in;
+  TG_TRY(decode_decimal_args(a, cols, n));
+  const int rc = update_after_decode(a, cols, n);
+  if (rc != TG_OK && !a->dist_cols.empty()) a->broken = true;
+  return rc;
 }
 
 static int64_t alogical_rows(const tg_chunk* c) { return c->sel ? c->nsel : (c->ncols > 0 ? c->cols[0].length : 0); }
@@ -1659,12 +1890,18 @@ int tg_agg_supported_ex(const tg_agg_desc_ex* desc) {
   return agg_setup(&tmp, desc ? &desc->base : nullptr, desc ? desc->col_flen : nullptr, desc ? desc->col_decimal : nullptr);
 }
 
-static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int32_t* col_dec, tg_agg** out) {
+int tg_agg_supported_ex2(const tg_agg_desc_ex2* desc) {
+  AggImpl tmp;
+  return agg_setup(&tmp, desc ? &desc->ex.base : nullptr, desc ? desc->ex.col_flen : nullptr, desc ? desc->ex.col_decimal : nullptr,
+                   desc ? desc->has_distinct : nullptr);
+}
+
+static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int32_t* col_dec, const uint8_t* has_distinct, tg_agg** out) {
   if (!out) return fail(TG_ERR_INVALID, "out is NULL");
   *out = nullptr;
   std::unique_ptr<tg_agg> shell(new tg_agg());
   std::unique_ptr<AggImpl> a(new AggImpl());
-  TG_TRY(agg_setup(a.get(), desc, col_flen, col_dec));
+  TG_TRY(agg_setup(a.get(), desc, col_flen, col_dec, has_distinct));
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(TG_ERR_CUDA, "no CUDA device: the GPU hash aggregation has no CPU fallback"); }
   if (a->device < 0 || a->device >= ndev) return fail(TG_ERR_INVALID, "device ordinal out of range");
@@ -1680,20 +1917,27 @@ static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int3
     a->dcols.emplace_back(new DevBuf()); a->dnulls.emplace_back(new DevBuf()); a->dscaled.emplace_back(new DevBuf());
   }
   a->stage.has_nulls.assign(a->ncols, 0);
+  for (size_t j = 0; j < a->dist_cols.size(); j++) a->dsets.emplace_back(new AggImpl::SetMem());
   shell->impl = a.release();
   *out = shell.release();
   return TG_OK;
 }
 
-int tg_agg_open(const tg_agg_desc* desc, tg_agg** out) { return agg_open(desc, nullptr, nullptr, out); }
+int tg_agg_open(const tg_agg_desc* desc, tg_agg** out) { return agg_open(desc, nullptr, nullptr, nullptr, out); }
 
 int tg_agg_open_ex(const tg_agg_desc_ex* desc, tg_agg** out) {
-  return agg_open(desc ? &desc->base : nullptr, desc ? desc->col_flen : nullptr, desc ? desc->col_decimal : nullptr, out);
+  return agg_open(desc ? &desc->base : nullptr, desc ? desc->col_flen : nullptr, desc ? desc->col_decimal : nullptr, nullptr, out);
+}
+
+int tg_agg_open_ex2(const tg_agg_desc_ex2* desc, tg_agg** out) {
+  return agg_open(desc ? &desc->ex.base : nullptr, desc ? desc->ex.col_flen : nullptr, desc ? desc->ex.col_decimal : nullptr,
+                  desc ? desc->has_distinct : nullptr, out);
 }
 
 int tg_agg_push(tg_agg* h, const tg_chunk* chk) {
   TGA_LOCK(h);
   if (a->finished) return fail(TG_ERR_STATE, "push after finish");
+  if (a->broken) return broken_fail();
   TG_TRY(avalidate(a, chk));
   TG_TRY(astage_append(a, chk));
   if (a->stage.rows >= (4ll << 20)) TG_TRY(aflush(a));
@@ -1718,6 +1962,7 @@ int tg_agg_push_dev(tg_agg* h, const tg_chunk* chk) {
 int tg_agg_finish(tg_agg* h) {
   TGA_LOCK(h);
   if (a->finished) return TG_OK;
+  if (a->broken) return broken_fail();
   TG_TRY(aflush(a));
   TG_TRY(afinalize(a));
   a->finished = true;
@@ -1787,6 +2032,15 @@ int tg_agg_get_stats(tg_agg* h, tg_agg_stats* out) {
   TGA_LOCK(h);
   if (!out) return fail(TG_ERR_INVALID, "out is NULL");
   *out = a->stats;
+  return TG_OK;
+}
+
+int tg_agg_get_distinct_stats(tg_agg* h, tg_agg_distinct_stats* out) {
+  TGA_LOCK(h);
+  if (!out) return fail(TG_ERR_INVALID, "out is NULL");
+  *out = a->dstats;
+  out->set_slots = 0;
+  for (const auto& m : a->dsets) out->set_slots += (int64_t)m->t.nslots;
   return TG_OK;
 }
 

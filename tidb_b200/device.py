@@ -93,9 +93,9 @@ class DeviceAgg:
     def __init__(self, plan: AggPlan):
         self.lib = abi.load_lib()
         self.plan = plan
-        desc, self._keep = plan.to_struct_ex()
+        desc, self._keep = plan.to_struct_ex2()
         self.h = C.c_void_p()
-        abi.check(self.lib.tg_agg_open_ex(C.byref(desc), C.byref(self.h)))
+        abi.check(self.lib.tg_agg_open_ex2(C.byref(desc), C.byref(self.h)))
         self.n_out = len(plan.funcs)
 
     def push(self, cols: Sequence[torch.Tensor], nulls=None) -> None:
@@ -113,6 +113,11 @@ class DeviceAgg:
     def stats(self) -> abi.TgAggStats:
         s = abi.TgAggStats()
         abi.check(self.lib.tg_agg_get_stats(self.h, C.byref(s)))
+        return s
+
+    def distinct_stats(self) -> abi.TgAggDistinctStats:
+        s = abi.TgAggDistinctStats()
+        abi.check(self.lib.tg_agg_get_distinct_stats(self.h, C.byref(s)))
         return s
 
     def close(self) -> None:

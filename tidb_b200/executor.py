@@ -199,9 +199,9 @@ class HashAggExec(Executor):
     def open(self) -> None:
         super().open()
         self._lib = abi.load_lib()
-        desc, self._keep = self.plan.to_struct_ex()
+        desc, self._keep = self.plan.to_struct_ex2()
         self._h = C.c_void_p()
-        abi.check(self._lib.tg_agg_open_ex(C.byref(desc), C.byref(self._h)))
+        abi.check(self._lib.tg_agg_open_ex2(C.byref(desc), C.byref(self._h)))
         self._prepared = False
 
     def next(self, required_rows: int = MAX_CHUNK_SIZE) -> Chunk:
@@ -225,6 +225,11 @@ class HashAggExec(Executor):
     def stats(self) -> abi.TgAggStats:
         s = abi.TgAggStats()
         abi.check(self._lib.tg_agg_get_stats(self._h, C.byref(s)))
+        return s
+
+    def distinct_stats(self) -> abi.TgAggDistinctStats:
+        s = abi.TgAggDistinctStats()
+        abi.check(self._lib.tg_agg_get_distinct_stats(self._h, C.byref(s)))
         return s
 
     def close(self) -> None:

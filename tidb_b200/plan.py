@@ -172,6 +172,7 @@ class AggFunc:
     ret_type: int = 0          # AggFuncDesc.RetTp.GetType(): abi.TYPE_NEWDECIMAL = exact DECIMAL SUM / AVG of an integer
                                # column, or SUM / AVG / MIN / MAX of a DECIMAL column
     ret_frac: int = 0          # AggFuncDesc.RetTp.GetDecimal()
+    distinct: bool = False     # AggFuncDesc.HasDistinct: COUNT / SUM / AVG of the distinct values (tg_agg_desc_ex2)
 
 
 @dataclass
@@ -212,6 +213,15 @@ class AggPlan:
         a = _i32([t.flen for t in self.col_types]); keep.append(a); ex.col_flen = a
         a = _i32([t.decimal for t in self.col_types]); keep.append(a); ex.col_decimal = a
         return ex, keep
+
+    def to_struct_ex2(self) -> Tuple[abi.TgAggDescEx2, list]:
+        """tg_agg_desc_ex2: to_struct_ex() plus HasDistinct per function (NULL when no function has it)"""
+        ex, keep = self.to_struct_ex()
+        d = abi.TgAggDescEx2()
+        d.ex = ex
+        if any(f.distinct for f in self.funcs):
+            a = (C.c_uint8 * len(self.funcs))(*[int(f.distinct) for f in self.funcs]); keep.append(a); d.has_distinct = a
+        return d, keep
 
 
 # ---------------------------------------------------------------------------------------------------------------
