@@ -150,6 +150,52 @@ __device__ __forceinline__ unsigned long long dec_ext(const AggFuncDev& f, unsig
 // its group
 __device__ __forceinline__ uint32_t agg_home(long long k, unsigned long long nslots) { return slot32(hash64((unsigned long long)k), (uint32_t)nslots); }
 
+// probe-length limit of every find-or-insert into the group table or a DISTINCT set: an item whose probe sequence is
+// longer finds the table overfull and is deferred, and the host grows the table (grow_and_retry)
+constexpr uint32_t kAggMaxProbe = 48;
+
+// find-or-insert `k` in the global table starting at slot s with the slot's current content `cur` already loaded;
+// returns false when the probe sequence exceeds max_probe (table overfull: defer)
+__device__ __forceinline__ bool global_find_or_insert(const AggTable& t, long long k, uint32_t& s, long long cur, uint32_t max_probe) {
+  const uint32_t S = (uint32_t)t.nslots;
+  uint32_t steps = 0;
+  for (;;) {
+    if (cur == k) return true;
+    if (cur == kEmptyKey) {
+      unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(&t.keys[s]), (unsigned long long)kEmptyKey, (unsigned long long)k);
+      if (old == (unsigned long long)kEmptyKey || old == (unsigned long long)k) return true;
+    }
+    if (++steps > max_probe) return false;
+    if (++s == S) s = 0;
+    cur = *reinterpret_cast<volatile long long*>(&t.keys[s]);
+  }
+}
+
+// fold one partial group (rows + states) into global slot s: MergePartialResult (func_sum.go:106, func_count.go:481,
+// func_avg.go:444, func_max_min.go merge)
+template <bool WIDE>
+__device__ __forceinline__ void agg_merge_into(const AggTable& t, const AggSpec& spec, unsigned long long s, unsigned long long rows, const unsigned long long* st) {
+  atomicAdd(&t.rows[s], rows);
+  for (int k = 0; k < spec.n; k++) {
+    const AggFuncDev& f = spec.f[k];
+    if (f.s0 >= 0) {
+      unsigned long long v = st[f.s0];
+      switch (f.name) {
+        case TG_AGG_COUNT: atomicAdd(&t.state[f.s0][s], v); break;
+        case TG_AGG_SUM: case TG_AGG_AVG:
+          if (WIDE && f.s3 >= 0) dec3_add(&t.state[f.s0][s], &t.state[f.s2][s], &t.state[f.s3][s], v, st[f.s2], st[f.s3]);
+          else if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, st[f.s2]);
+          else atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v));
+          break;
+        case TG_AGG_MIN: atomicMin(&t.state[f.s0][s], v); break;
+        case TG_AGG_MAX: atomicMax(&t.state[f.s0][s], v); break;
+        default: break;
+      }
+    }
+    if (f.s1 >= 0) atomicAdd(&t.state[f.s1][s], st[f.s1]);
+  }
+}
+
 __global__ void k_agg_init(AggTable t, AggSpec spec, unsigned long long n_total) {
   unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
   unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
@@ -238,13 +284,13 @@ __device__ __forceinline__ void agg_apply(const AggTable& t, const AggSpec& spec
   }
 }
 
-// One thread per row: find-or-insert the group slot, then atomics.  Rows whose NEW key would push the
-// table past max_fill are deferred (bit set in `deferred`) so the host can grow the table and re-run
+// One thread per row: find-or-insert the group slot, then atomics.  Rows whose NEW key finds no slot within
+// max_probe steps are deferred (bit set in `deferred`) so the host can grow the table and re-run
 // them; `only` restricts a re-run to those rows.
 template <bool WIDE>
 __global__ void __launch_bounds__(256)
-k_agg_update(GroupKey gk, DevCols cols, int64_t n, AggTable t, AggSpec spec, unsigned long long max_fill,
-             unsigned long long* fill, uint32_t* deferred, const uint32_t* only, unsigned long long* n_deferred) {
+k_agg_update(GroupKey gk, DevCols cols, int64_t n, AggTable t, AggSpec spec, uint32_t max_probe,
+             uint32_t* deferred, const uint32_t* only, unsigned long long* n_deferred) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (; i < n; i += stride) {
@@ -262,28 +308,16 @@ k_agg_update(GroupKey gk, DevCols cols, int64_t n, AggTable t, AggSpec spec, uns
       }
       if (k == kEmptyKey) s = t.nslots + 1;
       else {
-        s = agg_home(k, t.nslots);
-        bool defer = false;
         // No global fill counter: one atomic per NEW key on a single address serialised at ~3 ns each (1 M groups =
-        // 3 ms, twice the rest of the kernel).  A probe sequence longer than `max_fill` steps means the table is
+        // 3 ms, twice the rest of the kernel).  A probe sequence longer than `max_probe` steps means the table is
         // overfull: the row is deferred and the host grows the table.
-        unsigned int steps = 0;
-        for (;;) {
-          long long cur = *reinterpret_cast<volatile long long*>(&t.keys[s]);
-          if (cur == k) break;
-          if (cur == kEmptyKey) {
-            unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(&t.keys[s]), (unsigned long long)kEmptyKey,
-                                               (unsigned long long)k);
-            if (old == (unsigned long long)kEmptyKey || old == (unsigned long long)k) break;
-          }
-          if (++steps > (unsigned int)max_fill) { defer = true; break; }
-          if (++s == t.nslots) s = 0;
-        }
-        if (defer) {
+        uint32_t sl = agg_home(k, t.nslots);
+        if (!global_find_or_insert(t, k, sl, *reinterpret_cast<volatile long long*>(&t.keys[sl]), max_probe)) {
           atomicOr(&deferred[i >> 5], 1u << (i & 31));
           atomicAdd(n_deferred, 1ull);
           continue;
         }
+        s = sl;
       }
     }
     agg_apply<WIDE>(t, spec, cols, i, s);
@@ -497,7 +531,7 @@ k_agg_update_local(GroupKey gk, DevCols cols, int64_t row_lo, int64_t row_hi, Ag
 // fold partial results into the global table; same deferral protocol as k_agg_update
 template <bool WIDE>
 __global__ void __launch_bounds__(256)
-k_agg_merge(AggPartials in, int64_t m, AggTable t, AggSpec spec, unsigned long long max_fill, unsigned long long* fill,
+k_agg_merge(AggPartials in, int64_t m, int nstates, AggTable t, AggSpec spec, uint32_t max_probe,
             uint32_t* deferred, const uint32_t* only, unsigned long long* n_deferred) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -507,46 +541,23 @@ k_agg_merge(AggPartials in, int64_t m, AggTable t, AggSpec spec, unsigned long l
     if (in.kind[i] == 1) s = t.nslots;
     else if (in.kind[i] == 2) s = t.nslots + 1;
     else {
-      long long k = in.keys[i];
-      s = agg_home(k, t.nslots);
-      bool defer = false;
-      unsigned int steps = 0;
-      for (;;) {
-        long long cur = *reinterpret_cast<volatile long long*>(&t.keys[s]);
-        if (cur == k) break;
-        if (cur == kEmptyKey) {
-          unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(&t.keys[s]), (unsigned long long)kEmptyKey, (unsigned long long)k);
-          if (old == (unsigned long long)kEmptyKey || old == (unsigned long long)k) break;
-        }
-        if (++steps > (unsigned int)max_fill) { defer = true; break; }
-        if (++s == t.nslots) s = 0;
+      const long long k = in.keys[i];
+      uint32_t sl = agg_home(k, t.nslots);
+      if (!global_find_or_insert(t, k, sl, *reinterpret_cast<volatile long long*>(&t.keys[sl]), max_probe)) {
+        atomicOr(&deferred[i >> 5], 1u << (i & 31));
+        atomicAdd(n_deferred, 1ull);
+        continue;
       }
-      if (defer) { atomicOr(&deferred[i >> 5], 1u << (i & 31)); atomicAdd(n_deferred, 1ull); continue; }
+      s = sl;
     }
-    atomicAdd(&t.rows[s], in.rows[i]);
-    for (int k = 0; k < spec.n; k++) {
-      const AggFuncDev& f = spec.f[k];
-      if (f.s0 >= 0) {
-        unsigned long long v = in.state[f.s0][i];
-        switch (f.name) {
-          case TG_AGG_COUNT: atomicAdd(&t.state[f.s0][s], v); break;                                                  // countPartial merge func_count.go:481
-          case TG_AGG_SUM: case TG_AGG_AVG:   // func_sum.go:106, func_avg.go:444
-            if (WIDE && f.s3 >= 0) dec3_add(&t.state[f.s0][s], &t.state[f.s2][s], &t.state[f.s3][s], v, in.state[f.s2][i], in.state[f.s3][i]);
-            else if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, in.state[f.s2][i]);
-            else atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v));
-            break;
-          case TG_AGG_MIN: atomicMin(&t.state[f.s0][s], v); break;
-          case TG_AGG_MAX: atomicMax(&t.state[f.s0][s], v); break;
-          default: break;
-        }
-      }
-      if (f.s1 >= 0) atomicAdd(&t.state[f.s1][s], in.state[f.s1][i]);
-    }
+    unsigned long long st[AGG_LOCAL_MAX_STATES];
+    for (int a = 0; a < nstates; a++) st[a] = in.state[a][i];
+    agg_merge_into<WIDE>(t, spec, s, in.rows[i], st);
   }
 }
 
 // re-insert every group of an old table into a bigger one (no atomics on the states: keys are unique)
-__global__ void k_agg_rehash(AggTable oldt, AggTable newt, AggSpec spec, int nstates, unsigned long long* fill) {
+__global__ void k_agg_rehash(AggTable oldt, AggTable newt, int nstates) {
   unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
   unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
   for (; i < oldt.nslots + 2; i += stride) {
@@ -915,6 +926,19 @@ struct AggHostStage {
   int64_t rows = 0;
 };
 
+// words of AggImpl::scalars, the handle's device counters
+enum {
+  SC_COUNT = 0,            // k_agg_count: occupied slots
+  SC_DEFERRED = 1,         // rows an update round deferred
+  SC_CURSOR = 2,           // k_agg_finalize's output cursor
+  SC_V1_TUPLES = 3,        // partial tuples a v1 CTA-local pass emitted
+  SC_MERGE_DEFERRED = 4,   // partial tuples a merge round deferred
+  SC_SPILLED = 5,          // local groups a round-2 update spilled
+  SC_LOCAL_ROWS = 6,       // rows the CTA-local level absorbed, since the table was created (zeroed with it)
+  SC_OVERFLOW = 7,         // spec.err: a fused argument expression left the DOUBLE range
+  SC_DEC_ERR = 8,          // k_dec_to_scaled: a DECIMAL cell not in its column's stored form
+};
+
 }  // namespace tg
 
 using namespace tg;
@@ -968,8 +992,9 @@ struct AggImpl {
   DevBuf tbl_mem;
   AggTable tbl{};
   unsigned long long nslots = 0;
-  DevBuf scalars;              // [0] fill [1] n_deferred [2] out cursor ... [6] rows the CTA-local level absorbed (zeroed with the table) [7] overflow
-  DevBuf deferred, partials_mem;
+  DevBuf scalars;              // counters, SC_* words
+  DevBuf deferred[2];          // row bitmaps of grow_and_retry: one round's input and the next round's
+  DevBuf partials_mem;
   int64_t expected_groups = 0;
   int local_mode = -1;            // -1 undecided, 0 global atomics only, 1 CTA-local partial aggregation first
 
@@ -1261,6 +1286,8 @@ static void layout_table(AggImpl* a, uint8_t* mem, unsigned long long nslots, Ag
 }
 
 static int alloc_table(AggImpl* a, unsigned long long nslots, DevBuf& mem, AggTable& t) {
+  // slots are 32-bit (agg_home, slot32): a bigger table would send every key to one slot
+  if (nslots >= (1ull << 32)) return fail(TG_ERR_OOM, "the aggregation table would need 2^32 slots or more");
   size_t n = (size_t)nslots + 2;
   TG_TRY(mem.ensure(a->device, n * 8 * (size_t)table_record_words(a) + 64));
   layout_table(a, mem.as<uint8_t>(), nslots, t);
@@ -1269,14 +1296,19 @@ static int alloc_table(AggImpl* a, unsigned long long nslots, DevBuf& mem, AggTa
   return TG_OK;
 }
 
-static int grow_table(AggImpl* a, unsigned long long want_slots) {
+// x4, or more: the grown table is at most half full once `more` new groups (deferred items) join a table that was 60 % full
+static unsigned long long grown_slots(unsigned long long cur, unsigned long long more) {
+  return std::max<unsigned long long>(cur * 4, (unsigned long long)((cur * 0.6 + (double)more) * 2));
+}
+
+// grow the group table for `more` new groups: rehash into a grown_slots table
+static int grow_table(AggImpl* a, unsigned long long more) {
+  const unsigned long long want_slots = grown_slots(a->nslots, more);
   std::unique_ptr<DevBuf> nm(new DevBuf());
   AggTable nt{};
   TG_TRY(alloc_table(a, want_slots, *nm, nt));
-  unsigned long long* sc = a->scalars.as<unsigned long long>();
-  TG_CUDA(cudaMemsetAsync(sc, 0, 8, a->stream));
   if (a->nkw) k_agg_rehash_mk<<<agrid(a, (int64_t)a->tbl.nslots), 256, 0, a->stream>>>(a->tbl, nt, a->nstates);
-  else k_agg_rehash<<<agrid(a, (int64_t)a->tbl.nslots + 2), 256, 0, a->stream>>>(a->tbl, nt, a->spec, a->nstates, sc);
+  else k_agg_rehash<<<agrid(a, (int64_t)a->tbl.nslots + 2), 256, 0, a->stream>>>(a->tbl, nt, a->nstates);
   a->stats.kernel_launches++;
   TG_CUDA(cudaStreamSynchronize(a->stream));
   std::swap(a->tbl_mem.p, nm->p); std::swap(a->tbl_mem.cap, nm->cap); std::swap(a->tbl_mem.device, nm->device);
@@ -1293,7 +1325,7 @@ __global__ void k_mark_range(uint32_t* bits, int64_t lo, int64_t hi) {
 static int mark_range_deferred(AggImpl* a, int64_t lo, int64_t hi) {
   // whole 32-bit words with memset, ragged edges with a tiny kernel
   int64_t wlo = (lo + 31) / 32, whi = hi / 32;
-  uint32_t* bits = a->deferred.as<uint32_t>();
+  uint32_t* bits = a->deferred[0].as<uint32_t>();
   if (whi > wlo) TG_CUDA(cudaMemsetAsync(bits + wlo, 0xff, (size_t)(whi - wlo) * 4, a->stream));
   int64_t e1 = std::min<int64_t>(hi, wlo * 32);
   if (lo < e1) { k_mark_range<<<1, 64, 0, a->stream>>>(bits, lo, e1); a->stats.kernel_launches++; }
@@ -1302,184 +1334,185 @@ static int mark_range_deferred(AggImpl* a, int64_t lo, int64_t hi) {
   return TG_OK;
 }
 
-// fold `m` partial-result tuples into the global table, growing it until every tuple found a slot
-static int grow_table(AggImpl* a, unsigned long long want_slots);
-static int merge_partials(AggImpl* a, const AggPartials& pp, unsigned long long m, unsigned long long* sc) {
-  if (m == 0) return TG_OK;
-  DevBuf mdef, mprev;
-  size_t dwords = (size_t)((m + 31) / 32);
-  TG_TRY(mdef.ensure(a->device, dwords * 4 + 16));
-  TG_CUDA(cudaMemsetAsync(mdef.p, 0, dwords * 4, a->stream));
-  TG_CUDA(cudaMemsetAsync(sc + 4, 0, 8, a->stream));
-  const uint32_t* only = nullptr;
-  for (int round = 0; round < 40; round++) {
-    unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
-    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->tbl, a->spec, max_fill, sc, mdef.as<uint32_t>(), only, sc + 4);
-    a->stats.kernel_launches++;
-    a->stats.paths |= TG_AGG_PATH_MERGE;
+// Grow-and-retry, the protocol of every find-or-insert pass into the group table or a DISTINCT set.  launch(deferred,
+// only, nd) runs one round over the pass's `nitems` items (only == nullptr: all of them, else those whose bit is set),
+// sets in `deferred` the bit of every item that found no slot within kAggMaxProbe steps, and reads back their number
+// into nd; grow(nd) makes room for nd new entries.  The next round re-runs just the deferred items.  bits[0] and bits[1]
+// take turns as the bitmap a round writes and the one it reads; `resume`: the items of the first round are the ones
+// already marked in bits[0].
+template <class Launch, class Grow>
+static int grow_and_retry(AggImpl* a, DevBuf (&bits)[2], int64_t nitems, bool resume, const char* what, Launch launch, Grow grow) {
+  const size_t bytes = (size_t)((nitems + 31) / 32) * 4;
+  int cur = resume ? 1 : 0;
+  const uint32_t* only = resume ? bits[0].as<uint32_t>() : nullptr;
+  for (int round = 0;; round++) {
+    TG_TRY(bits[cur].ensure(a->device, bytes + 16));
+    TG_CUDA(cudaMemsetAsync(bits[cur].p, 0, bytes, a->stream));
     unsigned long long nd = 0;
-    TG_CUDA(cudaMemcpyAsync(&nd, sc + 4, 8, cudaMemcpyDeviceToHost, a->stream));
-    TG_CUDA(cudaStreamSynchronize(a->stream));
-    if (nd == 0) break;
-    unsigned long long want = std::max<unsigned long long>(a->nslots * 4, (unsigned long long)((a->nslots * 0.6 + (double)nd) * 2));
-    TG_TRY(grow_table(a, want));
-    TG_TRY(mprev.ensure(a->device, dwords * 4 + 16));
-    TG_CUDA(cudaMemcpyAsync(mprev.p, mdef.p, dwords * 4, cudaMemcpyDeviceToDevice, a->stream));
-    TG_CUDA(cudaMemsetAsync(mdef.p, 0, dwords * 4, a->stream));
-    TG_CUDA(cudaMemsetAsync(sc + 4, 0, 8, a->stream));
-    only = mprev.as<uint32_t>();
-    if (round == 39) return fail(TG_ERR_CUDA, "internal: aggregation merge failed to converge");
+    TG_TRY(launch(bits[cur].as<uint32_t>(), only, nd));
+    if (nd == 0) return TG_OK;
+    // x4 per round: 40 rounds are never reached
+    if (round == 39) return fail(TG_ERR_CUDA, std::string("internal: ") + what + " failed to converge");
+    TG_TRY(grow(nd));
+    only = bits[cur].as<uint32_t>();
+    cur ^= 1;
   }
+}
+
+// one 8-byte counter back to the host (synchronises the stream)
+static int read_back(AggImpl* a, const unsigned long long* counter, unsigned long long& v) {
+  TG_CUDA(cudaMemcpyAsync(&v, counter, 8, cudaMemcpyDeviceToHost, a->stream));
+  TG_CUDA(cudaStreamSynchronize(a->stream));
   return TG_OK;
 }
 
-static void layout_partials(uint8_t* base, size_t cap, int nstates, unsigned long long* count, AggPartials& pp) {
-  pp.keys = reinterpret_cast<long long*>(base); base += cap * 8;
-  pp.rows = reinterpret_cast<unsigned long long*>(base); base += cap * 8;
-  for (int s = 0; s < nstates; s++) { pp.state[s] = reinterpret_cast<unsigned long long*>(base); base += cap * 8; }
-  pp.kind = base;
-  pp.count = count;
+// fold `m` partial-result tuples into the global table, growing it until every tuple found a slot
+static int merge_partials(AggImpl* a, const AggPartials& pp, unsigned long long m, unsigned long long* sc) {
+  if (m == 0) return TG_OK;
+  DevBuf bits[2];
+  return grow_and_retry(a, bits, (int64_t)m, false, "aggregation merge", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+    TG_CUDA(cudaMemsetAsync(sc + SC_MERGE_DEFERRED, 0, 8, a->stream));
+    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->nstates, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_MERGE_DEFERRED);
+    a->stats.kernel_launches++;
+    a->stats.paths |= TG_AGG_PATH_MERGE;
+    return read_back(a, sc + SC_MERGE_DEFERRED, nd);
+  }, [&](unsigned long long nd) { return grow_table(a, nd); });
 }
 
-// several GROUP BY columns: global tag-claimed table only (k_agg_update_mk), same grow-and-retry protocol
+// columnar partial-result tuples of `cap` entries in partials_mem: keys, rows, one array per state, kind
+static int alloc_partials(AggImpl* a, size_t cap, unsigned long long* count, AggPartials& pp) {
+  TG_TRY(a->partials_mem.ensure(a->device, cap * (8 + 8 + 8 * (size_t)a->nstates + 1) + 256));
+  uint8_t* base = a->partials_mem.as<uint8_t>();
+  pp.keys = reinterpret_cast<long long*>(base); base += cap * 8;
+  pp.rows = reinterpret_cast<unsigned long long*>(base); base += cap * 8;
+  for (int s = 0; s < a->nstates; s++) { pp.state[s] = reinterpret_cast<unsigned long long*>(base); base += cap * 8; }
+  pp.kind = base;
+  pp.count = count;
+  return TG_OK;
+}
+
+// TG_AGG_LOCAL_SLOTS, the CTA-local table's slots for sweeps: 512, 1024, 2048 or 4096; 0 when unset or any other value
+static int env_local_slots() {
+  const int v = env_int("TG_AGG_LOCAL_SLOTS", 0);
+  return (v == 512 || v == 1024 || v == 2048 || v == 4096) ? v : 0;
+}
+
+// several GROUP BY columns: global tag-claimed table only (k_agg_update_mk)
 static int update_grouped_mk(AggImpl* a, const DevCols& cols, int64_t n, unsigned long long* sc) {
-  size_t dwords = (size_t)((n + 31) / 32);
-  TG_TRY(a->deferred.ensure(a->device, dwords * 4 + 16));
-  TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
   GroupKeys gk{};
   gk.n = (int)a->group_cols.size(); gk.nkw = a->nkw;
   for (int q = 0; q < gk.n; q++) { gk.data[q] = cols.data[a->group_cols[q]]; gk.nulls[q] = cols.nulls[a->group_cols[q]]; gk.kind[q] = a->group_kinds[q]; }
-  DevBuf prev_deferred;
-  const uint32_t* only = nullptr;
-  for (int round = 0; round < 40; round++) {
-    TG_CUDA(cudaMemsetAsync(sc + 1, 0, 8, a->stream));
-    (a->wide ? k_agg_update_mk<true> : k_agg_update_mk<false>)<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, 48u, a->deferred.as<uint32_t>(), only, sc + 1);
+  return grow_and_retry(a, a->deferred, n, false, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+    TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
+    (a->wide ? k_agg_update_mk<true> : k_agg_update_mk<false>)<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_DEFERRED);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_MULTI_KEY;
-    unsigned long long nd = 0;
-    TG_CUDA(cudaMemcpyAsync(&nd, sc + 1, 8, cudaMemcpyDeviceToHost, a->stream));
-    TG_CUDA(cudaStreamSynchronize(a->stream));
-    if (nd == 0) break;
-    unsigned long long want = std::max<unsigned long long>(a->nslots * 4, (unsigned long long)((a->nslots * 0.6 + (double)nd) * 2));
-    TG_TRY(grow_table(a, want));
-    TG_TRY(prev_deferred.ensure(a->device, dwords * 4 + 16));
-    TG_CUDA(cudaMemcpyAsync(prev_deferred.p, a->deferred.p, dwords * 4, cudaMemcpyDeviceToDevice, a->stream));
-    TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
-    only = prev_deferred.as<uint32_t>();
-    if (round == 39) return fail(TG_ERR_CUDA, "internal: aggregation table failed to converge");
-  }
-  return TG_OK;
+    return read_back(a, sc + SC_DEFERRED, nd);
+  }, [&](unsigned long long nd) { return grow_table(a, nd); });
 }
 
 // Round-2 update path (agg_update.cuh): one two-level kernel per round; rows / local groups that found no slot are re-run
 // after the table has grown.
 static int update_grouped_v2(AggImpl* a, const GroupKey& gk, const DevCols& cols, int64_t n, unsigned long long* sc) {
-  size_t dwords = (size_t)((n + 31) / 32);
-  TG_TRY(a->deferred.ensure(a->device, dwords * 4 + 16));
-  TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
   // CTA-local level: on for small / unknown cardinalities (a CTA turns it off by itself when its hit rate is low)
-  const int env_local = env_int("TG_AGG_LOCAL", 1), env_slots = env_int("TG_AGG_LOCAL_SLOTS", 0);
+  const int env_local = env_int("TG_AGG_LOCAL", 1), env_slots = env_local_slots();
   bool local = env_local != 0 && a->nstates <= AGG_LOCAL_MAX_STATES && (a->expected_groups == 0 || a->expected_groups <= 4096);
   if (env_local == 2) local = a->nstates <= AGG_LOCAL_MAX_STATES;
-  int local_slots = (env_slots == 512 || env_slots == 1024 || env_slots == 2048 || env_slots == 4096) ? env_slots : 2048;
+  int local_slots = env_slots ? env_slots : 2048;
   size_t smem = (size_t)(local_slots + 2) * 8 * (2 + a->nstates);
   while (local && smem > (100u << 10) && local_slots > 512) { local_slots /= 2; smem = (size_t)(local_slots + 2) * 8 * (2 + a->nstates); }
   int per_sm = local ? (int)std::max<size_t>(1, std::min<size_t>(4, (200u << 10) / smem)) : 8;
   int grid = (int)std::min<int64_t>((n + AGG2_TILE - 1) / AGG2_TILE, (int64_t)a->nsm * per_sm);
   if (grid < 1) grid = 1;
   Agg2Params p{};
-  p.gk = gk; p.n = n; p.max_probe = 48; p.nstates = a->nstates; p.local_slots = local ? local_slots : 0;
-  p.deferred = a->deferred.as<uint32_t>(); p.only = nullptr; p.n_deferred = sc + 1; p.local_rows = sc + 6;
+  p.gk = gk; p.n = n; p.max_probe = kAggMaxProbe; p.nstates = a->nstates; p.local_slots = local ? local_slots : 0;
+  p.n_deferred = sc + SC_DEFERRED; p.local_rows = sc + SC_LOCAL_ROWS;
   if (local) {
     p.spill_cap = (unsigned long long)grid * (size_t)(local_slots + 2);
-    size_t per = 8 + 8 + 8 * (size_t)a->nstates + 1;
-    TG_TRY(a->partials_mem.ensure(a->device, (size_t)p.spill_cap * per + 256));
-    layout_partials(a->partials_mem.as<uint8_t>(), (size_t)p.spill_cap, a->nstates, sc + 5, p.spill);
+    TG_TRY(alloc_partials(a, (size_t)p.spill_cap, sc + SC_SPILLED, p.spill));
     TG_CUDA(cudaFuncSetAttribute(a->wide ? k_agg_update2<true, true> : k_agg_update2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
-  DevBuf prev_deferred;
-  for (int round = 0; round < 40; round++) {
-    TG_CUDA(cudaMemsetAsync(sc + 1, 0, 8, a->stream));
-    TG_CUDA(cudaMemsetAsync(sc + 5, 0, 8, a->stream));
-    if (local && round == 0) (a->wide ? k_agg_update2<true, true> : k_agg_update2<true, false>)<<<grid, AGG2_BLOCK, smem, a->stream>>>(p, cols, a->tbl, a->spec);
+  // local groups of the first round that found no global slot (p.spill): the table grows for them as well, then merges them
+  unsigned long long spilled = 0;
+  auto grow = [&](unsigned long long nd) {
+    TG_TRY(grow_table(a, nd + spilled));
+    const unsigned long long m = spilled;
+    spilled = 0;
+    return merge_partials(a, p.spill, m, sc);
+  };
+  TG_TRY(grow_and_retry(a, a->deferred, n, false, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+    const bool lvl = local && !only;   // the CTA-local level runs in the first round
+    TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
+    TG_CUDA(cudaMemsetAsync(sc + SC_SPILLED, 0, 8, a->stream));
+    p.deferred = deferred; p.only = only;
+    if (lvl) (a->wide ? k_agg_update2<true, true> : k_agg_update2<true, false>)<<<grid, AGG2_BLOCK, smem, a->stream>>>(p, cols, a->tbl, a->spec);
     else (a->wide ? k_agg_update2<false, true> : k_agg_update2<false, false>)<<<grid, AGG2_BLOCK, 0, a->stream>>>(p, cols, a->tbl, a->spec);
     a->stats.kernel_launches++;
-    a->stats.paths |= (local && round == 0) ? TG_AGG_PATH_V2_LOCAL : TG_AGG_PATH_V2_GLOBAL;
+    a->stats.paths |= lvl ? TG_AGG_PATH_V2_LOCAL : TG_AGG_PATH_V2_GLOBAL;
     unsigned long long back[8] = {0};
     TG_CUDA(cudaMemcpyAsync(back, sc, 64, cudaMemcpyDeviceToHost, a->stream));
     TG_CUDA(cudaStreamSynchronize(a->stream));
-    a->stats.local_rows = (int64_t)back[6];   // cumulative since the table was created
-    const unsigned long long nd = back[1], spilled = (local && round == 0) ? back[5] : 0;
-    if (nd == 0 && spilled == 0) break;
+    a->stats.local_rows = (int64_t)back[SC_LOCAL_ROWS];
+    nd = back[SC_DEFERRED];
+    if (lvl) spilled = back[SC_SPILLED];
     if (spilled > p.spill_cap) return fail(TG_ERR_CUDA, "internal: aggregation spill buffer overflow");
-    // grow x4 (at least enough for every deferred row / spilled group to be a new group), then re-run just those
-    unsigned long long want = std::max<unsigned long long>(a->nslots * 4, (unsigned long long)((a->nslots * 0.6 + (double)(nd + spilled)) * 2));
-    TG_TRY(grow_table(a, want));
-    p.max_probe = 48;
-    if (spilled) TG_TRY(merge_partials(a, p.spill, spilled, sc));
-    if (nd == 0) break;
-    TG_TRY(prev_deferred.ensure(a->device, dwords * 4 + 16));
-    TG_CUDA(cudaMemcpyAsync(prev_deferred.p, a->deferred.p, dwords * 4, cudaMemcpyDeviceToDevice, a->stream));
-    TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
-    p.only = prev_deferred.as<uint32_t>();
-    if (round == 39) return fail(TG_ERR_CUDA, "internal: aggregation table failed to converge");
-  }
-  return TG_OK;
+    return TG_OK;
+  }, grow));
+  return spilled ? grow(0) : TG_OK;
 }
 
 // rows [lo, hi): CTA-local partial aggregation, then merge of the partial results into the global table
 static int local_partial_pass(AggImpl* a, const GroupKey& gk, const DevCols& cols, int64_t lo, int64_t hi, unsigned long long* sc) {
-  int local_slots = 1024;   // bigger tables lose more to occupancy than they gain (TG_AGG_LOCAL_SLOTS overrides for sweeps)
-  if (const char* e = getenv("TG_AGG_LOCAL_SLOTS")) { int v = atoi(e); if (v == 512 || v == 1024 || v == 2048 || v == 4096) local_slots = v; }
-  size_t smem_per_cta = (size_t)(local_slots + 2) * 8 * (2 + a->nstates);
-  int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (200u << 10) / smem_per_cta));
-  int grid = agrid(a, hi - lo, 256, per_sm);
-  size_t cap = (size_t)grid * (local_slots / 2 + 2);
-  size_t per = 8 /*keys*/ + 8 /*rows*/ + 8 * (size_t)a->nstates + 1 /*kind*/;
-  TG_TRY(a->partials_mem.ensure(a->device, cap * per + 256));
+  const int env_slots = env_local_slots();
+  const int local_slots = env_slots ? env_slots : 1024;   // bigger tables lose more to occupancy than they gain
+  const size_t smem = (size_t)(local_slots + 2) * 8 * (2 + a->nstates);
+  const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (200u << 10) / smem));
+  const int grid = agrid(a, hi - lo, 256, per_sm);
   AggPartials pp{};
-  uint8_t* base = a->partials_mem.as<uint8_t>();
-  pp.keys = reinterpret_cast<long long*>(base); base += cap * 8;
-  pp.rows = reinterpret_cast<unsigned long long*>(base); base += cap * 8;
-  for (int s = 0; s < a->nstates; s++) { pp.state[s] = reinterpret_cast<unsigned long long*>(base); base += cap * 8; }
-  pp.kind = base;
-  pp.count = sc + 3;
-  TG_CUDA(cudaMemsetAsync(sc + 3, 0, 8, a->stream));
-  size_t smem = (size_t)(local_slots + 2) * 8 * (2 + a->nstates);
+  TG_TRY(alloc_partials(a, (size_t)grid * (local_slots / 2 + 2), sc + SC_V1_TUPLES, pp));
+  TG_CUDA(cudaMemsetAsync(sc + SC_V1_TUPLES, 0, 8, a->stream));
   TG_CUDA(cudaFuncSetAttribute(a->wide ? k_agg_update_local<true> : k_agg_update_local<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  (a->wide ? k_agg_update_local<true> : k_agg_update_local<false>)<<<grid, 256, smem, a->stream>>>(gk, cols, lo, hi, a->spec, a->nstates, local_slots, pp, a->deferred.as<uint32_t>(), sc + 1);
+  (a->wide ? k_agg_update_local<true> : k_agg_update_local<false>)<<<grid, 256, smem, a->stream>>>(gk, cols, lo, hi, a->spec, a->nstates, local_slots, pp, a->deferred[0].as<uint32_t>(), sc + SC_DEFERRED);
   a->stats.kernel_launches++;
   a->stats.paths |= TG_AGG_PATH_V1_LOCAL;
   unsigned long long m = 0;
-  TG_CUDA(cudaMemcpyAsync(&m, sc + 3, 8, cudaMemcpyDeviceToHost, a->stream));
-  TG_CUDA(cudaStreamSynchronize(a->stream));
-  if (m == 0) return TG_OK;
-  // merge with its own grow-and-retry loop (tuples, not rows)
-  DevBuf mdef, mprev;
-  size_t dwords = (size_t)((m + 31) / 32);
-  TG_TRY(mdef.ensure(a->device, dwords * 4 + 16));
-  TG_CUDA(cudaMemsetAsync(mdef.p, 0, dwords * 4, a->stream));
-  TG_CUDA(cudaMemsetAsync(sc + 4, 0, 8, a->stream));
-  const uint32_t* only = nullptr;
-  for (int round = 0; round < 40; round++) {
-    unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
-    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->tbl, a->spec, max_fill, sc, mdef.as<uint32_t>(), only, sc + 4);
-    a->stats.kernel_launches++;
-    a->stats.paths |= TG_AGG_PATH_MERGE;
-    unsigned long long nd = 0;
-    TG_CUDA(cudaMemcpyAsync(&nd, sc + 4, 8, cudaMemcpyDeviceToHost, a->stream));
-    TG_CUDA(cudaStreamSynchronize(a->stream));
-    if (nd == 0) break;
-    unsigned long long want = std::max<unsigned long long>(a->nslots * 4, (unsigned long long)((a->nslots * 0.6 + (double)nd) * 2));
-    TG_TRY(grow_table(a, want));
-    TG_TRY(mprev.ensure(a->device, dwords * 4 + 16));
-    TG_CUDA(cudaMemcpyAsync(mprev.p, mdef.p, dwords * 4, cudaMemcpyDeviceToDevice, a->stream));
-    TG_CUDA(cudaMemsetAsync(mdef.p, 0, dwords * 4, a->stream));
-    TG_CUDA(cudaMemsetAsync(sc + 4, 0, 8, a->stream));
-    only = mprev.as<uint32_t>();
-    if (round == 39) return fail(TG_ERR_CUDA, "internal: aggregation merge failed to converge");
+  TG_TRY(read_back(a, sc + SC_V1_TUPLES, m));
+  return merge_partials(a, pp, m, sc);
+}
+
+// Legacy update (TG_AGG_V1=1).  Phase 1 (low cardinality): CTA-local partial passes, decided on a 1M-row sample when there
+// is no hint; phase 2: global atomics on every row, or on the rows phase 1 deferred, growing the table on demand.
+static int update_grouped_v1(AggImpl* a, const GroupKey& gk, const DevCols& cols, int64_t n, unsigned long long* sc) {
+  const bool try_local = a->nstates <= AGG_LOCAL_MAX_STATES && a->local_mode != 0 &&
+                         (a->local_mode == 1 || a->expected_groups == 0 || a->expected_groups <= 2 * AGG_LOCAL_SLOTS_MAX);
+  if (try_local) {
+    const size_t bytes = (size_t)((n + 31) / 32) * 4;
+    TG_TRY(a->deferred[0].ensure(a->device, bytes + 16));
+    TG_CUDA(cudaMemsetAsync(a->deferred[0].p, 0, bytes, a->stream));
+    TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
+    unsigned long long nd = 0;   // rows the passes so far deferred
+    int64_t done = 0;
+    while (done < n) {
+      int64_t hi = (a->local_mode == 1) ? n : std::min<int64_t>(n, done + (1ll << 20));
+      TG_TRY(local_partial_pass(a, gk, cols, done, hi, sc));
+      TG_TRY(read_back(a, sc + SC_DEFERRED, nd));
+      int64_t span = hi - done;
+      done = hi;
+      // Keep the CTA-local phase while it absorbs a useful share of the rows: shared-memory atomics (LSU) and L2 atomics
+      // are different engines, so splitting the rows between them beats sending all of them to either one.
+      if (a->local_mode < 0) a->local_mode = (nd * 10 <= (unsigned long long)span * 7) ? 1 : 0;
+      if (a->local_mode == 0) break;
+    }
+    if (done < n) TG_TRY(mark_range_deferred(a, done, n));   // the rest of the batch goes through the global kernel
+    else if (nd == 0) return TG_OK;
   }
-  return TG_OK;
+  return grow_and_retry(a, a->deferred, n, try_local, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+    TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
+    (a->wide ? k_agg_update<true> : k_agg_update<false>)<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_DEFERRED);
+    a->stats.kernel_launches++;
+    a->stats.paths |= TG_AGG_PATH_V1_GLOBAL;
+    return read_back(a, sc + SC_DEFERRED, nd);
+  }, [&](unsigned long long nd) { return grow_table(a, nd); });
 }
 
 // aggregate n device-resident rows
@@ -1488,7 +1521,7 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
   a->stats.input_rows += n;
   TG_TRY(a->scalars.ensure(a->device, 64));
   unsigned long long* sc = a->scalars.as<unsigned long long>();
-  a->spec.err = sc + 7;    // raised by a fused argument expression that left the DOUBLE range (types.ErrOverflow)
+  a->spec.err = sc + SC_OVERFLOW;    // raised by a fused argument expression that left the DOUBLE range (types.ErrOverflow)
   if (a->nslots == 0) {
     unsigned long long want = 1024;
     if (a->group_col >= 0) {
@@ -1504,84 +1537,11 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
     (a->wide ? k_agg_update_nogroup<true> : k_agg_update_nogroup<false>)<<<agrid(a, n, 256, 4), 256, 0, a->stream>>>(cols, n, a->tbl, a->spec);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_NOGROUP;
+  } else if (a->nkw) {
+    TG_TRY(update_grouped_mk(a, cols, n, sc));
   } else {
-    if (a->nkw) {
-      TG_TRY(update_grouped_mk(a, cols, n, sc));
-      TG_CUDA(cudaEventRecord(a->ev1, a->stream));
-      TG_CUDA(cudaStreamSynchronize(a->stream));
-      TG_CUDA(cudaGetLastError());
-      float ms3 = 0; cudaEventElapsedTime(&ms3, a->ev0, a->ev1); a->stats.update_ms += ms3;
-      return TG_OK;
-    }
-    GroupKey gk{cols.data[a->group_col], cols.nulls[a->group_col], a->gk_kind, 0};
-    if (!env_int("TG_AGG_V1", 0)) {
-      TG_TRY(update_grouped_v2(a, gk, cols, n, sc));
-      TG_CUDA(cudaEventRecord(a->ev1, a->stream));
-      TG_CUDA(cudaStreamSynchronize(a->stream));
-      TG_CUDA(cudaGetLastError());
-      float ms2 = 0; cudaEventElapsedTime(&ms2, a->ev0, a->ev1); a->stats.update_ms += ms2;
-      return TG_OK;
-    }
-    size_t dwords = (size_t)((n + 31) / 32);
-    TG_TRY(a->deferred.ensure(a->device, dwords * 4 + 16));
-    TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
-    TG_CUDA(cudaMemsetAsync(sc + 1, 0, 8, a->stream));
-    bool have_deferred = false;
-    // ---- phase 1 (low cardinality): CTA-local partial aggregation, decided on a 1M-row sample when there is no hint ----
-    bool try_local = a->nstates <= AGG_LOCAL_MAX_STATES && a->local_mode != 0 &&
-                     (a->local_mode == 1 || a->expected_groups == 0 || a->expected_groups <= 2 * AGG_LOCAL_SLOTS_MAX);
-    if (try_local) {
-      int64_t done = 0;
-      while (done < n) {
-        int64_t hi = (a->local_mode == 1) ? n : std::min<int64_t>(n, done + (1ll << 20));
-        TG_TRY(local_partial_pass(a, gk, cols, done, hi, sc));
-        unsigned long long nd = 0;
-        TG_CUDA(cudaMemcpyAsync(&nd, sc + 1, 8, cudaMemcpyDeviceToHost, a->stream));
-        TG_CUDA(cudaStreamSynchronize(a->stream));
-        int64_t span = hi - done;
-        done = hi;
-        if (nd) have_deferred = true;
-        // Keep the CTA-local phase while it absorbs a useful share of the rows: shared-memory atomics (LSU) and L2 atomics
-        // are different engines, so splitting the rows between them beats sending all of them to either one.
-        if (a->local_mode < 0) a->local_mode = (nd * 10 <= (unsigned long long)span * 7) ? 1 : 0;
-        if (a->local_mode == 0) break;
-      }
-      if (done < n) {   // the rest of the batch goes through the global kernel: mark it "deferred"
-        TG_TRY(mark_range_deferred(a, done, n));
-        have_deferred = true;
-      }
-      TG_CUDA(cudaMemsetAsync(sc + 1, 0, 8, a->stream));
-    }
-    // ---- phase 2: global atomics on every row (or only the deferred ones), growing the table on demand ----
-    if (!try_local || have_deferred) {
-      DevBuf prev_deferred;
-      const uint32_t* only = nullptr;
-      if (try_local) {
-        TG_TRY(prev_deferred.ensure(a->device, dwords * 4 + 16));
-        TG_CUDA(cudaMemcpyAsync(prev_deferred.p, a->deferred.p, dwords * 4, cudaMemcpyDeviceToDevice, a->stream));
-        TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
-        only = prev_deferred.as<uint32_t>();
-      }
-      for (int round = 0; round < 40; round++) {
-        unsigned long long max_fill = 48;   // probe-length limit (see k_agg_update)
-        (a->wide ? k_agg_update<true> : k_agg_update<false>)<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, max_fill, sc, a->deferred.as<uint32_t>(), only, sc + 1);
-        a->stats.kernel_launches++;
-        a->stats.paths |= TG_AGG_PATH_V1_GLOBAL;
-        unsigned long long nd = 0;
-        TG_CUDA(cudaMemcpyAsync(&nd, sc + 1, 8, cudaMemcpyDeviceToHost, a->stream));
-        TG_CUDA(cudaStreamSynchronize(a->stream));
-        if (nd == 0) break;
-        // grow x4 (at least enough for every deferred row to be a new group), re-run only the deferred rows
-        unsigned long long want = std::max<unsigned long long>(a->nslots * 4, (unsigned long long)((a->nslots * 0.6 + (double)nd) * 2));
-        TG_TRY(grow_table(a, want));
-        TG_TRY(prev_deferred.ensure(a->device, dwords * 4 + 16));
-        TG_CUDA(cudaMemcpyAsync(prev_deferred.p, a->deferred.p, dwords * 4, cudaMemcpyDeviceToDevice, a->stream));
-        TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
-        TG_CUDA(cudaMemsetAsync(sc + 1, 0, 8, a->stream));
-        only = prev_deferred.as<uint32_t>();
-        if (round == 39) return fail(TG_ERR_CUDA, "internal: aggregation table failed to converge");
-      }
-    }
+    const GroupKey gk{cols.data[a->group_col], cols.nulls[a->group_col], a->gk_kind, 0};
+    TG_TRY(env_int("TG_AGG_V1", 0) ? update_grouped_v1(a, gk, cols, n, sc) : update_grouped_v2(a, gk, cols, n, sc));
   }
   TG_CUDA(cudaEventRecord(a->ev1, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
@@ -1592,11 +1552,11 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
 
 // DECIMAL argument columns of the batch -> int64 scratch columns (k_dec_to_scaled), checked before any update kernel runs:
 // a cell not in its column's stored form fails the push with the group table untouched.  One 8-byte read-back and one
-// synchronisation per batch; the error word is scalars[8], next to the overflow word of spec.err.
+// synchronisation per batch; the error word is scalars[SC_DEC_ERR], next to the overflow word of spec.err.
 static int decode_decimal_args(AggImpl* a, DevCols& cols, int64_t n) {
   if (n == 0 || std::find(a->dec_decode.begin(), a->dec_decode.end(), 1) == a->dec_decode.end()) return TG_OK;
   TG_TRY(a->scalars.ensure(a->device, 72));
-  unsigned long long* err = a->scalars.as<unsigned long long>() + 8;
+  unsigned long long* err = a->scalars.as<unsigned long long>() + SC_DEC_ERR;
   TG_CUDA(cudaMemsetAsync(err, 0, 8, a->stream));
   for (int c = 0; c < a->ncols; c++) {
     if (!a->dec_decode[c]) continue;
@@ -1655,7 +1615,7 @@ static int grow_set(AggImpl* a, AggImpl::SetMem& m, unsigned long long want) {
 
 // k_agg_distinct_mark for every DISTINCT argument column of the batch (after decode_decimal_args: a DECIMAL value is its
 // int64 at the column's scale), then the virtual columns ncols + j point at the values and the mark bits.  A set is sized
-// from its first batch like the group table and grows x4 with the same defer / rehash / re-run loop.
+// from its first batch like the group table and grows x4 through the same grow_and_retry.
 static int distinct_mark(AggImpl* a, DevCols& cols, int64_t n) {
   if (a->dist_cols.empty() || n == 0) return TG_OK;
   TG_TRY(a->dcounters.ensure(a->device, 16));
@@ -1663,36 +1623,26 @@ static int distinct_mark(AggImpl* a, DevCols& cols, int64_t n) {
   GroupKeys gk{};
   gk.n = (int)a->group_cols.size(); gk.nkw = a->dist_gkw;
   for (int q = 0; q < gk.n; q++) { gk.data[q] = cols.data[a->group_cols[q]]; gk.nulls[q] = cols.nulls[a->group_cols[q]]; gk.kind[q] = a->group_kinds[q]; }
-  const size_t dwords = (size_t)((n + 31) / 32);
-  TG_TRY(a->deferred.ensure(a->device, dwords * 4 + 16));
   TG_CUDA(cudaEventRecord(a->ev0, a->stream));
   for (size_t j = 0; j < a->dist_cols.size(); j++) {
     AggImpl::SetMem& m = *a->dsets[j];
     const int c = a->dist_cols[j];
     if (m.t.nslots == 0) TG_TRY(alloc_set(a, std::max<unsigned long long>(1024, (unsigned long long)std::min<int64_t>(n, 1ll << 22) * 2), m.mem, m.t));
-    TG_TRY(m.mark.ensure(a->device, dwords * 4 + 16));
-    TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
-    DevBuf prev_deferred;
-    const uint32_t* only = nullptr;
-    for (int round = 0; round < 40; round++) {
+    TG_TRY(m.mark.ensure(a->device, (size_t)((n + 31) / 32) * 4 + 16));
+    TG_TRY(grow_and_retry(a, a->deferred, n, false, "DISTINCT set", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
       TG_CUDA(cudaMemsetAsync(cnt, 0, 16, a->stream));
       k_agg_distinct_mark<<<agrid(a, n), 256, 0, a->stream>>>(gk, static_cast<const long long*>(cols.data[c]), cols.nulls[c],
-                                                               a->types[c] == TG_TYPE_DOUBLE, n, m.t, 48u, m.mark.as<uint32_t>(),
-                                                               a->deferred.as<uint32_t>(), only, cnt);
+                                                               a->types[c] == TG_TYPE_DOUBLE, n, m.t, kAggMaxProbe, m.mark.as<uint32_t>(),
+                                                               deferred, only, cnt);
       a->stats.kernel_launches++;
       a->dstats.launches++;
       unsigned long long back[2] = {0, 0};
       TG_CUDA(cudaMemcpyAsync(back, cnt, 16, cudaMemcpyDeviceToHost, a->stream));
       TG_CUDA(cudaStreamSynchronize(a->stream));
       a->dstats.pairs += (int64_t)back[1];
-      if (back[0] == 0) break;
-      if (round == 39) return fail(TG_ERR_CUDA, "internal: DISTINCT set failed to converge");
-      TG_TRY(grow_set(a, m, std::max<unsigned long long>(m.t.nslots * 4, (unsigned long long)((m.t.nslots * 0.6 + (double)back[0]) * 2))));
-      TG_TRY(prev_deferred.ensure(a->device, dwords * 4 + 16));
-      TG_CUDA(cudaMemcpyAsync(prev_deferred.p, a->deferred.p, dwords * 4, cudaMemcpyDeviceToDevice, a->stream));
-      TG_CUDA(cudaMemsetAsync(a->deferred.p, 0, dwords * 4, a->stream));
-      only = prev_deferred.as<uint32_t>();
-    }
+      nd = back[0];
+      return TG_OK;
+    }, [&](unsigned long long nd) { return grow_set(a, m, grown_slots(m.t.nslots, nd)); }));
     cols.data[a->ncols + j] = cols.data[c];
     cols.nulls[a->ncols + j] = m.mark.as<uint8_t>();
     cols.elem_len[a->ncols + j] = 8;
@@ -1711,7 +1661,7 @@ static int update_after_decode(AggImpl* a, DevCols& cols, int64_t n) {
   for (int k = 0; k < a->spec.n; k++) has_expr |= a->spec.f[k].arg_expr != TG_ARGEXPR_COL;
   if (!has_expr || n == 0) return TG_OK;
   unsigned long long e = 0;
-  TG_CUDA(cudaMemcpyAsync(&e, a->scalars.as<unsigned long long>() + 7, 8, cudaMemcpyDeviceToHost, a->stream));
+  TG_CUDA(cudaMemcpyAsync(&e, a->scalars.as<unsigned long long>() + SC_OVERFLOW, 8, cudaMemcpyDeviceToHost, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
   if (e) return fail(TG_ERR_OVERFLOW, "ErrOverflow: DOUBLE value is out of range in an aggregate argument expression");
   return TG_OK;
@@ -1825,10 +1775,10 @@ static int afinalize(AggImpl* a) {
     a->nslots = 1024;
   }
   unsigned long long fill = 0;
-  TG_CUDA(cudaMemsetAsync(sc, 0, 8, a->stream));
-  k_agg_count<<<agrid(a, (int64_t)a->nslots + 2), 256, 0, a->stream>>>(a->tbl, sc);
+  TG_CUDA(cudaMemsetAsync(sc + SC_COUNT, 0, 8, a->stream));
+  k_agg_count<<<agrid(a, (int64_t)a->nslots + 2), 256, 0, a->stream>>>(a->tbl, sc + SC_COUNT);
   a->stats.kernel_launches++;
-  TG_CUDA(cudaMemcpyAsync(&fill, sc, 8, cudaMemcpyDeviceToHost, a->stream));
+  TG_CUDA(cudaMemcpyAsync(&fill, sc + SC_COUNT, 8, cudaMemcpyDeviceToHost, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
   int64_t cap = (int64_t)fill + 2 + 1;
   AggOut ao{};
@@ -1839,11 +1789,11 @@ static int afinalize(AggImpl* a) {
     if (a->out_nullable[k] || default_row) { TG_TRY(a->out_valid[k]->ensure(a->device, (size_t)cap + 16)); ao.valid[k] = a->out_valid[k]->as<uint8_t>(); }
   }
   TG_CUDA(cudaEventRecord(a->ev0, a->stream));
-  TG_CUDA(cudaMemsetAsync(sc + 2, 0, 8, a->stream));
-  (a->wide ? k_agg_finalize<true, true> : a->dec_out ? k_agg_finalize<true, false> : k_agg_finalize<false, false>)<<<agrid(a, (int64_t)a->nslots + 2), 256, 0, a->stream>>>(a->tbl, a->spec, a->gk_kind, ao, sc + 2);
+  TG_CUDA(cudaMemsetAsync(sc + SC_CURSOR, 0, 8, a->stream));
+  (a->wide ? k_agg_finalize<true, true> : a->dec_out ? k_agg_finalize<true, false> : k_agg_finalize<false, false>)<<<agrid(a, (int64_t)a->nslots + 2), 256, 0, a->stream>>>(a->tbl, a->spec, a->gk_kind, ao, sc + SC_CURSOR);
   a->stats.kernel_launches++;
   unsigned long long nrows = 0;
-  TG_CUDA(cudaMemcpyAsync(&nrows, sc + 2, 8, cudaMemcpyDeviceToHost, a->stream));
+  TG_CUDA(cudaMemcpyAsync(&nrows, sc + SC_CURSOR, 8, cudaMemcpyDeviceToHost, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
   if (default_row && nrows == 0) {
     // write the default row on the host side: COUNT → 0, everything else NULL

@@ -154,48 +154,6 @@ __device__ __forceinline__ void agg_apply2(const AggTable& t, const LocalTable& 
   }
 }
 
-// fold one partial group (rows + states) into global slot s: MergePartialResult (func_sum.go:106, func_count.go:481,
-// func_avg.go:444, func_max_min.go merge)
-template <bool WIDE>
-__device__ __forceinline__ void agg_merge_into(const AggTable& t, const AggSpec& spec, unsigned long long s, unsigned long long rows, const unsigned long long* st) {
-  atomicAdd(&t.rows[s], rows);
-  for (int k = 0; k < spec.n; k++) {
-    const AggFuncDev& f = spec.f[k];
-    if (f.s0 >= 0) {
-      unsigned long long v = st[f.s0];
-      switch (f.name) {
-        case TG_AGG_COUNT: atomicAdd(&t.state[f.s0][s], v); break;
-        case TG_AGG_SUM: case TG_AGG_AVG:
-          if (WIDE && f.s3 >= 0) dec3_add(&t.state[f.s0][s], &t.state[f.s2][s], &t.state[f.s3][s], v, st[f.s2], st[f.s3]);
-          else if (f.s2 >= 0) dec_add(&t.state[f.s0][s], &t.state[f.s2][s], v, st[f.s2]);
-          else atomicAdd(reinterpret_cast<double*>(&t.state[f.s0][s]), __longlong_as_double((long long)v));
-          break;
-        case TG_AGG_MIN: atomicMin(&t.state[f.s0][s], v); break;
-        case TG_AGG_MAX: atomicMax(&t.state[f.s0][s], v); break;
-        default: break;
-      }
-    }
-    if (f.s1 >= 0) atomicAdd(&t.state[f.s1][s], st[f.s1]);
-  }
-}
-
-// find-or-insert `k` in the global table starting at slot s with the slot's current content `cur` already loaded;
-// returns false when the probe sequence exceeds max_probe (table overfull: defer)
-__device__ __forceinline__ bool global_find_or_insert(const AggTable& t, long long k, uint32_t& s, long long cur, uint32_t max_probe) {
-  const uint32_t S = (uint32_t)t.nslots;
-  uint32_t steps = 0;
-  for (;;) {
-    if (cur == k) return true;
-    if (cur == kEmptyKey) {
-      unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(&t.keys[s]), (unsigned long long)kEmptyKey, (unsigned long long)k);
-      if (old == (unsigned long long)kEmptyKey || old == (unsigned long long)k) return true;
-    }
-    if (++steps > max_probe) return false;
-    if (++s == S) s = 0;
-    cur = *reinterpret_cast<volatile long long*>(&t.keys[s]);
-  }
-}
-
 struct Agg2Params {
   GroupKey gk;
   int64_t n;
