@@ -213,7 +213,11 @@ typedef struct tg_join_desc {
   const int32_t* left_key_idx;
   const int32_t* right_key_idx;
   /* output = LUsed columns of left ‖ RUsed columns of right (builder.go:1868-1871).
-   * NULL pointer with n = -1 means "all columns" (the reference's nil slice).                  */
+   * NULL pointer with n = -1 means "all columns" (the reference's nil slice).  Used columns may be 4/8-byte fixed-width
+   * columns or DECIMAL (TG_TYPE_NEWDECIMAL, 40-byte MyDecimal cells) on either side, for every join type: a DECIMAL cell
+   * is moved as its 40 raw bytes, never interpreted, so a non-NULL output cell is bit-identical to its input cell
+   * (non-canonical forms, resultFrac and unused words included) and a cell under NULL is zero bytes.  No key, filter
+   * item or OtherCondition operand may be a DECIMAL column (TG_ERR_UNSUPPORTED).                                    */
   int32_t n_lused; int32_t n_rused;
   const int32_t* lused; const int32_t* rused;
   /* optional filters evaluated on the build-side / probe-side child chunk                      */
@@ -274,7 +278,8 @@ int tg_join_probe_dev(tg_join* j, const tg_chunk* dev_chk, int64_t* out_rows,
  * 1024), segment s holding seg_cnt_dev[s] valid rows at its start; dev_chk->cols[*].length = nseg*seg_cap.  This is
  * the shape a count-free exchange delivers (tg_partition_exchange_cf: one fixed-capacity region per sending GPU,
  * fill counts known only on the device), so the receiver probes without compacting and without a host round trip.
- * Only for plans the fused fast path covers (tg_join_get_stats().table_mode == 1); others: TG_ERR_UNSUPPORTED.  */
+ * Only for plans the fused fast path covers (tg_join_get_stats().table_mode == 1); others: TG_ERR_UNSUPPORTED.
+ * DECIMAL probe and build output columns are accepted: the fused kernels carry them as row ids, as on the other paths. */
 int tg_join_probe_dev_seg(tg_join* j, const tg_chunk* dev_chk, const int64_t* seg_cnt_dev, int32_t nseg,
                           int64_t seg_cap, int64_t* out_rows, void** out_cols, void** out_nulls);
 
@@ -302,7 +307,8 @@ enum {
   TG_JOIN_PATH_PROBE_SEG = 1 << 3,      /* segment probe over L2-partitioned rows (k_probe_inner_u1_seg_lean)    */
   /* 1 << 4 is unassigned: older headers name a removed kernel with it, so a new path must not reuse it              */
   TG_JOIN_PATH_SCATTER_BULK = 1 << 5,   /* bulk partition scatter (k_partition_scatter_bulk)                     */
-  TG_JOIN_PATH_SCATTER = 1 << 6         /* LSU partition scatter over the whole input (k_partition_scatter)      */
+  TG_JOIN_PATH_SCATTER = 1 << 6,        /* LSU partition scatter over the whole input (k_partition_scatter)      */
+  TG_JOIN_PATH_CELL_GATHER = 0x80       /* 1 << 7: DECIMAL output cells gathered from row ids (k_gather_cells)      */
 };
 int tg_join_get_stats(tg_join* j, tg_join_stats* out);
 

@@ -140,6 +140,7 @@ class TgAggStats(C.Structure):
 # tg_join_stats.paths / tg_agg_stats.paths: kernel families a handle has launched
 JOIN_PATH_PROBE_UQ, JOIN_PATH_PROBE_GENERAL, JOIN_PATH_PROBE_DIRECT, JOIN_PATH_PROBE_SEG = 1 << 0, 1 << 1, 1 << 2, 1 << 3
 JOIN_PATH_SCATTER_BULK, JOIN_PATH_SCATTER = 1 << 5, 1 << 6   # 1 << 4 is unassigned
+JOIN_PATH_CELL_GATHER = 1 << 7
 AGG_PATH_NOGROUP, AGG_PATH_V2_GLOBAL, AGG_PATH_V2_LOCAL, AGG_PATH_MULTI_KEY = 1 << 0, 1 << 1, 1 << 2, 1 << 3
 AGG_PATH_V1_LOCAL, AGG_PATH_V1_GLOBAL, AGG_PATH_MERGE = 1 << 4, 1 << 5, 1 << 6
 

@@ -21,6 +21,8 @@ struct Side {
   std::vector<int> types;
   std::vector<uint32_t> flags;
   std::vector<int> elem;
+  std::vector<int> kelem;         // width the kernels see: a DECIMAL column reaches them as 8-byte row ids (kernel_view)
+  bool has_cells = false;         // some needed column is DECIMAL
   std::vector<char> needed;       // staged to the device (key ∪ used ∪ filter columns)
   int key_col = -1;               // the single equal-condition key; -1 when the join has several (key_cols)
   std::vector<int> key_cols;      // several equal conditions: the key columns in condition order
@@ -113,7 +115,8 @@ struct JoinImpl {
   int scan_mode = 0;
   bool has_flag_col = false;
   int n_out = 0;
-  std::vector<int> out_elem;
+  std::vector<int> out_elem;          // bytes per output cell, 40 for DECIMAL
+  std::vector<int> kout_elem;         // what the kernels write: 8-byte row ids for DECIMAL (gather_cells makes the cells)
   KeySpec build_key{}, probe_key{};   // data pointers filled per launch
   bool multi_key = false;             // several equal conditions: synthetic 64-bit candidate key + residual equalities (k_composite_key)
   DevBuf bkey_syn, bkey_syn_nn, pkey_syn, pkey_syn_nn;
@@ -147,6 +150,9 @@ struct JoinImpl {
   std::deque<std::unique_ptr<ResultBatch>> results;
   std::vector<std::unique_ptr<ResultBatch>> free_batches;   // recycled (cudaFree would synchronise the whole device)
   std::unique_ptr<ResultBatch> dev_result;      // tg_join_probe_dev output (reused across calls)
+  DevBuf iota;                                  // int64 0, 1, 2, ...: the row-id stand-in of every DECIMAL column
+  int64_t iota_rows = 0;
+  std::vector<std::unique_ptr<DevBuf>> out_ids; // per DECIMAL output column: the source row ids the kernels wrote
   std::atomic<bool> probe_finished{false};
   std::atomic<int64_t> d2h_bytes{0};
   // small-Next window
@@ -175,6 +181,8 @@ static int fill_side(Side& s, int n, const int32_t* types, const uint32_t* flags
   for (int i = 0; i < n; i++) s.flags[i] = flags ? flags[i] : 0;
   s.elem.resize(n);
   for (int i = 0; i < n; i++) s.elem[i] = fixed_len(types[i]);
+  s.kelem.resize(n);
+  for (int i = 0; i < n; i++) s.kelem[i] = s.elem[i] == kCellBytes ? 8 : s.elem[i];
   s.needed.assign(n, 0);
   return TG_OK;
 }
@@ -319,8 +327,10 @@ static int setup(JoinImpl* j, const tg_join_desc* d) {
     if (s->key_col >= 0) s->needed[s->key_col] = 1;
     for (int c : s->key_cols) s->needed[c] = 1;
     for (int c : s->used) {
-      if (s->elem[c] != 8 && s->elem[c] != 4) return fail(TG_ERR_UNSUPPORTED, "only 4/8-byte fixed-width columns are offloaded (no DECIMAL / var-len yet)");
+      if (s->elem[c] != 8 && s->elem[c] != 4 && s->elem[c] != kCellBytes)
+        return fail(TG_ERR_UNSUPPORTED, "only 4/8-byte fixed-width columns and DECIMAL cells are offloaded (no var-len yet)");
       s->needed[c] = 1;
+      s->has_cells |= s->elem[c] == kCellBytes;
     }
     for (int i = 0; i < s->filter.n; i++) {
       s->needed[s->filter.items[i].lhs_col] = 1;
@@ -338,10 +348,10 @@ static int setup(JoinImpl* j, const tg_join_desc* d) {
   }
   // output schema: LUsed of left ‖ RUsed of right [‖ matched flag]
   j->n_lused = (int)j->lused.size(); j->n_rused = (int)j->rused.size();
-  j->out_elem.clear();
-  for (int c : j->lused) j->out_elem.push_back(left.elem[c]);
-  for (int c : j->rused) j->out_elem.push_back(right.elem[c]);
-  if (j->has_flag_col) j->out_elem.push_back(8);
+  j->out_elem.clear(); j->kout_elem.clear();
+  for (int c : j->lused) { j->out_elem.push_back(left.elem[c]); j->kout_elem.push_back(left.kelem[c]); }
+  for (int c : j->rused) { j->out_elem.push_back(right.elem[c]); j->kout_elem.push_back(right.kelem[c]); }
+  if (j->has_flag_col) { j->out_elem.push_back(8); j->kout_elem.push_back(8); }
   j->n_out = (int)j->out_elem.size();
   if (j->n_out > TG_MAX_OUT) return fail(TG_ERR_UNSUPPORTED, "too many output columns");
   j->device = d->device;
@@ -378,6 +388,7 @@ static int stage_append(HostStage& st, const Side& s, const tg_chunk* chk) {
     uint8_t* dst = d.p + (size_t)st.rows * el;
     if (!chk->sel) std::memcpy(dst, col.data, (size_t)n * el);
     else if (el == 8) { auto* o = reinterpret_cast<uint64_t*>(dst); auto* in = reinterpret_cast<const uint64_t*>(col.data); for (int64_t i = 0; i < n; i++) o[i] = in[chk->sel[i]]; }
+    else if (el == kCellBytes) { auto* in = reinterpret_cast<const uint8_t*>(col.data); for (int64_t i = 0; i < n; i++) std::memcpy(dst + (size_t)i * el, in + (size_t)chk->sel[i] * el, el); }
     else { auto* o = reinterpret_cast<uint32_t*>(dst); auto* in = reinterpret_cast<const uint32_t*>(col.data); for (int64_t i = 0; i < n; i++) o[i] = in[chk->sel[i]]; }
     d.used = (size_t)(st.rows + n) * el;
     // null bitmap: materialised lazily, the first time a chunk brings one
@@ -476,6 +487,7 @@ static int devchunk_view(const tg_chunk* chk, const Side& s, DevCols& v, int64_t
     if (!s.needed[c]) continue;
     if (chk->cols[c].elem_len != s.elem[c]) return fail(TG_ERR_INVALID, "chunk column elem_len does not match the schema type");
     if (chk->cols[c].length != *rows) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
+    if (s.elem[c] == kCellBytes && (reinterpret_cast<uintptr_t>(chk->cols[c].data) & 7)) return fail(TG_ERR_INVALID, "DECIMAL device columns must be 8-byte aligned");
     v.data[c] = chk->cols[c].data;
     v.nulls[c] = chk->cols[c].null_bitmap;
   }
@@ -498,6 +510,30 @@ static int composite_key(JoinImpl* j, const Side& s, const DevCols& v, int64_t n
   }
   k_composite_key<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(src, n, key.as<int64_t>(), not_null.as<uint32_t>());
   j->stats.kernel_launches++;
+  return TG_OK;
+}
+
+// ---- DECIMAL cells: late materialisation --------------------------------------------------------------
+// The build and probe kernels move 8-byte words.  A used DECIMAL column (40-byte MyDecimal cells, moved, never interpreted)
+// reaches them as a row-id column instead: the shared iota of int64 row numbers, under the column's own null bitmap.  So
+// every path (U1 payload, row-store word, build-side scan, NULL padding) writes the source row's id and valid byte where
+// the cell belongs, and gather_cells then copies the 40 raw bytes of that row, or zero bytes under NULL.
+static int ensure_iota(JoinImpl* j, int64_t rows) {
+  if (rows <= j->iota_rows) return TG_OK;
+  rows = std::max(rows, 2 * j->iota_rows);
+  TG_TRY(j->iota.ensure(j->device, (size_t)rows * 8 + 16));
+  k_iota<<<grid_for(j, rows, 256, 8), 256, 0, j->stream>>>(j->iota.as<int64_t>(), rows);
+  j->stats.kernel_launches++;
+  j->iota_rows = rows;
+  return TG_OK;
+}
+
+// the view the kernels get of `rows` rows of side s: each needed DECIMAL column becomes the iota (8-byte row ids)
+static int kernel_view(JoinImpl* j, const Side& s, DevCols& v, int64_t rows) {
+  if (!s.has_cells) return TG_OK;
+  TG_TRY(ensure_iota(j, rows));
+  for (int c = 0; c < s.ncols; c++)
+    if (s.needed[c] && s.elem[c] == kCellBytes) { v.data[c] = j->iota.p; v.elem_len[c] = 8; }
   return TG_OK;
 }
 
@@ -569,6 +605,7 @@ static int build_table(JoinImpl* j) {
   int64_t n = j->bcols.rows;
   j->stats.build_rows = n;
   DevCols bview = j->bcols.view(b);
+  TG_TRY(kernel_view(j, b, bview, n));
   KeySpec ks = j->build_key;
   if (j->multi_key) {
     TG_TRY(composite_key(j, b, bview, n, j->bkey_syn, j->bkey_syn_nn));
@@ -618,7 +655,7 @@ static int build_table(JoinImpl* j) {
   bool u1 = host_sc[1] <= 1 && !j->need_scan && payload.size() <= 1 && (!key_out || j->build_key.kind == KEY_I64) && j->other.empty();
   if (u1 && payload.size() == 1) {
     int pc = payload[0];
-    if (b.elem[pc] != 8 || j->bcols.has_nulls[pc]) u1 = false;
+    if (b.kelem[pc] != 8 || j->bcols.has_nulls[pc]) u1 = false;
   }
   if (u1 && j->default_load_factor && n > 0) {
     // the partitioned probe will slice this table: rebuild it dense enough for TG_MAX_PARTS L2-sized slices (probe_slices)
@@ -657,7 +694,7 @@ static int build_table(JoinImpl* j) {
     for (int c : j->other_build_cols) if (std::find(cols.begin(), cols.end(), c) == cols.end()) cols.push_back(c);   // read by OtherCondition only
     if ((int)cols.size() + 1 > TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "too many build columns");
     for (int c : cols) {
-      rs.col[w] = c; rs.elem_len[w] = b.elem[c];
+      rs.col[w] = c; rs.elem_len[w] = b.kelem[c];
       rs.null_bit[w] = j->bcols.has_nulls[c] ? w : -1;
       any_nullable |= j->bcols.has_nulls[c] != 0;
       j->build_word_of_col[c] = w;
@@ -720,10 +757,45 @@ static int ensure_result(JoinImpl* j, ResultBatch& rb, int64_t cap_rows, bool pr
     rb.cols.clear(); rb.bitmaps.clear();
     for (int i = 0; i < j->n_out; i++) { rb.cols.emplace_back(new DevBuf()); rb.bitmaps.emplace_back(new DevBuf()); }
   }
+  if ((int)j->out_ids.size() != j->n_out) {
+    j->out_ids.clear();
+    for (int i = 0; i < j->n_out; i++) j->out_ids.emplace_back(new DevBuf());
+  }
   for (int c = 0; c < j->n_out; c++) {
     size_t bytes = (size_t)(cap_rows + 8) * j->out_elem[c];
     if (preserve) TG_TRY(rb.cols[c]->ensure_preserve(j->device, bytes, (size_t)used_rows * j->out_elem[c], j->stream));
     else TG_TRY(rb.cols[c]->ensure(j->device, bytes));
+    if (j->out_elem[c] != kCellBytes) continue;
+    // the ids of a call's output rows, laid out like its cells (every probe starts a fresh batch: ids index from row 0)
+    if (preserve) TG_TRY(j->out_ids[c]->ensure_preserve(j->device, (size_t)(cap_rows + 8) * 8, (size_t)used_rows * 8, j->stream));
+    else TG_TRY(j->out_ids[c]->ensure(j->device, (size_t)(cap_rows + 8) * 8));
+  }
+  return TG_OK;
+}
+
+// where the kernels write output column c of rb: the cells themselves, or the row ids of a DECIMAL column
+static uint8_t* kernel_out(JoinImpl* j, ResultBatch& rb, int c) {
+  return (j->out_elem[c] == kCellBytes ? j->out_ids[c] : rb.cols[c])->as<uint8_t>();
+}
+
+// Turn the row ids of every DECIMAL output column of rb into cells: rows [0, rb.rows), or [0, *dev_rows) when the fused
+// paths leave the count on the device.  `probe_cells` = the view the probe ids index (nullptr: the build-side scan, where
+// every probe-side cell is NULL); build ids index bcols, which hold the build rows for the handle's lifetime.  Enqueued
+// behind the last kernel that moves rows, before anything can reuse the probe batch's buffers.
+static int gather_cells(JoinImpl* j, ResultBatch& rb, const DevCols* probe_cells, const unsigned long long* dev_rows) {
+  const bool probe_is_left = j->build_is_right;
+  for (int o = 0; o < j->n_out; o++) {
+    if (j->out_elem[o] != kCellBytes) continue;
+    if (!dev_rows && rb.rows == 0) continue;
+    const bool from_left = o < j->n_lused;
+    const int col = from_left ? j->lused[o] : j->rused[o - j->n_lused];
+    const void* src = from_left == probe_is_left ? (probe_cells ? probe_cells->data[col] : nullptr) : j->bcols.data[col]->p;
+    const int grid = dev_rows ? j->nsm * 8 : grid_for(j, rb.rows * 5, 256, 8);
+    k_gather_cells<<<grid, 256, 0, j->stream>>>(j->out_ids[o]->as<int64_t>(), rb.bitmaps[o]->as<uint8_t>(),
+                                                reinterpret_cast<const unsigned long long*>(src), rb.cols[o]->as<unsigned long long>(),
+                                                rb.rows, dev_rows);
+    j->stats.kernel_launches++;
+    j->stats.paths |= TG_JOIN_PATH_CELL_GATHER;
   }
   return TG_OK;
 }
@@ -749,7 +821,7 @@ static void fill_outspec_probe(const JoinImpl* j, OutCols& oc) {
   oc.n = j->n_out;
   for (int o = 0; o < j->n_out; o++) {
     OutSpec& sp = oc.spec[o];
-    sp.elem_len = j->out_elem[o];
+    sp.elem_len = j->kout_elem[o];
     sp.null_bit = -1;
     if (j->has_flag_col && o == j->n_out - 1) { sp.src = SRC_FLAG; sp.idx = 0; continue; }
     bool from_left = o < n_l;
@@ -799,8 +871,8 @@ static bool fast_path_ok(const JoinImpl* j, const DevCols& pview) {
   if (j->tv.mode != TABLE_U1 || j->probe_kind != PK_INNER || j->need_scan) return false;
   if (j->probe.filter.n || j->probe_key.kind != KEY_I64 || j->probe_key.reject_negative) return false;
   if (pview.nulls[j->probe.key_col]) return false;
-  for (int c : j->probe.used) if (j->probe.elem[c] != 8 || pview.nulls[c]) return false;
-  for (int e : j->out_elem) if (e != 8) return false;
+  for (int c : j->probe.used) if (j->probe.kelem[c] != 8 || pview.nulls[c]) return false;
+  for (int e : j->kout_elem) if (e != 8) return false;
   return true;
 }
 
@@ -809,9 +881,9 @@ static bool fast_path_ok(const JoinImpl* j, const DevCols& pview) {
 static bool uq_path_ok(const JoinImpl* j, const DevCols& pview) {
   if (!env_int("TG_PROBE_UQ", 1) ||j->probe_kind != PK_INNER || j->need_scan || !j->other.empty() || j->stats.max_dup > 1) return false;
   if (j->tv.mode != TABLE_U1 && j->tv.mode != TABLE_G) return false;
-  for (int c : j->probe.used) if (j->probe.elem[c] != 8 || pview.nulls[c]) return false;
-  for (int c : j->build.used) if (j->build.elem[c] != 8 || j->bcols.has_nulls[c]) return false;
-  for (int e : j->out_elem) if (e != 8) return false;
+  for (int c : j->probe.used) if (j->probe.kelem[c] != 8 || pview.nulls[c]) return false;
+  for (int c : j->build.used) if (j->build.kelem[c] != 8 || j->bcols.has_nulls[c]) return false;
+  for (int e : j->kout_elem) if (e != 8) return false;
   return true;
 }
 
@@ -919,8 +991,10 @@ static int launch_probe_seg(JoinImpl* j, const int64_t* pkey, int64_t n, const F
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // probe `n` device-resident rows; results are appended to rb (rb.rows advanced)
-static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatch& rb, bool sync_count, const SegSpec* in_seg = nullptr) {
+static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBatch& rb, bool sync_count, const SegSpec* in_seg = nullptr) {
   const Side& p = j->probe;
+  DevCols pview = pcells;
+  TG_TRY(kernel_view(j, p, pview, n));
   j->stats.probe_rows += n;
   KeySpec ks = j->probe_key;
   if (j->multi_key) {
@@ -966,7 +1040,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
                          (tune.inplace >= 0 ? tune.inplace != 0 : j->seg_match >= kInplaceMinMatch);
     if (inplace) C = inplace_seg_cap(j, P, n_main, C);
     TG_TRY(ensure_result(j, rb, inplace ? std::max<int64_t>(n, (int64_t)P * C) : rb.rows + n, rb.rows > 0, rb.rows));
-    for (int c = 0; c < j->n_out; c++) { oc.data[c] = rb.cols[c]->as<uint8_t>() + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
+    for (int c = 0; c < j->n_out; c++) { oc.data[c] = kernel_out(j, rb, c) + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
     build_fast_out(j, oc, pview, fo);
     unsigned long long* cur = j->out_cursor.as<unsigned long long>();
     TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
@@ -1026,6 +1100,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
         j->stats.kernel_launches++;
       }
     }
+    TG_TRY(gather_cells(j, rb, &pcells, cur));   // after the hole fill and the gated fallback: *cur rows from row 0
     if (sync_count) {
       unsigned long long got = 0, part[2 * TG_MAX_PARTS + 1];   // fill counts | segment bases | overflow flag
       const bool learn = P && !in_seg;
@@ -1046,7 +1121,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
   // single-pass path: inner join on unique build keys with filters / several payload columns (k_probe_inner_uq)
   if (uq_path_ok(j, pview)) {
     TG_TRY(ensure_result(j, rb, rb.rows + n, rb.rows > 0, rb.rows));
-    for (int c = 0; c < j->n_out; c++) { oc.data[c] = rb.cols[c]->as<uint8_t>() + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
+    for (int c = 0; c < j->n_out; c++) { oc.data[c] = kernel_out(j, rb, c) + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
     unsigned long long* cur = j->out_cursor.as<unsigned long long>();
     TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
     if (n > 0) {
@@ -1056,6 +1131,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
       j->stats.kernel_launches++;
       j->stats.paths |= TG_JOIN_PATH_PROBE_UQ;
     }
+    TG_TRY(gather_cells(j, rb, &pcells, cur));
     // the output row count decides rb.rows (and the next append position): always needed on the host
     unsigned long long got = 0;
     TG_CUDA(cudaMemcpyAsync(&got, cur, 8, cudaMemcpyDeviceToHost, j->stream));
@@ -1079,7 +1155,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
     if (lo) {
       if (lo % 8) return fail(TG_ERR_CUDA, "internal: sub-batch offset not byte aligned");
       for (int c = 0; c < p.ncols; c++) {
-        if (sub.data[c]) sub.data[c] = reinterpret_cast<const uint8_t*>(sub.data[c]) + (size_t)lo * p.elem[c];
+        if (sub.data[c]) sub.data[c] = reinterpret_cast<const uint8_t*>(sub.data[c]) + (size_t)lo * p.kelem[c];
         if (sub.nulls[c]) sub.nulls[c] += lo / 8;
       }
     }
@@ -1099,7 +1175,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
       OutCols oc{};
       fill_outspec_probe(j, oc);
       for (int c = 0; c < j->n_out; c++) {
-        oc.data[c] = rb.cols[c]->p;
+        oc.data[c] = kernel_out(j, rb, c);
         oc.valid[c] = nullptr;
         if (nullable[c]) {
           TG_TRY(j->tmp_valid[c]->ensure_preserve(j->device, (size_t)(rb.rows + total) + 16, (size_t)rb.rows, j->stream));
@@ -1117,6 +1193,7 @@ static int probe_device(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatc
   (void)out_start;
   if ((int)rb.cols.size() != j->n_out) TG_TRY(ensure_result(j, rb, 8, false, 0));
   TG_TRY(finish_bitmaps(j, rb, nullable));
+  TG_TRY(gather_cells(j, rb, &pcells, nullptr));
   TG_CUDA(cudaStreamSynchronize(j->stream));
   TG_CUDA(cudaGetLastError());
   return TG_OK;
@@ -1128,6 +1205,7 @@ static int scan_build_side(JoinImpl* j, ResultBatch& rb) {
   int64_t n = j->bcols.rows;
   if (n == 0) { if ((int)rb.cols.size() != j->n_out) TG_TRY(ensure_result(j, rb, 8, false, 0)); return TG_OK; }
   DevCols bview = j->bcols.view(b);
+  TG_TRY(kernel_view(j, b, bview, n));
   TG_TRY(j->tmp_cnt.ensure(j->device, (size_t)(n + 1) * 4));
   k_build_scan_count<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(j->row_slot.as<uint32_t>(), j->slot_used.as<uint8_t>(), n, j->scan_mode, j->tmp_cnt.as<uint32_t>());
   j->stats.kernel_launches++;
@@ -1143,12 +1221,12 @@ static int scan_build_side(JoinImpl* j, ResultBatch& rb) {
     bool from_left = o < j->n_lused;
     int col = from_left ? j->lused[o] : j->rused[o - j->n_lused];
     bool from_probe = from_left == probe_is_left;
-    oc.spec[o].elem_len = j->out_elem[o];
+    oc.spec[o].elem_len = j->kout_elem[o];
     oc.spec[o].null_bit = -1;
     oc.spec[o].src = from_probe ? SRC_PROBE_COL : SRC_BUILD_WORD;
     oc.spec[o].idx = col;
     nullable[o] = from_probe || j->bcols.has_nulls[col];
-    oc.data[o] = rb.cols[o]->p;
+    oc.data[o] = kernel_out(j, rb, o);
     oc.valid[o] = nullptr;
     if (nullable[o]) { TG_TRY(j->tmp_valid[o]->ensure(j->device, (size_t)total + 16)); oc.valid[o] = j->tmp_valid[o]->as<uint8_t>(); }
   }
@@ -1159,6 +1237,7 @@ static int scan_build_side(JoinImpl* j, ResultBatch& rb) {
   rb.rows = (int64_t)total;
   j->stats.output_rows += (int64_t)total;
   TG_TRY(finish_bitmaps(j, rb, nullable));
+  TG_TRY(gather_cells(j, rb, nullptr, nullptr));
   TG_CUDA(cudaStreamSynchronize(j->stream));
   TG_CUDA(cudaGetLastError());
   return TG_OK;
