@@ -740,6 +740,10 @@ def test_product_path_simulated_world(W):
         for r in range(W):
             seg_cnt = guarded(W)[0]
             assert L.tg_mail_wait(0, ptr(counts[r][0]), W, C.c_int64(st + 1), ptr(seg_cnt), ptr(err), C.c_int64(5000), None) == 0
+            # the join reads seg_cnt on a stream of its own, unordered with the default stream the wait writes it on: let the
+            # wait finish first (mgpu_worker.py enqueues the wait on the join's stream instead).  Safe: every signal the wait
+            # needs was enqueued above
+            t.cuda.synchronize()
             collect(*joins[r].probe_segments([recv[r][0][0], recv[r][1][0]], seg_cnt, cap, sync=True)[:2])
         spilled.append(sum(int(host(c)[0]) for c in cursor) - sum(before))
     assert spilled[0] == 0 and spilled[1] > 0, spilled
