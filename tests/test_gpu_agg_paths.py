@@ -265,6 +265,33 @@ def test_sel_vectors(monkeypatch):
     check_all(plans()[:2], chunks, want=P.AGG_PATH_V1_LOCAL)
 
 
+def test_host_push_with_null_data_pointer_is_rejected():
+    # a needed column of a host chunk with rows but no data pointer is invalid input: the push fails before anything is
+    # staged, and the handle aggregates the next pushes as if it had never been offered
+    plan = AggPlan([INT_NN, INT_NN], [0], [AggFunc(P.AGG_FIRSTROW, 0), AggFunc(P.AGG_COUNT, -1), AggFunc(P.AGG_MIN, 1),
+                                           AggFunc(P.AGG_MAX, 1)])
+    vals = np.arange(1000, dtype=np.int64)
+    good = Chunk([Column(vals % 7), Column(vals)])
+    bad = Chunk(good.columns)
+    lib = abi.load_lib()
+    e = HashAggExec(plan, MockDataSource(plan.col_types, []))
+    e.open()
+    try:
+        bs = bad.to_struct()
+        bs.cols[1].data = None
+        assert lib.tg_agg_push(e._h, C.byref(bs)) == abi.TG_ERR_INVALID
+        assert b"data is NULL" in lib.tg_last_error()
+        gs = good.to_struct()
+        abi.check(lib.tg_agg_push(e._h, C.byref(gs)))
+        abi.check(lib.tg_agg_finish(e._h))
+        e._prepared = True
+        out = e.next(1 << 10)
+        rows = sorted(zip(*(c.data.tolist() for c in out.columns)))
+        assert rows == [(k, len(vals[k::7]), k, int(vals[k::7][-1])) for k in range(7)]
+    finally:
+        e.close()
+
+
 # ---- several GROUP BY columns ----------------------------------------------------------------------------------
 def mk_rows(rng, n, ncols, card):
     """ncols key columns (column 0 nullable with both 0 and NULL present, column 1 a DOUBLE with -0.0 and +0.0) + the TYPES

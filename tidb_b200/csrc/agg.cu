@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "tma.cuh"
 #include "decimal.cuh"
+#include "chunk_io.cuh"
 
 namespace tg {
 
@@ -679,17 +680,6 @@ k_agg_finalize(AggTable t, AggSpec spec, int gk_kind, AggOut out, unsigned long 
   }
 }
 
-__global__ void k_pack_bitmap_agg(const uint8_t* __restrict__ valid, int64_t n, uint8_t* __restrict__ bitmap) {
-  int64_t b = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  int64_t nbytes = (n + 7) / 8;
-  for (; b < nbytes; b += stride) {
-    uint8_t v = 0;
-    for (int j = 0; j < 8; j++) { int64_t r = b * 8 + j; if (r < n && valid[r]) v |= (uint8_t)(1u << j); }
-    bitmap[b] = v;
-  }
-}
-
 
 // ---- several GROUP BY columns: tag-claimed slots, global table only -------------------------------------------------
 // N key words: the group table's keys (the GROUP BY words and the NULL word), or a DISTINCT set's (those plus the value)
@@ -920,12 +910,6 @@ k_dec_to_scaled(const uint8_t* __restrict__ cells, const uint8_t* __restrict__ n
 #include "agg_update.cuh"
 namespace tg {
 
-struct AggHostStage {
-  std::vector<std::unique_ptr<PinBuf>> data, nulls;
-  std::vector<char> has_nulls;
-  int64_t rows = 0;
-};
-
 // words of AggImpl::scalars, the handle's device counters
 enum {
   SC_COUNT = 0,            // k_agg_count: occupied slots
@@ -952,13 +936,7 @@ struct tg_agg {
   AggImpl* impl = nullptr;
 };
 
-struct AggImpl {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  int nsm = 132;
-
+struct AggImpl : DeviceHandle {
   int ncols = 0;
   std::vector<int> types, elem;
   std::vector<uint32_t> flags;
@@ -999,7 +977,7 @@ struct AggImpl {
   int local_mode = -1;            // -1 undecided, 0 global atomics only, 1 CTA-local partial aggregation first
 
   // staging
-  AggHostStage stage;
+  HostStage stage;
   std::vector<std::unique_ptr<DevBuf>> dcols, dnulls;
 
   // result
@@ -1010,12 +988,6 @@ struct AggImpl {
 };
 
 namespace tg {
-
-static int agrid(const AggImpl* a, int64_t n, int block = 256, int per_sm = 8) {
-  int64_t need = (n + block - 1) / block, cap = (int64_t)a->nsm * per_sm;
-  if (need < 1) need = 1;
-  return (int)(need < cap ? need : cap);
-}
 
 static int dec_expr_rules(const AggImpl* a, const tg_agg_func& f);
 static long long pow10_i64(int k) { long long p = 1; while (k-- > 0) p *= 10; return p; }
@@ -1291,7 +1263,7 @@ static int alloc_table(AggImpl* a, unsigned long long nslots, DevBuf& mem, AggTa
   size_t n = (size_t)nslots + 2;
   TG_TRY(mem.ensure(a->device, n * 8 * (size_t)table_record_words(a) + 64));
   layout_table(a, mem.as<uint8_t>(), nslots, t);
-  k_agg_init<<<agrid(a, (int64_t)n), 256, 0, a->stream>>>(t, a->spec, n);
+  k_agg_init<<<grid_size(a->nsm, (int64_t)n, 256, 8), 256, 0, a->stream>>>(t, a->spec, n);
   a->stats.kernel_launches++;
   return TG_OK;
 }
@@ -1307,8 +1279,8 @@ static int grow_table(AggImpl* a, unsigned long long more) {
   std::unique_ptr<DevBuf> nm(new DevBuf());
   AggTable nt{};
   TG_TRY(alloc_table(a, want_slots, *nm, nt));
-  if (a->nkw) k_agg_rehash_mk<<<agrid(a, (int64_t)a->tbl.nslots), 256, 0, a->stream>>>(a->tbl, nt, a->nstates);
-  else k_agg_rehash<<<agrid(a, (int64_t)a->tbl.nslots + 2), 256, 0, a->stream>>>(a->tbl, nt, a->nstates);
+  if (a->nkw) k_agg_rehash_mk<<<grid_size(a->nsm, (int64_t)a->tbl.nslots, 256, 8), 256, 0, a->stream>>>(a->tbl, nt, a->nstates);
+  else k_agg_rehash<<<grid_size(a->nsm, (int64_t)a->tbl.nslots + 2, 256, 8), 256, 0, a->stream>>>(a->tbl, nt, a->nstates);
   a->stats.kernel_launches++;
   TG_CUDA(cudaStreamSynchronize(a->stream));
   std::swap(a->tbl_mem.p, nm->p); std::swap(a->tbl_mem.cap, nm->cap); std::swap(a->tbl_mem.device, nm->device);
@@ -1372,7 +1344,7 @@ static int merge_partials(AggImpl* a, const AggPartials& pp, unsigned long long 
   DevBuf bits[2];
   return grow_and_retry(a, bits, (int64_t)m, false, "aggregation merge", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
     TG_CUDA(cudaMemsetAsync(sc + SC_MERGE_DEFERRED, 0, 8, a->stream));
-    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<agrid(a, (int64_t)m), 256, 0, a->stream>>>(pp, (int64_t)m, a->nstates, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_MERGE_DEFERRED);
+    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<grid_size(a->nsm, (int64_t)m, 256, 8), 256, 0, a->stream>>>(pp, (int64_t)m, a->nstates, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_MERGE_DEFERRED);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_MERGE;
     return read_back(a, sc + SC_MERGE_DEFERRED, nd);
@@ -1404,7 +1376,7 @@ static int update_grouped_mk(AggImpl* a, const DevCols& cols, int64_t n, unsigne
   for (int q = 0; q < gk.n; q++) { gk.data[q] = cols.data[a->group_cols[q]]; gk.nulls[q] = cols.nulls[a->group_cols[q]]; gk.kind[q] = a->group_kinds[q]; }
   return grow_and_retry(a, a->deferred, n, false, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
     TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
-    (a->wide ? k_agg_update_mk<true> : k_agg_update_mk<false>)<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_DEFERRED);
+    (a->wide ? k_agg_update_mk<true> : k_agg_update_mk<false>)<<<grid_size(a->nsm, n, 256, 8), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_DEFERRED);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_MULTI_KEY;
     return read_back(a, sc + SC_DEFERRED, nd);
@@ -1467,7 +1439,7 @@ static int local_partial_pass(AggImpl* a, const GroupKey& gk, const DevCols& col
   const int local_slots = env_slots ? env_slots : 1024;   // bigger tables lose more to occupancy than they gain
   const size_t smem = (size_t)(local_slots + 2) * 8 * (2 + a->nstates);
   const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (200u << 10) / smem));
-  const int grid = agrid(a, hi - lo, 256, per_sm);
+  const int grid = grid_size(a->nsm, hi - lo, 256, per_sm);
   AggPartials pp{};
   TG_TRY(alloc_partials(a, (size_t)grid * (local_slots / 2 + 2), sc + SC_V1_TUPLES, pp));
   TG_CUDA(cudaMemsetAsync(sc + SC_V1_TUPLES, 0, 8, a->stream));
@@ -1508,7 +1480,7 @@ static int update_grouped_v1(AggImpl* a, const GroupKey& gk, const DevCols& cols
   }
   return grow_and_retry(a, a->deferred, n, try_local, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
     TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
-    (a->wide ? k_agg_update<true> : k_agg_update<false>)<<<agrid(a, n), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_DEFERRED);
+    (a->wide ? k_agg_update<true> : k_agg_update<false>)<<<grid_size(a->nsm, n, 256, 8), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_DEFERRED);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_V1_GLOBAL;
     return read_back(a, sc + SC_DEFERRED, nd);
@@ -1534,7 +1506,7 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
   }
   TG_CUDA(cudaEventRecord(a->ev0, a->stream));
   if (a->group_col < 0) {
-    (a->wide ? k_agg_update_nogroup<true> : k_agg_update_nogroup<false>)<<<agrid(a, n, 256, 4), 256, 0, a->stream>>>(cols, n, a->tbl, a->spec);
+    (a->wide ? k_agg_update_nogroup<true> : k_agg_update_nogroup<false>)<<<grid_size(a->nsm, n, 256, 4), 256, 0, a->stream>>>(cols, n, a->tbl, a->spec);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_NOGROUP;
   } else if (a->nkw) {
@@ -1546,7 +1518,7 @@ static int update_device_impl(AggImpl* a, const DevCols& cols, int64_t n) {
   TG_CUDA(cudaEventRecord(a->ev1, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
   TG_CUDA(cudaGetLastError());
-  float ms = 0; cudaEventElapsedTime(&ms, a->ev0, a->ev1); a->stats.update_ms += ms;
+  a->stats.update_ms += a->elapsed_ms();
   return TG_OK;
 }
 
@@ -1563,7 +1535,7 @@ static int decode_decimal_args(AggImpl* a, DevCols& cols, int64_t n) {
     TG_TRY(a->dscaled[c]->ensure(a->device, (size_t)n * 8 + 16));
     const uint8_t* cells = static_cast<const uint8_t*>(cols.data[c]);
     long long* out = a->dscaled[c]->as<long long>();
-    const int grid = agrid(a, (n + 1) / 2);
+    const int grid = grid_size(a->nsm, (n + 1) / 2, 256, 8);
     if ((reinterpret_cast<uintptr_t>(cells) & 15) == 0)
       k_dec_to_scaled<true><<<grid, 256, 0, a->stream>>>(cells, cols.nulls[c], n, a->col_flen[c], a->col_dec[c], out, err, (unsigned long long)c + 1);
     else
@@ -1604,7 +1576,7 @@ static int grow_set(AggImpl* a, AggImpl::SetMem& m, unsigned long long want) {
   DevBuf nm;
   DistinctSet nt{};
   TG_TRY(alloc_set(a, want, nm, nt));
-  k_agg_distinct_rehash<<<agrid(a, (int64_t)m.t.nslots), 256, 0, a->stream>>>(m.t, nt);
+  k_agg_distinct_rehash<<<grid_size(a->nsm, (int64_t)m.t.nslots, 256, 8), 256, 0, a->stream>>>(m.t, nt);
   a->stats.kernel_launches++;
   TG_CUDA(cudaStreamSynchronize(a->stream));
   std::swap(m.mem.p, nm.p); std::swap(m.mem.cap, nm.cap); std::swap(m.mem.device, nm.device);
@@ -1631,7 +1603,7 @@ static int distinct_mark(AggImpl* a, DevCols& cols, int64_t n) {
     TG_TRY(m.mark.ensure(a->device, (size_t)((n + 31) / 32) * 4 + 16));
     TG_TRY(grow_and_retry(a, a->deferred, n, false, "DISTINCT set", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
       TG_CUDA(cudaMemsetAsync(cnt, 0, 16, a->stream));
-      k_agg_distinct_mark<<<agrid(a, n), 256, 0, a->stream>>>(gk, static_cast<const long long*>(cols.data[c]), cols.nulls[c],
+      k_agg_distinct_mark<<<grid_size(a->nsm, n, 256, 8), 256, 0, a->stream>>>(gk, static_cast<const long long*>(cols.data[c]), cols.nulls[c],
                                                                a->types[c] == TG_TYPE_DOUBLE, n, m.t, kAggMaxProbe, m.mark.as<uint32_t>(),
                                                                deferred, only, cnt);
       a->stats.kernel_launches++;
@@ -1650,7 +1622,7 @@ static int distinct_mark(AggImpl* a, DevCols& cols, int64_t n) {
   TG_CUDA(cudaEventRecord(a->ev1, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
   TG_CUDA(cudaGetLastError());
-  float ms = 0; cudaEventElapsedTime(&ms, a->ev0, a->ev1); a->dstats.mark_ms += ms;
+  a->dstats.mark_ms += a->elapsed_ms();
   return TG_OK;
 }
 
@@ -1683,80 +1655,20 @@ static int update_device(AggImpl* a, const DevCols& in, int64_t n) {
   return rc;
 }
 
-static int64_t alogical_rows(const tg_chunk* c) { return c->sel ? c->nsel : (c->ncols > 0 ? c->cols[0].length : 0); }
-
-static int avalidate(const AggImpl* a, const tg_chunk* chk) {
-  if (!chk || chk->ncols != a->ncols) return fail(TG_ERR_INVALID, "chunk column count does not match the child schema");
-  int64_t phys = chk->cols[0].length;
-  for (int c = 0; c < a->ncols; c++) {
-    if (!a->needed[c]) continue;
-    if (chk->cols[c].elem_len != a->elem[c]) return fail(TG_ERR_INVALID, "chunk column elem_len does not match the schema type");
-    if (chk->cols[c].length != phys) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
-  }
-  return TG_OK;
-}
-
-static int astage_append(AggImpl* a, const tg_chunk* chk) {
-  AggHostStage& st = a->stage;
-  int64_t n = alogical_rows(chk);
-  if (n == 0) return TG_OK;
-  for (int c = 0; c < a->ncols; c++) {
-    if (!a->needed[c]) continue;
-    const tg_column& col = chk->cols[c];
-    PinBuf& d = *st.data[c];
-    const size_t el = (size_t)a->elem[c];   // 8, or 40 for a DECIMAL column
-    TG_TRY(d.reserve((size_t)(st.rows + n) * el));
-    uint8_t* dst = d.p + (size_t)st.rows * el;
-    if (!chk->sel) std::memcpy(dst, col.data, (size_t)n * el);
-    else if (el == 8) {
-      uint64_t* dst8 = reinterpret_cast<uint64_t*>(dst);
-      const uint64_t* src8 = reinterpret_cast<const uint64_t*>(col.data);
-      for (int64_t i = 0; i < n; i++) dst8[i] = src8[chk->sel[i]];
-    } else for (int64_t i = 0; i < n; i++) std::memcpy(dst + (size_t)i * el, col.data + (size_t)chk->sel[i] * el, el);
-    d.used = (size_t)(st.rows + n) * el;
-    bool bring = col.null_bitmap != nullptr;
-    if (bring || st.has_nulls[c]) {
-      PinBuf& nb = *st.nulls[c];
-      size_t need = (size_t)((st.rows + n + 7) / 8) + 1;
-      TG_TRY(nb.reserve(need));
-      if (!st.has_nulls[c]) { std::memset(nb.p, 0xff, (size_t)((st.rows + 7) / 8) + 1); st.has_nulls[c] = 1; }
-      if (bring && !chk->sel) append_bits(nb.p, st.rows, col.null_bitmap, n);
-      else for (int64_t i = 0; i < n; i++) {
-        bool nn = bring ? bit_not_null(col.null_bitmap, chk->sel ? chk->sel[i] : i) : true;
-        int64_t r = st.rows + i;
-        if (nn) nb.p[r >> 3] |= (uint8_t)(1u << (r & 7)); else nb.p[r >> 3] &= (uint8_t)~(1u << (r & 7));
-      }
-      nb.used = need;
-    }
-  }
-  st.rows += n;
-  return TG_OK;
-}
-
 static int aflush(AggImpl* a) {
-  AggHostStage& st = a->stage;
+  HostStage& st = a->stage;
   if (st.rows == 0) return TG_OK;
   DevCols v{};
   for (int c = 0; c < a->ncols; c++) {
     v.elem_len[c] = a->elem[c];
     if (!a->needed[c]) continue;
-    size_t bytes = (size_t)st.rows * a->elem[c];
-    TG_TRY(a->dcols[c]->ensure(a->device, bytes + 16));
-    TG_CUDA(cudaMemcpyAsync(a->dcols[c]->p, st.data[c]->p, bytes, cudaMemcpyHostToDevice, a->stream));
-    a->stats.h2d_bytes += bytes;
+    TG_TRY(upload_column(a->device, a->stream, st.data[c]->p, st.has_nulls[c] ? st.nulls[c]->p : nullptr, st.rows, a->elem[c],
+                         *a->dcols[c], *a->dnulls[c], &a->stats.h2d_bytes));
     v.data[c] = a->dcols[c]->p;
-    if (st.has_nulls[c]) {
-      size_t nb = (size_t)((st.rows + 7) / 8);
-      TG_TRY(a->dnulls[c]->ensure(a->device, nb + 16));
-      TG_CUDA(cudaMemcpyAsync(a->dnulls[c]->p, st.nulls[c]->p, nb, cudaMemcpyHostToDevice, a->stream));
-      a->stats.h2d_bytes += nb;
-      v.nulls[c] = a->dnulls[c]->as<uint8_t>();
-    }
+    if (st.has_nulls[c]) v.nulls[c] = a->dnulls[c]->as<uint8_t>();
   }
-  int64_t n = st.rows;
-  int rc = update_device(a, v, n);
-  st.rows = 0;
-  std::fill(st.has_nulls.begin(), st.has_nulls.end(), 0);
+  int rc = update_device(a, v, st.rows);
+  st.reset();
   return rc;
 }
 
@@ -1776,7 +1688,7 @@ static int afinalize(AggImpl* a) {
   }
   unsigned long long fill = 0;
   TG_CUDA(cudaMemsetAsync(sc + SC_COUNT, 0, 8, a->stream));
-  k_agg_count<<<agrid(a, (int64_t)a->nslots + 2), 256, 0, a->stream>>>(a->tbl, sc + SC_COUNT);
+  k_agg_count<<<grid_size(a->nsm, (int64_t)a->nslots + 2, 256, 8), 256, 0, a->stream>>>(a->tbl, sc + SC_COUNT);
   a->stats.kernel_launches++;
   TG_CUDA(cudaMemcpyAsync(&fill, sc + SC_COUNT, 8, cudaMemcpyDeviceToHost, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
@@ -1790,7 +1702,7 @@ static int afinalize(AggImpl* a) {
   }
   TG_CUDA(cudaEventRecord(a->ev0, a->stream));
   TG_CUDA(cudaMemsetAsync(sc + SC_CURSOR, 0, 8, a->stream));
-  (a->wide ? k_agg_finalize<true, true> : a->dec_out ? k_agg_finalize<true, false> : k_agg_finalize<false, false>)<<<agrid(a, (int64_t)a->nslots + 2), 256, 0, a->stream>>>(a->tbl, a->spec, a->gk_kind, ao, sc + SC_CURSOR);
+  (a->wide ? k_agg_finalize<true, true> : a->dec_out ? k_agg_finalize<true, false> : k_agg_finalize<false, false>)<<<grid_size(a->nsm, (int64_t)a->nslots + 2, 256, 8), 256, 0, a->stream>>>(a->tbl, a->spec, a->gk_kind, ao, sc + SC_CURSOR);
   a->stats.kernel_launches++;
   unsigned long long nrows = 0;
   TG_CUDA(cudaMemcpyAsync(&nrows, sc + SC_CURSOR, 8, cudaMemcpyDeviceToHost, a->stream));
@@ -1811,25 +1723,16 @@ static int afinalize(AggImpl* a) {
   for (int k = 0; k < nf; k++) {
     if (!ao.valid[k]) continue;
     TG_TRY(a->out_bitmaps[k]->ensure(a->device, (size_t)((a->out_rows + 7) / 8) + 16));
-    if (a->out_rows) { k_pack_bitmap_agg<<<agrid(a, (a->out_rows + 7) / 8), 256, 0, a->stream>>>(ao.valid[k], a->out_rows, a->out_bitmaps[k]->as<uint8_t>()); a->stats.kernel_launches++; }
+    if (a->out_rows) { launch_pack_bitmap(ao.valid[k], a->out_rows, a->out_bitmaps[k]->as<uint8_t>(), a->nsm, a->stream); a->stats.kernel_launches++; }
   }
   TG_CUDA(cudaEventRecord(a->ev1, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
   TG_CUDA(cudaGetLastError());
-  float ms = 0; cudaEventElapsedTime(&ms, a->ev0, a->ev1); a->stats.finalize_ms += ms;
+  a->stats.finalize_ms += a->elapsed_ms();
   return TG_OK;
 }
 
 }  // namespace tg
-
-#define TGA_LOCK(h)                                                            \
-  if (!(h)) return tg::fail(TG_ERR_INVALID, "handle is NULL");                 \
-  if ((h)->closed.load()) return tg::fail(TG_ERR_CANCELLED, "handle is closed"); \
-  std::lock_guard<std::mutex> lock__((h)->mu);                                 \
-  if ((h)->closed.load() || !(h)->impl) return tg::fail(TG_ERR_CANCELLED, "handle is closed"); \
-  AggImpl* a = (h)->impl;                                                      \
-  tg::DeviceGuard guard__(a->device);                                          \
-  if (!guard__.ok) return tg::fail(TG_ERR_CUDA, "cudaSetDevice failed (no usable CUDA device)")
 
 extern "C" {
 
@@ -1853,20 +1756,15 @@ static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int3
   std::unique_ptr<AggImpl> a(new AggImpl());
   TG_TRY(agg_setup(a.get(), desc, col_flen, col_dec, has_distinct));
   int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(TG_ERR_CUDA, "no CUDA device: the GPU hash aggregation has no CPU fallback"); }
+  TG_TRY(require_device("the GPU hash aggregation", &ndev));
   if (a->device < 0 || a->device >= ndev) return fail(TG_ERR_INVALID, "device ordinal out of range");
   DeviceGuard g(a->device);
   if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
-  if (desc->stream) { a->stream = (cudaStream_t)desc->stream; a->own_stream = false; }
-  else { TG_CUDA(cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking)); a->own_stream = true; }
-  TG_CUDA(cudaEventCreate(&a->ev0));
-  TG_CUDA(cudaEventCreate(&a->ev1));
-  a->nsm = device_sm_count(a->device);
+  TG_TRY(a->open(a->device, desc->stream));
+  a->stage.init(a->ncols);
   for (int c = 0; c < a->ncols; c++) {
-    a->stage.data.emplace_back(new PinBuf()); a->stage.nulls.emplace_back(new PinBuf());
     a->dcols.emplace_back(new DevBuf()); a->dnulls.emplace_back(new DevBuf()); a->dscaled.emplace_back(new DevBuf());
   }
-  a->stage.has_nulls.assign(a->ncols, 0);
   for (size_t j = 0; j < a->dist_cols.size(); j++) a->dsets.emplace_back(new AggImpl::SetMem());
   shell->impl = a.release();
   *out = shell.release();
@@ -1885,32 +1783,26 @@ int tg_agg_open_ex2(const tg_agg_desc_ex2* desc, tg_agg** out) {
 }
 
 int tg_agg_push(tg_agg* h, const tg_chunk* chk) {
-  TGA_LOCK(h);
+  TG_LOCK(h, AggImpl, a);
   if (a->finished) return fail(TG_ERR_STATE, "push after finish");
   if (a->broken) return broken_fail();
-  TG_TRY(avalidate(a, chk));
-  TG_TRY(astage_append(a, chk));
-  if (a->stage.rows >= (4ll << 20)) TG_TRY(aflush(a));
+  TG_TRY(validate_chunk(a->ncols, a->needed, a->elem, chk));
+  TG_TRY(stage_append(a->stage, a->needed, a->elem, chk));
+  if (a->stage.rows >= kStageBatchRows) TG_TRY(aflush(a));
   return TG_OK;
 }
 
 int tg_agg_push_dev(tg_agg* h, const tg_chunk* chk) {
-  TGA_LOCK(h);
+  TG_LOCK(h, AggImpl, a);
   if (a->finished) return fail(TG_ERR_STATE, "push after finish");
-  TG_TRY(avalidate(a, chk));
-  if (chk->sel) return fail(TG_ERR_UNSUPPORTED, "device-resident chunks must not carry a sel vector");
+  DevCols v;
+  TG_TRY(device_view(chk, a->ncols, a->needed, a->elem, v));
   TG_TRY(aflush(a));
-  DevCols v{};
-  for (int c = 0; c < a->ncols; c++) {
-    v.elem_len[c] = a->elem[c];
-    if (!a->needed[c]) continue;
-    v.data[c] = chk->cols[c].data; v.nulls[c] = chk->cols[c].null_bitmap;
-  }
-  return update_device(a, v, chk->cols[0].length);
+  return update_device(a, v, logical_rows(chk));
 }
 
 int tg_agg_finish(tg_agg* h) {
-  TGA_LOCK(h);
+  TG_LOCK(h, AggImpl, a);
   if (a->finished) return TG_OK;
   if (a->broken) return broken_fail();
   TG_TRY(aflush(a));
@@ -1920,7 +1812,7 @@ int tg_agg_finish(tg_agg* h) {
 }
 
 int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) {
-  TGA_LOCK(h);
+  TG_LOCK(h, AggImpl, a);
   if (!out || !nrows) return fail(TG_ERR_INVALID, "out / nrows is NULL");
   *nrows = 0;
   if (!a->finished) return fail(TG_ERR_STATE, "next before finish (hash aggregation is a pipeline breaker)");
@@ -1928,9 +1820,6 @@ int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) 
   int64_t lo = a->consumed;
   int64_t want = std::min<int64_t>(std::min<int64_t>(max_rows, out->capacity_rows), a->out_rows - lo);
   if (want <= 0) return TG_OK;
-  // any RequiredRows >= 1 is served: bitmaps that start inside a byte are fetched whole and shifted on the host
-  const int shift = (int)(lo & 7);
-  std::vector<std::vector<uint8_t>> shifted;
   for (int k = 0; k < a->spec.n; k++)
     if (a->out_elem[k] == TG_DEC_CELL_BYTES && out->cols[k].elem_len != TG_DEC_CELL_BYTES)
       return fail(TG_ERR_INVALID, "a DECIMAL result column needs elem_len 40 (MyDecimal cells)");
@@ -1938,37 +1827,17 @@ int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) 
     const size_t el = (size_t)a->out_elem[k];
     TG_CUDA(cudaMemcpyAsync(out->cols[k].data, a->out_cols[k]->as<uint8_t>() + (size_t)lo * el, (size_t)want * el, cudaMemcpyDeviceToHost, a->stream));
     a->stats.d2h_bytes += want * (int64_t)el;
-    size_t nb = (size_t)((want + 7) / 8);
-    if (a->out_bitmaps[k]->p) {
-      if (!out->cols[k].null_bitmap) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");
-      if (shift == 0) TG_CUDA(cudaMemcpyAsync(out->cols[k].null_bitmap, a->out_bitmaps[k]->as<uint8_t>() + lo / 8, nb, cudaMemcpyDeviceToHost, a->stream));
-      else {
-        shifted.emplace_back((size_t)((shift + want + 7) / 8) + 1, (uint8_t)0);
-        TG_CUDA(cudaMemcpyAsync(shifted.back().data(), a->out_bitmaps[k]->as<uint8_t>() + lo / 8, shifted.back().size() - 1, cudaMemcpyDeviceToHost, a->stream));
-      }
-    } else if (out->cols[k].null_bitmap) {
-      std::memset(out->cols[k].null_bitmap, 0xff, nb);
-      if (want & 7) out->cols[k].null_bitmap[nb - 1] = (uint8_t)((1u << (want & 7)) - 1);
-    }
   }
-  TG_CUDA(cudaStreamSynchronize(a->stream));
-  if (shift) {
-    size_t q = 0;
-    for (int k = 0; k < a->spec.n; k++) {
-      if (!a->out_bitmaps[k]->p) continue;
-      const std::vector<uint8_t>& src = shifted[q++];
-      size_t nb = (size_t)((want + 7) / 8);
-      for (size_t b = 0; b < nb; b++) out->cols[k].null_bitmap[b] = (uint8_t)((src[b] >> shift) | (src[b + 1] << (8 - shift)));
-    }
-  }
-  if (want & 7) for (int k = 0; k < a->spec.n; k++) if (a->out_bitmaps[k]->p) out->cols[k].null_bitmap[want >> 3] &= (uint8_t)((1u << (want & 7)) - 1);
+  // any RequiredRows >= 1 is served (download_bitmaps re-aligns bitmaps that start inside a byte); d2h_bytes counts the
+  // result cells only
+  TG_TRY(download_bitmaps(a->out_bitmaps, out, lo, want, a->stream, nullptr));
   a->consumed += want;
   *nrows = want;
   return TG_OK;
 }
 
 int tg_agg_result_dev(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls) {
-  TGA_LOCK(h);
+  TG_LOCK(h, AggImpl, a);
   if (!a->finished) return fail(TG_ERR_STATE, "result before finish");
   if (out_rows) *out_rows = a->out_rows;
   for (int k = 0; k < a->spec.n; k++) {
@@ -1979,14 +1848,14 @@ int tg_agg_result_dev(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_
 }
 
 int tg_agg_get_stats(tg_agg* h, tg_agg_stats* out) {
-  TGA_LOCK(h);
+  TG_LOCK(h, AggImpl, a);
   if (!out) return fail(TG_ERR_INVALID, "out is NULL");
   *out = a->stats;
   return TG_OK;
 }
 
 int tg_agg_get_distinct_stats(tg_agg* h, tg_agg_distinct_stats* out) {
-  TGA_LOCK(h);
+  TG_LOCK(h, AggImpl, a);
   if (!out) return fail(TG_ERR_INVALID, "out is NULL");
   *out = a->dstats;
   out->set_slots = 0;
@@ -2004,10 +1873,7 @@ int tg_agg_close(tg_agg* h) {
     h->impl = nullptr;
     if (a) {
       DeviceGuard g(a->device);
-      if (a->stream) cudaStreamSynchronize(a->stream);
-      if (a->ev0) cudaEventDestroy(a->ev0);
-      if (a->ev1) cudaEventDestroy(a->ev1);
-      if (a->own_stream && a->stream) cudaStreamDestroy(a->stream);
+      a->release();
       cudaGetLastError();
       delete a;
     }

@@ -8,11 +8,11 @@
 #include <condition_variable>
 #include "join_kernels.cuh"
 #include "partition_kernels.cuh"
+#include "chunk_io.cuh"
 
 namespace tg {
 
 static const int64_t kGeneralBatchRows = 16ll << 20;   // sub-batch of the general probe path (bounds temp memory)
-static const int64_t kStageBatchRows = 4ll << 20;      // host staging batch for small pushed chunks
 static const int64_t kDirectPushRows = 128ll << 10;    // chunks at least this big are copied straight from the caller
 static const int64_t kNextWindowRows = 1ll << 20;      // D2H window that serves small tg_join_next calls
 
@@ -53,20 +53,6 @@ struct ColStore {
   }
 };
 
-// host staging of pushed chunks (pinned), one buffer per needed column
-struct HostStage {
-  std::vector<std::unique_ptr<PinBuf>> data, nulls;
-  std::vector<char> has_nulls;
-  int64_t rows = 0;
-  void init(int ncols) {
-    data.clear(); nulls.clear();
-    for (int i = 0; i < ncols; i++) { data.emplace_back(new PinBuf()); nulls.emplace_back(new PinBuf()); }
-    has_nulls.assign(ncols, 0);
-    rows = 0;
-  }
-  void reset() { rows = 0; std::fill(has_nulls.begin(), has_nulls.end(), 0); for (auto& d : data) d->used = 0; for (auto& d : nulls) d->used = 0; }
-};
-
 struct ResultBatch {
   std::vector<std::unique_ptr<DevBuf>> cols, bitmaps;
   int64_t rows = 0;
@@ -92,16 +78,11 @@ struct tg_join {
   JoinImpl* impl = nullptr;          // guarded by mu + res_mu; nullptr once closed
 };
 
-struct JoinImpl {
+struct JoinImpl : DeviceHandle {
   std::mutex& res_mu;                // the shell's (see tg_join)
   std::condition_variable& res_cv;
   explicit JoinImpl(tg_join& shell) : res_mu(shell.res_mu), res_cv(shell.res_cv) {}
-  int device = 0;
-  cudaStream_t stream = nullptr;
   cudaStream_t d2h_stream = nullptr; // tg_join_next copies results on its own stream: D2H overlaps the next H2D + probe
-  bool own_stream = false;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  int nsm = 132;
   double load_factor = 0.5;
   bool default_load_factor = true;
 
@@ -164,13 +145,6 @@ struct JoinImpl {
 };
 
 namespace tg {
-
-static int grid_for(const JoinImpl* j, int64_t n, int block, int per_sm) {
-  int64_t need = (n + block - 1) / block;
-  int64_t cap = (int64_t)j->nsm * per_sm;
-  if (need < 1) need = 1;
-  return (int)(need < cap ? need : cap);
-}
 
 // ---- descriptor → handle -------------------------------------------------------------------------------
 static int fill_side(Side& s, int n, const int32_t* types, const uint32_t* flags) {
@@ -360,94 +334,17 @@ static int setup(JoinImpl* j, const tg_join_desc* d) {
   return TG_OK;
 }
 
-// ---- host chunk → staging ---------------------------------------------------------------------------
-static int64_t chunk_logical_rows(const tg_chunk* c) { return c->sel ? c->nsel : (c->ncols > 0 ? c->cols[0].length : 0); }
-
-static int validate_chunk(const Side& s, const tg_chunk* chk) {
-  if (!chk || chk->ncols != s.ncols) return fail(TG_ERR_INVALID, "chunk column count does not match the child schema");
-  int64_t phys = chk->ncols ? chk->cols[0].length : 0;
+// ---- host chunk → device ---------------------------------------------------------------------------
+// the rows of side s → cs (replaces its contents): from the host staging st, or (st = nullptr) straight from the
+// buffers of a big pushed chunk
+static int upload_side(JoinImpl* j, const Side& s, const HostStage* st, const tg_chunk* chk, ColStore& cs) {
+  cs.rows = st ? st->rows : chk->cols[0].length;
   for (int c = 0; c < s.ncols; c++) {
     if (!s.needed[c]) continue;
-    if (chk->cols[c].elem_len != s.elem[c]) return fail(TG_ERR_INVALID, "chunk column elem_len does not match the schema type");
-    if (chk->cols[c].length != phys) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
-    if (phys && !chk->cols[c].data) return fail(TG_ERR_INVALID, "chunk column data is NULL");
-  }
-  return TG_OK;
-}
-
-// append the logical rows of a host chunk to the staging buffers (gathers through sel)
-static int stage_append(HostStage& st, const Side& s, const tg_chunk* chk) {
-  int64_t n = chunk_logical_rows(chk);
-  if (n == 0) return TG_OK;
-  for (int c = 0; c < s.ncols; c++) {
-    if (!s.needed[c]) continue;
-    const tg_column& col = chk->cols[c];
-    int el = s.elem[c];
-    PinBuf& d = *st.data[c];
-    TG_TRY(d.reserve((size_t)(st.rows + n) * el));
-    uint8_t* dst = d.p + (size_t)st.rows * el;
-    if (!chk->sel) std::memcpy(dst, col.data, (size_t)n * el);
-    else if (el == 8) { auto* o = reinterpret_cast<uint64_t*>(dst); auto* in = reinterpret_cast<const uint64_t*>(col.data); for (int64_t i = 0; i < n; i++) o[i] = in[chk->sel[i]]; }
-    else if (el == kCellBytes) { auto* in = reinterpret_cast<const uint8_t*>(col.data); for (int64_t i = 0; i < n; i++) std::memcpy(dst + (size_t)i * el, in + (size_t)chk->sel[i] * el, el); }
-    else { auto* o = reinterpret_cast<uint32_t*>(dst); auto* in = reinterpret_cast<const uint32_t*>(col.data); for (int64_t i = 0; i < n; i++) o[i] = in[chk->sel[i]]; }
-    d.used = (size_t)(st.rows + n) * el;
-    // null bitmap: materialised lazily, the first time a chunk brings one
-    PinBuf& nb = *st.nulls[c];
-    bool bring = col.null_bitmap != nullptr;
-    if (bring || st.has_nulls[c]) {
-      size_t need = (size_t)((st.rows + n + 7) / 8) + 1;
-      TG_TRY(nb.reserve(need));
-      if (!st.has_nulls[c]) { std::memset(nb.p, 0xff, (size_t)((st.rows + 7) / 8) + 1); st.has_nulls[c] = 1; }
-      if (bring && !chk->sel) append_bits(nb.p, st.rows, col.null_bitmap, n);
-      else {
-        for (int64_t i = 0; i < n; i++) {
-          bool nn = bring ? bit_not_null(col.null_bitmap, chk->sel ? chk->sel[i] : i) : true;
-          int64_t r = st.rows + i;
-          if (nn) nb.p[r >> 3] |= (uint8_t)(1u << (r & 7)); else nb.p[r >> 3] &= (uint8_t)~(1u << (r & 7));
-        }
-      }
-      nb.used = need;
-    }
-  }
-  st.rows += n;
-  return TG_OK;
-}
-
-// staging → device column store (replaces its contents)
-static int stage_to_device(JoinImpl* j, HostStage& st, const Side& s, ColStore& cs) {
-  cs.rows = st.rows;
-  for (int c = 0; c < s.ncols; c++) {
-    if (!s.needed[c]) continue;
-    size_t bytes = (size_t)st.rows * s.elem[c];
-    TG_TRY(cs.data[c]->ensure(j->device, bytes + 16));
-    if (bytes) { TG_CUDA(cudaMemcpyAsync(cs.data[c]->p, st.data[c]->p, bytes, cudaMemcpyHostToDevice, j->stream)); j->stats.h2d_bytes += bytes; }
-    cs.has_nulls[c] = st.has_nulls[c];
-    if (st.has_nulls[c]) {
-      size_t nb = (size_t)((st.rows + 7) / 8);
-      TG_TRY(cs.nulls[c]->ensure(j->device, nb + 16));
-      if (nb) { TG_CUDA(cudaMemcpyAsync(cs.nulls[c]->p, st.nulls[c]->p, nb, cudaMemcpyHostToDevice, j->stream)); j->stats.h2d_bytes += nb; }
-    }
-  }
-  return TG_OK;
-}
-
-// a whole (large) host chunk → device column store, straight from the caller's buffers
-static int chunk_to_device(JoinImpl* j, const tg_chunk* chk, const Side& s, ColStore& cs) {
-  int64_t n = chk->cols[0].length;
-  cs.rows = n;
-  for (int c = 0; c < s.ncols; c++) {
-    if (!s.needed[c]) continue;
-    size_t bytes = (size_t)n * s.elem[c];
-    TG_TRY(cs.data[c]->ensure(j->device, bytes + 16));
-    TG_CUDA(cudaMemcpyAsync(cs.data[c]->p, chk->cols[c].data, bytes, cudaMemcpyHostToDevice, j->stream));
-    j->stats.h2d_bytes += bytes;
-    cs.has_nulls[c] = chk->cols[c].null_bitmap != nullptr;
-    if (cs.has_nulls[c]) {
-      size_t nb = (size_t)((n + 7) / 8);
-      TG_TRY(cs.nulls[c]->ensure(j->device, nb + 16));
-      TG_CUDA(cudaMemcpyAsync(cs.nulls[c]->p, chk->cols[c].null_bitmap, nb, cudaMemcpyHostToDevice, j->stream));
-      j->stats.h2d_bytes += nb;
-    }
+    const void* data = st ? st->data[c]->p : chk->cols[c].data;
+    const uint8_t* nulls = st ? (st->has_nulls[c] ? st->nulls[c]->p : nullptr) : chk->cols[c].null_bitmap;
+    cs.has_nulls[c] = nulls != nullptr;
+    TG_TRY(upload_column(j->device, j->stream, data, nulls, cs.rows, s.elem[c], *cs.data[c], *cs.nulls[c], &j->stats.h2d_bytes));
   }
   return TG_OK;
 }
@@ -476,21 +373,12 @@ static int devchunk_append(JoinImpl* j, const tg_chunk* chk, const Side& s, ColS
   return TG_OK;
 }
 
-// borrow a device chunk as a column view (no copy)
-static int devchunk_view(const tg_chunk* chk, const Side& s, DevCols& v, int64_t* rows) {
-  if (!chk || chk->ncols != s.ncols) return fail(TG_ERR_INVALID, "chunk column count does not match the child schema");
-  if (chk->sel) return fail(TG_ERR_UNSUPPORTED, "device-resident chunks must not carry a sel vector");
-  std::memset(&v, 0, sizeof(v));
-  *rows = chk->ncols ? chk->cols[0].length : 0;
-  for (int c = 0; c < s.ncols; c++) {
-    v.elem_len[c] = s.elem[c];
-    if (!s.needed[c]) continue;
-    if (chk->cols[c].elem_len != s.elem[c]) return fail(TG_ERR_INVALID, "chunk column elem_len does not match the schema type");
-    if (chk->cols[c].length != *rows) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
-    if (s.elem[c] == kCellBytes && (reinterpret_cast<uintptr_t>(chk->cols[c].data) & 7)) return fail(TG_ERR_INVALID, "DECIMAL device columns must be 8-byte aligned");
-    v.data[c] = chk->cols[c].data;
-    v.nulls[c] = chk->cols[c].null_bitmap;
-  }
+// borrow a device chunk of the probe side as a column view (no copy)
+static int probe_view(JoinImpl* j, const tg_chunk* chk, DevCols& v) {
+  const Side& s = j->probe;
+  TG_TRY(device_view(chk, s.ncols, s.needed, s.elem, v));
+  for (int c = 0; c < s.ncols; c++)
+    if (s.needed[c] && s.elem[c] == kCellBytes && (reinterpret_cast<uintptr_t>(v.data[c]) & 7)) return fail(TG_ERR_INVALID, "DECIMAL device columns must be 8-byte aligned");
   return TG_OK;
 }
 
@@ -508,7 +396,7 @@ static int composite_key(JoinImpl* j, const Side& s, const DevCols& v, int64_t n
     src.reject[q] = s.key_reject[q];
     if (!src.data[q]) return fail(TG_ERR_INVALID, "key column data is NULL");
   }
-  k_composite_key<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(src, n, key.as<int64_t>(), not_null.as<uint32_t>());
+  k_composite_key<<<grid_size(j->nsm, n, 256, 8), 256, 0, j->stream>>>(src, n, key.as<int64_t>(), not_null.as<uint32_t>());
   j->stats.kernel_launches++;
   return TG_OK;
 }
@@ -522,7 +410,7 @@ static int ensure_iota(JoinImpl* j, int64_t rows) {
   if (rows <= j->iota_rows) return TG_OK;
   rows = std::max(rows, 2 * j->iota_rows);
   TG_TRY(j->iota.ensure(j->device, (size_t)rows * 8 + 16));
-  k_iota<<<grid_for(j, rows, 256, 8), 256, 0, j->stream>>>(j->iota.as<int64_t>(), rows);
+  k_iota<<<grid_size(j->nsm, rows, 256, 8), 256, 0, j->stream>>>(j->iota.as<int64_t>(), rows);
   j->stats.kernel_launches++;
   j->iota_rows = rows;
   return TG_OK;
@@ -630,14 +518,14 @@ static int build_table(JoinImpl* j) {
   unsigned long long* sc = j->scalars.as<unsigned long long>();   // [0] distinct [1] maxcnt [2] cursor
   TG_CUDA(cudaEventRecord(j->ev0, j->stream));
   TG_CUDA(cudaMemsetAsync(sc, 0, 64, j->stream));
-  k_table_init<<<grid_for(j, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, nslots);
+  k_table_init<<<grid_size(j->nsm, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, nslots);
   j->stats.kernel_launches++;
   if (n > 0) {
-    k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots,
+    k_build_insert<<<grid_size(j->nsm, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots,
                                                                   j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>());
     j->stats.kernel_launches++;
   }
-  k_table_stats<<<grid_for(j, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, sc, sc + 1);
+  k_table_stats<<<grid_size(j->nsm, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, sc, sc + 1);
   j->stats.kernel_launches++;
   unsigned long long host_sc[3] = {0, 0, 0};
   TG_CUDA(cudaMemcpyAsync(host_sc, sc, 16, cudaMemcpyDeviceToHost, j->stream));
@@ -668,8 +556,8 @@ static int build_table(JoinImpl* j) {
       j->table.release();
       TG_TRY(j->table.ensure(j->device, (size_t)(nslots + 2) * sizeof(Slot)));   // + the side slot and a spare (probe_rows_u1)
       slots = j->table.as<Slot>();
-      k_table_init<<<grid_for(j, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, nslots);
-      k_build_insert<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots,
+      k_table_init<<<grid_size(j->nsm, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, nslots);
+      k_build_insert<<<grid_size(j->nsm, n, 256, 8), 256, 0, j->stream>>>(ks, bview, b.filter, n, slots, nslots,
                                                                     j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>());
       j->stats.kernel_launches += 2;
       j->stats.table_slots = (int64_t)nslots;
@@ -681,7 +569,7 @@ static int build_table(JoinImpl* j) {
     j->u1_payload_col = payload.empty() ? -1 : payload[0];
     if (n > 0) {
       const unsigned long long* pl = j->u1_payload_col >= 0 ? reinterpret_cast<const unsigned long long*>(bview.data[j->u1_payload_col]) : nullptr;
-      k_build_scatter_u1<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(j->row_slot.as<uint32_t>(), pl, n, slots);
+      k_build_scatter_u1<<<grid_size(j->nsm, n, 256, 8), 256, 0, j->stream>>>(j->row_slot.as<uint32_t>(), pl, n, slots);
       j->stats.kernel_launches++;
     }
     j->tv.mode = TABLE_U1;
@@ -704,11 +592,11 @@ static int build_table(JoinImpl* j) {
     rs.nwords = w + (any_nullable ? 1 : 0);
     if (rs.nwords == 0) rs.nwords = 1;   // semi joins: no payload at all, keep a dummy word so offsets stay valid
     j->rowspec = rs;
-    k_table_assign<<<grid_for(j, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, sc + 2);
+    k_table_assign<<<grid_size(j->nsm, (int64_t)nslots + 1, 256, 8), 256, 0, j->stream>>>(slots, nslots + 1, sc + 2);
     j->stats.kernel_launches++;
     TG_TRY(j->rows_store.ensure(j->device, (size_t)(n + 1) * rs.nwords * 8));
     if (n > 0 && w > 0) {
-      k_build_scatter_rows<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>(), n, slots,
+      k_build_scatter_rows<<<grid_size(j->nsm, n, 256, 8), 256, 0, j->stream>>>(j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>(), n, slots,
                                                                           bview, rs, j->rows_store.as<unsigned long long>());
       j->stats.kernel_launches++;
     }
@@ -741,9 +629,7 @@ static int build_table(JoinImpl* j) {
   TG_CUDA(cudaEventRecord(j->ev1, j->stream));
   TG_CUDA(cudaStreamSynchronize(j->stream));
   TG_CUDA(cudaGetLastError());
-  float ms = 0;
-  cudaEventElapsedTime(&ms, j->ev0, j->ev1);
-  j->stats.build_ms = ms;
+  j->stats.build_ms = j->elapsed_ms();
   j->stats.table_mode = j->tv.mode;
   // valid keys = rows that landed in the table
   j->stats.build_valid_keys = -1;
@@ -790,7 +676,7 @@ static int gather_cells(JoinImpl* j, ResultBatch& rb, const DevCols* probe_cells
     const bool from_left = o < j->n_lused;
     const int col = from_left ? j->lused[o] : j->rused[o - j->n_lused];
     const void* src = from_left == probe_is_left ? (probe_cells ? probe_cells->data[col] : nullptr) : j->bcols.data[col]->p;
-    const int grid = dev_rows ? j->nsm * 8 : grid_for(j, rb.rows * 5, 256, 8);
+    const int grid = dev_rows ? j->nsm * 8 : grid_size(j->nsm, rb.rows * 5, 256, 8);
     k_gather_cells<<<grid, 256, 0, j->stream>>>(j->out_ids[o]->as<int64_t>(), rb.bitmaps[o]->as<uint8_t>(),
                                                 reinterpret_cast<const unsigned long long*>(src), rb.cols[o]->as<unsigned long long>(),
                                                 rb.rows, dev_rows);
@@ -860,7 +746,7 @@ static int finish_bitmaps(JoinImpl* j, ResultBatch& rb, const std::vector<char>&
     if (!nullable[c]) { rb.bitmaps[c]->release(); continue; }
     TG_TRY(rb.bitmaps[c]->ensure(j->device, (size_t)((rb.rows + 7) / 8) + 16));
     if (rb.rows) {
-      k_pack_bitmap<<<grid_for(j, (rb.rows + 7) / 8, 256, 8), 256, 0, j->stream>>>(j->tmp_valid[c]->as<uint8_t>(), rb.rows, rb.bitmaps[c]->as<uint8_t>());
+      launch_pack_bitmap(j->tmp_valid[c]->as<uint8_t>(), rb.rows, rb.bitmaps[c]->as<uint8_t>(), j->nsm, j->stream);
       j->stats.kernel_launches++;
     }
   }
@@ -1076,7 +962,7 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
           TG_TRY(j->tmp_cnt.ensure(j->device, (size_t)(2 * ntiles + 1) * 4));
           j->stats.paths |= TG_JOIN_PATH_PROBE_SEG;
           TG_TRY(dispatch_shape<LaunchInplace>(fo, j, (int64_t)P * C, fo, cur, tune, seg, j->tile_cnt.as<uint32_t>()));
-          k_inplace_holes<<<grid_for(j, ntiles, 256, 4), 256, 0, j->stream>>>(j->tile_cnt.as<uint32_t>(), ntiles, cur, flag, j->tmp_cnt.as<uint32_t>());
+          k_inplace_holes<<<grid_size(j->nsm, ntiles, 256, 4), 256, 0, j->stream>>>(j->tile_cnt.as<uint32_t>(), ntiles, cur, flag, j->tmp_cnt.as<uint32_t>());
           int64_t nblocks = 0;
           TG_TRY(enqueue_scan(j, 2 * ntiles, &nblocks));
           k_inplace_fill<<<j->nsm * 8, 256, 0, j->stream>>>(j->tile_cnt.as<uint32_t>(), ntiles, j->tmp_off.as<unsigned long long>(), cur, flag, fo);
@@ -1164,7 +1050,7 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
     else { sks.data = sub.data[p.key_col]; sks.nulls = sub.nulls[p.key_col]; }
     TG_TRY(j->tmp_cnt.ensure(j->device, (size_t)(m + 1) * 4));
     TG_TRY(j->tmp_slot.ensure(j->device, (size_t)(m + 1) * 4));
-    k_probe_count<<<grid_for(j, m, 256, 8), 256, 0, j->stream>>>(sks, sub, p.filter, j->dev_other, m, j->tv, j->probe_kind, j->tmp_cnt.as<uint32_t>(),
+    k_probe_count<<<grid_size(j->nsm, m, 256, 8), 256, 0, j->stream>>>(sks, sub, p.filter, j->dev_other, m, j->tv, j->probe_kind, j->tmp_cnt.as<uint32_t>(),
                                                                  j->tmp_slot.as<uint32_t>(), j->need_scan ? j->slot_used.as<uint8_t>() : nullptr);
     j->stats.kernel_launches++;
     j->stats.paths |= TG_JOIN_PATH_PROBE_GENERAL;
@@ -1182,7 +1068,7 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
           oc.valid[c] = j->tmp_valid[c]->as<uint8_t>();
         }
       }
-      k_probe_write<<<grid_for(j, m, 256, 8), 256, 0, j->stream>>>(m, j->tmp_off.as<unsigned long long>(), j->tmp_slot.as<uint32_t>(),
+      k_probe_write<<<grid_size(j->nsm, m, 256, 8), 256, 0, j->stream>>>(m, j->tmp_off.as<unsigned long long>(), j->tmp_slot.as<uint32_t>(),
                                                                    reinterpret_cast<const int64_t*>(sks.data), sks, j->tv, sub, oc, j->probe_kind,
                                                                    (unsigned long long)rb.rows, j->dev_other);
       j->stats.kernel_launches++;
@@ -1207,7 +1093,7 @@ static int scan_build_side(JoinImpl* j, ResultBatch& rb) {
   DevCols bview = j->bcols.view(b);
   TG_TRY(kernel_view(j, b, bview, n));
   TG_TRY(j->tmp_cnt.ensure(j->device, (size_t)(n + 1) * 4));
-  k_build_scan_count<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(j->row_slot.as<uint32_t>(), j->slot_used.as<uint8_t>(), n, j->scan_mode, j->tmp_cnt.as<uint32_t>());
+  k_build_scan_count<<<grid_size(j->nsm, n, 256, 8), 256, 0, j->stream>>>(j->row_slot.as<uint32_t>(), j->slot_used.as<uint8_t>(), n, j->scan_mode, j->tmp_cnt.as<uint32_t>());
   j->stats.kernel_launches++;
   unsigned long long total = 0;
   TG_TRY(scan_counts(j, n, &total));
@@ -1231,7 +1117,7 @@ static int scan_build_side(JoinImpl* j, ResultBatch& rb) {
     if (nullable[o]) { TG_TRY(j->tmp_valid[o]->ensure(j->device, (size_t)total + 16)); oc.valid[o] = j->tmp_valid[o]->as<uint8_t>(); }
   }
   if (total) {
-    k_build_scan_write<<<grid_for(j, n, 256, 8), 256, 0, j->stream>>>(n, j->tmp_off.as<unsigned long long>(), bview, oc, 0ull);
+    k_build_scan_write<<<grid_size(j->nsm, n, 256, 8), 256, 0, j->stream>>>(n, j->tmp_off.as<unsigned long long>(), bview, oc, 0ull);
     j->stats.kernel_launches++;
   }
   rb.rows = (int64_t)total;
@@ -1260,18 +1146,52 @@ static void queue_result(JoinImpl* j, std::unique_ptr<ResultBatch> rb) {
   j->res_cv.notify_all();
 }
 
+// probe n rows into rb, timed into probe_ms; with sync_count = false the probe is left in flight and its time uncounted
+static int timed_probe(JoinImpl* j, const DevCols& pview, int64_t n, ResultBatch& rb, bool sync_count, const SegSpec* seg = nullptr) {
+  TG_CUDA(cudaEventRecord(j->ev0, j->stream));
+  TG_TRY(probe_device(j, pview, n, rb, sync_count, seg));
+  TG_CUDA(cudaEventRecord(j->ev1, j->stream));
+  if (!sync_count) return TG_OK;
+  TG_CUDA(cudaStreamSynchronize(j->stream));
+  j->stats.probe_ms += j->elapsed_ms();
+  return TG_OK;
+}
+
+// probe a batch of host rows (the staging st, or a big chunk when st = nullptr) and queue its result for *_next
+static int probe_host_rows(JoinImpl* j, const HostStage* st, const tg_chunk* chk) {
+  TG_TRY(upload_side(j, j->probe, st, chk, j->pcols_dev));
+  std::unique_ptr<ResultBatch> rb = new_batch(j);
+  TG_TRY(timed_probe(j, j->pcols_dev.view(j->probe), j->pcols_dev.rows, *rb, true));
+  queue_result(j, std::move(rb));
+  return TG_OK;
+}
+
 static int flush_probe_stage(JoinImpl* j) {
   if (j->pstage.rows == 0) return TG_OK;
-  TG_TRY(stage_to_device(j, j->pstage, j->probe, j->pcols_dev));
-  std::unique_ptr<ResultBatch> rb = new_batch(j);
-  DevCols pview = j->pcols_dev.view(j->probe);
-  TG_CUDA(cudaEventRecord(j->ev0, j->stream));
-  TG_TRY(probe_device(j, pview, j->pstage.rows, *rb, true));
-  TG_CUDA(cudaEventRecord(j->ev1, j->stream));
-  TG_CUDA(cudaStreamSynchronize(j->stream));
-  float ms = 0; cudaEventElapsedTime(&ms, j->ev0, j->ev1); j->stats.probe_ms += ms;
+  TG_TRY(probe_host_rows(j, &j->pstage, nullptr));
   j->pstage.reset();
-  queue_result(j, std::move(rb));
+  return TG_OK;
+}
+
+// tg_join_probe_dev(_seg): probe a device-resident chunk into dev_result; seg = the segment layout of its rows
+static int probe_dev_chunk(JoinImpl* j, const tg_chunk* dev_chk, const SegSpec* seg, int64_t nseg, int64_t* out_rows,
+                           void** out_cols, void** out_nulls) {
+  DevCols pview;
+  TG_TRY(probe_view(j, dev_chk, pview));
+  const int64_t n = logical_rows(dev_chk);
+  if (seg) {
+    if (n != nseg * seg->cap) return fail(TG_ERR_INVALID, "column length must be nseg * seg_cap");
+    if (n / 128 >= (1ll << 31)) return fail(TG_ERR_UNSUPPORTED, "segmented chunk too large");
+  }
+  if (!j->dev_result) j->dev_result.reset(new ResultBatch());
+  ResultBatch& rb = *j->dev_result;
+  rb.rows = 0; rb.consumed = 0;
+  TG_TRY(timed_probe(j, pview, n, rb, out_rows != nullptr, seg));
+  if (out_rows) *out_rows = rb.rows;
+  for (int c = 0; c < j->n_out; c++) {
+    if (out_cols) out_cols[c] = rb.cols[c]->p;
+    if (out_nulls) out_nulls[c] = rb.bitmaps[c]->p;
+  }
   return TG_OK;
 }
 
@@ -1280,15 +1200,6 @@ static int flush_probe_stage(JoinImpl* j) {
 // ---------------------------------------------------------------------------------------------------
 // C entry points
 // ---------------------------------------------------------------------------------------------------
-#define TG_LOCK(h)                                                             \
-  if (!(h)) return tg::fail(TG_ERR_INVALID, "handle is NULL");                 \
-  if ((h)->closed.load()) return tg::fail(TG_ERR_CANCELLED, "handle is closed"); \
-  std::lock_guard<std::mutex> lock__((h)->mu);                                 \
-  if ((h)->closed.load() || !(h)->impl) return tg::fail(TG_ERR_CANCELLED, "handle is closed"); \
-  JoinImpl* j = (h)->impl;                                                     \
-  tg::DeviceGuard guard__(j->device);                                          \
-  if (!guard__.ok) return tg::fail(TG_ERR_CUDA, "cudaSetDevice failed (no usable CUDA device)")
-
 extern "C" {
 
 int tg_join_supported(const tg_join_desc* desc) {
@@ -1304,16 +1215,12 @@ int tg_join_open(const tg_join_desc* desc, tg_join** out) {
   std::unique_ptr<JoinImpl> j(new JoinImpl(*shell));
   TG_TRY(setup(j.get(), desc));
   int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(TG_ERR_CUDA, "no CUDA device: the GPU hash join has no CPU fallback"); }
+  TG_TRY(require_device("the GPU hash join", &ndev));
   if (j->device < 0 || j->device >= ndev) return fail(TG_ERR_INVALID, "device ordinal out of range");
   DeviceGuard g(j->device);
   if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
-  if (desc->stream) { j->stream = (cudaStream_t)desc->stream; j->own_stream = false; }
-  else { TG_CUDA(cudaStreamCreateWithFlags(&j->stream, cudaStreamNonBlocking)); j->own_stream = true; }
-  TG_CUDA(cudaEventCreate(&j->ev0));
-  TG_CUDA(cudaEventCreate(&j->ev1));
+  TG_TRY(j->open(j->device, desc->stream));
   TG_CUDA(cudaStreamCreateWithFlags(&j->d2h_stream, cudaStreamNonBlocking));
-  j->nsm = device_sm_count(j->device);
   j->bstage.init(j->build.ncols); j->bcols.init(j->build.ncols);
   j->pstage.init(j->probe.ncols); j->pcols_dev.init(j->probe.ncols);
   shell->impl = j.release();
@@ -1322,24 +1229,24 @@ int tg_join_open(const tg_join_desc* desc, tg_join** out) {
 }
 
 int tg_join_build_push(tg_join* h, const tg_chunk* chk) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (j->built) return fail(TG_ERR_STATE, "build_push after build_finish");
-  TG_TRY(validate_chunk(j->build, chk));
-  return stage_append(j->bstage, j->build, chk);
+  TG_TRY(validate_chunk(j->build.ncols, j->build.needed, j->build.elem, chk));
+  return stage_append(j->bstage, j->build.needed, j->build.elem, chk);
 }
 
 int tg_join_build_push_dev(tg_join* h, const tg_chunk* chk) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (j->built) return fail(TG_ERR_STATE, "build_push after build_finish");
   if (j->bstage.rows) return fail(TG_ERR_STATE, "host and device build pushes cannot be mixed");
-  TG_TRY(validate_chunk(j->build, chk));
+  TG_TRY(validate_chunk(j->build.ncols, j->build.needed, j->build.elem, chk));
   return devchunk_append(j, chk, j->build, j->bcols);
 }
 
 int tg_join_build_finish(tg_join* h) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (j->built) return fail(TG_ERR_STATE, "build_finish called twice");
-  if (j->bstage.rows) { TG_TRY(stage_to_device(j, j->bstage, j->build, j->bcols)); }
+  if (j->bstage.rows) { TG_TRY(upload_side(j, j->build, &j->bstage, nullptr, j->bcols)); }
   int rc = build_table(j);
   // pinned staging of the build side is no longer needed
   j->bstage.init(j->build.ncols);
@@ -1347,32 +1254,23 @@ int tg_join_build_finish(tg_join* h) {
 }
 
 int tg_join_probe_push(tg_join* h, const tg_chunk* chk) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (!j->built) return fail(TG_ERR_STATE, "probe_push before build_finish");
   if (j->probe_finished.load()) return fail(TG_ERR_STATE, "probe_push after probe_finish");
-  TG_TRY(validate_chunk(j->probe, chk));
-  int64_t n = chunk_logical_rows(chk);
+  TG_TRY(validate_chunk(j->probe.ncols, j->probe.needed, j->probe.elem, chk));
+  int64_t n = logical_rows(chk);
   if (n == 0) return TG_OK;
   if (!chk->sel && n >= kDirectPushRows) {
     TG_TRY(flush_probe_stage(j));
-    TG_TRY(chunk_to_device(j, chk, j->probe, j->pcols_dev));
-    std::unique_ptr<ResultBatch> rb = new_batch(j);
-    DevCols pview = j->pcols_dev.view(j->probe);
-    TG_CUDA(cudaEventRecord(j->ev0, j->stream));
-    TG_TRY(probe_device(j, pview, n, *rb, true));
-    TG_CUDA(cudaEventRecord(j->ev1, j->stream));
-    TG_CUDA(cudaStreamSynchronize(j->stream));
-    float ms = 0; cudaEventElapsedTime(&ms, j->ev0, j->ev1); j->stats.probe_ms += ms;
-    queue_result(j, std::move(rb));
-    return TG_OK;
+    return probe_host_rows(j, nullptr, chk);
   }
-  TG_TRY(stage_append(j->pstage, j->probe, chk));
+  TG_TRY(stage_append(j->pstage, j->probe.needed, j->probe.elem, chk));
   if (j->pstage.rows >= kStageBatchRows) TG_TRY(flush_probe_stage(j));
   return TG_OK;
 }
 
 int tg_join_probe_finish(tg_join* h) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (!j->built) return fail(TG_ERR_STATE, "probe_finish before build_finish");
   if (j->probe_finished.load()) return TG_OK;
   TG_TRY(flush_probe_stage(j));
@@ -1414,7 +1312,7 @@ static int join_next_impl(tg_join* h, tg_mut_chunk* out, int64_t max_rows, int64
   int64_t want = std::min<int64_t>(std::min<int64_t>(max_rows, out->capacity_rows), rb.rows - rb.consumed);
   if (want <= 0) return TG_OK;
   // any RequiredRows >= 1 is served (LIMIT 1, MaxOneRow): the result's bit-packed NULL bitmaps are re-aligned on the host
-  // when the read cursor is not on a byte boundary (see below)
+  // when the read cursor is not on a byte boundary (download_bitmaps)
   int64_t lo = rb.consumed;
   // row bytes of all columns, for the small-request window
   size_t row_bytes = 0;
@@ -1448,42 +1346,16 @@ static int join_next_impl(tg_join* h, tg_mut_chunk* out, int64_t max_rows, int64
       offb += (size_t)wn * el;
     }
   }
-  const int shift = (int)(lo & 7);
-  std::vector<std::vector<uint8_t>> shifted;    // bitmaps that start inside a byte: fetched whole, shifted below
-  for (int c = 0; c < j->n_out; c++) {
-    size_t nb = (size_t)((want + 7) / 8);
-    if (rb.bitmaps[c]->p) {
-      if (!out->cols[c].null_bitmap) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");
-      if (shift == 0) TG_CUDA(cudaMemcpyAsync(out->cols[c].null_bitmap, rb.bitmaps[c]->as<uint8_t>() + lo / 8, nb, cudaMemcpyDeviceToHost, cstream));
-      else {
-        shifted.emplace_back((size_t)((shift + want + 7) / 8) + 1, (uint8_t)0);
-        TG_CUDA(cudaMemcpyAsync(shifted.back().data(), rb.bitmaps[c]->as<uint8_t>() + lo / 8, shifted.back().size() - 1, cudaMemcpyDeviceToHost, cstream));
-      }
-      j->d2h_bytes += nb;
-    } else if (out->cols[c].null_bitmap) {
-      std::memset(out->cols[c].null_bitmap, 0xff, nb);
-      if (want & 7) out->cols[c].null_bitmap[nb - 1] = (uint8_t)((1u << (want & 7)) - 1);
-    }
-  }
-  TG_CUDA(cudaStreamSynchronize(cstream));
-  if (shift) {
-    size_t q = 0;
-    for (int c = 0; c < j->n_out; c++) {
-      if (!rb.bitmaps[c]->p) continue;
-      const std::vector<uint8_t>& src = shifted[q++];
-      size_t nb = (size_t)((want + 7) / 8);
-      for (size_t b = 0; b < nb; b++) out->cols[c].null_bitmap[b] = (uint8_t)((src[b] >> shift) | (src[b + 1] << (8 - shift)));
-    }
-  }
-  // mask the tail bits of copied bitmaps (Column.nullBitmap keeps unused bits zero)
-  if (want & 7) for (int c = 0; c < j->n_out; c++) if (rb.bitmaps[c]->p) out->cols[c].null_bitmap[(want >> 3)] &= (uint8_t)((1u << (want & 7)) - 1);
+  int64_t bitmap_bytes = 0;
+  TG_TRY(download_bitmaps(rb.bitmaps, out, lo, want, cstream, &bitmap_bytes));
+  j->d2h_bytes += bitmap_bytes;
   rb.consumed += want;
   *nrows = want;
   return TG_OK;
 }
 
 int tg_join_probe_rewind(tg_join* h) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (!j->built) return fail(TG_ERR_STATE, "rewind before build_finish");
   if (j->need_scan) return fail(TG_ERR_UNSUPPORTED, "joins that scan the build side afterwards cannot be re-probed (used flags accumulate)");
   j->pstage.reset();
@@ -1498,58 +1370,22 @@ int tg_join_next(tg_join* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows
 int tg_join_next_wait(tg_join* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) { return join_next_impl(h, out, max_rows, nrows, true); }
 
 int tg_join_probe_dev(tg_join* h, const tg_chunk* dev_chk, int64_t* out_rows, void** out_cols, void** out_nulls) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (!j->built) return fail(TG_ERR_STATE, "probe before build_finish");
-  DevCols pview; int64_t n = 0;
-  TG_TRY(devchunk_view(dev_chk, j->probe, pview, &n));
-  if (!j->dev_result) j->dev_result.reset(new ResultBatch());
-  ResultBatch& rb = *j->dev_result;
-  rb.rows = 0; rb.consumed = 0;
-  TG_CUDA(cudaEventRecord(j->ev0, j->stream));
-  TG_TRY(probe_device(j, pview, n, rb, out_rows != nullptr));
-  TG_CUDA(cudaEventRecord(j->ev1, j->stream));
-  if (out_rows) {
-    TG_CUDA(cudaStreamSynchronize(j->stream));
-    float ms = 0; cudaEventElapsedTime(&ms, j->ev0, j->ev1); j->stats.probe_ms += ms;
-    *out_rows = rb.rows;
-  }
-  for (int c = 0; c < j->n_out; c++) {
-    if (out_cols) out_cols[c] = rb.cols[c]->p;
-    if (out_nulls) out_nulls[c] = rb.bitmaps[c]->p;
-  }
-  return TG_OK;
+  return probe_dev_chunk(j, dev_chk, nullptr, 0, out_rows, out_cols, out_nulls);
 }
 
 int tg_join_probe_dev_seg(tg_join* h, const tg_chunk* dev_chk, const int64_t* seg_cnt_dev, int32_t nseg, int64_t seg_cap,
                           int64_t* out_rows, void** out_cols, void** out_nulls) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (!j->built) return fail(TG_ERR_STATE, "probe before build_finish");
   if (!seg_cnt_dev || nseg < 1 || seg_cap < 1024 || seg_cap % 1024) return fail(TG_ERR_INVALID, "seg_cnt_dev required; seg_cap must be a positive multiple of 1024");
-  DevCols pview; int64_t n = 0;
-  TG_TRY(devchunk_view(dev_chk, j->probe, pview, &n));
-  if (n != (int64_t)nseg * seg_cap) return fail(TG_ERR_INVALID, "column length must be nseg * seg_cap");
-  if (n / 128 >= (1ll << 31)) return fail(TG_ERR_UNSUPPORTED, "segmented chunk too large");
-  if (!j->dev_result) j->dev_result.reset(new ResultBatch());
-  ResultBatch& rb = *j->dev_result;
-  rb.rows = 0; rb.consumed = 0;
   SegSpec seg{reinterpret_cast<const unsigned long long*>(seg_cnt_dev), (uint32_t)(seg_cap / 128), 0, seg_cap, nullptr};
-  TG_CUDA(cudaEventRecord(j->ev0, j->stream));
-  TG_TRY(probe_device(j, pview, n, rb, out_rows != nullptr, &seg));
-  TG_CUDA(cudaEventRecord(j->ev1, j->stream));
-  if (out_rows) {
-    TG_CUDA(cudaStreamSynchronize(j->stream));
-    float ms = 0; cudaEventElapsedTime(&ms, j->ev0, j->ev1); j->stats.probe_ms += ms;
-    *out_rows = rb.rows;
-  }
-  for (int c = 0; c < j->n_out; c++) {
-    if (out_cols) out_cols[c] = rb.cols[c]->p;
-    if (out_nulls) out_nulls[c] = rb.bitmaps[c]->p;
-  }
-  return TG_OK;
+  return probe_dev_chunk(j, dev_chk, &seg, nseg, out_rows, out_cols, out_nulls);
 }
 
 int tg_join_get_stats(tg_join* h, tg_join_stats* out) {
-  TG_LOCK(h);
+  TG_LOCK(h, JoinImpl, j);
   if (!out) return fail(TG_ERR_INVALID, "out is NULL");
   TG_CUDA(cudaStreamSynchronize(j->stream));
   *out = j->stats;
@@ -1577,9 +1413,7 @@ int tg_join_close(tg_join* h) {
       j->results.clear();
       j->free_batches.clear();
       j->dev_result.reset();
-      if (j->ev0) cudaEventDestroy(j->ev0);
-      if (j->ev1) cudaEventDestroy(j->ev1);
-      if (j->own_stream && j->stream) cudaStreamDestroy(j->stream);
+      j->release();
       cudaGetLastError();
       delete j;
     }

@@ -1250,16 +1250,4 @@ k_gather_cells(const int64_t* __restrict__ ids, const uint8_t* __restrict__ bitm
   }
 }
 
-// valid bytes (1 = NOT NULL) → Column.nullBitmap bits
-__global__ void k_pack_bitmap(const uint8_t* __restrict__ valid, int64_t n, uint8_t* __restrict__ bitmap) {
-  int64_t b = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  int64_t nbytes = (n + 7) / 8;
-  for (; b < nbytes; b += stride) {
-    uint8_t v = 0;
-    for (int j = 0; j < 8; j++) { int64_t r = b * 8 + j; if (r < n && valid[r]) v |= (uint8_t)(1u << j); }
-    bitmap[b] = v;
-  }
-}
-
 }  // namespace tg

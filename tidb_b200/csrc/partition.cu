@@ -19,12 +19,6 @@ static int check_parts(int32_t nparts, int32_t ncols) {
   return TG_OK;
 }
 
-static int pgrid(int device, int64_t n, int per_block, int per_sm) {
-  int64_t need = (n + per_block - 1) / per_block, cap = (int64_t)device_sm_count(device) * per_sm;
-  if (need < 1) need = 1;
-  return (int)(need < cap ? need : cap);
-}
-
 // Per-device scratch of the counted calls (counts | cursors): allocated once, never freed — a DevBuf per call would run
 // pool_free's device-wide synchronisation on every exchange step.  The counted calls synchronise their stream before
 // returning, so holding the device's mutex for the duration of a call makes the shared scratch safe.

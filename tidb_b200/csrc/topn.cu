@@ -11,9 +11,9 @@
 //                      are returned.  Ties are broken arbitrarily, as by the reference's heap.
 // HBM-bound: the rank pass reads 8 B/row + bitmap, each histogram pass 8 B/row.
 #include <algorithm>
-#include <memory>
 #include <vector>
 #include "common.cuh"
+#include "chunk_io.cuh"
 
 namespace tg {
 
@@ -126,8 +126,7 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
     if (items[q].col < 0 || items[q].col >= nc) return fail(TG_ERR_INVALID, "ORDER BY column out of range");
     if (kinds[items[q].col] < 0) return fail(TG_ERR_UNSUPPORTED, "ORDER BY column type is not offloaded (int family / double / time)");
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(TG_ERR_CUDA, "no CUDA device: TopN has no CPU fallback"); }
+  TG_TRY(require_device("TopN"));
   DeviceGuard g(device);
   if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
   cudaStream_t st = (cudaStream_t)stream;
@@ -135,25 +134,18 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
   if (n == 0 || count == 0 || offset >= n) return TG_OK;
   const int64_t want = count >= n - offset ? n : offset + count;   // min(n, offset + count) without overflowing int64
   // device-resident columns
-  std::vector<std::unique_ptr<DevBuf>> hold;
+  std::vector<DevBuf> hdata(nc), hnulls(nc);
   std::vector<const unsigned long long*> dcol(nc);
   std::vector<const uint8_t*> dnul(nc, nullptr);
   for (int c = 0; c < nc; c++) {
     if (chk->cols[c].length != n) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
     if (on_device) { dcol[c] = reinterpret_cast<const unsigned long long*>(chk->cols[c].data); dnul[c] = chk->cols[c].null_bitmap; continue; }
-    hold.emplace_back(new DevBuf());
-    TG_TRY(hold.back()->ensure(device, (size_t)n * 8 + 16));
-    TG_CUDA(cudaMemcpyAsync(hold.back()->p, chk->cols[c].data, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    dcol[c] = hold.back()->as<unsigned long long>();
-    if (chk->cols[c].null_bitmap) {
-      hold.emplace_back(new DevBuf());
-      size_t nb = (size_t)((n + 7) / 8);
-      TG_TRY(hold.back()->ensure(device, nb + 16));
-      TG_CUDA(cudaMemcpyAsync(hold.back()->p, chk->cols[c].null_bitmap, nb, cudaMemcpyHostToDevice, st));
-      dnul[c] = hold.back()->as<uint8_t>();
-    }
+    TG_TRY(upload_column(device, st, chk->cols[c].data, chk->cols[c].null_bitmap, n, 8, hdata[c], hnulls[c], nullptr));
+    dcol[c] = hdata[c].as<unsigned long long>();
+    if (chk->cols[c].null_bitmap) dnul[c] = hnulls[c].as<uint8_t>();
   }
-  const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)device_sm_count(device) * 8);
+  const int nsm = device_sm_count(device);
+  const int grid = grid_size(nsm, n, 256, 8);
   DevBuf rank, scratch, idx;
   TG_TRY(rank.ensure(device, (size_t)n * 8 + 16));
   TG_TRY(scratch.ensure(device, 257 * 8));
@@ -191,7 +183,7 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
   DevBuf gcol, gval;
   TG_TRY(gcol.ensure(device, (size_t)m * 8 + 16));
   TG_TRY(gval.ensure(device, (size_t)m + 16));
-  const int ggrid = (int)std::min<int64_t>(((int64_t)m + 255) / 256, (int64_t)device_sm_count(device) * 8);
+  const int ggrid = grid_size(nsm, (int64_t)m, 256, 8);
   for (int c = 0; c < nc; c++) {
     k_topn_gather<<<ggrid, 256, 0, st>>>(dcol[c], dnul[c], idx.as<long long>(), (int64_t)m, gcol.as<unsigned long long>(), gval.as<uint8_t>());
     TG_CUDA(cudaMemcpyAsync(hv[c].data(), gcol.p, (size_t)m * 8, cudaMemcpyDeviceToHost, st));

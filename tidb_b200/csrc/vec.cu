@@ -8,6 +8,7 @@
 // 8 B (+8 B) read and 8 B written per row, null bitmaps merged bytewise (Column.MergeNulls column.go:906).
 #include <memory>
 #include "common.cuh"
+#include "chunk_io.cuh"
 
 namespace tg {
 
@@ -194,32 +195,19 @@ struct ArgDev {
     if (!c) return TG_OK;
     if (c->elem_len != 8) return fail(TG_ERR_UNSUPPORTED, "VecEval kernels take 8-byte columns");
     if (on_device) { v.data = c->data; v.nulls = c->null_bitmap; return TG_OK; }
-    size_t bytes = (size_t)c->length * 8, nb = (size_t)((c->length + 7) / 8);
-    TG_TRY(data.ensure(device, bytes + 16));
-    if (bytes) TG_CUDA(cudaMemcpyAsync(data.p, c->data, bytes, cudaMemcpyHostToDevice, st));
+    TG_TRY(upload_column(device, st, c->data, c->null_bitmap, c->length, 8, data, nulls, nullptr));
     v.data = data.p;
-    if (c->null_bitmap) {
-      TG_TRY(nulls.ensure(device, nb + 16));
-      if (nb) TG_CUDA(cudaMemcpyAsync(nulls.p, c->null_bitmap, nb, cudaMemcpyHostToDevice, st));
-      v.nulls = nulls.as<uint8_t>();
-    }
+    if (c->null_bitmap) v.nulls = nulls.as<uint8_t>();
     return TG_OK;
   }
 };
-
-static int vgrid(int device, int64_t n_threads) {
-  int64_t need = (n_threads + 255) / 256, cap = (int64_t)device_sm_count(device) * 8;
-  if (need < 1) need = 1;
-  return (int)(need < cap ? need : cap);
-}
 
 template <typename Launch>
 static int run_binary(int device, int on_device, const tg_column* a, const tg_column* b, void* result, uint8_t* rnulls,
                       void* stream, bool has_overflow, Launch launch) {
   if (!a || !result || !rnulls) return fail(TG_ERR_INVALID, "a / result / result_nulls is NULL");
   if (b && b->length != a->length) return fail(TG_ERR_INVALID, "argument columns have different lengths");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(TG_ERR_CUDA, "no CUDA device: VecEval kernels have no CPU fallback"); }
+  TG_TRY(require_device("VecEval"));
   DeviceGuard g(device);
   if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
   cudaStream_t st = (cudaStream_t)stream;
@@ -240,7 +228,7 @@ static int run_binary(int device, int on_device, const tg_column* a, const tg_co
   }
   if (!dovf) TG_CUDA(cudaMalloc(reinterpret_cast<void**>(&dovf), 16));
   TG_CUDA(cudaMemsetAsync(dovf, 0, 4, st));
-  if (n > 0) launch(vgrid(device, (n + VEC_ITEMS - 1) / VEC_ITEMS), st, da.v, db.v, n, res_dev, nul_dev, dovf);
+  if (n > 0) launch(grid_size(device_sm_count(device), (n + VEC_ITEMS - 1) / VEC_ITEMS, 256, 8), st, da.v, db.v, n, res_dev, nul_dev, dovf);
   int ovf = 0;
   if (has_overflow) TG_CUDA(cudaMemcpyAsync(&ovf, dovf, 4, cudaMemcpyDeviceToHost, st));
   if (!on_device && n > 0) {
@@ -298,8 +286,7 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk, const tg_filte
   if (!chk || !selected) return fail(TG_ERR_INVALID, "chunk / selected is NULL");
   if (n_items < 0 || n_items > TG_MAX_FILTER) return fail(TG_ERR_UNSUPPORTED, "at most 8 CNF filter items are offloaded");
   if (chk->ncols <= 0 || chk->ncols > TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "chunk must have 1..16 columns");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(TG_ERR_CUDA, "no CUDA device: VecEval kernels have no CPU fallback"); }
+  TG_TRY(require_device("VecEval"));
   DeviceGuard g(device);
   if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
   cudaStream_t st = (cudaStream_t)stream;
@@ -336,7 +323,7 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk, const tg_filte
   TG_CUDA(cudaMemsetAsync(dcount.p, 0, 8, st));
   TG_CUDA(cudaMemsetAsync(selected_dev, 0, (size_t)nphys, st));
   int64_t n = chk->sel ? chk->nsel : nphys;
-  if (n > 0) k_vec_filter<<<vgrid(device, n), 256, 0, st>>>(cols, f, sel_dev, chk->nsel, nphys, selected_dev, dcount.as<unsigned long long>());
+  if (n > 0) k_vec_filter<<<grid_size(device_sm_count(device), n, 256, 8), 256, 0, st>>>(cols, f, sel_dev, chk->nsel, nphys, selected_dev, dcount.as<unsigned long long>());
   unsigned long long cnt = 0;
   TG_CUDA(cudaMemcpyAsync(&cnt, dcount.p, 8, cudaMemcpyDeviceToHost, st));
   if (!on_device && nphys) TG_CUDA(cudaMemcpyAsync(selected, selected_dev, (size_t)nphys, cudaMemcpyDeviceToHost, st));
