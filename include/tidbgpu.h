@@ -527,9 +527,23 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk,
  * ORDER BY items over plain columns, LIMIT offset, count.  Rows [offset, offset + count) of the child's rows in item
  * order (NULL sorts before every value, DESC reverses: chunk.GetCompareFunc) are written to `out` (child schema, host
  * buffers, capacity >= min(count, rows - offset)); ties are broken arbitrarily, as by the reference's heap.
- * `on_device` as in the VecEval calls.  8-byte int-family / double / time columns.  DOUBLE compares as Go cmp.Compare
- * (NaN first, -0 == +0); DATE / DATETIME / TIMESTAMP compare by calendar value and microseconds, ignoring the fsp and
- * type bits (types/core_time.go compareTime).  The output rows keep the input's bits.
+ * `on_device` as in the VecEval calls.  8-byte int-family / double / time columns, and DECIMAL columns of 40-byte
+ * MyDecimal cells (elem_len 40 and col_types TG_TYPE_NEWDECIMAL; a 40-byte column of any other type, or an 8-byte column
+ * typed NEWDECIMAL as an ORDER BY item, is TG_ERR_UNSUPPORTED), as ORDER BY items, payload or both.  These argument checks
+ * need no device.  DOUBLE compares as Go cmp.Compare (NaN first, -0 == +0); DATE / DATETIME / TIMESTAMP compare by
+ * calendar value and microseconds, ignoring the fsp and type bits (types/core_time.go compareTime).
+ * DECIMAL compares as cmpMyDecimal / MyDecimal.Compare (types/mydecimal.go): the sign first, so a cell with `negative`
+ * set and a zero value sorts after every negative value and before +0 (all such negative zeros are equal); then the
+ * magnitudes by their words as doSub does: ceil(digitsInt / 9) integer words, then ceil(digitsFrac / 9) fraction words,
+ * left-aligned, with leading zero integer words and trailing zero fraction words not counted (1.50 == 1.5 whatever the
+ * digitsInt).  resultFrac and the words after the used ones are ignored.  Any well-formed cell of up to 9 words is
+ * accepted, whatever its declared precision.  A non-NULL cell of a DECIMAL ORDER BY column is malformed when digitsInt
+ * or digitsFrac is negative, its integer and fraction words number more than 9, or one of them is >= 10^9: every
+ * non-NULL cell of such a column is checked (whatever offset and count select), and one malformed cell fails the call
+ * with TG_ERR_INVALID, *nrows = 0 and `out` not written.  Payload cells are never interpreted.
+ * The output rows keep the input's bits: a DECIMAL cell is copied whole (header, resultFrac and unused words included),
+ * and a NULL row's cell is 40 zero bytes.  The output column of a DECIMAL column must have elem_len 40 (TG_ERR_INVALID
+ * otherwise); device-resident DECIMAL columns must be 8-byte aligned.
  * ------------------------------------------------------------------------------------------- */
 typedef struct tg_sort_item { int32_t col; int32_t desc; } tg_sort_item;
 int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_types, const uint32_t* col_flags,

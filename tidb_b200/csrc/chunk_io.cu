@@ -1,5 +1,6 @@
 // chunk_io.cu — the host side of the chunk contract shared by the operators (chunk_io.cuh).
 #include "chunk_io.cuh"
+#include "decimal.cuh"
 
 namespace tg {
 
@@ -133,6 +134,27 @@ __global__ void k_pack_bitmap(const uint8_t* __restrict__ valid, int64_t n, uint
 
 void launch_pack_bitmap(const uint8_t* valid, int64_t n, uint8_t* bitmap, int nsm, cudaStream_t s) {
   k_pack_bitmap<<<grid_size(nsm, (n + 7) / 8, 256, 8), 256, 0, s>>>(valid, n, bitmap);
+}
+
+// five lanes per row, one 8-byte word each: coalesced stores
+__global__ void __launch_bounds__(256)
+k_gather_cells(const int64_t* __restrict__ ids, const uint8_t* __restrict__ bitmap, const unsigned long long* __restrict__ src,
+               unsigned long long* __restrict__ dst, int64_t rows, const unsigned long long* dev_rows) {
+  constexpr int W = TG_DEC_CELL_BYTES / 8;
+  const int64_t n = (dev_rows ? (int64_t)*dev_rows : rows) * W;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / W;
+    unsigned long long v = 0;
+    if (!bitmap || bit_not_null(bitmap, r)) v = src[ids[r] * W + (i - r * W)];
+    dst[i] = v;
+  }
+}
+
+void launch_gather_cells(const int64_t* ids, const uint8_t* bitmap, const void* src, void* dst, int64_t rows,
+                         const unsigned long long* dev_rows, int nsm, cudaStream_t s) {
+  const int grid = dev_rows ? nsm * 8 : grid_size(nsm, rows * (TG_DEC_CELL_BYTES / 8), 256, 8);
+  k_gather_cells<<<grid, 256, 0, s>>>(ids, bitmap, reinterpret_cast<const unsigned long long*>(src),
+                                      reinterpret_cast<unsigned long long*>(dst), rows, dev_rows);
 }
 
 int require_device(const char* what, int* ndev) {

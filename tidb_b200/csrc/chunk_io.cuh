@@ -1,7 +1,7 @@
 // chunk_io.cuh — how the operators read a pushed tg_chunk and fill a caller's tg_mut_chunk: validation, pinned host
-// staging (sel gather, lazy NULL bitmaps), host → device column uploads, views of device-resident chunks and the NULL
-// bitmaps of *_next; plus what every operator handle needs of its device: the launch grid, the device check, and a
-// stream with two timing events.
+// staging (sel gather, lazy NULL bitmaps), host → device column uploads, views of device-resident chunks, the NULL
+// bitmaps of *_next and the gather of DECIMAL cells by row id; plus what every operator handle needs of its device: the
+// launch grid, the device check, and a stream with two timing events.
 #pragma once
 #include <algorithm>
 #include <memory>
@@ -60,6 +60,12 @@ inline int grid_size(int nsm, int64_t n, int block, int per_sm) {
 
 // valid bytes (1 = NOT NULL) of n rows → Column.nullBitmap bits, on stream s (k_pack_bitmap)
 void launch_pack_bitmap(const uint8_t* valid, int64_t n, uint8_t* bitmap, int nsm, cudaStream_t s);
+
+// 40-byte DECIMAL cells by row id, on stream s (k_gather_cells): dst row r = src row ids[r], 40 zero bytes where `bitmap`
+// (indexed by r, may be NULL) says NULL.  The row count is *dev_rows when given (kept on the device), else `rows`.
+// src and dst are 8-byte aligned.
+void launch_gather_cells(const int64_t* ids, const uint8_t* bitmap, const void* src, void* dst, int64_t rows,
+                         const unsigned long long* dev_rows, int nsm, cudaStream_t s);
 
 // TG_OK when the process sees a CUDA device (*ndev = how many); `what` names the operator in the error
 int require_device(const char* what, int* ndev = nullptr);

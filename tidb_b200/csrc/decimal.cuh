@@ -1,5 +1,5 @@
 // decimal.cuh — the MyDecimal cell of an exact DECIMAL aggregate result and of a DECIMAL argument column (included by agg.cu:
-// k_agg_finalize writes cells, k_dec_to_scaled parses them).
+// k_agg_finalize writes cells, k_dec_to_scaled parses them), and the order of cells (included by topn.cu).
 //
 // A cell is the 40-byte types.MyDecimal (types/mydecimal.go:236-248) that chunk.Column copies whole (util/chunk/column.go:41):
 //   byte 0 digitsInt (int8), byte 1 digitsFrac (int8), byte 2 resultFrac (int8), byte 3 negative (bool),
@@ -87,7 +87,7 @@ __device__ __forceinline__ bool dec_parse_cell(const uint32_t (&c)[10], int flen
 // SUM: the exact sum at the argument's scale (sum4Decimal, func_sum.go:207-253; its final Round to the scale leaves the sum
 // alone).  The integer part is |sum| / 10^scale; the remainder, left-aligned, gives the ceil(scale / 9) fraction words.  A
 // DECIMAL MIN / MAX writes its int64 here too (hi = the sign extension).
-__device__ __noinline__ void dec_sum_cell(uint8_t* cell, unsigned long long lo, unsigned long long hi, int scale) {
+static __device__ __noinline__ void dec_sum_cell(uint8_t* cell, unsigned long long lo, unsigned long long hi, int scale) {
   const __int128 s = dec_sum_of(lo, hi);
   const bool neg = s < 0;
   unsigned __int128 m = neg ? (unsigned __int128)(-s) : (unsigned __int128)s;
@@ -117,7 +117,7 @@ __device__ __noinline__ void dec_sum_cell(uint8_t* cell, unsigned long long lo, 
 // The value is sum / (count * 10^scale), and count * 10^scale can pass 64 bits: the digits are those of m / n (m = |sum|),
 // with the point moved `scale` places, so the integer part is q / 10^scale (q = m / n), the fraction digits are the low
 // `scale` digits of q, then the digits of r / n (r = m % n).  `n` < 2^63, so r * 10^9 fits 128 bits.  frac >= scale.
-__device__ __noinline__ void dec_avg_cell(uint8_t* cell, unsigned long long lo, unsigned long long hi, unsigned long long n, int scale, int frac) {
+static __device__ __noinline__ void dec_avg_cell(uint8_t* cell, unsigned long long lo, unsigned long long hi, unsigned long long n, int scale, int frac) {
   const __int128 s = dec_sum_of(lo, hi);
   const bool neg = s < 0;
   const unsigned __int128 m = neg ? (unsigned __int128)(-s) : (unsigned __int128)s;
@@ -166,7 +166,7 @@ __device__ __noinline__ void dec_avg_cell(uint8_t* cell, unsigned long long lo, 
 
 // the one call k_agg_finalize makes for a non-NULL DECIMAL result: AVG, or SUM / MIN / MAX (one call site instead of two
 // keeps the kernel at 64 registers)
-__device__ __noinline__ void dec_result_cell(uint8_t* cell, bool avg, unsigned long long lo, unsigned long long hi, unsigned long long n, int scale, int frac) {
+static __device__ __noinline__ void dec_result_cell(uint8_t* cell, bool avg, unsigned long long lo, unsigned long long hi, unsigned long long n, int scale, int frac) {
   if (avg) dec_avg_cell(cell, lo, hi, n, scale, frac);
   else dec_sum_cell(cell, lo, hi, scale);
 }
@@ -226,7 +226,7 @@ __device__ __forceinline__ void dec3_store(uint8_t* cell, bool neg, unsigned lon
 
 // SUM: the integer part is |sum| / 10^scale; the remainder, left-aligned, gives the ceil(scale / 9) fraction words: the
 // last scale % 9 digits first (padded to a whole word), then whole words towards the point.
-__device__ __noinline__ void dec3_sum_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, int scale) {
+static __device__ __noinline__ void dec3_sum_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, int scale) {
   unsigned long long m[3];
   const bool neg = dec_magnitude(m, lo, mid, top);
   const int aw = scale / 9, nfw = (scale + 8) / 9;   // scale <= 30
@@ -242,7 +242,7 @@ __device__ __noinline__ void dec3_sum_cell(uint8_t* cell, unsigned long long lo,
 // AVG: dec_avg_cell's rule (the truncation at 9 * ceil(frac / 9) digits derived there holds for any scale <= 30: a product
 // has digitsFrac s_a + s_b, so the sum does too).  q = m / n by 192-bit long division (n < 2^63); the integer part is
 // q / 10^scale, the fraction digits are the low `scale` digits of q, then the digits of r / n (r * 10^9 fits 128 bits).
-__device__ __noinline__ void dec3_avg_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, unsigned long long n, int scale, int frac) {
+static __device__ __noinline__ void dec3_avg_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, unsigned long long n, int scale, int frac) {
   unsigned long long q[3];
   const bool neg = dec_magnitude(q, lo, mid, top);
   unsigned long long r = dec_divmod192(q, n);
@@ -282,10 +282,80 @@ __device__ __noinline__ void dec3_avg_cell(uint8_t* cell, unsigned long long lo,
 
 // the one call k_agg_finalize<true, true> makes for a non-NULL product result (the scale, AVG's scale and the AVG flag in
 // one word `how` = scale | frac << 8 | avg << 16: fewer argument registers)
-__device__ __noinline__ void dec3_result_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, unsigned long long n, int how) {
+static __device__ __noinline__ void dec3_result_cell(uint8_t* cell, unsigned long long lo, unsigned long long mid, unsigned long long top, unsigned long long n, int how) {
   const int scale = how & 0xff, frac = (how >> 8) & 0xff;
   if (how >> 16) dec3_avg_cell(cell, lo, mid, top, n, scale, frac);
   else dec3_sum_cell(cell, lo, mid, top, scale);
+}
+
+// ---- ordering cells of any form (TopN: k_topn_rank_dec on the device, the exact comparator on the host) ---------------
+// The order is MyDecimal.Compare (mydecimal.go:1623, through chunk cmpMyDecimal): the sign first, so a negative zero sorts
+// after every negative value and before +0 (and all negative zeros are equal); then doSub's word comparison of the
+// magnitudes: ceil(digitsInt / 9) integer words, then ceil(digitsFrac / 9) fraction words, left-aligned, with leading zero
+// integer words and trailing zero fraction words not counted.  resultFrac and the words after the used ones are not
+// looked at.  c[0] is the header word, c[1..9] the words, as in dec_parse_cell.
+
+__host__ __device__ __forceinline__ int dec_int_words(uint32_t hdr) { return ((int)(int8_t)(hdr & 0xffu) + 8) / 9; }
+__host__ __device__ __forceinline__ int dec_frac_words(uint32_t hdr) { return ((int)(int8_t)((hdr >> 8) & 0xffu) + 8) / 9; }
+__host__ __device__ __forceinline__ bool dec_negative(uint32_t hdr) { return (hdr >> 24) != 0; }
+
+// a cell Compare can read: digitsInt >= 0, digitsFrac >= 0, at most 9 integer and fraction words, each below 10^9
+__host__ __device__ __forceinline__ bool dec_cell_ok(const uint32_t (&c)[10]) {
+  const int di = (int)(int8_t)(c[0] & 0xffu), df = (int)(int8_t)((c[0] >> 8) & 0xffu);
+  if (di < 0 || df < 0) return false;
+  const int n = (di + 8) / 9 + (df + 8) / 9;
+  if (n > 9) return false;
+  bool ok = true;
+#pragma unroll
+  for (int j = 0; j < 9; j++) ok &= j >= n || c[1 + j] < TG_DEC_WORD_BASE;
+  return ok;
+}
+
+// -1 / 0 / 1: MyDecimal.Compare of two well-formed cells.  Integer words are right-aligned and fraction words left-aligned
+// on the point (a missing word is 0), which is doSub's comparison once leading and trailing zero words are dropped.
+__host__ __device__ inline int dec_cell_cmp(const uint32_t* a, const uint32_t* b) {
+  const bool na = dec_negative(a[0]), nb = dec_negative(b[0]);
+  if (na != nb) return na ? -1 : 1;
+  const int ia = dec_int_words(a[0]), ib = dec_int_words(b[0]);
+  const int ea = ia + dec_frac_words(a[0]), eb = ib + dec_frac_words(b[0]);
+  const int top = ia > ib ? ia : ib, fr = (ea - ia > eb - ib) ? ea - ia : eb - ib;
+  int r = 0;
+  for (int k = -top; k < fr && r == 0; k++) {   // k < 0: integer word 10^(9 * (-k - 1)); k >= 0: fraction word k
+    const int ja = ia + k, jb = ib + k;
+    const uint32_t wa = (ja >= 0 && ja < ea) ? a[1 + ja] : 0u, wb = (jb >= 0 && jb < eb) ? b[1 + jb] : 0u;
+    r = wa < wb ? -1 : (wa > wb ? 1 : 0);
+  }
+  return na ? -r : r;
+}
+
+// A monotone 64-bit key of a well-formed cell: a < b implies key(a) <= key(b), equal values give equal keys, and values
+// that differ within their first 16 significant digits give different keys.  Bit 63 is 1 for a cell without the negative
+// flag; below it the magnitude M = 0 for a zero, else (e + 82) << 54 | m, where e in [-81, 80] is the decimal exponent of
+// the leading digit and m in [10^15, 10^16) the first 16 significant digits; a negative cell takes ~M (63 bits).  Every
+// index into c is a constant, so c stays in registers.
+__host__ __device__ __forceinline__ unsigned long long dec_order_key(const uint32_t (&c)[10]) {
+  const int wi = dec_int_words(c[0]), n = wi + dec_frac_words(c[0]);
+  uint32_t w = 0, w1 = 0, w2 = 0;   // the first nonzero word and the two after it
+  int j0 = -1;
+#pragma unroll
+  for (int j = 0; j < 9; j++) {
+    const uint32_t v = j < n ? c[1 + j] : 0u;
+    if (j0 < 0) { if (v) { j0 = j; w = v; } }
+    else if (j == j0 + 1) w1 = v;
+    else if (j == j0 + 2) w2 = v;
+  }
+  unsigned long long mag = 0;
+  if (j0 >= 0) {
+    int d = 1;          // digits of w
+    uint32_t p = 10;    // 10^d
+#pragma unroll
+    for (int k = 1; k < 9; k++) if (w >= p) { d++; p *= 10u; }
+    const int e = 9 * (wi - 1 - j0) + d - 1;
+    // the first 18 significant digits: w (d digits), w1 (9), then the first 9 - d digits of w2; p = 10^d here
+    const unsigned long long z = ((unsigned long long)w * TG_DEC_WORD_BASE + w1) * (TG_DEC_WORD_BASE / p) + w2 / p;
+    mag = ((unsigned long long)(e + 82) << 54) | (z / 100ull);
+  }
+  return dec_negative(c[0]) ? (~mag & 0x7FFFFFFFFFFFFFFFull) : (mag | 0x8000000000000000ull);
 }
 
 }  // namespace tg

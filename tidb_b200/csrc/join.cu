@@ -676,10 +676,8 @@ static int gather_cells(JoinImpl* j, ResultBatch& rb, const DevCols* probe_cells
     const bool from_left = o < j->n_lused;
     const int col = from_left ? j->lused[o] : j->rused[o - j->n_lused];
     const void* src = from_left == probe_is_left ? (probe_cells ? probe_cells->data[col] : nullptr) : j->bcols.data[col]->p;
-    const int grid = dev_rows ? j->nsm * 8 : grid_size(j->nsm, rb.rows * 5, 256, 8);
-    k_gather_cells<<<grid, 256, 0, j->stream>>>(j->out_ids[o]->as<int64_t>(), rb.bitmaps[o]->as<uint8_t>(),
-                                                reinterpret_cast<const unsigned long long*>(src), rb.cols[o]->as<unsigned long long>(),
-                                                rb.rows, dev_rows);
+    launch_gather_cells(j->out_ids[o]->as<int64_t>(), rb.bitmaps[o]->as<uint8_t>(), src, rb.cols[o]->p, rb.rows, dev_rows,
+                        j->nsm, j->stream);
     j->stats.kernel_launches++;
     j->stats.paths |= TG_JOIN_PATH_CELL_GATHER;
   }

@@ -1226,28 +1226,14 @@ k_build_scan_write(int64_t n, const unsigned long long* __restrict__ off, DevCol
 
 // ---------------------------------------------------------------------------------------------
 // DECIMAL payload (late materialisation, join.cu kernel_view / gather_cells): the kernels above move a used DECIMAL column
-// as 8-byte row ids; these two kernels make the ids and turn them back into cells.  A cell is copied as 40 raw bytes, as
-// the reference copies a fixed-length column's bytes into its row table and back (row_table_builder.go fillRowData).
+// as 8-byte row ids; k_iota makes the ids and launch_gather_cells (chunk_io.cuh) turns them back into cells.  A cell is
+// copied as 40 raw bytes, as the reference copies a fixed-length column's bytes into its row table and back
+// (row_table_builder.go fillRowData).
 // ---------------------------------------------------------------------------------------------
 static constexpr int kCellBytes = 40;   // one MyDecimal cell in a chunk column
 
 __global__ void k_iota(int64_t* __restrict__ out, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = i;
-}
-
-// dst row r = src row ids[r] (five lanes per row, one 8-byte word each: coalesced stores), zero bytes where `bitmap` says
-// NULL; the row count is *dev_rows when given (the fused probe paths keep it on the device), else `rows`
-__global__ void __launch_bounds__(256)
-k_gather_cells(const int64_t* __restrict__ ids, const uint8_t* __restrict__ bitmap, const unsigned long long* __restrict__ src,
-               unsigned long long* __restrict__ dst, int64_t rows, const unsigned long long* dev_rows) {
-  constexpr int W = kCellBytes / 8;
-  const int64_t n = (dev_rows ? (int64_t)*dev_rows : rows) * W;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t r = i / W;
-    unsigned long long v = 0;
-    if (!bitmap || bit_not_null(bitmap, r)) v = src[ids[r] * W + (i - r * W)];
-    dst[i] = v;
-  }
 }
 
 }  // namespace tg
