@@ -16,6 +16,9 @@
  *     tg_last_error() returns a thread-local human readable message for the last failure.
  *   - input buffers are BORROWED for the duration of the call only (cgo pointer rule);
  *     output buffers are caller-owned and caller-sized.
+ *   - a tg_join_next / tg_join_next_wait / tg_agg_next / tg_topn call that fails does not write `out` (no cell, no
+ *     bitmap byte) and leaves no copy into it running: *nrows = 0, and the handle's read cursor and d2h_bytes stay
+ *     where they were, so the next valid call returns the rows the failed one would have.
  *   - the library never falls back to a CPU implementation: if no CUDA device is usable every
  *     compute entry point fails with TG_ERR_CUDA.
  *   - calls on one handle are serialised internally; tg_*_close may race with an in-flight
@@ -454,7 +457,9 @@ int tg_agg_push_dev(tg_agg* a, const tg_chunk* dev_chk);
 /* end of input: HashAggFinalWorker merge + result generation (agg_hash_final_worker.go:73,:121) */
 int tg_agg_finish(tg_agg* a);
 /* HashAggExec.Next (agg_hash_executor.go:441). Output schema = one column per agg func in
- * desc order (the reference emits group columns through firstrow() funcs, SURVEY §8 note 4).   */
+ * desc order (the reference emits group columns through firstrow() funcs, SURVEY §8 note 4).
+ * Each output column's elem_len must be its result's width (40 for a DECIMAL result, else 8) and a column that can be
+ * NULL needs a null_bitmap; otherwise TG_ERR_INVALID, with nothing written.                       */
 int tg_agg_next(tg_agg* a, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows);
 int tg_agg_close(tg_agg* a);
 /* device-resident result: number of groups + device pointers of the output columns            */

@@ -1820,9 +1820,8 @@ int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) 
   int64_t lo = a->consumed;
   int64_t want = std::min<int64_t>(std::min<int64_t>(max_rows, out->capacity_rows), a->out_rows - lo);
   if (want <= 0) return TG_OK;
-  for (int k = 0; k < a->spec.n; k++)
-    if (a->out_elem[k] == TG_DEC_CELL_BYTES && out->cols[k].elem_len != TG_DEC_CELL_BYTES)
-      return fail(TG_ERR_INVALID, "a DECIMAL result column needs elem_len 40 (MyDecimal cells)");
+  // every output column is checked before the first copy is enqueued: a rejected call writes nothing
+  TG_TRY(check_out_columns(a->out_bitmaps, a->out_elem, out));
   for (int k = 0; k < a->spec.n; k++) {
     const size_t el = (size_t)a->out_elem[k];
     TG_CUDA(cudaMemcpyAsync(out->cols[k].data, a->out_cols[k]->as<uint8_t>() + (size_t)lo * el, (size_t)want * el, cudaMemcpyDeviceToHost, a->stream));

@@ -83,6 +83,14 @@ int device_view(const tg_chunk* chk, int ncols, const std::vector<char>& needed,
   return TG_OK;
 }
 
+int check_out_columns(const std::vector<std::unique_ptr<DevBuf>>& bitmaps, const std::vector<int>& elem, const tg_mut_chunk* out) {
+  for (int c = 0; c < out->ncols; c++) {
+    if (out->cols[c].elem_len != elem[c]) return fail(TG_ERR_INVALID, "output column elem_len does not match its result column (a DECIMAL result needs elem_len 40, every other one 8)");
+    if (bitmaps[c]->p && !out->cols[c].null_bitmap) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");
+  }
+  return TG_OK;
+}
+
 int download_bitmaps(const std::vector<std::unique_ptr<DevBuf>>& bitmaps, tg_mut_chunk* out, int64_t lo, int64_t want,
                      cudaStream_t s, int64_t* copied) {
   const int shift = (int)(lo & 7);
@@ -92,7 +100,6 @@ int download_bitmaps(const std::vector<std::unique_ptr<DevBuf>>& bitmaps, tg_mut
   for (int c = 0; c < out->ncols; c++) {
     uint8_t* dst = out->cols[c].null_bitmap;
     if (bitmaps[c]->p) {
-      if (!dst) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");
       if (shift == 0) TG_CUDA(cudaMemcpyAsync(dst, bitmaps[c]->as<uint8_t>() + lo / 8, nb, cudaMemcpyDeviceToHost, s));
       else {
         shifted.emplace_back((size_t)((shift + want + 7) / 8) + 1, (uint8_t)0);

@@ -44,10 +44,15 @@ int upload_column(int device, cudaStream_t s, const void* src, const uint8_t* bi
 // borrow a validated device-resident chunk (no sel vector) as a column view of its needed columns; no copy
 int device_view(const tg_chunk* chk, int ncols, const std::vector<char>& needed, const std::vector<int>& elem, DevCols& v);
 
-// The NULL bitmaps of result rows [lo, lo + want) into out's columns.  bitmaps[c] holds column c's bitmap from row 0,
-// or no memory when the column cannot be NULL: out then gets all-valid bits if it passed a bitmap.  Copies on s, then
-// synchronises s, re-aligns bitmaps that start inside a byte and zeroes the bits past `want`.  *copied (when given) =
-// the bitmap bytes the rows cover.
+// TG_OK when every output column of `out` can take its result column: elem_len == elem[c], and a bitmap wherever
+// bitmaps[c] has memory (the column can be NULL).  A *_next call runs it before it enqueues any copy, so a call it
+// rejects writes nothing.
+int check_out_columns(const std::vector<std::unique_ptr<DevBuf>>& bitmaps, const std::vector<int>& elem, const tg_mut_chunk* out);
+
+// The NULL bitmaps of result rows [lo, lo + want) into out's columns, which check_out_columns accepted.  bitmaps[c]
+// holds column c's bitmap from row 0, or no memory when the column cannot be NULL: out then gets all-valid bits if it
+// passed a bitmap.  Copies on s, then synchronises s, re-aligns bitmaps that start inside a byte and zeroes the bits
+// past `want`.  *copied (when given) = the bitmap bytes the rows cover.
 int download_bitmaps(const std::vector<std::unique_ptr<DevBuf>>& bitmaps, tg_mut_chunk* out, int64_t lo, int64_t want,
                      cudaStream_t s, int64_t* copied);
 

@@ -1309,6 +1309,8 @@ static int join_next_impl(tg_join* h, tg_mut_chunk* out, int64_t max_rows, int64
   ResultBatch& rb = *j->results.front();
   int64_t want = std::min<int64_t>(std::min<int64_t>(max_rows, out->capacity_rows), rb.rows - rb.consumed);
   if (want <= 0) return TG_OK;
+  // every output column is checked before the first copy is enqueued: a rejected call writes nothing
+  TG_TRY(check_out_columns(rb.bitmaps, j->out_elem, out));
   // any RequiredRows >= 1 is served (LIMIT 1, MaxOneRow): the result's bit-packed NULL bitmaps are re-aligned on the host
   // when the read cursor is not on a byte boundary (download_bitmaps)
   int64_t lo = rb.consumed;

@@ -290,10 +290,16 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
   });
   const int64_t take = std::min<int64_t>(want - offset, std::min<int64_t>(out->capacity_rows, (int64_t)m - offset));
   if (want - offset > out->capacity_rows) return fail(TG_ERR_CAPACITY, "TopN output chunk is smaller than `count`");
+  // every output column is checked before the first write: a rejected call leaves `out` as it was
   for (int c = 0; c < nc; c++)
     if (kinds[c] == KIND_DECIMAL && out->cols[c].elem_len != TG_DEC_CELL_BYTES) return fail(TG_ERR_INVALID, "a DECIMAL output column must have elem_len 40");
   for (int c = 0; c < nc; c++) {
     if (out->cols[c].elem_len != elem[c]) return fail(TG_ERR_INVALID, "output column elem_len mismatch");
+    if (out->cols[c].null_bitmap) continue;
+    for (int64_t i = 0; i < take; i++)
+      if (!hn[c][(size_t)order[(size_t)(offset + i)]]) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");
+  }
+  for (int c = 0; c < nc; c++) {
     uint8_t* dst = reinterpret_cast<uint8_t*>(out->cols[c].data);
     uint8_t* nb = out->cols[c].null_bitmap;
     if (nb) std::memset(nb, 0, (size_t)((take + 7) / 8));
@@ -303,8 +309,7 @@ int tg_topn(int device, int on_device, const tg_chunk* chk, const int32_t* col_t
       // a NULL row's value is zero bytes (a DECIMAL cell: 40 of them, as the join writes)
       if (valid) std::memcpy(dst + i * elem[c], hv[c].data() + (size_t)r * w[c], (size_t)elem[c]);
       else std::memset(dst + i * elem[c], 0, (size_t)elem[c]);
-      if (nb) { if (valid) nb[i >> 3] |= (uint8_t)(1u << (i & 7)); }
-      else if (!valid) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");
+      if (nb && valid) nb[i >> 3] |= (uint8_t)(1u << (i & 7));
     }
   }
   *nrows = take;
