@@ -527,6 +527,51 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk,
                   const tg_filter_item* items, int32_t n_items,
                   uint8_t* selected, int64_t* n_selected, void* stream);
 
+/* DECIMAL comparisons over 40-byte MyDecimal cells (the layout of tg_agg_func.ret_type), for Selection and Projection.
+ *   Order: cells compare exactly as tg_topn orders DECIMAL cells, which is MyDecimal.Compare (types/mydecimal.go:1623):
+ *     the sign first, so a cell with `negative` set and a zero value is below +0 and above every negative value; then the
+ *     word magnitudes, integer words right-aligned and fraction words left-aligned on the point, leading and trailing
+ *     zero words not counted, so 1.50 == 1.5 whatever the digitsInt.  resultFrac and the unused words are ignored.
+ *   Any well-formed cell of any precision is accepted: no flen or scale is needed, so HAVING runs over SUM results wider
+ *     than 18 digits.  A non-NULL cell is malformed when digitsInt or digitsFrac is negative, it has more than 9 integer
+ *     and fraction words, or one of those words is >= 10^9 (tg_topn's definition).  Every non-NULL cell of a DECIMAL
+ *     operand column is checked at every row the call evaluates (the rows in `sel` when the chunk has one, else every
+ *     physical row), whatever the other items and the other operand give; one malformed cell fails the call with
+ *     TG_ERR_INVALID.  Cells under NULL and outside `sel` are never read as values.  A malformed constant cell, a missing
+ *     one, or an operand column whose elem_len is not 40 is TG_ERR_INVALID.
+ *   A failed call with host buffers (on_device == 0) writes nothing: no result value, no bitmap byte, no `selected` byte
+ *     and no *n_selected.  With device buffers, `result` / `result_nulls` / `selected` may have been written; *n_selected
+ *     is not.
+ *   These argument checks (descriptor, types, elem_len, alignment, constant cells) answer before the device is looked
+ *     for.  Device-resident DECIMAL columns must be 8-byte aligned. */
+/* tg_filter_item.is_real values understood by tg_vec_filter_ex */
+enum { TG_FILTER_INT = 0, TG_FILTER_REAL = 1, TG_FILTER_DECIMAL = 2 };
+
+/* builtin{LT,LE,GT,GE,EQ,NE}DecimalSig.vecEvalInt (expression/builtin_compare_vec_generated.go:64, :960, :1184):
+ * result int64 0/1, NULL if either side is NULL (MergeNulls).  b == NULL -> compare with the 40-byte constant cell
+ * b_const_cell (host memory).  A NULL row has its result bit cleared and the value 0. */
+int tg_vec_compare_decimal(int device, int on_device, int op, const tg_column* a, const tg_column* b,
+                           const uint8_t* b_const_cell, int64_t* result, uint8_t* result_nulls, void* stream);
+
+/* tg_vec_filter plus DECIMAL items: col_types[c] is the MySQL type of chunk column c; an item with
+ * is_real == TG_FILTER_DECIMAL compares 40-byte MyDecimal cells, against column rhs_col or, when rhs_col < 0, against
+ * the constant cell at dec_consts + 40 * i (host memory; may be NULL when no DECIMAL item has a constant).
+ *   A DECIMAL item needs col_types TG_TYPE_NEWDECIMAL and elem_len 40 on both operands.  A DECIMAL column in an INT or
+ *   REAL item, or a column of another type in a DECIMAL item, is TG_ERR_UNSUPPORTED: the planner casts before it
+ *   compares a DECIMAL with an integer or real operand.  INT and REAL items (is_real 0 / 1) keep exactly their
+ *   tg_vec_filter meaning, so items of all kinds mix in one CNF of at most TG_MAX_FILTER (8) items over at most 16
+ *   columns.  Any other is_real value, an op outside TG_CMP_*, or operand columns of different lengths is
+ *   TG_ERR_INVALID.  With no DECIMAL item the call is tg_vec_filter: the same `selected` and count. */
+int tg_vec_filter_ex(int device, int on_device, const tg_chunk* chk, const int32_t* col_types,
+                     const tg_filter_item* items, int32_t n_items, const uint8_t* dec_consts,
+                     uint8_t* selected, int64_t* n_selected, void* stream);
+
+/* The form the two calls above compare a constant cell in (host code, no device): `out` gets the cell's sign and value
+ * without leading zero integer words and trailing zero fraction words, digitsInt / digitsFrac = 9 * the words kept,
+ * resultFrac and the unused words 0.  It compares with every cell as `cell` does.  A malformed cell is TG_ERR_INVALID
+ * with `out` not written. */
+int tg_decimal_normalize(const uint8_t* cell, uint8_t* out);
+
 /* ---------------------------------------------------------------------------------------------
  * TopN                         replaces sortexec.TopNExec (pkg/executor/sortexec/topn.go:74, :230)
  * ORDER BY items over plain columns, LIMIT offset, count.  Rows [offset, offset + count) of the child's rows in item

@@ -27,6 +27,7 @@ AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_FIRSTROW = 0, 1, 2, 3, 4, 5
 AGGMODE_COMPLETE, AGGMODE_FINAL, AGGMODE_PARTIAL1, AGGMODE_PARTIAL2, AGGMODE_DEDUP = 0, 1, 2, 3, 4
 CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_EQ, CMP_NE = 0, 1, 2, 3, 4, 5
 ARITH_PLUS, ARITH_MINUS, ARITH_MUL = 0, 1, 2
+FILTER_INT, FILTER_REAL, FILTER_DECIMAL = 0, 1, 2    # tg_filter_item.is_real as tg_vec_filter_ex reads it
 
 
 class TgColumn(C.Structure):
@@ -157,7 +158,7 @@ EXPORTED_SYMBOLS = [
     "tg_agg_supported", "tg_agg_supported_ex", "tg_agg_supported_ex2", "tg_agg_open", "tg_agg_open_ex", "tg_agg_open_ex2", "tg_agg_push",
     "tg_agg_push_dev", "tg_agg_finish", "tg_agg_next", "tg_agg_close", "tg_agg_result_dev", "tg_agg_get_stats", "tg_agg_get_distinct_stats",
     "tg_vec_compare_int", "tg_vec_compare_real", "tg_vec_arith_int", "tg_vec_arith_real",
-    "tg_vec_filter", "tg_topn",
+    "tg_vec_filter", "tg_vec_compare_decimal", "tg_vec_filter_ex", "tg_decimal_normalize", "tg_topn",
     "tg_partition_by_key", "tg_partition_of_key", "tg_partition_exchange", "tg_partition_exchange_cf", "tg_partition_exchange_cf_ex", "tg_partition_exchange_cf_spill", "tg_partition_count",
     "tg_mail_signal", "tg_mail_wait", "tg_peer_copy_regions",
     "tg_ipc_export", "tg_ipc_open", "tg_ipc_close",

@@ -1,5 +1,6 @@
 // decimal.cuh — the MyDecimal cell of an exact DECIMAL aggregate result and of a DECIMAL argument column (included by agg.cu:
-// k_agg_finalize writes cells, k_dec_to_scaled parses them), and the order of cells (included by topn.cu).
+// k_agg_finalize writes cells, k_dec_to_scaled parses them), and the order of cells (included by topn.cu, and by vec.cu
+// for the DECIMAL compares and filters).
 //
 // A cell is the 40-byte types.MyDecimal (types/mydecimal.go:236-248) that chunk.Column copies whole (util/chunk/column.go:41):
 //   byte 0 digitsInt (int8), byte 1 digitsFrac (int8), byte 2 resultFrac (int8), byte 3 negative (bool),
@@ -311,21 +312,60 @@ __host__ __device__ __forceinline__ bool dec_cell_ok(const uint32_t (&c)[10]) {
   return ok;
 }
 
-// -1 / 0 / 1: MyDecimal.Compare of two well-formed cells.  Integer words are right-aligned and fraction words left-aligned
-// on the point (a missing word is 0), which is doSub's comparison once leading and trailing zero words are dropped.
-__host__ __device__ inline int dec_cell_cmp(const uint32_t* a, const uint32_t* b) {
-  const bool na = dec_negative(a[0]), nb = dec_negative(b[0]);
+// Word j (0..8) of a cell, for dec_cmp_words: DecWordsPtr reads a cell in memory (the host comparator, a constant in
+// kernel parameter space); DecWordsReg reads a cell held in registers, selecting among its nine words so that every
+// index into c is a constant (a dynamic index would move the cell to local memory).
+struct DecWordsPtr {
+  const uint32_t* c;
+  __host__ __device__ __forceinline__ uint32_t operator()(int j) const { return c[1 + j]; }
+};
+struct DecWordsReg {
+  const uint32_t (&c)[10];
+  __device__ __forceinline__ uint32_t operator()(int j) const {
+    uint32_t w = 0;
+#pragma unroll
+    for (int t = 0; t < 9; t++) w = t == j ? c[1 + t] : w;
+    return w;
+  }
+};
+
+// -1 / 0 / 1: MyDecimal.Compare of two well-formed cells (header words ha / hb, words read through wa / wb).  Integer
+// words are right-aligned and fraction words left-aligned on the point (a missing word is 0), which is doSub's comparison
+// once leading and trailing zero words are dropped.  On a malformed cell it returns some value and reads no memory
+// outside the cell's nine words through DecWordsReg.
+template <typename WA, typename WB>
+__host__ __device__ __forceinline__ int dec_cmp_words(uint32_t ha, const WA& wa_at, uint32_t hb, const WB& wb_at) {
+  const bool na = dec_negative(ha), nb = dec_negative(hb);
   if (na != nb) return na ? -1 : 1;
-  const int ia = dec_int_words(a[0]), ib = dec_int_words(b[0]);
-  const int ea = ia + dec_frac_words(a[0]), eb = ib + dec_frac_words(b[0]);
+  const int ia = dec_int_words(ha), ib = dec_int_words(hb);
+  const int ea = ia + dec_frac_words(ha), eb = ib + dec_frac_words(hb);
   const int top = ia > ib ? ia : ib, fr = (ea - ia > eb - ib) ? ea - ia : eb - ib;
   int r = 0;
   for (int k = -top; k < fr && r == 0; k++) {   // k < 0: integer word 10^(9 * (-k - 1)); k >= 0: fraction word k
     const int ja = ia + k, jb = ib + k;
-    const uint32_t wa = (ja >= 0 && ja < ea) ? a[1 + ja] : 0u, wb = (jb >= 0 && jb < eb) ? b[1 + jb] : 0u;
+    const uint32_t wa = (ja >= 0 && ja < ea) ? wa_at(ja) : 0u, wb = (jb >= 0 && jb < eb) ? wb_at(jb) : 0u;
     r = wa < wb ? -1 : (wa > wb ? 1 : 0);
   }
   return na ? -r : r;
+}
+
+__host__ __device__ inline int dec_cell_cmp(const uint32_t* a, const uint32_t* b) {
+  return dec_cmp_words(a[0], DecWordsPtr{a}, b[0], DecWordsPtr{b});
+}
+
+// The comparison form of a well-formed cell (host; the constant of a DECIMAL compare or filter item): the same sign (a
+// negative zero stays negative) and value, without its leading zero integer words and trailing zero fraction words, so
+// digitsInt / digitsFrac = 9 * the integer / fraction words kept; resultFrac and the unused words are 0.  dec_cell_cmp
+// orders it against every cell as it orders the input cell, and a row's comparison with it walks no word pair that
+// only the constant's zero words would add.
+inline void dec_normalize(const uint32_t (&c)[10], uint32_t (&o)[10]) {
+  const int wi = dec_int_words(c[0]), n = wi + dec_frac_words(c[0]);
+  int lo = 0, hi = n;
+  while (lo < wi && c[1 + lo] == 0) lo++;
+  while (hi > wi && c[hi] == 0) hi--;   // c[hi] is word hi - 1
+  for (int j = 0; j < 10; j++) o[j] = 0;
+  o[0] = (uint32_t)(9 * (wi - lo)) | ((uint32_t)(9 * (hi - wi)) << 8) | (dec_negative(c[0]) ? 1u << 24 : 0u);
+  for (int j = lo; j < hi; j++) o[1 + j - lo] = c[1 + j];
 }
 
 // A monotone 64-bit key of a well-formed cell: a < b implies key(a) <= key(b), equal values give equal keys, and values

@@ -6,9 +6,12 @@
 // (builtin_arithmetic_vec.go:856, :365, :646, :1011, :496, :300, :40) and
 // expression.VectorizedFilter (chunk_executor.go:413).  All are streaming kernels bounded by HBM:
 // 8 B (+8 B) read and 8 B written per row, null bitmaps merged bytewise (Column.MergeNulls column.go:906).
+// The DECIMAL compare and filter (tg_vec_compare_decimal, tg_vec_filter_ex) read 40-byte MyDecimal cells and compare
+// them as MyDecimal.Compare (builtin{LT,LE,GT,GE,EQ,NE}DecimalSig, builtin_compare_vec_generated.go:64, :960, :1184).
 #include <memory>
 #include "common.cuh"
 #include "chunk_io.cuh"
+#include "decimal.cuh"
 
 namespace tg {
 
@@ -187,15 +190,122 @@ k_vec_filter(DevCols cols, DevFilter f, const long long* __restrict__ sel, int64
   if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
 }
 
-// a column argument made device-resident (copies host buffers when on_device == 0)
+// ---- DECIMAL compares and filters: 40-byte MyDecimal cells (decimal.cuh) -------------------------------------------
+// The cell of row i in registers: five 8-byte loads.  Lane l's cell starts 40 * l bytes into its warp's 1280 contiguous
+// bytes, so the warp's five loads cover those bytes and L1 serves the sectors each load leaves to the next (TopN's
+// k_topn_rank_dec reads its cells the same way; see DESIGN.md §6b for the measurement).
+__device__ __forceinline__ void dec_load(const void* data, int64_t i, uint32_t (&c)[10]) {
+  const unsigned long long* p = reinterpret_cast<const unsigned long long*>(data) + i * 5;
+#pragma unroll
+  for (int j = 0; j < 5; j++) {
+    const unsigned long long v = p[j];
+    c[2 * j] = (uint32_t)v; c[2 * j + 1] = (uint32_t)(v >> 32);
+  }
+}
+
+// a constant cell in its comparison form (dec_normalize), passed by value
+struct DecConst { uint32_t c[10]; };
+
+// the DECIMAL items of a tg_vec_filter_ex CNF: `op` lhs_col (rhs_col, or the constant k when rhs_col < 0)
+struct DecItem { int32_t op, lhs_col, rhs_col, pad; uint32_t k[10]; };
+struct DecFilter { int32_t n, pad; DecItem items[TG_MAX_FILTER]; };
+
+// tg_vec_compare_decimal: k_vec_compare's warp-row layout over cells.  A NULL row's value is 0 and its cells are not
+// compared; a malformed non-NULL cell of either operand sets *bad (decimal.cuh dec_cell_ok) whatever the other side holds.
+__global__ void __launch_bounds__(256)
+k_vec_compare_dec(int op, VArg a, VArg b, const __grid_constant__ DecConst k, int64_t n, long long* __restrict__ result,
+                  uint8_t* __restrict__ rnulls, unsigned int* __restrict__ bad) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int64_t tile = 32 * VEC_ITEMS;
+  bool malformed = false;
+  for (int64_t base = warp * tile; base < n; base += nwarps * tile) {
+    uint32_t x[VEC_ITEMS][10], y[VEC_ITEMS][10];
+#pragma unroll
+    for (int j = 0; j < VEC_ITEMS; j++) {
+      const int64_t i = base + j * 32 + lane;
+      if (i < n) {
+        dec_load(a.data, i, x[j]);
+        if (b.data) dec_load(b.data, i, y[j]);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < VEC_ITEMS; j++) {
+      const int64_t i = base + j * 32 + lane;
+      const bool in = i < n;
+      const bool va = in && arg_valid(a, i), vb = in && arg_valid(b, i);
+      malformed |= va && !dec_cell_ok(x[j]);
+      bool r = false;
+      if (b.data) {
+        malformed |= vb && !dec_cell_ok(y[j]);
+        if (va && vb) r = apply_cmp(op, dec_cmp_words(x[j][0], DecWordsReg{x[j]}, y[j][0], DecWordsReg{y[j]}));
+      } else if (va) {
+        r = apply_cmp(op, dec_cmp_words(x[j][0], DecWordsReg{x[j]}, k.c[0], DecWordsPtr{k.c}));
+      }
+      if (in) __stcs(result + i, r ? 1ll : 0ll);
+      const unsigned bal = __ballot_sync(0xffffffffu, va && vb);
+      store_valid_word(rnulls, base + j * 32, n, bal, lane);
+    }
+  }
+  if (malformed) *bad = 1u;
+}
+
+// tg_vec_filter_ex with DECIMAL items: k_vec_filter's row loop; the DECIMAL items are evaluated first and all of them,
+// so every non-NULL cell of their operands is checked at every row evaluated (*bad), then the INT / REAL items by
+// eval_filter, unchanged.
+__global__ void __launch_bounds__(256)
+k_vec_filter_dec(DevCols cols, DevFilter f, const __grid_constant__ DecFilter d, const long long* __restrict__ sel,
+                 int64_t nsel, int64_t nphys, uint8_t* __restrict__ selected, unsigned long long* count,
+                 unsigned int* __restrict__ bad) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  unsigned long long local = 0;
+  bool malformed = false;
+  const int64_t n = sel ? nsel : nphys;
+  for (; i < n; i += stride) {
+    const int64_t p = sel ? sel[i] : i;
+    bool s = true;
+    for (int q = 0; q < d.n; q++) {
+      const DecItem& it = d.items[q];
+      uint32_t x[10];
+      dec_load(cols.data[it.lhs_col], p, x);
+      const uint8_t* ln = cols.nulls[it.lhs_col];
+      const bool vx = !ln || bit_not_null(ln, p);
+      malformed |= vx && !dec_cell_ok(x);
+      int c;
+      bool vy = true;
+      if (it.rhs_col >= 0) {
+        uint32_t y[10];
+        dec_load(cols.data[it.rhs_col], p, y);
+        const uint8_t* rn = cols.nulls[it.rhs_col];
+        vy = !rn || bit_not_null(rn, p);
+        malformed |= vy && !dec_cell_ok(y);
+        c = dec_cmp_words(x[0], DecWordsReg{x}, y[0], DecWordsReg{y});
+      } else {
+        c = dec_cmp_words(x[0], DecWordsReg{x}, it.k[0], DecWordsPtr{it.k});
+      }
+      s &= vx && vy && apply_cmp(it.op, c);
+    }
+    s = s && eval_filter(f, cols, p);
+    selected[p] = s ? 1 : 0;
+    local += s;
+  }
+  for (int o = 16; o; o >>= 1) local += __shfl_xor_sync(0xffffffffu, local, o);
+  if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
+  if (malformed) *bad = 1u;
+}
+
+// a column argument made device-resident (copies host buffers when on_device == 0); `elem` is the width the kernel
+// reads: 8, or 40 for DECIMAL cells
 struct ArgDev {
   DevBuf data, nulls;
   VArg v{nullptr, nullptr};
-  int load(int device, int on_device, const tg_column* c, cudaStream_t st) {
+  int load(int device, int on_device, const tg_column* c, cudaStream_t st, int elem = 8) {
     if (!c) return TG_OK;
-    if (c->elem_len != 8) return fail(TG_ERR_UNSUPPORTED, "VecEval kernels take 8-byte columns");
+    if (c->elem_len != elem) return fail(TG_ERR_UNSUPPORTED, elem == 8 ? "VecEval kernels take 8-byte columns" : "DECIMAL operands are 40-byte cells");
     if (on_device) { v.data = c->data; v.nulls = c->null_bitmap; return TG_OK; }
-    TG_TRY(upload_column(device, st, c->data, c->null_bitmap, c->length, 8, data, nulls, nullptr));
+    TG_TRY(upload_column(device, st, c->data, c->null_bitmap, c->length, elem, data, nulls, nullptr));
     v.data = data.p;
     if (c->null_bitmap) v.nulls = nulls.as<uint8_t>();
     return TG_OK;
@@ -238,6 +348,27 @@ static int run_binary(int device, int on_device, const tg_column* a, const tg_co
   TG_CUDA(cudaStreamSynchronize(st));
   TG_CUDA(cudaGetLastError());
   if (ovf) return fail(TG_ERR_OVERFLOW, "ErrOverflow: value is out of range in arithmetic VecEval kernel");
+  return TG_OK;
+}
+
+static const char* kMalformedCell =
+    "malformed DECIMAL cell (digitsInt / digitsFrac < 0, more than 9 words, or a word >= 10^9)";
+
+// the checks of a DECIMAL operand column that need no device
+static int check_dec_column(const tg_column& c, int on_device) {
+  if (c.elem_len != TG_DEC_CELL_BYTES) return fail(TG_ERR_INVALID, "a DECIMAL operand column must have elem_len 40 (MyDecimal cells)");
+  if (c.length < 0 || (c.length > 0 && !c.data)) return fail(TG_ERR_INVALID, "DECIMAL operand column without data");
+  if (on_device && (reinterpret_cast<uintptr_t>(c.data) & 7)) return fail(TG_ERR_INVALID, "DECIMAL device columns must be 8-byte aligned");
+  return TG_OK;
+}
+
+// a constant cell (host memory) -> its comparison form; a missing or malformed cell is TG_ERR_INVALID
+static int load_dec_const(const uint8_t* cell, uint32_t (&k)[10]) {
+  if (!cell) return fail(TG_ERR_INVALID, "DECIMAL comparison with a constant, but the constant cell is NULL");
+  uint32_t c[10];
+  std::memcpy(c, cell, TG_DEC_CELL_BYTES);
+  if (!dec_cell_ok(c)) return fail(TG_ERR_INVALID, std::string(kMalformedCell) + " as the constant");
+  dec_normalize(c, k);
   return TG_OK;
 }
 
@@ -330,6 +461,144 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk, const tg_filte
   TG_CUDA(cudaStreamSynchronize(st));
   TG_CUDA(cudaGetLastError());
   if (n_selected) *n_selected = (int64_t)cnt;
+  return TG_OK;
+}
+
+int tg_decimal_normalize(const uint8_t* cell, uint8_t* out) {
+  if (!out) return fail(TG_ERR_INVALID, "out is NULL");
+  uint32_t k[10];
+  TG_TRY(load_dec_const(cell, k));
+  std::memcpy(out, k, TG_DEC_CELL_BYTES);
+  return TG_OK;
+}
+
+int tg_vec_compare_decimal(int device, int on_device, int op, const tg_column* a, const tg_column* b,
+                           const uint8_t* b_const_cell, int64_t* result, uint8_t* result_nulls, void* stream) {
+  if (!a || !result || !result_nulls) return fail(TG_ERR_INVALID, "a / result / result_nulls is NULL");
+  if (op < TG_CMP_LT || op > TG_CMP_NE) return fail(TG_ERR_INVALID, "unknown comparison");
+  if (b && b->length != a->length) return fail(TG_ERR_INVALID, "argument columns have different lengths");
+  TG_TRY(check_dec_column(*a, on_device));
+  if (b) TG_TRY(check_dec_column(*b, on_device));
+  DecConst k{};
+  if (!b) TG_TRY(load_dec_const(b_const_cell, k.c));
+  TG_TRY(require_device("VecEval"));
+  DeviceGuard g(device);
+  if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t n = a->length;
+  ArgDev da, db;
+  TG_TRY(da.load(device, on_device, a, st, TG_DEC_CELL_BYTES));
+  TG_TRY(db.load(device, on_device, b, st, TG_DEC_CELL_BYTES));
+  DevBuf dres, dnul, dbad;
+  long long* res_dev = reinterpret_cast<long long*>(result);
+  uint8_t* nul_dev = result_nulls;
+  const size_t nb = (size_t)((n + 7) / 8);
+  if (!on_device) {
+    TG_TRY(dres.ensure(device, (size_t)n * 8 + 16)); TG_TRY(dnul.ensure(device, nb + 16));
+    res_dev = dres.as<long long>(); nul_dev = dnul.as<uint8_t>();
+  }
+  TG_TRY(dbad.ensure(device, 16));
+  TG_CUDA(cudaMemsetAsync(dbad.p, 0, 4, st));
+  if (n > 0)
+    k_vec_compare_dec<<<grid_size(device_sm_count(device), (n + VEC_ITEMS - 1) / VEC_ITEMS, 256, 8), 256, 0, st>>>(
+        op, da.v, db.v, k, n, res_dev, nul_dev, dbad.as<unsigned int>());
+  unsigned int bad = 0;
+  TG_CUDA(cudaMemcpyAsync(&bad, dbad.p, 4, cudaMemcpyDeviceToHost, st));
+  TG_CUDA(cudaStreamSynchronize(st));
+  TG_CUDA(cudaGetLastError());
+  if (bad) return fail(TG_ERR_INVALID, kMalformedCell);
+  // host buffers are written only once the cells are known to be well-formed
+  if (!on_device && n > 0) {
+    TG_CUDA(cudaMemcpyAsync(result, res_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaMemcpyAsync(result_nulls, nul_dev, nb, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaStreamSynchronize(st));
+  }
+  return TG_OK;
+}
+
+int tg_vec_filter_ex(int device, int on_device, const tg_chunk* chk, const int32_t* col_types,
+                     const tg_filter_item* items, int32_t n_items, const uint8_t* dec_consts,
+                     uint8_t* selected, int64_t* n_selected, void* stream) {
+  if (!chk || !selected || !col_types) return fail(TG_ERR_INVALID, "chunk / col_types / selected is NULL");
+  if (n_items < 0 || n_items > TG_MAX_FILTER) return fail(TG_ERR_UNSUPPORTED, "at most 8 CNF filter items are offloaded");
+  if (n_items > 0 && !items) return fail(TG_ERR_INVALID, "items is NULL");
+  if (chk->ncols <= 0 || chk->ncols > TG_MAX_COLS || !chk->cols) return fail(TG_ERR_UNSUPPORTED, "chunk must have 1..16 columns");
+  const int64_t nphys = chk->cols[0].length;
+  DecFilter d{};
+  DevFilter f{};
+  std::vector<char> needed(chk->ncols, 0);
+  for (int i = 0; i < n_items; i++) {
+    const tg_filter_item& it = items[i];
+    if (it.lhs_col < 0 || it.lhs_col >= chk->ncols || it.rhs_col >= chk->ncols) return fail(TG_ERR_INVALID, "filter column out of range");
+    if (it.op < TG_CMP_LT || it.op > TG_CMP_NE) return fail(TG_ERR_INVALID, "unknown comparison");
+    if (it.is_real < TG_FILTER_INT || it.is_real > TG_FILTER_DECIMAL) return fail(TG_ERR_INVALID, "unknown filter item kind (is_real)");
+    const bool dec = it.is_real == TG_FILTER_DECIMAL;
+    for (int side = 0; side < 2; side++) {
+      const int c = side ? it.rhs_col : it.lhs_col;
+      if (c < 0) continue;
+      const tg_column& col = chk->cols[c];
+      const bool dec_col = col_types[c] == TG_TYPE_NEWDECIMAL;
+      if (dec && !dec_col) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL filter item compares DECIMAL columns only (the planner casts the other operand)");
+      if (!dec && dec_col) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL column in an INT / REAL filter item");
+      if (dec) TG_TRY(check_dec_column(col, on_device));
+      else if (col.elem_len != 8) return fail(TG_ERR_UNSUPPORTED, "VecEval kernels take 8-byte columns");
+      if (col.length != nphys) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
+      needed[c] = 1;
+    }
+    if (dec) {
+      DecItem& di = d.items[d.n++];
+      di.op = it.op; di.lhs_col = it.lhs_col; di.rhs_col = it.rhs_col;
+      if (it.rhs_col < 0) TG_TRY(load_dec_const(dec_consts ? dec_consts + (size_t)TG_DEC_CELL_BYTES * i : nullptr, di.k));
+    } else {
+      f.items[f.n++] = it;
+    }
+  }
+  if (d.n == 0) return tg_vec_filter(device, on_device, chk, items, n_items, selected, n_selected, stream);
+  TG_TRY(require_device("VecEval"));
+  DeviceGuard g(device);
+  if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<std::unique_ptr<ArgDev>> args;
+  DevCols cols{};
+  for (int c = 0; c < chk->ncols; c++) {
+    args.emplace_back(new ArgDev());
+    cols.elem_len[c] = chk->cols[c].elem_len;
+    if (!needed[c]) continue;
+    TG_TRY(args[c]->load(device, on_device, &chk->cols[c], st, chk->cols[c].elem_len));
+    cols.data[c] = args[c]->v.data; cols.nulls[c] = args[c]->v.nulls;
+  }
+  DevBuf dsel_idx, dselected, dflags;
+  const long long* sel_dev = reinterpret_cast<const long long*>(chk->sel);
+  uint8_t* selected_dev = selected;
+  if (!on_device) {
+    if (chk->sel) {
+      TG_TRY(dsel_idx.ensure(device, (size_t)chk->nsel * 8 + 16));
+      TG_CUDA(cudaMemcpyAsync(dsel_idx.p, chk->sel, (size_t)chk->nsel * 8, cudaMemcpyHostToDevice, st));
+      sel_dev = dsel_idx.as<long long>();
+    }
+    TG_TRY(dselected.ensure(device, (size_t)nphys + 16));
+    selected_dev = dselected.as<uint8_t>();
+  }
+  TG_TRY(dflags.ensure(device, 16));   // the count (8 bytes), then the malformed flag (4 bytes)
+  TG_CUDA(cudaMemsetAsync(dflags.p, 0, 16, st));
+  TG_CUDA(cudaMemsetAsync(selected_dev, 0, (size_t)nphys, st));
+  const int64_t n = chk->sel ? chk->nsel : nphys;
+  unsigned long long* dcount = dflags.as<unsigned long long>();
+  unsigned int* dbad = reinterpret_cast<unsigned int*>(dcount + 1);
+  if (n > 0)
+    k_vec_filter_dec<<<grid_size(device_sm_count(device), n, 256, 8), 256, 0, st>>>(cols, f, d, sel_dev, chk->nsel, nphys,
+                                                                                     selected_dev, dcount, dbad);
+  unsigned long long flags[2] = {0, 0};
+  TG_CUDA(cudaMemcpyAsync(flags, dflags.p, 16, cudaMemcpyDeviceToHost, st));
+  TG_CUDA(cudaStreamSynchronize(st));
+  TG_CUDA(cudaGetLastError());
+  if ((unsigned int)flags[1]) return fail(TG_ERR_INVALID, kMalformedCell);
+  // host buffers are written only once the cells are known to be well-formed
+  if (!on_device && nphys) {
+    TG_CUDA(cudaMemcpyAsync(selected, selected_dev, (size_t)nphys, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaStreamSynchronize(st));
+  }
+  if (n_selected) *n_selected = (int64_t)flags[0];
   return TG_OK;
 }
 

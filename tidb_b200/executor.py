@@ -261,8 +261,9 @@ def _concat_chunks(chunks: Sequence[Chunk]) -> Chunk:
 class SelectionExec(Executor):
     """GPU replacement of executor.SelectionExec (pkg/executor/select.go:746-785): pulls child chunks, evaluates the
     CNF filter list with expression.VectorizedFilter semantics (chunk_executor.go:413: a row is selected iff every item is
-    non-NULL true) on the device (tg_vec_filter) and hands the selected rows on, at most `required_rows` per Next.
-    Child chunks are batched (`batch_rows`) so that one launch filters many 1024-row chunks."""
+    non-NULL true) on the device (tg_vec_filter; tg_vec_filter_ex when an item compares DECIMAL cells) and hands the
+    selected rows on, at most `required_rows` per Next.  Child chunks are batched (`batch_rows`) so that one launch filters
+    many 1024-row chunks."""
 
     def __init__(self, child: Executor, filters: Sequence, device: int = 0, batch_rows: int = 64 * MAX_CHUNK_SIZE):
         super().__init__(child.schema, [child])
@@ -280,7 +281,7 @@ class SelectionExec(Executor):
         self._pending, self._eof = [], False
 
     def _fill(self) -> None:
-        from .plan import filter_array
+        from .plan import dec_const_array, filter_array
         batch, rows = [], 0
         while rows < self.batch_rows:
             chk = self.children[0].next(MAX_CHUNK_SIZE)
@@ -296,7 +297,14 @@ class SelectionExec(Executor):
         nsel = C.c_int64(0)
         cs = dense.to_struct()
         arr = filter_array(self.filters)
-        abi.check(self._lib.tg_vec_filter(self.device, 0, C.byref(cs), arr, len(self.filters), selected.ctypes.data_as(C.c_void_p), C.byref(nsel), None))
+        if any(f.is_decimal for f in self.filters):
+            # DECIMAL items compare MyDecimal cells: tg_vec_filter_ex, told the child schema's types
+            tps = (C.c_int32 * len(self.schema))(*[t.tp for t in self.schema])
+            consts = dec_const_array(self.filters)
+            abi.check(self._lib.tg_vec_filter_ex(self.device, 0, C.byref(cs), tps, arr, len(self.filters), consts,
+                                                 selected.ctypes.data_as(C.c_void_p), C.byref(nsel), None))
+        else:
+            abi.check(self._lib.tg_vec_filter(self.device, 0, C.byref(cs), arr, len(self.filters), selected.ctypes.data_as(C.c_void_p), C.byref(nsel), None))
         self.launches += 1
         keep = selected.astype(bool)
         assert int(keep.sum()) == nsel.value
@@ -320,7 +328,8 @@ class SelectionExec(Executor):
 class ProjectionExec(Executor):
     """GPU replacement of executor.ProjectionExec (pkg/executor/projection.go:450-483 -> EvaluatorSuite.Run,
     expression/evaluator.go:128): plain column references are passed through (the reference SWAPS them, ColumnSwapHelper),
-    scalar functions are evaluated column-at-a-time by the VecEval kernels (tg_vec_arith_* / tg_vec_compare_*), constants
+    scalar functions are evaluated column-at-a-time by the VecEval kernels (tg_vec_arith_* / tg_vec_compare_*, DECIMAL
+    comparisons by tg_vec_compare_decimal), constants
     are scalars (the reference materialises them as columns, vectorized.go:23).  Errors keep the reference's meaning:
     overflow on a non-NULL row fails the Next call (types.ErrOverflow <-> TG_ERR_OVERFLOW)."""
 
@@ -361,7 +370,16 @@ class ProjectionExec(Executor):
         pb = C.byref(sb) if sb is not None else None
         rp, np_ = res.ctypes.data_as(C.c_void_p), nulls.ctypes.data_as(C.c_void_p)
         k = b.value if isinstance(b, Const) else 0
-        if e.kind == "arith" and real:
+        if e.is_decimal:
+            if e.kind != "cmp":
+                raise abi.TgError(abi.TG_ERR_UNSUPPORTED, "DECIMAL arithmetic is not offloaded to the VecEval kernels")
+            cell = None
+            if isinstance(b, Const):
+                if b.cell is None:
+                    raise abi.TgError(abi.TG_ERR_UNSUPPORTED, "a DECIMAL comparison takes a DECIMAL constant (the planner casts it)")
+                cell = (C.c_uint8 * 40).from_buffer_copy(bytes(b.cell))
+            rc = self._lib.tg_vec_compare_decimal(self.device, 0, e.op, C.byref(sa), pb, cell, rp, np_, None)
+        elif e.kind == "arith" and real:
             rc = self._lib.tg_vec_arith_real(self.device, 0, e.op, C.byref(sa), pb, C.c_double(float(k)), rp, np_, None)
         elif e.kind == "arith":
             rc = self._lib.tg_vec_arith_int(self.device, 0, e.op, int(e.a_unsigned), int(e.b_unsigned), C.byref(sa), pb, C.c_int64(int(k)), rp, np_, None)

@@ -46,7 +46,8 @@ def _u32(vals: Sequence[int]):
 
 @dataclass
 class FilterItem:
-    """One CNF item `col OP const` / `col OP col` (tg_filter_item)."""
+    """One CNF item `col OP const` / `col OP col` (tg_filter_item).  is_decimal: a DECIMAL item of tg_vec_filter_ex over
+    40-byte MyDecimal cell columns, whose constant is the 40-byte cell const_cell (Constant.Value.GetMysqlDecimal())."""
     op: int
     lhs_col: int
     rhs_col: int = -1
@@ -55,11 +56,13 @@ class FilterItem:
     const_i64: int = 0
     const_f64: float = 0.0
     rhs_unsigned: bool = False
+    is_decimal: bool = False
+    const_cell: Optional[bytes] = None
 
     def to_struct(self) -> abi.TgFilterItem:
         s = abi.TgFilterItem()
         s.op, s.lhs_col, s.rhs_col = self.op, self.lhs_col, self.rhs_col
-        s.is_real, s.lhs_unsigned = int(self.is_real), int(self.lhs_unsigned)
+        s.is_real, s.lhs_unsigned = (abi.FILTER_DECIMAL if self.is_decimal else int(self.is_real)), int(self.lhs_unsigned)
         s.rhs_unsigned = int(self.rhs_unsigned)
         s.const_i64, s.const_f64 = self.const_i64, self.const_f64
         return s
@@ -70,6 +73,19 @@ def filter_array(items: Sequence[FilterItem]):
     for i, it in enumerate(items):
         arr[i] = it.to_struct()
     return arr
+
+
+def dec_const_array(items: Sequence[FilterItem]):
+    """tg_vec_filter_ex's dec_consts: 40 bytes per item, item i's constant cell at byte 40 * i (zeros where an item has
+    none); None when no item has a constant cell"""
+    if not any(it.const_cell is not None for it in items):
+        return None
+    buf = bytearray(40 * len(items))
+    for i, it in enumerate(items):
+        if it.const_cell is not None:
+            assert len(it.const_cell) == 40, "a DECIMAL constant is one 40-byte MyDecimal cell"
+            buf[40 * i:40 * i + 40] = bytes(it.const_cell)
+    return (C.c_uint8 * len(buf)).from_buffer(buf)
 
 
 @dataclass
@@ -243,24 +259,30 @@ class ColRef(Expr):
 
 @dataclass
 class Const(Expr):
-    """expression.Constant: handed to the kernels as a scalar (the reference materialises a column, vectorized.go:23)"""
-    value: float
+    """expression.Constant: handed to the kernels as a scalar (the reference materialises a column, vectorized.go:23).
+    cell: a DECIMAL constant, its 40-byte MyDecimal cell (value is then not used)."""
+    value: float = 0
     is_real: bool = False
+    cell: Optional[bytes] = None
 
     def ret_type(self, schema):
+        if self.cell is not None:
+            return FieldType(abi.TYPE_NEWDECIMAL, abi.FLAG_NOT_NULL)
         return FieldType(abi.TYPE_DOUBLE if self.is_real else abi.TYPE_LONGLONG, abi.FLAG_NOT_NULL)
 
 
 @dataclass
 class ScalarFunc(Expr):
-    """builtinArithmetic{Plus,Minus,Multiply}{Int,Real}Sig / builtin{LT,LE,GT,GE,EQ,NE}{Int,Real}Sig over two arguments
-    (kind "arith": op = abi.ARITH_*, kind "cmp": op = abi.CMP_*); the right argument may be a Const"""
+    """builtinArithmetic{Plus,Minus,Multiply}{Int,Real}Sig / builtin{LT,LE,GT,GE,EQ,NE}{Int,Real,Decimal}Sig over two
+    arguments (kind "arith": op = abi.ARITH_*, kind "cmp": op = abi.CMP_*); the right argument may be a Const.
+    is_decimal (kind "cmp" only): both arguments are DECIMAL (cell columns; a Const with a cell)."""
     kind: str
     op: int
     args: Tuple[Expr, Expr]
     is_real: bool = False
     a_unsigned: bool = False
     b_unsigned: bool = False
+    is_decimal: bool = False
 
     def ret_type(self, schema):
         if self.kind == "arith" and self.is_real:
