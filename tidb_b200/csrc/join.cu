@@ -111,6 +111,8 @@ struct JoinImpl : DeviceHandle {
   bool built = false;
   DevBuf table, rows_store, row_slot, row_rank, slot_used, scalars;
   TableView tv{};
+  DevBuf pidx_slots, pidx_pilot;   // slice index of a sliced U1 table (build_slice_index); pidx.P == 0: none
+  SliceIndex pidx{};
   RowSpec rowspec{};
   std::vector<int> build_word_of_col;   // build column → row-store word (mode G)
   int u1_payload_col = -1;
@@ -470,6 +472,73 @@ static const double kMaxDenseLoad = 0.5;
 // 4.34, 99 % 4.63 / 4.35, 50 % 5.63 / 4.33.
 static const double kInplaceMinMatch = 0.995;
 
+// ---- slice index of a sliced U1 table (SliceIndex, join_kernels.cuh) ----------------------------------------------------
+// Load factor and mean keys per bucket: tools/scratch/pilot_lab.cu on bench.py's 10 M keys in 16 slices (H100 80GB HBM3,
+// 700 W) — load factor 0.7 with 4 keys per bucket places every key with one-byte pilots (153 KiB of pilots per slice), and
+// the in-place probe kernel with the pilots in shared memory took 1.70 ms against 2.07 ms on the linear-probe table.
+// Denser or with bigger buckets, one-byte pilots leave keys unplaced (0.9 with 4–6 keys: 1–10 % of them); with more
+// pilot bytes per CTA than kPidxMaxPilotBytes the kernel lost a third (204 KiB: 2.71–2.83 ms).  DESIGN.md §4.1.
+static const double kPidxLoad = 0.7;
+static const double kPidxKeysPerBucket = 4.0;
+static const size_t kPidxMaxPilotBytes = 160 << 10;
+static int enqueue_scan(JoinImpl* j, int64_t n, int64_t* nblocks_out);
+static int build_slice_index(JoinImpl* j, const Slot* slots, unsigned long long nslots) {
+  const ProbeTuning& tune = probe_tuning();
+  const uint32_t P = (uint32_t)probe_slices((size_t)nslots * sizeof(Slot), j->device, tune.parts);
+  if (P < 2) return TG_OK;
+  DevBuf cnt;
+  TG_TRY(cnt.ensure(j->device, (size_t)(TG_MAX_PARTS + 1) * 8));
+  unsigned long long* pcnt = cnt.as<unsigned long long>();
+  TG_CUDA(cudaMemsetAsync(pcnt, 0, (size_t)(TG_MAX_PARTS + 1) * 8, j->stream));
+  k_pidx_part_count<<<grid_size(j->nsm, (int64_t)nslots, 256, 8), 256, 0, j->stream>>>(slots, nslots, P, pcnt);
+  unsigned long long hc[TG_MAX_PARTS];
+  TG_CUDA(cudaMemcpyAsync(hc, pcnt, P * 8, cudaMemcpyDeviceToHost, j->stream));
+  TG_CUDA(cudaStreamSynchronize(j->stream));
+  unsigned long long mx = 0;
+  for (uint32_t p = 0; p < P; p++) mx = std::max(mx, hc[p]);
+  SliceIndex ix{};
+  ix.P = P;
+  ix.S = (uint32_t)std::ceil((double)mx / kPidxLoad) + 1;
+  ix.B = ((uint32_t)std::ceil((double)mx / kPidxKeysPerBucket) + 16) & ~15u;
+  int optin = 0;
+  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, j->device);
+  if (ix.B > kPidxMaxPilotBytes || ix.B > (uint32_t)optin) return TG_OK;   // slices too big: the linear-probe kernels
+  const size_t nb = (size_t)P * ix.B, ns = (size_t)P * ix.S;
+  TG_TRY(j->pidx_slots.ensure(j->device, ns * sizeof(Slot)));
+  TG_TRY(j->pidx_pilot.ensure(j->device, nb));
+  DevBuf owner, list;
+  TG_TRY(owner.ensure(j->device, ns * 4));
+  TG_TRY(list.ensure(j->device, (size_t)(mx * P + 1) * 4));
+  TG_TRY(j->tmp_cnt.ensure(j->device, (nb + 1) * 4));
+  Slot* islots = j->pidx_slots.as<Slot>();
+  ix.slots = islots;
+  ix.pilot = j->pidx_pilot.as<uint8_t>();
+  TG_CUDA(cudaMemsetAsync(j->pidx_pilot.p, (int)kPilotNone, nb, j->stream));
+  TG_CUDA(cudaMemsetAsync(owner.p, 0xFF, ns * 4, j->stream));
+  TG_CUDA(cudaMemsetAsync(j->tmp_cnt.p, 0, (nb + 1) * 4, j->stream));
+  k_table_init<<<grid_size(j->nsm, (int64_t)ns, 256, 8), 256, 0, j->stream>>>(islots, ns, ns);   // all empty: no side slot
+  const unsigned g = (unsigned)grid_size(j->nsm, (int64_t)nslots, 256, 8);
+  k_pidx_bucket_count<<<g, 256, 0, j->stream>>>(slots, nslots, ix, j->tmp_cnt.as<uint32_t>());
+  int64_t nblocks = 0;
+  TG_TRY(enqueue_scan(j, (int64_t)nb, &nblocks));
+  const unsigned long long* off = j->tmp_off.as<unsigned long long>();
+  k_pidx_lists<<<g, 256, 0, j->stream>>>(slots, nslots, ix, off, j->tmp_cnt.as<uint32_t>(), list.as<uint32_t>());
+  const unsigned gb = (unsigned)grid_size(j->nsm, (int64_t)nb, 256, 8);
+  for (uint32_t size = kPidxMaxBucket; size >= 1; size--)   // largest buckets first
+    k_pidx_place<<<gb, 256, 0, j->stream>>>(slots, ix, off, list.as<uint32_t>(), size, owner.as<uint32_t>(), j->pidx_pilot.as<uint8_t>());
+  unsigned long long* bad = pcnt + TG_MAX_PARTS;
+  k_pidx_write<<<g, 256, 0, j->stream>>>(slots, nslots, ix, islots, 0, bad);
+  k_pidx_write<<<g, 256, 0, j->stream>>>(slots, nslots, ix, islots, 1, bad);
+  j->stats.kernel_launches += 8 + kPidxMaxBucket;
+  unsigned long long hbad = 0;
+  TG_CUDA(cudaMemcpyAsync(&hbad, bad, 8, cudaMemcpyDeviceToHost, j->stream));
+  TG_CUDA(cudaStreamSynchronize(j->stream));
+  if (hbad) { j->pidx_slots.release(); j->pidx_pilot.release(); return TG_OK; }   // never seen: the linear-probe kernels
+  j->pidx = ix;
+  return TG_OK;
+}
+
+
 // Segment capacity of the in-place segment probe.  The fallback C0 = 1.05·n/P + 16 K leaves ≈ 330 K rows of slack per segment
 // at 100 M rows and P = 16, about 130 σ of a uniform multinomial fill (σ ≈ sqrt(n/P) ≈ 2.5 K), and every unused row below the
 // output count costs the hole fill a move of the whole output row.  So once the host has read the fills of a partitioned
@@ -545,6 +614,9 @@ static int build_table(JoinImpl* j) {
     int pc = payload[0];
     if (b.kelem[pc] != 8 || j->bcols.has_nulls[pc]) u1 = false;
   }
+  bool sliced = false;   // a U1 table rebuilt dense for the partitioned probe: it gets a slice index (build_slice_index)
+  j->pidx = SliceIndex{};
+  j->pidx_slots.release(); j->pidx_pilot.release();
   if (u1 && j->default_load_factor && n > 0) {
     // the partitioned probe will slice this table: rebuild it dense enough for TG_MAX_PARTS L2-sized slices (probe_slices)
     const ProbeTuning& tune = probe_tuning();
@@ -561,6 +633,7 @@ static int build_table(JoinImpl* j) {
                                                                     j->row_slot.as<uint32_t>(), j->row_rank.as<uint32_t>());
       j->stats.kernel_launches += 2;
       j->stats.table_slots = (int64_t)nslots;
+      sliced = true;
     }
   }
   j->tv = TableView{slots, nslots, nullptr, 0, -1, TABLE_NONE};
@@ -571,6 +644,7 @@ static int build_table(JoinImpl* j) {
       const unsigned long long* pl = j->u1_payload_col >= 0 ? reinterpret_cast<const unsigned long long*>(bview.data[j->u1_payload_col]) : nullptr;
       k_build_scatter_u1<<<grid_size(j->nsm, n, 256, 8), 256, 0, j->stream>>>(j->row_slot.as<uint32_t>(), pl, n, slots);
       j->stats.kernel_launches++;
+      if (sliced) TG_TRY(build_slice_index(j, slots, nslots));
     }
     j->tv.mode = TABLE_U1;
   } else {
@@ -858,6 +932,17 @@ struct LaunchInplace {
       int64_t ctas = (n / 128 + 7) / 8;
       int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
       int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
+      if (j->pidx.P == (uint32_t)(n / seg.cap)) {
+        // the slice index of this table, cut for this P: one CTA per SM holding one slice's pilots
+        static bool attr = false;
+        if (!attr) {
+          TG_CUDA(cudaFuncSetAttribute(k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)kPidxMaxPilotBytes));
+          attr = true;
+        }
+        k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD><<<j->nsm, kPidxThreads, j->pidx.B, j->stream>>>(n, j->tv, j->pidx, fo, cur, seg, tile_cnt);
+        return TG_OK;
+      }
       k_probe_inner_u1_seg_inplace<NPC, NKD, NMD><<<grid, 256, 0, j->stream>>>(n, j->tv, fo, cur, seg, tile_cnt);
       return TG_OK;
     }

@@ -840,6 +840,195 @@ k_probe_inner_u1_seg_inplace(int64_t n, TableView t, FastOut out, unsigned long 
   if (lane == 0 && kept) atomicAdd(out_cursor, kept);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Slice index of a U1 table the partitioned probe slices (hash-and-displace, PTHash style): slice p holds the keys of
+// partition mulhi32(hi32(h), P) in S slots of 16 bytes; a key's bucket is mulhi32(lo32(h), B), bits the partition does not
+// use; its slot is p·S + pidx_slot(h, pilot[p·B + bucket], S).  A probe row costs one pilot byte and ONE 16-byte gather,
+// no linear-probe run.  Pilot kPilotNone = the bucket found no placement: its keys are looked up in the linear-probe
+// table, which keeps every key.  DESIGN.md §4.1.
+// ---------------------------------------------------------------------------------------------
+static constexpr uint32_t kPilotNone = 255;
+static constexpr int kPidxMaxBucket = 32;   // a bigger bucket is never placed (Poisson(4) tail: none at 10 M keys)
+static constexpr int kPidxThreads = 1024;   // CTA of the index probe: the CTA's warps share one slice's pilots
+
+struct SliceIndex {
+  const Slot* slots;        // [P][S]
+  const uint8_t* pilot;     // [P][B], B a multiple of 16
+  uint32_t P, S, B, pad;
+};
+
+__host__ __device__ __forceinline__ uint32_t pidx_slot(uint64_t h, uint32_t q, uint32_t S) {
+  return slot32(hash64(h ^ ((uint64_t)(q + 1) * 0xC2B2AE3D27D4EB4Full)), S);
+}
+__host__ __device__ __forceinline__ uint32_t pidx_bucket(uint64_t h, uint32_t B) { return mulhi32((uint32_t)h, B); }
+
+// keys per partition (block-aggregated in shared memory)
+__global__ void __launch_bounds__(256) k_pidx_part_count(const Slot* __restrict__ slots, unsigned long long nslots, uint32_t P,
+                                                         unsigned long long* __restrict__ pcnt) {
+  __shared__ unsigned int c[64];   // P <= TG_MAX_PARTS (partition_kernels.cuh: 16)
+  for (int i = threadIdx.x; i < 64; i += blockDim.x) c[i] = 0;
+  __syncthreads();
+  for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nslots; i += (unsigned long long)gridDim.x * blockDim.x) {
+    const int64_t k = slots[i].key;
+    if (k != kEmptyKey) atomicAdd(&c[slot32(hash64((uint64_t)k), P)], 1u);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < (int)P; i += blockDim.x) if (c[i]) atomicAdd(&pcnt[i], (unsigned long long)c[i]);
+}
+
+// keys per bucket (global bucket id p·B + b)
+__global__ void __launch_bounds__(256) k_pidx_bucket_count(const Slot* __restrict__ slots, unsigned long long nslots, SliceIndex ix,
+                                                           uint32_t* __restrict__ bcnt) {
+  for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nslots; i += (unsigned long long)gridDim.x * blockDim.x) {
+    const int64_t k = slots[i].key;
+    if (k == kEmptyKey) continue;
+    const uint64_t h = hash64((uint64_t)k);
+    atomicAdd(&bcnt[(size_t)slot32(h, ix.P) * ix.B + pidx_bucket(h, ix.B)], 1u);
+  }
+}
+
+// the table slots of each bucket's keys, at off[bucket] (exclusive scan of the counts); bcnt counts back down to 0
+__global__ void __launch_bounds__(256) k_pidx_lists(const Slot* __restrict__ slots, unsigned long long nslots, SliceIndex ix,
+                                                    const unsigned long long* __restrict__ off, uint32_t* __restrict__ bcnt,
+                                                    uint32_t* __restrict__ list) {
+  for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nslots; i += (unsigned long long)gridDim.x * blockDim.x) {
+    const int64_t k = slots[i].key;
+    if (k == kEmptyKey) continue;
+    const uint64_t h = hash64((uint64_t)k);
+    const size_t b = (size_t)slot32(h, ix.P) * ix.B + pidx_bucket(h, ix.B);
+    list[off[b] + atomicSub(&bcnt[b], 1u) - 1] = (uint32_t)i;
+  }
+}
+
+// place every bucket of exactly `size` keys (launched largest size first): try pilots 0, 1, ...; a try claims each key's
+// slot with atomicCAS from empty to the bucket id, and a bucket that loses any claim (to another bucket or to one of its own
+// keys) releases the claims it won and tries its next pilot.  No placement within kPilotNone pilots leaves kPilotNone.
+__global__ void __launch_bounds__(256) k_pidx_place(const Slot* __restrict__ slots, SliceIndex ix, const unsigned long long* __restrict__ off,
+                                                    const uint32_t* __restrict__ list, uint32_t size, uint32_t* __restrict__ owner,
+                                                    uint8_t* __restrict__ pilot) {
+  const size_t nb = (size_t)ix.P * ix.B;
+  for (size_t b = blockIdx.x * (size_t)blockDim.x + threadIdx.x; b < nb; b += (size_t)gridDim.x * blockDim.x) {
+    const unsigned long long o = off[b];
+    if (off[b + 1] - o != size) continue;
+    uint64_t h[kPidxMaxBucket];
+    for (uint32_t j = 0; j < size; j++) h[j] = hash64((uint64_t)slots[list[o + j]].key);
+    uint32_t* const base = owner + (b / ix.B) * ix.S;
+    for (uint32_t q = 0; q < kPilotNone; q++) {
+      uint32_t won = 0;
+      for (; won < size; won++)
+        if (atomicCAS(base + pidx_slot(h[won], q, ix.S), 0xFFFFFFFFu, (uint32_t)b) != 0xFFFFFFFFu) break;
+      if (won == size) { pilot[b] = (uint8_t)q; break; }
+      for (uint32_t j = 0; j < won; j++) atomicExch(base + pidx_slot(h[j], q, ix.S), 0xFFFFFFFFu);
+    }
+  }
+}
+
+// write each placed key's {key, payload} into its index slot, then (second launch, check = 1) verify that every placed key
+// is at its computed slot; *bad != 0 drops the index
+__global__ void __launch_bounds__(256) k_pidx_write(const Slot* __restrict__ slots, unsigned long long nslots, SliceIndex ix,
+                                                    Slot* __restrict__ islots, int check, unsigned long long* __restrict__ bad) {
+  for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nslots; i += (unsigned long long)gridDim.x * blockDim.x) {
+    const Slot s = slots[i];
+    if (s.key == kEmptyKey) continue;
+    const uint64_t h = hash64((uint64_t)s.key);
+    const uint32_t p = slot32(h, ix.P);
+    const uint32_t q = ix.pilot[(size_t)p * ix.B + pidx_bucket(h, ix.B)];
+    if (q == kPilotNone) continue;
+    Slot* d = islots + (size_t)p * ix.S + pidx_slot(h, q, ix.S);
+    if (!check) *d = s;
+    else if (d->key != s.key || d->meta != s.meta) atomicAdd(bad, 1ull);
+  }
+}
+
+// In-place segment probe through the slice index: the contract of k_probe_inner_u1_seg_inplace (tile_cnt, one cursor
+// atomic per warp, compaction of partly matched tiles), but CTA-cooperative: one CTA of kPidxThreads per SM loads the
+// pilots of slice p into shared memory, its warps sweep segment p's tiles, and a barrier precedes the next slice.  A full
+// tile reads its keys, one pilot byte and ONE 16-byte slot per row; a tile with a sentinel-valued key or a key whose
+// bucket has no pilot, and a segment's partial last tile, take inplace_tile_generic on the linear-probe table.
+template <int NPC, int NKD, int NMD>
+__global__ void __launch_bounds__(kPidxThreads, 1)
+k_probe_inner_u1_seg_inplace_pidx(int64_t n, TableView t, SliceIndex ix, FastOut out, unsigned long long* __restrict__ out_cursor,
+                                  SegSpec seg, uint32_t* __restrict__ tile_cnt) {
+  static_assert(NKD >= 1, "the probe key is read from the first key destination");
+  constexpr int R = 4, G = 2, NP = NPC > 0 ? NPC : 1;
+  extern __shared__ __align__(16) uint8_t spil[];
+  if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) return;
+  const int lane = threadIdx.x & 31;
+  const int64_t warps_total = (int64_t)gridDim.x * (kPidxThreads / 32);
+  const int64_t warp_id = (int64_t)blockIdx.x * (kPidxThreads / 32) + (threadIdx.x >> 5);
+  const int64_t* __restrict__ pkey = reinterpret_cast<const int64_t*>(out.key_dst[0]);
+  const int nseg = (int)(n / 128 / seg.tiles_per_seg);
+  unsigned long long kept = 0;
+  for (int p = 0; p < nseg; p++) {
+    __syncthreads();   // every warp is done with the previous slice's pilots
+    const uint4* src = reinterpret_cast<const uint4*>(ix.pilot + (size_t)p * ix.B);
+    for (uint32_t i = threadIdx.x; i < ix.B / 16; i += kPidxThreads) reinterpret_cast<uint4*>(spil)[i] = __ldcs(src + i);
+    __syncthreads();
+    const unsigned long long c = seg.cnt[p];
+    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+    const int64_t t0 = (int64_t)p * seg.tiles_per_seg, t1 = t0 + seg.tiles_per_seg;
+    const Slot* __restrict__ islots = ix.slots + (size_t)p * ix.S;
+    for (int64_t tile = t0 + warp_id; tile < t1; tile += warps_total) {
+      const int64_t base = tile * 128;
+      uint32_t m = 0;
+      if (limit - base >= 128) {
+        int64_t k[R];
+#pragma unroll
+        for (int g = 0; g < G; g++) {
+          const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + base + g * 64 + 2 * lane));
+          k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
+        }
+        uint32_t q[R];
+        bool generic = false;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+          q[j] = spil[pidx_bucket(hash64((uint64_t)k[j]), ix.B)];
+          generic |= (k[j] == kEmptyKey) | (q[j] == kPilotNone);
+        }
+        if (__any_sync(0xffffffffu, generic)) {
+          m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
+        } else {
+          unsigned long long meta[R];
+          unsigned hit = 0;
+#pragma unroll
+          for (int j = 0; j < R; j++) {
+            const Slot v = load_slot(islots + pidx_slot(hash64((uint64_t)k[j]), q[j], ix.S));
+            meta[j] = v.meta;
+            if (v.key == k[j]) hit |= 1u << j;
+          }
+          if (__all_sync(0xffffffffu, hit == 0xFu)) {
+            m = 128;
+#pragma unroll
+            for (int g = 0; g < G; g++) {
+              const int64_t o = base + g * 64 + 2 * lane;
+              const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
+#pragma unroll
+              for (int d = 1; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
+#pragma unroll
+              for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
+            }
+          } else {
+            unsigned long long pv[R][NP];
+            inplace_load_pv<NPC>(base, out, pv, lane);
+            unsigned bal[R];
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+              bal[j] = __ballot_sync(0xffffffffu, (hit >> j) & 1u);
+              m += __popc(bal[j]);
+            }
+            inplace_store<NPC, NKD, NMD>(base, k, meta, pv, bal, out, lane);
+          }
+        }
+      } else if (limit > base) {
+        m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
+      }
+      if (lane == 0) tile_cnt[tile] = m;
+      kept += m;
+    }
+  }
+  if (lane == 0 && kept) atomicAdd(out_cursor, kept);
+}
+
 // Hole fill behind k_probe_inner_u1_seg_inplace, R = *out_cursor: tile t keeps rows [128t, 128t + m_t).  cnt[t] = its holes
 // below R, [128t + m_t, min(128t + 128, R)); cnt[ntiles + t] = its kept rows at or beyond R.  Both sum to the same total;
 // one exclusive scan over the 2·ntiles counts numbers the holes and the rows that fill them.

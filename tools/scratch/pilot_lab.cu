@@ -1,0 +1,344 @@
+// pilot_lab.cu — can a per-slice pilot index (hash-and-displace, one 16-byte gather per row) beat the linear-probe table
+// in the in-place segment probe at the bench shape?  100 M partition-ordered probe rows, 100 % match, against 10 M unique
+// build keys (bench.py's keys: id * ODD), 16 slices.
+//
+//   (a) k_probe_inner_u1_seg_inplace<1,2,1> from the library against the linear-probe table at load factor 0.5
+//   (b) a prototype of the same kernel that reads the key's pilot byte and gathers ONE 16-byte slot of a dense slice table
+//       at load factor ALPHA; the pilots come from global memory through L1 (`gl`), or from shared memory, where a CTA
+//       loads the pilots of one slice and its warps sweep that slice's tiles together (`sm`)
+//
+// build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I include -I tidb_b200/csrc \
+//          -o tools/scratch/pilot_lab tools/scratch/pilot_lab.cu
+// run:   tools/scratch/pilot_lab [ALPHA LAMBDA]...        (GPU: kernel times, median of 30 alternating launches per variant,
+//                                                          for each (load factor, mean keys per bucket) pair; default
+//                                                          0.9 2  0.8 3  0.75 4)
+//        tools/scratch/pilot_lab --host [ALPHA LAMBDA]   (CPU only: placement statistics of the pilot index)
+//
+// The index is built on the host here (sequential, largest bucket first, one byte per pilot, 255 = not placed: such a
+// key's tile takes the library's generic path on the linear-probe table).  Results: DESIGN.md §4.1 "Pilot index".
+#include "join_kernels.cuh"
+#include <algorithm>
+#include <cstdio>
+#include <cstring>
+#include <numeric>
+#include <random>
+#include <vector>
+
+using namespace tg;
+#define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { printf("CUDA %s at %d\n", cudaGetErrorString(e_), __LINE__); exit(1); } } while (0)
+
+static const uint64_t ODD = 0x9E3779B97F4A7C15ull;
+static const int P = 16;
+
+// slot of a key within its slice under pilot q
+__host__ __device__ __forceinline__ uint32_t pilot_slot(uint64_t h, uint32_t q, uint32_t S) {
+  return slot32(hash64(h ^ ((uint64_t)(q + 1) * 0xC2B2AE3D27D4EB4Full)), S);
+}
+__host__ __device__ __forceinline__ uint32_t bucket_of(uint64_t h, uint32_t B) { return mulhi32((uint32_t)h, B); }
+
+struct Index {
+  uint32_t S = 0, B = 0;
+  std::vector<uint8_t> pilot;   // [P][B]
+  std::vector<Slot> slots;      // [P][S]
+  long long bad_buckets = 0, bad_keys = 0;
+};
+
+// sequential hash-and-displace per slice, largest bucket first; pilot 255 = not placed
+static Index build_index(const std::vector<uint64_t>& keys, const std::vector<uint64_t>& payload, double alpha, double lambda,
+                         bool fill_slots) {
+  std::vector<std::vector<uint32_t>> part(P);
+  for (uint32_t i = 0; i < keys.size(); i++) part[slot32(hash64(keys[i]), P)].push_back(i);
+  size_t mx = 0;
+  for (auto& v : part) mx = std::max(mx, v.size());
+  Index ix;
+  ix.S = (uint32_t)std::ceil(mx / alpha);
+  ix.B = ((uint32_t)std::ceil(mx / lambda) + 15) & ~15u;   // whole uint4 rows for the shared-memory copy
+  ix.pilot.assign((size_t)P * ix.B, 255);
+  if (fill_slots) ix.slots.assign((size_t)P * ix.S, Slot{kEmptyKey, 0});
+  std::vector<uint8_t> taken(ix.S);
+  for (int p = 0; p < P; p++) {
+    std::fill(taken.begin(), taken.end(), 0);
+    std::vector<uint32_t> cnt(ix.B + 1, 0), ord(part[p].size());
+    for (uint32_t i : part[p]) cnt[bucket_of(hash64(keys[i]), ix.B) + 1]++;
+    std::partial_sum(cnt.begin(), cnt.end(), cnt.begin());
+    std::vector<uint32_t> pos(cnt.begin(), cnt.end() - 1);
+    for (uint32_t i : part[p]) ord[pos[bucket_of(hash64(keys[i]), ix.B)]++] = i;
+    std::vector<uint32_t> bs(ix.B);
+    std::iota(bs.begin(), bs.end(), 0);
+    std::stable_sort(bs.begin(), bs.end(), [&](uint32_t a, uint32_t b) { return cnt[a + 1] - cnt[a] > cnt[b + 1] - cnt[b]; });
+    uint32_t sl[64];
+    for (uint32_t b : bs) {
+      const uint32_t n = cnt[b + 1] - cnt[b];
+      if (!n) break;
+      int q = 0;
+      for (; q < 255; q++) {
+        bool ok = n <= 64;
+        for (uint32_t j = 0; ok && j < n; j++) {
+          sl[j] = pilot_slot(hash64(keys[ord[cnt[b] + j]]), q, ix.S);
+          if (taken[sl[j]]) ok = false;
+          for (uint32_t i = 0; ok && i < j; i++) ok = sl[i] != sl[j];
+        }
+        if (ok) break;
+      }
+      if (q == 255) { ix.bad_buckets++; ix.bad_keys += n; continue; }
+      ix.pilot[(size_t)p * ix.B + b] = (uint8_t)q;
+      for (uint32_t j = 0; j < n; j++) {
+        taken[sl[j]] = 1;
+        if (fill_slots) {
+          const uint32_t i = ord[cnt[b] + j];
+          ix.slots[(size_t)p * ix.S + sl[j]] = Slot{(int64_t)keys[i], payload[i]};
+        }
+      }
+    }
+  }
+  return ix;
+}
+
+// ---- (b) prototype: pilot → slot → one LDG.128 → compare ---------------------------------------------------------------
+struct PilotView {
+  const Slot* slots; const uint8_t* pilot; uint32_t S, B;
+};
+
+template <bool SMEM>
+__device__ __forceinline__ void pilot_tile(int64_t base, int64_t limit, const PilotView& ix, const uint8_t* spil, const TableView& t,
+                                           const FastOut& out, int lane, uint32_t& m) {
+  constexpr int R = 4, G = 2, NPC = 1, NKD = 2, NMD = 1, NP = 1;
+  const int64_t* pkey = reinterpret_cast<const int64_t*>(out.key_dst[0]);
+  if (limit - base < 128) { m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane); return; }
+  int64_t k[R];
+#pragma unroll
+  for (int g = 0; g < G; g++) {
+    const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + base + g * 64 + 2 * lane));
+    k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
+  }
+  uint32_t q[R];
+  bool odd = false;
+#pragma unroll
+  for (int j = 0; j < R; j++) {
+    const uint64_t h = hash64((uint64_t)k[j]);
+    const uint32_t p = slot32(h, P), b = bucket_of(h, ix.B);
+    q[j] = SMEM ? spil[b] : __ldg(ix.pilot + (size_t)p * ix.B + b);
+    odd |= (k[j] == kEmptyKey) | (q[j] == 255u);
+  }
+  if (__any_sync(0xffffffffu, odd)) { m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane); return; }
+  unsigned long long meta[R];
+  unsigned hit = 0;
+#pragma unroll
+  for (int j = 0; j < R; j++) {
+    const uint64_t h = hash64((uint64_t)k[j]);
+    const Slot v = load_slot(ix.slots + (size_t)slot32(h, P) * ix.S + pilot_slot(h, q[j], ix.S));
+    meta[j] = v.meta;
+    if (v.key == k[j]) hit |= 1u << j;
+  }
+  if (__all_sync(0xffffffffu, hit == 0xFu)) {
+    m = 128;
+#pragma unroll
+    for (int g = 0; g < G; g++) {
+      const int64_t o = base + g * 64 + 2 * lane;
+      const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
+#pragma unroll
+      for (int d = 1; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
+#pragma unroll
+      for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
+    }
+  } else {
+    unsigned long long pv[R][NP];
+    inplace_load_pv<NPC>(base, out, pv, lane);
+    unsigned bal[R];
+    m = 0;
+#pragma unroll
+    for (int j = 0; j < R; j++) { bal[j] = __ballot_sync(0xffffffffu, (hit >> j) & 1u); m += __popc(bal[j]); }
+    inplace_store<NPC, NKD, NMD>(base, k, meta, pv, bal, out, lane);
+  }
+}
+
+// warp-autonomous, pilots through L1
+__global__ void __launch_bounds__(256, 3)
+k_pilot_gl(int64_t n, TableView t, PilotView ix, FastOut out, unsigned long long* out_cursor, SegSpec seg, uint32_t* tile_cnt) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const int64_t warp_id = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t ntiles = n / 128;
+  unsigned long long kept = 0;
+  for (int64_t tile = warp_id; tile < ntiles; tile += warps_total) {
+    const int64_t base = tile * 128;
+    const uint32_t p = (uint32_t)tile / seg.tiles_per_seg;
+    const unsigned long long c = seg.cnt[p];
+    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+    uint32_t m = 0;
+    if (limit > base) pilot_tile<false>(base, limit, ix, nullptr, t, out, lane, m);
+    if (lane == 0) tile_cnt[tile] = m;
+    kept += m;
+  }
+  if (lane == 0 && kept) atomicAdd(out_cursor, kept);
+}
+
+// CTA per slice in turn: the CTA's pilots of slice p in shared memory, its warps stride over slice p's tiles
+template <int NT>
+__global__ void __launch_bounds__(NT, 1)
+k_pilot_sm(int64_t n, TableView t, PilotView ix, FastOut out, unsigned long long* out_cursor, SegSpec seg, uint32_t* tile_cnt) {
+  extern __shared__ uint8_t spil[];
+  const int lane = threadIdx.x & 31;
+  const int64_t warps_total = (int64_t)gridDim.x * (NT >> 5);
+  const int64_t warp_id = (int64_t)blockIdx.x * (NT >> 5) + (threadIdx.x >> 5);
+  unsigned long long kept = 0;
+  const int nseg = (int)(n / 128 / seg.tiles_per_seg);
+  for (int p = 0; p < nseg; p++) {
+    __syncthreads();
+    const uint4* src = reinterpret_cast<const uint4*>(ix.pilot + (size_t)p * ix.B);
+    for (uint32_t i = threadIdx.x; i < ix.B / 16; i += NT) reinterpret_cast<uint4*>(spil)[i] = __ldcs(src + i);
+    __syncthreads();
+    const unsigned long long c = seg.cnt[p];
+    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+    const int64_t t0 = (int64_t)p * seg.tiles_per_seg, t1 = t0 + seg.tiles_per_seg;
+    for (int64_t tile = t0 + warp_id; tile < t1; tile += warps_total) {
+      const int64_t base = tile * 128;
+      uint32_t m = 0;
+      if (limit > base) pilot_tile<true>(base, limit, ix, spil, t, out, lane, m);
+      if (lane == 0) tile_cnt[tile] = m;
+      kept += m;
+    }
+  }
+  if (lane == 0 && kept) atomicAdd(out_cursor, kept);
+}
+
+// linear-probe insert (the library's k_build_insert without its column plumbing): U1, meta = payload
+__global__ void k_lp_insert(const unsigned long long* keys, const unsigned long long* pay, int64_t n, Slot* slots, unsigned long long nslots) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t k = (int64_t)keys[i];
+  unsigned long long s = home_slot(hash64((uint64_t)k), nslots);
+  for (;;) {
+    const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(&slots[s].key), (unsigned long long)kEmptyKey, (unsigned long long)k);
+    if (old == (unsigned long long)kEmptyKey) { slots[s].meta = pay[i]; return; }
+    if (++s == nslots) s = 0;
+  }
+}
+
+static void host_stats(const std::vector<double>& as, const std::vector<double>& ls) {
+  std::vector<uint64_t> keys(10000000), pay(keys.size());
+  for (uint64_t i = 0; i < keys.size(); i++) { keys[i] = i * ODD; pay[i] = i * 7; }
+  for (double a : as)
+    for (double l : ls) {
+      Index ix = build_index(keys, pay, a, l, false);
+      printf("alpha %.2f lambda %.1f: S %u (%.2f MiB per slice) B %u (%.0f KiB of pilots)  unplaced buckets %lld keys %lld\n", a, l,
+             ix.S, ix.S * 16.0 / (1 << 20), ix.B, ix.B / 1024.0, ix.bad_buckets, ix.bad_keys);
+      fflush(stdout);
+    }
+}
+
+int main(int argc, char** argv) {
+  if (argc > 1 && !strcmp(argv[1], "--host")) {
+    if (argc == 4) host_stats({atof(argv[2])}, {atof(argv[3])});
+    else host_stats({0.8, 0.85, 0.9}, {4.0, 5.0, 6.0});
+    return 0;
+  }
+  std::vector<std::pair<double, double>> cfg;   // (ALPHA, LAMBDA) pairs from the command line
+  for (int i = 1; i + 1 < argc; i += 2) cfg.push_back({atof(argv[i]), atof(argv[i + 1])});
+  if (cfg.empty()) cfg = {{0.9, 2.0}, {0.8, 3.0}, {0.75, 4.0}};
+  const int64_t nb = 10000000, np = 100000000;
+  cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, 0));
+  printf("card %s, %d SMs, L2 %d MiB\n", prop.name, prop.multiProcessorCount, prop.l2CacheSize >> 20);
+  std::vector<uint64_t> bk(nb), bv(nb);
+  std::vector<uint64_t> ids(nb);
+  std::iota(ids.begin(), ids.end(), 0);
+  std::mt19937_64 rng(42);
+  std::shuffle(ids.begin(), ids.end(), rng);
+  for (int64_t i = 0; i < nb; i++) { bk[i] = ids[i] * ODD; bv[i] = ids[i] * 7; }
+  // probe side: uniform ids, partition-ordered into P segments of capacity cap (learned-capacity slack)
+  std::vector<std::vector<uint64_t>> seg(P);
+  std::uniform_int_distribution<uint64_t> U(0, nb - 1);
+  for (int64_t i = 0; i < np; i++) { const uint64_t k = U(rng) * ODD; seg[slot32(hash64(k), P)].push_back(k); }
+  size_t mx = 0;
+  for (auto& s : seg) mx = std::max(mx, s.size());
+  const long long cap = ((long long)(mx + 8 * std::sqrt((double)mx)) + 4096 + 127) / 128 * 128;   // whole 128-row tiles
+  const int64_t ntot = cap * P;
+  std::vector<uint64_t> hk(ntot, 0), hcnt(P), hpv(ntot, 0);
+  for (int p = 0; p < P; p++) {
+    std::copy(seg[p].begin(), seg[p].end(), hk.begin() + p * cap);
+    for (size_t i = 0; i < seg[p].size(); i++) hpv[p * cap + i] = p * cap + i;
+    hcnt[p] = seg[p].size();
+  }
+  unsigned long long *d_bk, *d_bv, *d_key0, *d_key1, *d_meta, *d_pv, *d_cnt, *d_cur;
+  uint32_t* d_tc;
+  Slot *d_lp, *d_ix;
+  uint8_t* d_pil;
+  const unsigned long long nslots = (unsigned long long)(nb / 0.5 + 32) & ~3ull;
+  CK(cudaMalloc(&d_bk, nb * 8)); CK(cudaMalloc(&d_bv, nb * 8));
+  CK(cudaMalloc(&d_key0, ntot * 8)); CK(cudaMalloc(&d_key1, ntot * 8)); CK(cudaMalloc(&d_meta, ntot * 8)); CK(cudaMalloc(&d_pv, ntot * 8));
+  CK(cudaMalloc(&d_cnt, P * 8)); CK(cudaMalloc(&d_cur, 8)); CK(cudaMalloc(&d_tc, ntot / 128 * 4));
+  CK(cudaMalloc(&d_lp, (nslots + 2) * sizeof(Slot)));
+  CK(cudaMemcpy(d_bk, bk.data(), nb * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(d_bv, bv.data(), nb * 8, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(d_key0, hk.data(), ntot * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(d_pv, hpv.data(), ntot * 8, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(d_cnt, hcnt.data(), P * 8, cudaMemcpyHostToDevice));
+  k_table_init<<<(nslots + 256) / 256, 256>>>(d_lp, nslots + 2, nslots);
+  k_lp_insert<<<(nb + 255) / 256, 256>>>(d_bk, d_bv, nb, d_lp, nslots);
+  CK(cudaDeviceSynchronize());
+  TableView t{d_lp, nslots, nullptr, 0, -1, TABLE_U1, 0};
+  FastOut out{};
+  out.n_pcols = 1; out.n_key_dst = 2; out.n_meta_dst = 1;
+  out.psrc[0] = d_pv; out.pdst[0] = d_pv; out.key_dst[0] = d_key0; out.key_dst[1] = d_key1; out.meta_dst[0] = d_meta;
+  SegSpec sg{d_cnt, (uint32_t)(cap / 128), 0, cap, nullptr, 0};
+  int occ_a = 0, occ_g = 0;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_a, k_probe_inner_u1_seg_inplace<1, 2, 1>, 256, 0));
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_g, k_pilot_gl, 256, 0));
+  const int sms = prop.multiProcessorCount;
+  cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+  for (auto [alpha, lambda] : cfg) {
+    Index ix = build_index(bk, bv, alpha, lambda, true);
+    printf("\nindex: alpha %.2f lambda %.1f  S %u (%.2f MiB per slice)  B %u  unplaced buckets %lld keys %lld\n", alpha, lambda, ix.S,
+           ix.S * 16.0 / (1 << 20), ix.B, ix.bad_buckets, ix.bad_keys);
+    CK(cudaMalloc(&d_ix, ix.slots.size() * sizeof(Slot))); CK(cudaMalloc(&d_pil, ix.pilot.size()));
+    CK(cudaMemcpy(d_ix, ix.slots.data(), ix.slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_pil, ix.pilot.data(), ix.pilot.size(), cudaMemcpyHostToDevice));
+    PilotView pv{d_ix, d_pil, ix.S, ix.B};
+    const size_t smem = ix.B;
+    const int nv = smem <= prop.sharedMemPerBlockOptin ? 3 : 2;   // the shared-memory variant needs the slice's pilots in one CTA
+    if (nv == 3) CK(cudaFuncSetAttribute(k_pilot_sm<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    printf("resident CTAs per SM: (a) %d, (b/gl) %d, (b/sm) %s, %zu B of pilots per slice\n", occ_a, occ_g, nv == 3 ? "1 x 1024 threads" : "n/a", smem);
+    auto run = [&](int v) {
+      CK(cudaMemsetAsync(d_cur, 0, 8));
+      if (v == 0) k_probe_inner_u1_seg_inplace<1, 2, 1><<<occ_a * sms, 256>>>(ntot, t, out, d_cur, sg, d_tc);
+      else if (v == 1) k_pilot_gl<<<occ_g * sms, 256>>>(ntot, t, pv, out, d_cur, sg, d_tc);
+      else k_pilot_sm<1024><<<sms, 1024, smem>>>(ntot, t, pv, out, d_cur, sg, d_tc);
+    };
+    const char* name[3] = {"(a) seg_inplace, linear probe, alpha 0.5", "(b) pilot index, pilots via L1", "(b) pilot index, pilots in smem"};
+    // correctness: every variant matches every row and writes the same build payload
+    for (int v = 0; v < nv; v++) {
+      CK(cudaMemset(d_meta, 0, ntot * 8));
+      CK(cudaMemcpy(d_key0, hk.data(), ntot * 8, cudaMemcpyHostToDevice));   // a variant with misses compacts the keys in place
+      run(v); CK(cudaDeviceSynchronize()); CK(cudaGetLastError());
+      unsigned long long cur; CK(cudaMemcpy(&cur, d_cur, 8, cudaMemcpyDeviceToHost));
+      // a tile that takes the generic path is compacted in lane order, so rows may move within their tile: check each output
+      // row's build payload against the key at the same position, and the keys as a multiset (sum and xor)
+      std::vector<uint64_t> m(ntot), ko(ntot);
+      CK(cudaMemcpy(m.data(), d_meta, ntot * 8, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(ko.data(), d_key0, ntot * 8, cudaMemcpyDeviceToHost));
+      long long bad = 0;
+      uint64_t s0 = 0, x0 = 0, s1 = 0, x1 = 0;
+      for (int p = 0; p < P; p++)
+        for (size_t i = 0; i < seg[p].size(); i++) {
+          bad += m[p * cap + i] * ODD != ko[p * cap + i] * 7;
+          s0 += seg[p][i]; x0 ^= seg[p][i] * 0x2545F4914F6CDD1Dull; s1 += ko[p * cap + i]; x1 ^= ko[p * cap + i] * 0x2545F4914F6CDD1Dull;
+        }
+      printf("%s: rows %llu (want %lld), wrong payloads %lld, keys %s\n", name[v], cur, (long long)np, bad,
+             s0 == s1 && x0 == x1 ? "kept" : "CHANGED");
+    }
+    std::vector<float> ms[3];
+    for (int r = 0; r < nv; r++) run(r);
+    for (int it = 0; it < 30; it++)
+      for (int v = 0; v < nv; v++) {
+        CK(cudaEventRecord(e0)); run(v); CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
+        float x; CK(cudaEventElapsedTime(&x, e0, e1)); ms[v].push_back(x);
+      }
+    for (int v = 0; v < nv; v++) {
+      std::sort(ms[v].begin(), ms[v].end());
+      printf("%-44s median %.3f ms  (min %.3f, max %.3f, 30 launches)", name[v], ms[v][15], ms[v][0], ms[v][29]);
+      if (v) printf("  %+.1f %% against (a)", 100.0 * (ms[v][15] / ms[0][15] - 1));
+      printf("\n");
+    }
+    fflush(stdout);
+    CK(cudaFree(d_ix)); CK(cudaFree(d_pil));
+  }
+  return 0;
+}
