@@ -70,7 +70,10 @@ enum {
   TG_TYPE_TINY = 1, TG_TYPE_SHORT = 2, TG_TYPE_LONG = 3, TG_TYPE_FLOAT = 4, TG_TYPE_DOUBLE = 5,
   TG_TYPE_TIMESTAMP = 7, TG_TYPE_LONGLONG = 8, TG_TYPE_INT24 = 9, TG_TYPE_DATE = 10,
   TG_TYPE_DURATION = 11, TG_TYPE_DATETIME = 12, TG_TYPE_YEAR = 13, TG_TYPE_NEWDECIMAL = 0xf6,
-  TG_TYPE_VARSTRING = 0xfd
+  TG_TYPE_VARSTRING = 0xfd,
+  TG_TYPE_VARCHAR = 15, TG_TYPE_BIT = 16, TG_TYPE_JSON = 0xf5, TG_TYPE_ENUM = 0xf7, TG_TYPE_SET = 0xf8,
+  TG_TYPE_TINY_BLOB = 0xf9, TG_TYPE_MEDIUM_BLOB = 0xfa, TG_TYPE_LONG_BLOB = 0xfb, TG_TYPE_BLOB = 0xfc,
+  TG_TYPE_STRING = 0xfe
 };
 /* pkg/parser/mysql/type.go:54-77 */
 enum { TG_FLAG_NOT_NULL = 1u << 0, TG_FLAG_UNSIGNED = 1u << 5 };
@@ -571,6 +574,70 @@ int tg_vec_filter_ex(int device, int on_device, const tg_chunk* chk, const int32
  * resultFrac and the unused words 0.  It compares with every cell as `cell` does.  A malformed cell is TG_ERR_INVALID
  * with `out` not written. */
 int tg_decimal_normalize(const uint8_t* cell, uint8_t* out);
+
+/* String comparisons and LIKE over var-length columns, for Selection and Projection.
+ *   Columns: a string column is a chunk column with elem_len = -1, `offsets` of length + 1 int64 values and `data`
+ *     (Column.GetString, pkg/util/chunk/column.go:715; the layout tg_chunk_decode returns).  Row r holds the bytes
+ *     data[offsets[r] .. offsets[r+1]).  Offsets need not start at 0: a view into a larger buffer is valid, and the call
+ *     reads only [offsets[0], offsets[length]).  In tg_vec_filter_ex2 its col_types entry is TG_TYPE_VARCHAR,
+ *     TG_TYPE_VARSTRING, TG_TYPE_STRING or one of the four BLOB / TEXT types; ENUM, SET, JSON and BIT are var-length but
+ *     not strings, so an item over them is TG_ERR_UNSUPPORTED.  Device-resident `data` and `offsets` need only their
+ *     natural (1- and 8-byte) alignment.
+ *   Offsets: checked at every row the call evaluates, NULL or not (the rows in `sel` when the chunk has one, else every
+ *     physical row).  A row is bad when offsets[r] > offsets[r+1] or either value lies outside
+ *     [offsets[0], offsets[length]]; a bad row fails the call with TG_ERR_INVALID.  With host columns,
+ *     offsets[length] < offsets[0] is TG_ERR_INVALID before any device work.  A failed call with host buffers writes
+ *     nothing (no result, no bitmap byte, no `selected` byte, no *n_selected), as for malformed DECIMAL cells.
+ *   Collation: the MySQL collation id of the comparison (the builtin's collation), one of three collator behaviours
+ *     (pkg/util/collate/bin.go, collate.go newCollatorIDMap):
+ *       63 binary                                          compare: strings.Compare on the bytes; LIKE: over bytes
+ *                                                          (CompilePatternBinary / DoMatchBinary)
+ *       46 utf8mb4_bin, 83 utf8_bin, 65 ascii_bin, 47 latin1_bin
+ *                                                          compare: strings.Compare after the trailing 0x20 bytes are cut
+ *                                                          from both sides (truncateTailingSpace; a tab is kept, so
+ *                                                          "a\t" > "a"); LIKE: over runes (CompilePattern / DoMatch),
+ *                                                          trailing spaces count
+ *       309 utf8mb4_0900_bin                               compare: strings.Compare on the bytes; LIKE: over runes
+ *     Any other id (the _ci collations, gbk, gb18030) is TG_ERR_UNSUPPORTED.  Bytes compare unsigned; a proper prefix sorts
+ *     first.
+ *   LIKE: `column LIKE 'pattern' ESCAPE e` as builtinLikeSig.vecEvalInt (expression/builtin_like_vec.go) with a constant
+ *     pattern and escape byte e (0..255, else TG_ERR_INVALID).  The escape is tested before '_' and '%' (so either may be
+ *     the escape), an escape as the last character is a literal, "%%" is "%" and "%_" is "_%"; the match is
+ *     stringutil.doMatchInner with its single restart point.  Over runes, the string and the pattern decode as Go's
+ *     []rune(s): every byte that does not start a valid UTF-8 sequence (truncated, overlong, surrogate, above U+10FFFF)
+ *     is one U+FFFD, so such bytes and a valid U+FFFD match each other, and the escape is the rune e (0xE9 is 'é', not
+ *     the byte 0xE9).  A pattern from a column or a non-constant escape is not offloaded (the shim keeps the CPU path).
+ *   The constant and the pattern have no length cap.  These argument checks (types, collation ids, kind, escape, host
+ *     offsets bounds) answer before the device is looked for. */
+enum { TG_FILTER_STRING = 3 };   /* tg_filter_item.is_real value understood by tg_vec_filter_ex2 */
+enum { TG_STR_CMP = 0, TG_STR_LIKE = 1, TG_STR_NOT_LIKE = 2 };
+typedef struct tg_str_arg {
+  const uint8_t* bytes; int64_t len;  /* the constant (TG_STR_CMP with rhs_col < 0) or the LIKE pattern; host memory;
+                                         may be NULL when len == 0                                                      */
+  int32_t collation;                  /* MySQL collation id                                                             */
+  int32_t kind;                       /* TG_STR_*; LIKE items ignore op and rhs_col                                     */
+  int32_t escape;                     /* LIKE escape byte                                                               */
+  int32_t reserved;
+} tg_str_arg;
+
+/* tg_vec_filter_ex plus STRING items (is_real == TG_FILTER_STRING): str_args[i] describes item i (read for STRING items
+ * only; may be NULL when there is none).  A TG_STR_CMP item compares lhs_col with rhs_col or, when rhs_col < 0, with
+ * the constant; TG_STR_LIKE / TG_STR_NOT_LIKE match lhs_col against the pattern.  NULL stays NULL, so a NOT LIKE item
+ * does not select a NULL row.  STRING items mix with INT, REAL and DECIMAL items in one CNF of at most TG_MAX_FILTER (8)
+ * items over at most 16 columns; a string column in a non-STRING item, or a non-string column in a STRING item, is
+ * TG_ERR_UNSUPPORTED.  With no STRING item the call is tg_vec_filter_ex: the same `selected` and count. */
+int tg_vec_filter_ex2(int device, int on_device, const tg_chunk* chk, const int32_t* col_types,
+                      const tg_filter_item* items, int32_t n_items, const uint8_t* dec_consts,
+                      const tg_str_arg* str_args, uint8_t* selected, int64_t* n_selected, void* stream);
+/* builtin{LT,LE,GT,GE,EQ,NE}StringSig.vecEvalInt (expression/builtin_compare_vec_generated.go, types.CompareString):
+ * result int64 0/1, NULL if either side is NULL (a NULL row's value is 0).  b == NULL -> compare with the constant
+ * b_const[0 .. b_len) (host memory). */
+int tg_vec_compare_string(int device, int on_device, int op, int32_t collation, const tg_column* a,
+                          const tg_column* b, const uint8_t* b_const, int64_t b_len,
+                          int64_t* result, uint8_t* result_nulls, void* stream);
+/* builtinLikeSig.vecEvalInt with a constant pattern (host memory) and escape: result int64 0/1, NULL where a is NULL. */
+int tg_vec_like(int device, int on_device, int32_t collation, const tg_column* a, const uint8_t* pattern,
+                int64_t pattern_len, int32_t escape, int64_t* result, uint8_t* result_nulls, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * TopN                         replaces sortexec.TopNExec (pkg/executor/sortexec/topn.go:74, :230)

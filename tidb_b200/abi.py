@@ -20,6 +20,9 @@ TG_ERR_STATE, TG_ERR_CANCELLED, TG_ERR_OVERFLOW, TG_ERR_CAPACITY = 5, 6, 7, 8
 TYPE_TINY, TYPE_SHORT, TYPE_LONG, TYPE_FLOAT, TYPE_DOUBLE = 1, 2, 3, 4, 5
 TYPE_TIMESTAMP, TYPE_LONGLONG, TYPE_INT24, TYPE_DATE, TYPE_DURATION = 7, 8, 9, 10, 11
 TYPE_DATETIME, TYPE_YEAR, TYPE_NEWDECIMAL, TYPE_VARSTRING = 12, 13, 0xF6, 0xFD
+TYPE_VARCHAR, TYPE_BIT, TYPE_JSON, TYPE_ENUM, TYPE_SET = 15, 16, 0xF5, 0xF7, 0xF8
+TYPE_TINY_BLOB, TYPE_MEDIUM_BLOB, TYPE_LONG_BLOB, TYPE_BLOB, TYPE_STRING = 0xF9, 0xFA, 0xFB, 0xFC, 0xFE
+STRING_TYPES = (TYPE_VARCHAR, TYPE_VARSTRING, TYPE_STRING, TYPE_TINY_BLOB, TYPE_MEDIUM_BLOB, TYPE_LONG_BLOB, TYPE_BLOB)
 FLAG_NOT_NULL, FLAG_UNSIGNED = 1 << 0, 1 << 5
 JOIN_INNER, JOIN_LEFT_OUTER, JOIN_RIGHT_OUTER, JOIN_SEMI, JOIN_ANTI_SEMI = 0, 1, 2, 3, 4
 JOIN_LEFT_OUTER_SEMI, JOIN_ANTI_LEFT_OUTER_SEMI = 5, 6
@@ -28,6 +31,11 @@ AGGMODE_COMPLETE, AGGMODE_FINAL, AGGMODE_PARTIAL1, AGGMODE_PARTIAL2, AGGMODE_DED
 CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_EQ, CMP_NE = 0, 1, 2, 3, 4, 5
 ARITH_PLUS, ARITH_MINUS, ARITH_MUL = 0, 1, 2
 FILTER_INT, FILTER_REAL, FILTER_DECIMAL = 0, 1, 2    # tg_filter_item.is_real as tg_vec_filter_ex reads it
+FILTER_STRING = 3                                     # ... and as tg_vec_filter_ex2 reads it
+STR_CMP, STR_LIKE, STR_NOT_LIKE = 0, 1, 2             # tg_str_arg.kind
+# MySQL collation ids of the offloaded string collators (tidbgpu.h; pkg/parser/charset collations)
+COLLATION_BINARY, COLLATION_UTF8MB4_BIN, COLLATION_UTF8_BIN, COLLATION_ASCII_BIN, COLLATION_LATIN1_BIN = 63, 46, 83, 65, 47
+COLLATION_UTF8MB4_0900_BIN = 309
 
 
 class TgColumn(C.Structure):
@@ -54,6 +62,12 @@ class TgFilterItem(C.Structure):
     _fields_ = [("op", C.c_int32), ("lhs_col", C.c_int32), ("rhs_col", C.c_int32),
                 ("is_real", C.c_int32), ("lhs_unsigned", C.c_int32), ("rhs_unsigned", C.c_int32),
                 ("const_i64", C.c_int64), ("const_f64", C.c_double)]
+
+
+class TgStrArg(C.Structure):
+    """tg_str_arg: the constant or LIKE pattern (host bytes), collation id, kind and escape of one STRING filter item"""
+    _fields_ = [("bytes", C.c_void_p), ("len", C.c_int64), ("collation", C.c_int32), ("kind", C.c_int32),
+                ("escape", C.c_int32), ("reserved", C.c_int32)]
 
 
 class TgOtherItem(C.Structure):
@@ -159,6 +173,7 @@ EXPORTED_SYMBOLS = [
     "tg_agg_push_dev", "tg_agg_finish", "tg_agg_next", "tg_agg_close", "tg_agg_result_dev", "tg_agg_get_stats", "tg_agg_get_distinct_stats",
     "tg_vec_compare_int", "tg_vec_compare_real", "tg_vec_arith_int", "tg_vec_arith_real",
     "tg_vec_filter", "tg_vec_compare_decimal", "tg_vec_filter_ex", "tg_decimal_normalize", "tg_topn",
+    "tg_vec_filter_ex2", "tg_vec_compare_string", "tg_vec_like",
     "tg_partition_by_key", "tg_partition_of_key", "tg_partition_exchange", "tg_partition_exchange_cf", "tg_partition_exchange_cf_ex", "tg_partition_exchange_cf_spill", "tg_partition_count",
     "tg_mail_signal", "tg_mail_wait", "tg_peer_copy_regions",
     "tg_ipc_export", "tg_ipc_open", "tg_ipc_close",

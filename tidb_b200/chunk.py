@@ -3,7 +3,7 @@
 Mirrors pkg/util/chunk/column.go:74-82 (Column{length, nullBitmap, offsets, data}) and
 pkg/util/chunk/chunk.go:35-54 (Chunk{columns, sel, ...}): fixed-width little-endian `data`,
 LSB-first `nullBitmap` where bit 1 means NOT NULL, optional selection vector `sel`.
-Only fixed-width columns are modelled (the GPU path's scope).
+Fixed-width columns and var-length string columns (int64 `offsets`, uint8 `data`) are modelled.
 """
 from __future__ import annotations
 
@@ -17,6 +17,7 @@ from . import abi
 
 DECIMAL_CELL = 40   # bytes of one MyDecimal cell in a chunk column
 DECIMAL_DTYPE = np.dtype((np.uint8, DECIMAL_CELL))   # numpy allocates it as (n, 40) uint8
+VARLEN = -1         # elem_len of a var-length column (getFixedLen, codec.go:165)
 
 
 def pack_not_null_bitmap(nulls: np.ndarray) -> np.ndarray:
@@ -31,19 +32,27 @@ def unpack_nulls(bitmap: np.ndarray, n: int) -> np.ndarray:
 
 
 class Column:
-    """One fixed-width chunk.Column.  `data` is a 1-D numpy array of int64/uint64/float64/float32, or an (n, 40) uint8
-    array of MyDecimal cells (a DECIMAL column: types/mydecimal.go:236, copied whole into the column, column.go:41)."""
+    """One chunk.Column.  Fixed width: `data` is a 1-D numpy array of int64/uint64/float64/float32, or an (n, 40) uint8
+    array of MyDecimal cells (a DECIMAL column: types/mydecimal.go:236, copied whole into the column, column.go:41).
+    Var-length (a string column, `offsets` given): `offsets` holds length + 1 int64 values and row r is the bytes
+    data[offsets[r]:offsets[r + 1]] of the uint8 `data` (Column.GetString, column.go:715); elem_len is -1."""
 
-    def __init__(self, data: np.ndarray, nulls: Optional[np.ndarray] = None):
-        data = np.ascontiguousarray(data)
-        if data.ndim == 2 and data.dtype == np.uint8 and data.shape[1] == DECIMAL_CELL:
-            self.elem_len = DECIMAL_CELL
-        elif data.dtype.itemsize in (4, 8):
-            self.elem_len = int(data.dtype.itemsize)
+    def __init__(self, data: np.ndarray, nulls: Optional[np.ndarray] = None, offsets: Optional[np.ndarray] = None):
+        self.offsets: Optional[np.ndarray] = None
+        if offsets is not None:
+            self.offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+            data = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
+            self.elem_len = VARLEN
         else:
-            raise ValueError("only 4/8-byte fixed-width columns and 40-byte DECIMAL cells are modelled")
+            data = np.ascontiguousarray(data)
+            if data.ndim == 2 and data.dtype == np.uint8 and data.shape[1] == DECIMAL_CELL:
+                self.elem_len = DECIMAL_CELL
+            elif data.dtype.itemsize in (4, 8):
+                self.elem_len = int(data.dtype.itemsize)
+            else:
+                raise ValueError("only 4/8-byte fixed-width columns, 40-byte DECIMAL cells and var-length columns are modelled")
         self.data = data
-        self.length = int(data.shape[0])
+        self.length = int(data.shape[0]) if offsets is None else int(self.offsets.shape[0]) - 1
         if nulls is not None:
             nulls = np.asarray(nulls, dtype=bool)
             if nulls.shape[0] != self.length:
@@ -51,6 +60,43 @@ class Column:
             self.null_bitmap: Optional[np.ndarray] = pack_not_null_bitmap(nulls)
         else:
             self.null_bitmap = None
+
+    @classmethod
+    def strings(cls, values: Sequence[Optional[bytes]]) -> "Column":
+        """A var-length column of the given rows; None is NULL (an empty row under the bitmap)."""
+        lens = np.array([0 if v is None else len(v) for v in values], dtype=np.int64)
+        offsets = np.zeros(len(values) + 1, dtype=np.int64)
+        np.cumsum(lens, out=offsets[1:])
+        data = np.frombuffer(b"".join(b"" if v is None else bytes(v) for v in values), dtype=np.uint8).copy()
+        nulls = np.array([v is None for v in values], dtype=bool)
+        return cls(data, nulls if nulls.any() else None, offsets)
+
+    @property
+    def is_varlen(self) -> bool:
+        return self.offsets is not None
+
+    def get_bytes(self, i: int) -> bytes:
+        """Column.GetString: the bytes of row i of a var-length column"""
+        return self.data[self.offsets[i]:self.offsets[i + 1]].tobytes()
+
+    def values(self) -> list:
+        """the rows of a var-length column as bytes, None where NULL"""
+        nl = self.nulls()
+        return [None if nl[i] else self.get_bytes(i) for i in range(self.length)]
+
+    def take(self, idx: np.ndarray) -> "Column":
+        """rows idx (int array) of the column, in that order, as a new dense column (the gather of a sel vector)"""
+        idx = np.asarray(idx, dtype=np.int64)
+        nl = self.nulls()[idx] if self.null_bitmap is not None else None
+        if nl is not None and not nl.any():
+            nl = None
+        if not self.is_varlen:
+            return Column(self.data[idx], nl)
+        starts, ends = self.offsets[idx], self.offsets[idx + 1]
+        offsets = np.zeros(len(idx) + 1, dtype=np.int64)
+        np.cumsum(ends - starts, out=offsets[1:])
+        pos = np.repeat(starts - offsets[:-1], ends - starts) + np.arange(int(offsets[-1]), dtype=np.int64)
+        return Column(self.data[pos], nl, offsets)
 
     # Column.IsNull column.go:225
     def is_null(self, i: int) -> bool:
@@ -67,14 +113,32 @@ class Column:
         s = abi.TgColumn()
         s.length = self.length
         s.null_bitmap = self.null_bitmap.ctypes.data if self.null_bitmap is not None else None
-        s.offsets = None
-        s.data = self.data.ctypes.data if self.length else None
+        s.offsets = self.offsets.ctypes.data if self.is_varlen else None
+        s.data = self.data.ctypes.data if (self.data.size if self.is_varlen else self.length) else None
         s.elem_len = self.elem_len
         return s
 
     def slice(self, lo: int, hi: int) -> "Column":
         nl = self.nulls()[lo:hi] if self.null_bitmap is not None else None
+        if self.is_varlen:
+            o = self.offsets[lo:hi + 1]
+            return Column(self.data[o[0]:o[-1]].copy(), nl, o - o[0])
         return Column(self.data[lo:hi].copy(), nl)
+
+
+def concat_columns(cols: Sequence[Column]) -> Column:
+    """the rows of several columns of one type, one after the other, as one dense column (sel vectors not applied)"""
+    nl = np.concatenate([c.nulls() for c in cols]) if any(c.null_bitmap is not None for c in cols) else None
+    if nl is not None and not nl.any():
+        nl = None
+    if not cols[0].is_varlen:
+        return Column(np.concatenate([c.data for c in cols]), nl)
+    offsets, data, at = [np.zeros(1, dtype=np.int64)], [], 0
+    for c in cols:
+        offsets.append(c.offsets[1:] - c.offsets[0] + at)
+        data.append(c.data[c.offsets[0]:c.offsets[-1]])
+        at += int(c.offsets[-1] - c.offsets[0])
+    return Column(np.concatenate(data) if data else np.zeros(0, np.uint8), nl, np.concatenate(offsets))
 
 
 class Chunk:

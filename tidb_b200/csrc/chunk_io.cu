@@ -70,6 +70,25 @@ int upload_column(int device, cudaStream_t s, const void* src, const uint8_t* bi
   return TG_OK;
 }
 
+int upload_varlen_column(int device, cudaStream_t s, const tg_column& c, DevBuf& offs, DevBuf& data, DevBuf& nulls,
+                         int64_t* h2d_bytes) {
+  const size_t ob = (size_t)(c.length + 1) * 8;
+  const int64_t lo = c.offsets[0];
+  const size_t bytes = (size_t)(c.offsets[c.length] - lo);
+  TG_TRY(offs.ensure(device, ob + 16));
+  TG_CUDA(cudaMemcpyAsync(offs.p, c.offsets, ob, cudaMemcpyHostToDevice, s));
+  TG_TRY(data.ensure(device, bytes + 16));
+  if (bytes) TG_CUDA(cudaMemcpyAsync(data.p, c.data + lo, bytes, cudaMemcpyHostToDevice, s));
+  size_t nb = 0;
+  if (c.null_bitmap) {
+    nb = (size_t)((c.length + 7) / 8);
+    TG_TRY(nulls.ensure(device, nb + 16));
+    if (nb) TG_CUDA(cudaMemcpyAsync(nulls.p, c.null_bitmap, nb, cudaMemcpyHostToDevice, s));
+  }
+  if (h2d_bytes) *h2d_bytes += (int64_t)(ob + bytes + nb);
+  return TG_OK;
+}
+
 int device_view(const tg_chunk* chk, int ncols, const std::vector<char>& needed, const std::vector<int>& elem, DevCols& v) {
   TG_TRY(validate_chunk(ncols, needed, elem, chk));
   if (chk->sel) return fail(TG_ERR_UNSUPPORTED, "device-resident chunks must not carry a sel vector");

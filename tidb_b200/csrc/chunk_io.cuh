@@ -41,6 +41,14 @@ int stage_append(HostStage& st, const std::vector<char>& needed, const std::vect
 int upload_column(int device, cudaStream_t s, const void* src, const uint8_t* bitmap, int64_t rows, int elem,
                   DevBuf& data, DevBuf& nulls, int64_t* h2d_bytes);
 
+// A var-length host column (elem_len -1) → device, on stream s: its length + 1 offsets as they are → offs, the bytes
+// [offsets[0], offsets[length]) → data (data's byte 0 is the byte at offsets[0], so offsets need not start at 0) and its
+// NULL bitmap (when it has one) → nulls; each buffer gets 16 bytes past what is copied.  The caller has checked
+// offsets[0] <= offsets[length]; offsets between them are not read here.  The bytes copied are added to *h2d_bytes when
+// it is given.
+int upload_varlen_column(int device, cudaStream_t s, const tg_column& c, DevBuf& offs, DevBuf& data, DevBuf& nulls,
+                         int64_t* h2d_bytes);
+
 // borrow a validated device-resident chunk (no sel vector) as a column view of its needed columns; no copy
 int device_view(const tg_chunk* chk, int ncols, const std::vector<char>& needed, const std::vector<int>& elem, DevCols& v);
 

@@ -8,32 +8,14 @@
 // 8 B (+8 B) read and 8 B written per row, null bitmaps merged bytewise (Column.MergeNulls column.go:906).
 // The DECIMAL compare and filter (tg_vec_compare_decimal, tg_vec_filter_ex) read 40-byte MyDecimal cells and compare
 // them as MyDecimal.Compare (builtin{LT,LE,GT,GE,EQ,NE}DecimalSig, builtin_compare_vec_generated.go:64, :960, :1184).
-#include <memory>
-#include "common.cuh"
-#include "chunk_io.cuh"
-#include "decimal.cuh"
+#include "vec.cuh"
 
 namespace tg {
-
-struct VArg { const void* data; const uint8_t* nulls; };
 
 // Streaming layout: lane l of a warp owns rows base+l, base+32+l, ... (VEC_ITEMS per thread, all loads issued before
 // use) so every load/store instruction is one fully coalesced 256-byte request; the 32 validity bits of a warp-row are
 // one ballot, written as one aligned 32-bit word of the result bitmap.
 #define VEC_ITEMS 4
-__device__ __forceinline__ bool arg_valid(const VArg& a, int64_t i) { return !a.nulls || bit_not_null(a.nulls, i); }
-
-// write the 32 validity bits of rows [wbase, wbase+32) (wbase % 32 == 0); tail rows are masked off
-__device__ __forceinline__ void store_valid_word(uint8_t* rnulls, int64_t wbase, int64_t n, unsigned bal, int lane) {
-  if (lane == 0 && wbase < n) {
-    int64_t rem = n - wbase;
-    if (rem >= 32) *reinterpret_cast<uint32_t*>(rnulls + (wbase >> 3)) = bal;
-    else {
-      bal &= (1u << rem) - 1u;
-      for (int b = 0; b < (int)((rem + 7) / 8); b++) rnulls[(wbase >> 3) + b] = (uint8_t)(bal >> (8 * b));
-    }
-  }
-}
 
 template <bool REAL>
 __global__ void __launch_bounds__(256)
@@ -190,25 +172,9 @@ k_vec_filter(DevCols cols, DevFilter f, const long long* __restrict__ sel, int64
   if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
 }
 
-// ---- DECIMAL compares and filters: 40-byte MyDecimal cells (decimal.cuh) -------------------------------------------
-// The cell of row i in registers: five 8-byte loads.  Lane l's cell starts 40 * l bytes into its warp's 1280 contiguous
-// bytes, so the warp's five loads cover those bytes and L1 serves the sectors each load leaves to the next (TopN's
-// k_topn_rank_dec reads its cells the same way; see DESIGN.md §6b for the measurement).
-__device__ __forceinline__ void dec_load(const void* data, int64_t i, uint32_t (&c)[10]) {
-  const unsigned long long* p = reinterpret_cast<const unsigned long long*>(data) + i * 5;
-#pragma unroll
-  for (int j = 0; j < 5; j++) {
-    const unsigned long long v = p[j];
-    c[2 * j] = (uint32_t)v; c[2 * j + 1] = (uint32_t)(v >> 32);
-  }
-}
-
+// ---- DECIMAL compares and filters: 40-byte MyDecimal cells (dec_load, DecFilter: vec.cuh) ----------------------------
 // a constant cell in its comparison form (dec_normalize), passed by value
 struct DecConst { uint32_t c[10]; };
-
-// the DECIMAL items of a tg_vec_filter_ex CNF: `op` lhs_col (rhs_col, or the constant k when rhs_col < 0)
-struct DecItem { int32_t op, lhs_col, rhs_col, pad; uint32_t k[10]; };
-struct DecFilter { int32_t n, pad; DecItem items[TG_MAX_FILTER]; };
 
 // tg_vec_compare_decimal: k_vec_compare's warp-row layout over cells.  A NULL row's value is 0 and its cells are not
 // compared; a malformed non-NULL cell of either operand sets *bad (decimal.cuh dec_cell_ok) whatever the other side holds.
@@ -251,9 +217,9 @@ k_vec_compare_dec(int op, VArg a, VArg b, const __grid_constant__ DecConst k, in
   if (malformed) *bad = 1u;
 }
 
-// tg_vec_filter_ex with DECIMAL items: k_vec_filter's row loop; the DECIMAL items are evaluated first and all of them,
-// so every non-NULL cell of their operands is checked at every row evaluated (*bad), then the INT / REAL items by
-// eval_filter, unchanged.
+// tg_vec_filter_ex with DECIMAL items: k_vec_filter's row loop; the DECIMAL items are evaluated first and all of them
+// (eval_dec_items), so every non-NULL cell of their operands is checked at every row evaluated (*bad), then the INT /
+// REAL items by eval_filter, unchanged.
 __global__ void __launch_bounds__(256)
 k_vec_filter_dec(DevCols cols, DevFilter f, const __grid_constant__ DecFilter d, const long long* __restrict__ sel,
                  int64_t nsel, int64_t nphys, uint8_t* __restrict__ selected, unsigned long long* count,
@@ -265,28 +231,7 @@ k_vec_filter_dec(DevCols cols, DevFilter f, const __grid_constant__ DecFilter d,
   const int64_t n = sel ? nsel : nphys;
   for (; i < n; i += stride) {
     const int64_t p = sel ? sel[i] : i;
-    bool s = true;
-    for (int q = 0; q < d.n; q++) {
-      const DecItem& it = d.items[q];
-      uint32_t x[10];
-      dec_load(cols.data[it.lhs_col], p, x);
-      const uint8_t* ln = cols.nulls[it.lhs_col];
-      const bool vx = !ln || bit_not_null(ln, p);
-      malformed |= vx && !dec_cell_ok(x);
-      int c;
-      bool vy = true;
-      if (it.rhs_col >= 0) {
-        uint32_t y[10];
-        dec_load(cols.data[it.rhs_col], p, y);
-        const uint8_t* rn = cols.nulls[it.rhs_col];
-        vy = !rn || bit_not_null(rn, p);
-        malformed |= vy && !dec_cell_ok(y);
-        c = dec_cmp_words(x[0], DecWordsReg{x}, y[0], DecWordsReg{y});
-      } else {
-        c = dec_cmp_words(x[0], DecWordsReg{x}, it.k[0], DecWordsPtr{it.k});
-      }
-      s &= vx && vy && apply_cmp(it.op, c);
-    }
+    bool s = eval_dec_items(d, cols, p, malformed);
     s = s && eval_filter(f, cols, p);
     selected[p] = s ? 1 : 0;
     local += s;
@@ -295,22 +240,6 @@ k_vec_filter_dec(DevCols cols, DevFilter f, const __grid_constant__ DecFilter d,
   if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
   if (malformed) *bad = 1u;
 }
-
-// a column argument made device-resident (copies host buffers when on_device == 0); `elem` is the width the kernel
-// reads: 8, or 40 for DECIMAL cells
-struct ArgDev {
-  DevBuf data, nulls;
-  VArg v{nullptr, nullptr};
-  int load(int device, int on_device, const tg_column* c, cudaStream_t st, int elem = 8) {
-    if (!c) return TG_OK;
-    if (c->elem_len != elem) return fail(TG_ERR_UNSUPPORTED, elem == 8 ? "VecEval kernels take 8-byte columns" : "DECIMAL operands are 40-byte cells");
-    if (on_device) { v.data = c->data; v.nulls = c->null_bitmap; return TG_OK; }
-    TG_TRY(upload_column(device, st, c->data, c->null_bitmap, c->length, elem, data, nulls, nullptr));
-    v.data = data.p;
-    if (c->null_bitmap) v.nulls = nulls.as<uint8_t>();
-    return TG_OK;
-  }
-};
 
 template <typename Launch>
 static int run_binary(int device, int on_device, const tg_column* a, const tg_column* b, void* result, uint8_t* rnulls,
@@ -351,7 +280,7 @@ static int run_binary(int device, int on_device, const tg_column* a, const tg_co
   return TG_OK;
 }
 
-static const char* kMalformedCell =
+const char* const kMalformedCell =
     "malformed DECIMAL cell (digitsInt / digitsFrac < 0, more than 9 words, or a word >= 10^9)";
 
 // the checks of a DECIMAL operand column that need no device
@@ -369,6 +298,40 @@ static int load_dec_const(const uint8_t* cell, uint32_t (&k)[10]) {
   std::memcpy(c, cell, TG_DEC_CELL_BYTES);
   if (!dec_cell_ok(c)) return fail(TG_ERR_INVALID, std::string(kMalformedCell) + " as the constant");
   dec_normalize(c, k);
+  return TG_OK;
+}
+
+int check_filter_items(int on_device, const tg_chunk* chk, const int32_t* col_types, const tg_filter_item* items,
+                       int32_t n_items, const uint8_t* dec_consts, const std::vector<char>& skip, DecFilter& d,
+                       DevFilter& f, std::vector<char>& needed) {
+  const int64_t nphys = chk->cols[0].length;
+  for (int i = 0; i < n_items; i++) {
+    if (skip[i]) continue;
+    const tg_filter_item& it = items[i];
+    if (it.lhs_col < 0 || it.lhs_col >= chk->ncols || it.rhs_col >= chk->ncols) return fail(TG_ERR_INVALID, "filter column out of range");
+    if (it.op < TG_CMP_LT || it.op > TG_CMP_NE) return fail(TG_ERR_INVALID, "unknown comparison");
+    if (it.is_real < TG_FILTER_INT || it.is_real > TG_FILTER_DECIMAL) return fail(TG_ERR_INVALID, "unknown filter item kind (is_real)");
+    const bool dec = it.is_real == TG_FILTER_DECIMAL;
+    for (int side = 0; side < 2; side++) {
+      const int c = side ? it.rhs_col : it.lhs_col;
+      if (c < 0) continue;
+      const tg_column& col = chk->cols[c];
+      const bool dec_col = col_types[c] == TG_TYPE_NEWDECIMAL;
+      if (dec && !dec_col) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL filter item compares DECIMAL columns only (the planner casts the other operand)");
+      if (!dec && dec_col) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL column in an INT / REAL filter item");
+      if (dec) TG_TRY(check_dec_column(col, on_device));
+      else if (col.elem_len != 8) return fail(TG_ERR_UNSUPPORTED, "VecEval kernels take 8-byte columns");
+      if (col.length != nphys) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
+      needed[c] = 1;
+    }
+    if (dec) {
+      DecItem& di = d.items[d.n++];
+      di.op = it.op; di.lhs_col = it.lhs_col; di.rhs_col = it.rhs_col;
+      if (it.rhs_col < 0) TG_TRY(load_dec_const(dec_consts ? dec_consts + (size_t)TG_DEC_CELL_BYTES * i : nullptr, di.k));
+    } else {
+      f.items[f.n++] = it;
+    }
+  }
   return TG_OK;
 }
 
@@ -523,37 +486,12 @@ int tg_vec_filter_ex(int device, int on_device, const tg_chunk* chk, const int32
   if (n_items < 0 || n_items > TG_MAX_FILTER) return fail(TG_ERR_UNSUPPORTED, "at most 8 CNF filter items are offloaded");
   if (n_items > 0 && !items) return fail(TG_ERR_INVALID, "items is NULL");
   if (chk->ncols <= 0 || chk->ncols > TG_MAX_COLS || !chk->cols) return fail(TG_ERR_UNSUPPORTED, "chunk must have 1..16 columns");
-  const int64_t nphys = chk->cols[0].length;
   DecFilter d{};
   DevFilter f{};
   std::vector<char> needed(chk->ncols, 0);
-  for (int i = 0; i < n_items; i++) {
-    const tg_filter_item& it = items[i];
-    if (it.lhs_col < 0 || it.lhs_col >= chk->ncols || it.rhs_col >= chk->ncols) return fail(TG_ERR_INVALID, "filter column out of range");
-    if (it.op < TG_CMP_LT || it.op > TG_CMP_NE) return fail(TG_ERR_INVALID, "unknown comparison");
-    if (it.is_real < TG_FILTER_INT || it.is_real > TG_FILTER_DECIMAL) return fail(TG_ERR_INVALID, "unknown filter item kind (is_real)");
-    const bool dec = it.is_real == TG_FILTER_DECIMAL;
-    for (int side = 0; side < 2; side++) {
-      const int c = side ? it.rhs_col : it.lhs_col;
-      if (c < 0) continue;
-      const tg_column& col = chk->cols[c];
-      const bool dec_col = col_types[c] == TG_TYPE_NEWDECIMAL;
-      if (dec && !dec_col) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL filter item compares DECIMAL columns only (the planner casts the other operand)");
-      if (!dec && dec_col) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL column in an INT / REAL filter item");
-      if (dec) TG_TRY(check_dec_column(col, on_device));
-      else if (col.elem_len != 8) return fail(TG_ERR_UNSUPPORTED, "VecEval kernels take 8-byte columns");
-      if (col.length != nphys) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
-      needed[c] = 1;
-    }
-    if (dec) {
-      DecItem& di = d.items[d.n++];
-      di.op = it.op; di.lhs_col = it.lhs_col; di.rhs_col = it.rhs_col;
-      if (it.rhs_col < 0) TG_TRY(load_dec_const(dec_consts ? dec_consts + (size_t)TG_DEC_CELL_BYTES * i : nullptr, di.k));
-    } else {
-      f.items[f.n++] = it;
-    }
-  }
+  TG_TRY(check_filter_items(on_device, chk, col_types, items, n_items, dec_consts, std::vector<char>(n_items, 0), d, f, needed));
   if (d.n == 0) return tg_vec_filter(device, on_device, chk, items, n_items, selected, n_selected, stream);
+  const int64_t nphys = chk->cols[0].length;
   TG_TRY(require_device("VecEval"));
   DeviceGuard g(device);
   if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");

@@ -17,13 +17,16 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 from . import abi
-from .chunk import DECIMAL_DTYPE, Chunk, Column, MutChunk
+from .chunk import DECIMAL_DTYPE, Chunk, Column, MutChunk, concat_columns
 from .plan import AggPlan, FieldType, JoinPlan
 
 MAX_CHUNK_SIZE = 1024  # tidb_max_chunk_size default (vardef/tidb_vars.go:1464)
 
 
 def np_dtype_of(t: FieldType):
+    """the numpy dtype of a fixed-width column's data; a string column's data is its uint8 bytes (with int64 offsets)"""
+    if t.tp in abi.STRING_TYPES:
+        return np.uint8
     if t.tp == abi.TYPE_DOUBLE:
         return np.float64
     if t.tp == abi.TYPE_FLOAT:
@@ -52,7 +55,8 @@ class Executor:
             c.close()
 
     def empty_chunk(self) -> Chunk:
-        return Chunk([Column(np.zeros(0, dtype=np_dtype_of(t))) for t in self.schema])
+        return Chunk([Column.strings([]) if t.tp in abi.STRING_TYPES else Column(np.zeros(0, dtype=np_dtype_of(t)))
+                      for t in self.schema])
 
 
 class MockDataSource(Executor):
@@ -246,6 +250,9 @@ def _concat_chunks(chunks: Sequence[Chunk]) -> Chunk:
     """child chunks -> one dense chunk (sel vectors applied), the batch a device call works on"""
     cols = []
     for c in range(chunks[0].num_cols()):
+        if chunks[0].columns[c].is_varlen:
+            cols.append(concat_columns([ck.columns[c] if ck.sel is None else ck.columns[c].take(ck.sel) for ck in chunks]))
+            continue
         vals, nls, any_null = [], [], False
         for ck in chunks:
             col = ck.columns[c]
@@ -258,11 +265,30 @@ def _concat_chunks(chunks: Sequence[Chunk]) -> Chunk:
     return Chunk(cols)
 
 
+def _rows(c: Column, lo: int, hi: int) -> Column:
+    """rows [lo, hi) of a column handed on by Next"""
+    if c.is_varlen:
+        return c.slice(lo, hi)
+    return Column(c.data[lo:hi], c.nulls()[lo:hi] if c.nulls().any() else None)
+
+
+def _split_head(pending: List[Chunk], required_rows: int) -> Chunk:
+    """the next at most required_rows rows of the pending chunks"""
+    head = pending[0]
+    if head.num_rows() <= required_rows:
+        pending.pop(0)
+        return head
+    n = head.num_rows()
+    pending[0] = Chunk([_rows(c, required_rows, n) for c in head.columns])
+    return Chunk([_rows(c, 0, required_rows) for c in head.columns])
+
+
 class SelectionExec(Executor):
     """GPU replacement of executor.SelectionExec (pkg/executor/select.go:746-785): pulls child chunks, evaluates the
     CNF filter list with expression.VectorizedFilter semantics (chunk_executor.go:413: a row is selected iff every item is
-    non-NULL true) on the device (tg_vec_filter; tg_vec_filter_ex when an item compares DECIMAL cells) and hands the
-    selected rows on, at most `required_rows` per Next.  Child chunks are batched (`batch_rows`) so that one launch filters
+    non-NULL true) on the device (tg_vec_filter; tg_vec_filter_ex when an item compares DECIMAL cells; tg_vec_filter_ex2
+    when an item compares or matches strings) and hands the selected rows on, at most `required_rows` per Next; string
+    payload columns are handed on bit for bit.  Child chunks are batched (`batch_rows`) so that one launch filters
     many 1024-row chunks."""
 
     def __init__(self, child: Executor, filters: Sequence, device: int = 0, batch_rows: int = 64 * MAX_CHUNK_SIZE):
@@ -281,7 +307,7 @@ class SelectionExec(Executor):
         self._pending, self._eof = [], False
 
     def _fill(self) -> None:
-        from .plan import dec_const_array, filter_array
+        from .plan import dec_const_array, filter_array, str_arg_array
         batch, rows = [], 0
         while rows < self.batch_rows:
             chk = self.children[0].next(MAX_CHUNK_SIZE)
@@ -297,7 +323,12 @@ class SelectionExec(Executor):
         nsel = C.c_int64(0)
         cs = dense.to_struct()
         arr = filter_array(self.filters)
-        if any(f.is_decimal for f in self.filters):
+        if any(f.is_string for f in self.filters):
+            # STRING items read var-length columns: tg_vec_filter_ex2, with one tg_str_arg per item
+            tps = (C.c_int32 * len(self.schema))(*[t.tp for t in self.schema])
+            abi.check(self._lib.tg_vec_filter_ex2(self.device, 0, C.byref(cs), tps, arr, len(self.filters), dec_const_array(self.filters),
+                                                  str_arg_array(self.filters), selected.ctypes.data_as(C.c_void_p), C.byref(nsel), None))
+        elif any(f.is_decimal for f in self.filters):
             # DECIMAL items compare MyDecimal cells: tg_vec_filter_ex, told the child schema's types
             tps = (C.c_int32 * len(self.schema))(*[t.tp for t in self.schema])
             consts = dec_const_array(self.filters)
@@ -309,27 +340,23 @@ class SelectionExec(Executor):
         keep = selected.astype(bool)
         assert int(keep.sum()) == nsel.value
         if nsel.value:
-            self._pending.append(Chunk([Column(c.data[keep], c.nulls()[keep] if c.nulls().any() else None) for c in dense.columns]))
+            rows = np.flatnonzero(keep)
+            self._pending.append(Chunk([c.take(rows) if c.is_varlen else Column(c.data[keep], c.nulls()[keep] if c.nulls().any() else None)
+                                        for c in dense.columns]))
 
     def next(self, required_rows: int = MAX_CHUNK_SIZE) -> Chunk:
         while not self._pending and not self._eof:
             self._fill()
         if not self._pending:
             return self.empty_chunk()
-        head = self._pending[0]
-        if head.num_rows() <= required_rows:
-            self._pending.pop(0)
-            return head
-        out = Chunk([Column(c.data[:required_rows], c.nulls()[:required_rows] if c.nulls().any() else None) for c in head.columns])
-        self._pending[0] = Chunk([Column(c.data[required_rows:], c.nulls()[required_rows:] if c.nulls().any() else None) for c in head.columns])
-        return out
+        return _split_head(self._pending, required_rows)
 
 
 class ProjectionExec(Executor):
     """GPU replacement of executor.ProjectionExec (pkg/executor/projection.go:450-483 -> EvaluatorSuite.Run,
     expression/evaluator.go:128): plain column references are passed through (the reference SWAPS them, ColumnSwapHelper),
     scalar functions are evaluated column-at-a-time by the VecEval kernels (tg_vec_arith_* / tg_vec_compare_*, DECIMAL
-    comparisons by tg_vec_compare_decimal), constants
+    comparisons by tg_vec_compare_decimal, string comparisons by tg_vec_compare_string, LIKE by tg_vec_like), constants
     are scalars (the reference materialises them as columns, vectorized.go:23).  Errors keep the reference's meaning:
     overflow on a non-NULL row fails the Next call (types.ErrOverflow <-> TG_ERR_OVERFLOW)."""
 
@@ -370,7 +397,19 @@ class ProjectionExec(Executor):
         pb = C.byref(sb) if sb is not None else None
         rp, np_ = res.ctypes.data_as(C.c_void_p), nulls.ctypes.data_as(C.c_void_p)
         k = b.value if isinstance(b, Const) else 0
-        if e.is_decimal:
+        if e.kind == "like" or e.is_string:
+            if not isinstance(b, Const) and e.kind == "like":
+                raise abi.TgError(abi.TG_ERR_UNSUPPORTED, "LIKE with a pattern from a column is not offloaded")
+            if isinstance(b, Const) and b.bytes_value is None:
+                raise abi.TgError(abi.TG_ERR_UNSUPPORTED, "a string comparison takes a string constant (the planner casts it)")
+            kb = bytes(b.bytes_value) if isinstance(b, Const) else b""
+            kbuf = (C.c_uint8 * max(len(kb), 1)).from_buffer_copy(kb.ljust(1, b"\0"))
+            kp = C.cast(kbuf, C.c_void_p) if kb else None
+            if e.kind == "like":
+                rc = self._lib.tg_vec_like(self.device, 0, e.collation, C.byref(sa), kp, C.c_int64(len(kb)), e.escape, rp, np_, None)
+            else:
+                rc = self._lib.tg_vec_compare_string(self.device, 0, e.op, e.collation, C.byref(sa), pb, kp, C.c_int64(len(kb)), rp, np_, None)
+        elif e.is_decimal:
             if e.kind != "cmp":
                 raise abi.TgError(abi.TG_ERR_UNSUPPORTED, "DECIMAL arithmetic is not offloaded to the VecEval kernels")
             cell = None
@@ -406,13 +445,7 @@ class ProjectionExec(Executor):
                 self._pending.append(Chunk([self._eval(e, dense) for e in self.exprs]))
         if not self._pending:
             return self.empty_chunk()
-        head = self._pending[0]
-        if head.num_rows() <= required_rows:
-            self._pending.pop(0)
-            return head
-        out = Chunk([Column(c.data[:required_rows], c.nulls()[:required_rows] if c.nulls().any() else None) for c in head.columns])
-        self._pending[0] = Chunk([Column(c.data[required_rows:], c.nulls()[required_rows:] if c.nulls().any() else None) for c in head.columns])
-        return out
+        return _split_head(self._pending, required_rows)
 
 
 class TopNExec(Executor):

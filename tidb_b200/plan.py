@@ -47,7 +47,10 @@ def _u32(vals: Sequence[int]):
 @dataclass
 class FilterItem:
     """One CNF item `col OP const` / `col OP col` (tg_filter_item).  is_decimal: a DECIMAL item of tg_vec_filter_ex over
-    40-byte MyDecimal cell columns, whose constant is the 40-byte cell const_cell (Constant.Value.GetMysqlDecimal())."""
+    40-byte MyDecimal cell columns, whose constant is the 40-byte cell const_cell (Constant.Value.GetMysqlDecimal()).
+    is_string: a STRING item of tg_vec_filter_ex2 over var-length string columns: str_kind abi.STR_CMP compares with
+    rhs_col or the constant const_bytes, abi.STR_LIKE / STR_NOT_LIKE match the pattern const_bytes with `escape`, under
+    the MySQL collation id `collation`."""
     op: int
     lhs_col: int
     rhs_col: int = -1
@@ -58,11 +61,17 @@ class FilterItem:
     rhs_unsigned: bool = False
     is_decimal: bool = False
     const_cell: Optional[bytes] = None
+    is_string: bool = False
+    const_bytes: Optional[bytes] = None
+    collation: int = abi.COLLATION_UTF8MB4_BIN
+    str_kind: int = abi.STR_CMP
+    escape: int = ord("\\")
 
     def to_struct(self) -> abi.TgFilterItem:
         s = abi.TgFilterItem()
         s.op, s.lhs_col, s.rhs_col = self.op, self.lhs_col, self.rhs_col
-        s.is_real, s.lhs_unsigned = (abi.FILTER_DECIMAL if self.is_decimal else int(self.is_real)), int(self.lhs_unsigned)
+        kind = abi.FILTER_STRING if self.is_string else (abi.FILTER_DECIMAL if self.is_decimal else int(self.is_real))
+        s.is_real, s.lhs_unsigned = kind, int(self.lhs_unsigned)
         s.rhs_unsigned = int(self.rhs_unsigned)
         s.const_i64, s.const_f64 = self.const_i64, self.const_f64
         return s
@@ -86,6 +95,24 @@ def dec_const_array(items: Sequence[FilterItem]):
             assert len(it.const_cell) == 40, "a DECIMAL constant is one 40-byte MyDecimal cell"
             buf[40 * i:40 * i + 40] = bytes(it.const_cell)
     return (C.c_uint8 * len(buf)).from_buffer(buf)
+
+
+def str_arg_array(items: Sequence[FilterItem]):
+    """tg_vec_filter_ex2's str_args: one tg_str_arg per item (zeros for the items that are not STRING); None when no item
+    is STRING.  The constant and pattern buffers are kept alive on the array (`_keep`)."""
+    if not any(it.is_string for it in items):
+        return None
+    arr = (abi.TgStrArg * len(items))()
+    arr._keep = []
+    for i, it in enumerate(items):
+        if not it.is_string:
+            continue
+        b = bytes(it.const_bytes or b"")
+        buf = (C.c_uint8 * max(len(b), 1)).from_buffer_copy(b.ljust(1, b"\0"))
+        arr._keep.append(buf)
+        arr[i].bytes = C.cast(buf, C.c_void_p) if b else None
+        arr[i].len, arr[i].collation, arr[i].kind, arr[i].escape = len(b), it.collation, it.str_kind, it.escape
+    return arr
 
 
 @dataclass
@@ -260,12 +287,16 @@ class ColRef(Expr):
 @dataclass
 class Const(Expr):
     """expression.Constant: handed to the kernels as a scalar (the reference materialises a column, vectorized.go:23).
-    cell: a DECIMAL constant, its 40-byte MyDecimal cell (value is then not used)."""
+    cell: a DECIMAL constant, its 40-byte MyDecimal cell (value is then not used).  bytes_value: a string constant (or
+    a LIKE pattern), its bytes."""
     value: float = 0
     is_real: bool = False
     cell: Optional[bytes] = None
+    bytes_value: Optional[bytes] = None
 
     def ret_type(self, schema):
+        if self.bytes_value is not None:
+            return FieldType(abi.TYPE_VARSTRING, abi.FLAG_NOT_NULL)
         if self.cell is not None:
             return FieldType(abi.TYPE_NEWDECIMAL, abi.FLAG_NOT_NULL)
         return FieldType(abi.TYPE_DOUBLE if self.is_real else abi.TYPE_LONGLONG, abi.FLAG_NOT_NULL)
@@ -275,7 +306,10 @@ class Const(Expr):
 class ScalarFunc(Expr):
     """builtinArithmetic{Plus,Minus,Multiply}{Int,Real}Sig / builtin{LT,LE,GT,GE,EQ,NE}{Int,Real,Decimal}Sig over two
     arguments (kind "arith": op = abi.ARITH_*, kind "cmp": op = abi.CMP_*); the right argument may be a Const.
-    is_decimal (kind "cmp" only): both arguments are DECIMAL (cell columns; a Const with a cell)."""
+    is_decimal (kind "cmp" only): both arguments are DECIMAL (cell columns; a Const with a cell).
+    is_string (kind "cmp"): both arguments are strings (var-length columns; a Const with bytes_value), compared under the
+    MySQL collation id `collation`.  Kind "like": builtinLikeSig, the first argument LIKE the Const pattern (bytes_value)
+    with `escape`, under `collation`."""
     kind: str
     op: int
     args: Tuple[Expr, Expr]
@@ -283,6 +317,9 @@ class ScalarFunc(Expr):
     a_unsigned: bool = False
     b_unsigned: bool = False
     is_decimal: bool = False
+    is_string: bool = False
+    collation: int = abi.COLLATION_UTF8MB4_BIN
+    escape: int = ord("\\")
 
     def ret_type(self, schema):
         if self.kind == "arith" and self.is_real:
