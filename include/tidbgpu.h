@@ -500,6 +500,11 @@ int tg_agg_get_distinct_stats(tg_agg* a, tg_agg_distinct_stats* out);
  * VecEval* kernels             replace pkg/expression builtin_*_vec.go signatures
  * All operate on one column-at-a-time over host or device buffers (`on_device` flag).
  * Result null bitmap = MergeNulls of the argument bitmaps (pkg/util/chunk/column.go:906).
+ * Every call below checks its arguments (descriptors, types, elem_len, alignment, items, constants, collations, host
+ * offsets bounds) before it looks for the device: a bad argument gets the same status on a machine without a device.
+ * A failed call with host buffers (on_device == 0) writes nothing: no result value, no bitmap byte, no `selected` byte,
+ * and *n_selected is left unset.  With device buffers, `result` / `result_nulls` / `selected` may have been written;
+ * *n_selected is not.
  * ------------------------------------------------------------------------------------------- */
 enum { TG_ARITH_PLUS = 0, TG_ARITH_MINUS = 1, TG_ARITH_MUL = 2 };
 
@@ -542,11 +547,7 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk,
  *     physical row), whatever the other items and the other operand give; one malformed cell fails the call with
  *     TG_ERR_INVALID.  Cells under NULL and outside `sel` are never read as values.  A malformed constant cell, a missing
  *     one, or an operand column whose elem_len is not 40 is TG_ERR_INVALID.
- *   A failed call with host buffers (on_device == 0) writes nothing: no result value, no bitmap byte, no `selected` byte
- *     and no *n_selected.  With device buffers, `result` / `result_nulls` / `selected` may have been written; *n_selected
- *     is not.
- *   These argument checks (descriptor, types, elem_len, alignment, constant cells) answer before the device is looked
- *     for.  Device-resident DECIMAL columns must be 8-byte aligned. */
+ *   Device-resident DECIMAL columns must be 8-byte aligned. */
 /* tg_filter_item.is_real values understood by tg_vec_filter_ex */
 enum { TG_FILTER_INT = 0, TG_FILTER_REAL = 1, TG_FILTER_DECIMAL = 2 };
 
@@ -586,8 +587,7 @@ int tg_decimal_normalize(const uint8_t* cell, uint8_t* out);
  *   Offsets: checked at every row the call evaluates, NULL or not (the rows in `sel` when the chunk has one, else every
  *     physical row).  A row is bad when offsets[r] > offsets[r+1] or either value lies outside
  *     [offsets[0], offsets[length]]; a bad row fails the call with TG_ERR_INVALID.  With host columns,
- *     offsets[length] < offsets[0] is TG_ERR_INVALID before any device work.  A failed call with host buffers writes
- *     nothing (no result, no bitmap byte, no `selected` byte, no *n_selected), as for malformed DECIMAL cells.
+ *     offsets[length] < offsets[0] is TG_ERR_INVALID.
  *   Collation: the MySQL collation id of the comparison (the builtin's collation), one of three collator behaviours
  *     (pkg/util/collate/bin.go, collate.go newCollatorIDMap):
  *       63 binary                                          compare: strings.Compare on the bytes; LIKE: over bytes
@@ -607,8 +607,7 @@ int tg_decimal_normalize(const uint8_t* cell, uint8_t* out);
  *     []rune(s): every byte that does not start a valid UTF-8 sequence (truncated, overlong, surrogate, above U+10FFFF)
  *     is one U+FFFD, so such bytes and a valid U+FFFD match each other, and the escape is the rune e (0xE9 is 'é', not
  *     the byte 0xE9).  A pattern from a column or a non-constant escape is not offloaded (the shim keeps the CPU path).
- *   The constant and the pattern have no length cap.  These argument checks (types, collation ids, kind, escape, host
- *     offsets bounds) answer before the device is looked for. */
+ *   The constant and the pattern have no length cap. */
 enum { TG_FILTER_STRING = 3 };   /* tg_filter_item.is_real value understood by tg_vec_filter_ex2 */
 enum { TG_STR_CMP = 0, TG_STR_LIKE = 1, TG_STR_NOT_LIKE = 2 };
 typedef struct tg_str_arg {

@@ -5,9 +5,11 @@ import ctypes as C
 import os
 import re
 
+import numpy as np
 import pytest
 
 from tidb_b200 import abi
+from tidb_b200.chunk import Column
 from tidb_b200.plan import AggFunc, AggPlan, FieldType, JoinPlan
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -89,6 +91,23 @@ def test_no_cpu_fallback_without_device(lib):
     assert b"no CPU fallback" in lib.tg_last_error()
     p = C.c_void_p()
     assert lib.tg_dev_alloc(0, C.c_size_t(16), C.byref(p)) == abi.TG_ERR_CUDA
+
+
+def test_vec_compare_and_arith_refuse_4_byte_operands_without_a_device(lib):
+    # a 4-byte operand, as a or as b, is TG_ERR_UNSUPPORTED on every machine: the argument checks answer before the
+    # device is looked for, and a refused call writes nothing
+    wide, narrow = Column(np.arange(5, dtype=np.int64)).to_struct(), Column(np.arange(5, dtype=np.int32)).to_struct()
+    assert narrow.elem_len == 4
+    for name, const in (("tg_vec_compare_int", C.c_int64(1)), ("tg_vec_arith_int", C.c_int64(1)),
+                        ("tg_vec_compare_real", C.c_double(1.0)), ("tg_vec_arith_real", C.c_double(1.0))):
+        signs = (0, 0) if name.endswith("_int") else ()
+        for a, b in ((narrow, None), (narrow, wide), (wide, narrow)):
+            res, nulls = np.full(5, 0x5A5A5A5A, np.int64), np.full(1, 0xA5, np.uint8)
+            rc = getattr(lib, name)(0, 0, abi.CMP_LT, *signs, C.byref(a), None if b is None else C.byref(b), const,
+                                    res.ctypes.data_as(C.c_void_p), nulls.ctypes.data_as(C.c_void_p), None)
+            assert rc == abi.TG_ERR_UNSUPPORTED, (name, a is narrow, b is narrow)
+            assert b"8-byte columns" in lib.tg_last_error()
+            assert (res == 0x5A5A5A5A).all() and nulls[0] == 0xA5
 
 
 def test_partition_function_is_stable(lib):

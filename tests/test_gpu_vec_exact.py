@@ -210,8 +210,9 @@ def test_vec_arith_int_exact(pools, n):
                     b2, bn2 = (None, None) if b is None else (b.copy(), bn.copy())
                     if b2 is not None:
                         b2[pos], bn2[pos] = pool[1][j], False
-                    rc, _, _ = call_binary("tg_vec_arith_int", op, signs, a2, an2, b2, bn2, k)
+                    rc, res2, bm2 = call_binary("tg_vec_arith_int", op, signs, a2, an2, b2, bn2, k)
                     assert rc == abi.TG_ERR_OVERFLOW, (what, pos)
+                    assert (res2 == 0x5A5A5A5A).all() and (bm2 == 0xA5).all(), (what, pos)   # host buffers untouched
 
 
 @pytest.mark.parametrize("n", SIZES)
@@ -241,7 +242,9 @@ def test_vec_arith_real_exact(pools, n):
                 b2, bn2 = (None, None) if b is None else (b.copy(), bn.copy())
                 if b2 is not None:
                     b2[pos], bn2[pos] = pool[1][j], False
-                assert call_binary("tg_vec_arith_real", op, None, a2, an2, b2, bn2, k)[0] == abi.TG_ERR_OVERFLOW, what
+                rc, res2, bm2 = call_binary("tg_vec_arith_real", op, None, a2, an2, b2, bn2, k)
+                assert rc == abi.TG_ERR_OVERFLOW, what
+                assert (res2.view(np.int64) == 0x5A5A5A5A).all() and (bm2 == 0xA5).all(), what   # host buffers untouched
 
 
 def test_vec_real_signed_zero_nan_and_inf_times_zero():

@@ -241,46 +241,7 @@ k_vec_filter_dec(DevCols cols, DevFilter f, const __grid_constant__ DecFilter d,
   if (malformed) *bad = 1u;
 }
 
-template <typename Launch>
-static int run_binary(int device, int on_device, const tg_column* a, const tg_column* b, void* result, uint8_t* rnulls,
-                      void* stream, bool has_overflow, Launch launch) {
-  if (!a || !result || !rnulls) return fail(TG_ERR_INVALID, "a / result / result_nulls is NULL");
-  if (b && b->length != a->length) return fail(TG_ERR_INVALID, "argument columns have different lengths");
-  TG_TRY(require_device("VecEval"));
-  DeviceGuard g(device);
-  if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
-  cudaStream_t st = (cudaStream_t)stream;
-  int64_t n = a->length;
-  ArgDev da, db;
-  TG_TRY(da.load(device, on_device, a, st));
-  TG_TRY(db.load(device, on_device, b, st));
-  DevBuf dres, dnul;
-  static std::mutex flag_mu;
-  static int* ovf_flag[16];   // one overflow flag per device, allocated once and intentionally never freed
-  std::lock_guard<std::mutex> flag_lock(flag_mu);   // VecEval calls are serialised per process
-  int*& dovf = ovf_flag[device & 15];
-  void* res_dev = result; uint8_t* nul_dev = rnulls;
-  size_t nb = (size_t)((n + 7) / 8);
-  if (!on_device) {
-    TG_TRY(dres.ensure(device, (size_t)n * 8 + 16)); TG_TRY(dnul.ensure(device, nb + 16));
-    res_dev = dres.p; nul_dev = dnul.as<uint8_t>();
-  }
-  if (!dovf) TG_CUDA(cudaMalloc(reinterpret_cast<void**>(&dovf), 16));
-  TG_CUDA(cudaMemsetAsync(dovf, 0, 4, st));
-  if (n > 0) launch(grid_size(device_sm_count(device), (n + VEC_ITEMS - 1) / VEC_ITEMS, 256, 8), st, da.v, db.v, n, res_dev, nul_dev, dovf);
-  int ovf = 0;
-  if (has_overflow) TG_CUDA(cudaMemcpyAsync(&ovf, dovf, 4, cudaMemcpyDeviceToHost, st));
-  if (!on_device && n > 0) {
-    TG_CUDA(cudaMemcpyAsync(result, res_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaMemcpyAsync(rnulls, nul_dev, nb, cudaMemcpyDeviceToHost, st));
-  }
-  TG_CUDA(cudaStreamSynchronize(st));
-  TG_CUDA(cudaGetLastError());
-  if (ovf) return fail(TG_ERR_OVERFLOW, "ErrOverflow: value is out of range in arithmetic VecEval kernel");
-  return TG_OK;
-}
-
-const char* const kMalformedCell =
+static const char* const kMalformedCell =
     "malformed DECIMAL cell (digitsInt / digitsFrac < 0, more than 9 words, or a word >= 10^9)";
 
 // the checks of a DECIMAL operand column that need no device
@@ -335,6 +296,139 @@ int check_filter_items(int on_device, const tg_chunk* chk, const int32_t* col_ty
   return TG_OK;
 }
 
+static const char* const kBadOffsets =
+    "malformed string offsets: offsets[r] > offsets[r+1], or an offset outside [offsets[0], offsets[length]], at a row the call evaluates";
+
+static int fault_status(VecFault f) {
+  if (f == FAULT_OVERFLOW) return fail(TG_ERR_OVERFLOW, "ErrOverflow: value is out of range in arithmetic VecEval kernel");
+  return fail(TG_ERR_INVALID, f == FAULT_BAD_CELL ? kMalformedCell : kBadOffsets);
+}
+
+// one VecFlags block per device, allocated on first use and never freed; its mutex holds the block from the zeroing
+// through the read-back of one call
+struct FlagSlot { std::mutex mu; VecFlags* p = nullptr; };
+static FlagSlot& flag_slot(int device, int ndev) {
+  static std::unique_ptr<FlagSlot[]> slots(new FlagSlot[ndev]);
+  return slots[device];
+}
+
+int run_vec(int device, int on_device, const tg_chunk* chk, const std::vector<char>& needed, uint8_t* selected,
+            int64_t* n_selected, void* result, uint8_t* rnulls, void* stream, std::initializer_list<VecFault> faults,
+            const VecKernel& launch) {
+  int ndev = 0;
+  TG_TRY(require_device("VecEval", &ndev));
+  DeviceGuard g(device);
+  if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
+  const bool filter = selected != nullptr;
+  const int64_t nphys = chk->cols[0].length;
+  const size_t nb = (size_t)((nphys + 7) / 8);
+  VecLaunch v{};
+  v.device = device; v.nsm = device_sm_count(device); v.ncols = chk->ncols; v.st = (cudaStream_t)stream;
+  v.sel = reinterpret_cast<const long long*>(chk->sel); v.nsel = chk->nsel; v.nphys = nphys;
+  v.n = chk->sel ? chk->nsel : nphys;
+  v.selected = selected; v.result = static_cast<long long*>(result); v.rnulls = rnulls;
+  // the needed columns: borrowed when device-resident, else uploaded (a var-length one from its offsets[0])
+  DevBuf offs[TG_MAX_COLS], data[TG_MAX_COLS], nulls[TG_MAX_COLS];
+  for (int c = 0; c < chk->ncols; c++) {
+    const tg_column& col = chk->cols[c];
+    v.cols.elem_len[c] = col.elem_len;
+    if (!needed[c]) continue;
+    const bool varlen = col.elem_len < 0;
+    if (on_device) {
+      if (varlen) { v.sc.offs[c] = col.offsets; v.sc.data[c] = col.data; }
+      else v.cols.data[c] = col.data;
+      v.cols.nulls[c] = col.null_bitmap;
+      continue;
+    }
+    if (varlen) {
+      TG_TRY(upload_varlen_column(device, v.st, col, offs[c], data[c], nulls[c], nullptr));
+      v.sc.offs[c] = offs[c].as<int64_t>(); v.sc.data[c] = data[c].as<uint8_t>(); v.sc.base[c] = col.offsets[0];
+    } else {
+      TG_TRY(upload_column(device, v.st, col.data, col.null_bitmap, col.length, col.elem_len, data[c], nulls[c], nullptr));
+      v.cols.data[c] = data[c].p;
+    }
+    if (col.null_bitmap) v.cols.nulls[c] = nulls[c].as<uint8_t>();
+  }
+  // a host chunk: its sel vector goes up, and the outputs are computed into device scratch
+  DevBuf dsel, dout, dnul;
+  if (!on_device) {
+    if (chk->sel) {
+      TG_TRY(dsel.ensure(device, (size_t)chk->nsel * 8 + 16));
+      TG_CUDA(cudaMemcpyAsync(dsel.p, chk->sel, (size_t)chk->nsel * 8, cudaMemcpyHostToDevice, v.st));
+      v.sel = dsel.as<long long>();
+    }
+    if (filter) {
+      TG_TRY(dout.ensure(device, (size_t)nphys + 16));
+      v.selected = dout.as<uint8_t>();
+    } else {
+      TG_TRY(dout.ensure(device, (size_t)nphys * 8 + 16)); TG_TRY(dnul.ensure(device, nb + 16));
+      v.result = dout.as<long long>(); v.rnulls = dnul.as<uint8_t>();
+    }
+  }
+  VecFlags flags{};
+  std::unique_lock<std::mutex> flag_lock;
+  if (filter || faults.size()) {
+    FlagSlot& slot = flag_slot(device, ndev);
+    flag_lock = std::unique_lock<std::mutex>(slot.mu);
+    if (!slot.p) TG_CUDA(cudaMalloc(reinterpret_cast<void**>(&slot.p), sizeof(VecFlags)));
+    v.flags = slot.p;
+    TG_CUDA(cudaMemsetAsync(v.flags, 0, sizeof(VecFlags), v.st));
+  }
+  if (filter) TG_CUDA(cudaMemsetAsync(v.selected, 0, (size_t)nphys, v.st));
+  if (v.n > 0) TG_TRY(launch(v));
+  if (v.flags) TG_CUDA(cudaMemcpyAsync(&flags, v.flags, sizeof(VecFlags), cudaMemcpyDeviceToHost, v.st));
+  TG_CUDA(cudaStreamSynchronize(v.st));
+  if (flag_lock) flag_lock.unlock();
+  TG_CUDA(cudaGetLastError());
+  for (size_t w = 0; w < faults.size(); w++)
+    if (flags.fault[w]) return fault_status(faults.begin()[w]);
+  if (!on_device && nphys > 0) {
+    if (filter) {
+      TG_CUDA(cudaMemcpyAsync(selected, v.selected, (size_t)nphys, cudaMemcpyDeviceToHost, v.st));
+    } else {
+      TG_CUDA(cudaMemcpyAsync(result, v.result, (size_t)nphys * 8, cudaMemcpyDeviceToHost, v.st));
+      TG_CUDA(cudaMemcpyAsync(rnulls, v.rnulls, nb, cudaMemcpyDeviceToHost, v.st));
+    }
+    TG_CUDA(cudaStreamSynchronize(v.st));
+  }
+  if (n_selected) *n_selected = (int64_t)flags.count;
+  return TG_OK;
+}
+
+int run_column(int device, int on_device, const tg_column* a, const tg_column* b, void* result, uint8_t* rnulls,
+               void* stream, std::initializer_list<VecFault> faults, const VecKernel& launch) {
+  const tg_column cols[2] = {*a, b ? *b : *a};
+  const tg_chunk chk{b ? 2 : 1, 0, cols, nullptr, 0};
+  return run_vec(device, on_device, &chk, std::vector<char>(chk.ncols, 1), nullptr, nullptr, result, rnulls, stream,
+                 faults, launch);
+}
+
+int run_filter(int device, int on_device, const tg_chunk* chk, const std::vector<char>& needed, StrPrep* prep,
+               const DecFilter& d, const DevFilter& f, uint8_t* selected, int64_t* n_selected, void* stream) {
+  // fault word 0: bad string offsets (STRING items only); word 1: malformed DECIMAL cells
+  return run_vec(device, on_device, chk, needed, selected, n_selected, nullptr, nullptr, stream,
+                 {FAULT_BAD_OFFSETS, FAULT_BAD_CELL}, [&](const VecLaunch& v) -> int {
+    if (prep) return launch_string(v, *prep, d, f);
+    const int grid = grid_size(v.nsm, v.n, 256, 8);
+    if (d.n)
+      k_vec_filter_dec<<<grid, 256, 0, v.st>>>(v.cols, f, d, v.sel, v.nsel, v.nphys, v.selected, &v.flags->count, &v.flags->fault[1]);
+    else
+      k_vec_filter<<<grid, 256, 0, v.st>>>(v.cols, f, v.sel, v.nsel, v.nphys, v.selected, &v.flags->count);
+    return TG_OK;
+  });
+}
+
+// the checks of the four compare / arith calls
+static int check_binary(const tg_column* a, const tg_column* b, const void* result, const uint8_t* rnulls) {
+  if (!a || !result || !rnulls) return fail(TG_ERR_INVALID, "a / result / result_nulls is NULL");
+  if (b && b->length != a->length) return fail(TG_ERR_INVALID, "argument columns have different lengths");
+  if (a->elem_len != 8 || (b && b->elem_len != 8)) return fail(TG_ERR_UNSUPPORTED, "VecEval kernels take 8-byte columns");
+  return TG_OK;
+}
+
+// the grid of the warp-row kernels: VEC_ITEMS rows per thread
+static int warp_row_grid(const VecLaunch& v) { return grid_size(v.nsm, (v.n + VEC_ITEMS - 1) / VEC_ITEMS, 256, 8); }
+
 }  // namespace tg
 
 using namespace tg;
@@ -343,36 +437,41 @@ extern "C" {
 
 int tg_vec_compare_int(int device, int on_device, int op, int a_unsigned, int b_unsigned, const tg_column* a,
                        const tg_column* b, int64_t b_const, int64_t* result, uint8_t* result_nulls, void* stream) {
-  return run_binary(device, on_device, a, b, result, result_nulls, stream, false,
-                    [&](int grid, cudaStream_t st, VArg va, VArg vb, int64_t n, void* r, uint8_t* rn, int*) {
-                      k_vec_compare<false><<<grid, 256, 0, st>>>(op, a_unsigned, b_unsigned, va, vb, (long long)b_const, 0.0, n,
-                                                                 reinterpret_cast<long long*>(r), rn);
-                    });
+  TG_TRY(check_binary(a, b, result, result_nulls));
+  return run_column(device, on_device, a, b, result, result_nulls, stream, {}, [&](const VecLaunch& v) {
+    k_vec_compare<false><<<warp_row_grid(v), 256, 0, v.st>>>(op, a_unsigned, b_unsigned, v.arg(0), v.arg(1), (long long)b_const,
+                                                             0.0, v.n, v.result, v.rnulls);
+    return TG_OK;
+  });
 }
 
 int tg_vec_compare_real(int device, int on_device, int op, const tg_column* a, const tg_column* b, double b_const,
                         int64_t* result, uint8_t* result_nulls, void* stream) {
-  return run_binary(device, on_device, a, b, result, result_nulls, stream, false,
-                    [&](int grid, cudaStream_t st, VArg va, VArg vb, int64_t n, void* r, uint8_t* rn, int*) {
-                      k_vec_compare<true><<<grid, 256, 0, st>>>(op, 0, 0, va, vb, 0, b_const, n, reinterpret_cast<long long*>(r), rn);
-                    });
+  TG_TRY(check_binary(a, b, result, result_nulls));
+  return run_column(device, on_device, a, b, result, result_nulls, stream, {}, [&](const VecLaunch& v) {
+    k_vec_compare<true><<<warp_row_grid(v), 256, 0, v.st>>>(op, 0, 0, v.arg(0), v.arg(1), 0, b_const, v.n, v.result, v.rnulls);
+    return TG_OK;
+  });
 }
 
 int tg_vec_arith_int(int device, int on_device, int op, int a_unsigned, int b_unsigned, const tg_column* a,
                      const tg_column* b, int64_t b_const, int64_t* result, uint8_t* result_nulls, void* stream) {
-  return run_binary(device, on_device, a, b, result, result_nulls, stream, true,
-                    [&](int grid, cudaStream_t st, VArg va, VArg vb, int64_t n, void* r, uint8_t* rn, int* ovf) {
-                      k_vec_arith_int<<<grid, 256, 0, st>>>(op, a_unsigned, b_unsigned, va, vb, (long long)b_const, n,
-                                                            reinterpret_cast<long long*>(r), rn, ovf);
-                    });
+  TG_TRY(check_binary(a, b, result, result_nulls));
+  return run_column(device, on_device, a, b, result, result_nulls, stream, {FAULT_OVERFLOW}, [&](const VecLaunch& v) {
+    k_vec_arith_int<<<warp_row_grid(v), 256, 0, v.st>>>(op, a_unsigned, b_unsigned, v.arg(0), v.arg(1), (long long)b_const, v.n,
+                                                        v.result, v.rnulls, reinterpret_cast<int*>(&v.flags->fault[0]));
+    return TG_OK;
+  });
 }
 
 int tg_vec_arith_real(int device, int on_device, int op, const tg_column* a, const tg_column* b, double b_const,
                       double* result, uint8_t* result_nulls, void* stream) {
-  return run_binary(device, on_device, a, b, result, result_nulls, stream, true,
-                    [&](int grid, cudaStream_t st, VArg va, VArg vb, int64_t n, void* r, uint8_t* rn, int* ovf) {
-                      k_vec_arith_real<<<grid, 256, 0, st>>>(op, va, vb, b_const, n, reinterpret_cast<double*>(r), rn, ovf);
-                    });
+  TG_TRY(check_binary(a, b, result, result_nulls));
+  return run_column(device, on_device, a, b, result, result_nulls, stream, {FAULT_OVERFLOW}, [&](const VecLaunch& v) {
+    k_vec_arith_real<<<warp_row_grid(v), 256, 0, v.st>>>(op, v.arg(0), v.arg(1), b_const, v.n, reinterpret_cast<double*>(v.result),
+                                                         v.rnulls, reinterpret_cast<int*>(&v.flags->fault[0]));
+    return TG_OK;
+  });
 }
 
 int tg_vec_filter(int device, int on_device, const tg_chunk* chk, const tg_filter_item* items, int32_t n_items,
@@ -380,10 +479,6 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk, const tg_filte
   if (!chk || !selected) return fail(TG_ERR_INVALID, "chunk / selected is NULL");
   if (n_items < 0 || n_items > TG_MAX_FILTER) return fail(TG_ERR_UNSUPPORTED, "at most 8 CNF filter items are offloaded");
   if (chk->ncols <= 0 || chk->ncols > TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "chunk must have 1..16 columns");
-  TG_TRY(require_device("VecEval"));
-  DeviceGuard g(device);
-  if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
-  cudaStream_t st = (cudaStream_t)stream;
   DevFilter f{}; f.n = n_items;
   std::vector<char> needed(chk->ncols, 0);
   for (int i = 0; i < n_items; i++) {
@@ -391,40 +486,9 @@ int tg_vec_filter(int device, int on_device, const tg_chunk* chk, const tg_filte
     if (it.lhs_col < 0 || it.lhs_col >= chk->ncols || it.rhs_col >= chk->ncols) return fail(TG_ERR_INVALID, "filter column out of range");
     f.items[i] = it; needed[it.lhs_col] = 1; if (it.rhs_col >= 0) needed[it.rhs_col] = 1;
   }
-  int64_t nphys = chk->cols[0].length;
-  std::vector<std::unique_ptr<ArgDev>> args;
-  DevCols cols{};
-  for (int c = 0; c < chk->ncols; c++) {
-    args.emplace_back(new ArgDev());
-    cols.elem_len[c] = chk->cols[c].elem_len;
-    if (!needed[c]) continue;
-    TG_TRY(args[c]->load(device, on_device, &chk->cols[c], st));
-    cols.data[c] = args[c]->v.data; cols.nulls[c] = args[c]->v.nulls;
-  }
-  DevBuf dsel_idx, dselected, dcount;
-  const long long* sel_dev = reinterpret_cast<const long long*>(chk->sel);
-  uint8_t* selected_dev = selected;
-  if (!on_device) {
-    if (chk->sel) {
-      TG_TRY(dsel_idx.ensure(device, (size_t)chk->nsel * 8 + 16));
-      TG_CUDA(cudaMemcpyAsync(dsel_idx.p, chk->sel, (size_t)chk->nsel * 8, cudaMemcpyHostToDevice, st));
-      sel_dev = dsel_idx.as<long long>();
-    }
-    TG_TRY(dselected.ensure(device, (size_t)nphys + 16));
-    selected_dev = dselected.as<uint8_t>();
-  }
-  TG_TRY(dcount.ensure(device, 16));
-  TG_CUDA(cudaMemsetAsync(dcount.p, 0, 8, st));
-  TG_CUDA(cudaMemsetAsync(selected_dev, 0, (size_t)nphys, st));
-  int64_t n = chk->sel ? chk->nsel : nphys;
-  if (n > 0) k_vec_filter<<<grid_size(device_sm_count(device), n, 256, 8), 256, 0, st>>>(cols, f, sel_dev, chk->nsel, nphys, selected_dev, dcount.as<unsigned long long>());
-  unsigned long long cnt = 0;
-  TG_CUDA(cudaMemcpyAsync(&cnt, dcount.p, 8, cudaMemcpyDeviceToHost, st));
-  if (!on_device && nphys) TG_CUDA(cudaMemcpyAsync(selected, selected_dev, (size_t)nphys, cudaMemcpyDeviceToHost, st));
-  TG_CUDA(cudaStreamSynchronize(st));
-  TG_CUDA(cudaGetLastError());
-  if (n_selected) *n_selected = (int64_t)cnt;
-  return TG_OK;
+  for (int c = 0; c < chk->ncols; c++)
+    if (needed[c] && chk->cols[c].elem_len != 8) return fail(TG_ERR_UNSUPPORTED, "VecEval kernels take 8-byte columns");
+  return run_filter(device, on_device, chk, needed, nullptr, DecFilter{}, f, selected, n_selected, stream);
 }
 
 int tg_decimal_normalize(const uint8_t* cell, uint8_t* out) {
@@ -444,39 +508,10 @@ int tg_vec_compare_decimal(int device, int on_device, int op, const tg_column* a
   if (b) TG_TRY(check_dec_column(*b, on_device));
   DecConst k{};
   if (!b) TG_TRY(load_dec_const(b_const_cell, k.c));
-  TG_TRY(require_device("VecEval"));
-  DeviceGuard g(device);
-  if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t n = a->length;
-  ArgDev da, db;
-  TG_TRY(da.load(device, on_device, a, st, TG_DEC_CELL_BYTES));
-  TG_TRY(db.load(device, on_device, b, st, TG_DEC_CELL_BYTES));
-  DevBuf dres, dnul, dbad;
-  long long* res_dev = reinterpret_cast<long long*>(result);
-  uint8_t* nul_dev = result_nulls;
-  const size_t nb = (size_t)((n + 7) / 8);
-  if (!on_device) {
-    TG_TRY(dres.ensure(device, (size_t)n * 8 + 16)); TG_TRY(dnul.ensure(device, nb + 16));
-    res_dev = dres.as<long long>(); nul_dev = dnul.as<uint8_t>();
-  }
-  TG_TRY(dbad.ensure(device, 16));
-  TG_CUDA(cudaMemsetAsync(dbad.p, 0, 4, st));
-  if (n > 0)
-    k_vec_compare_dec<<<grid_size(device_sm_count(device), (n + VEC_ITEMS - 1) / VEC_ITEMS, 256, 8), 256, 0, st>>>(
-        op, da.v, db.v, k, n, res_dev, nul_dev, dbad.as<unsigned int>());
-  unsigned int bad = 0;
-  TG_CUDA(cudaMemcpyAsync(&bad, dbad.p, 4, cudaMemcpyDeviceToHost, st));
-  TG_CUDA(cudaStreamSynchronize(st));
-  TG_CUDA(cudaGetLastError());
-  if (bad) return fail(TG_ERR_INVALID, kMalformedCell);
-  // host buffers are written only once the cells are known to be well-formed
-  if (!on_device && n > 0) {
-    TG_CUDA(cudaMemcpyAsync(result, res_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaMemcpyAsync(result_nulls, nul_dev, nb, cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaStreamSynchronize(st));
-  }
-  return TG_OK;
+  return run_column(device, on_device, a, b, result, result_nulls, stream, {FAULT_BAD_CELL}, [&](const VecLaunch& v) {
+    k_vec_compare_dec<<<warp_row_grid(v), 256, 0, v.st>>>(op, v.arg(0), v.arg(1), k, v.n, v.result, v.rnulls, &v.flags->fault[0]);
+    return TG_OK;
+  });
 }
 
 int tg_vec_filter_ex(int device, int on_device, const tg_chunk* chk, const int32_t* col_types,
@@ -490,54 +525,7 @@ int tg_vec_filter_ex(int device, int on_device, const tg_chunk* chk, const int32
   DevFilter f{};
   std::vector<char> needed(chk->ncols, 0);
   TG_TRY(check_filter_items(on_device, chk, col_types, items, n_items, dec_consts, std::vector<char>(n_items, 0), d, f, needed));
-  if (d.n == 0) return tg_vec_filter(device, on_device, chk, items, n_items, selected, n_selected, stream);
-  const int64_t nphys = chk->cols[0].length;
-  TG_TRY(require_device("VecEval"));
-  DeviceGuard g(device);
-  if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
-  cudaStream_t st = (cudaStream_t)stream;
-  std::vector<std::unique_ptr<ArgDev>> args;
-  DevCols cols{};
-  for (int c = 0; c < chk->ncols; c++) {
-    args.emplace_back(new ArgDev());
-    cols.elem_len[c] = chk->cols[c].elem_len;
-    if (!needed[c]) continue;
-    TG_TRY(args[c]->load(device, on_device, &chk->cols[c], st, chk->cols[c].elem_len));
-    cols.data[c] = args[c]->v.data; cols.nulls[c] = args[c]->v.nulls;
-  }
-  DevBuf dsel_idx, dselected, dflags;
-  const long long* sel_dev = reinterpret_cast<const long long*>(chk->sel);
-  uint8_t* selected_dev = selected;
-  if (!on_device) {
-    if (chk->sel) {
-      TG_TRY(dsel_idx.ensure(device, (size_t)chk->nsel * 8 + 16));
-      TG_CUDA(cudaMemcpyAsync(dsel_idx.p, chk->sel, (size_t)chk->nsel * 8, cudaMemcpyHostToDevice, st));
-      sel_dev = dsel_idx.as<long long>();
-    }
-    TG_TRY(dselected.ensure(device, (size_t)nphys + 16));
-    selected_dev = dselected.as<uint8_t>();
-  }
-  TG_TRY(dflags.ensure(device, 16));   // the count (8 bytes), then the malformed flag (4 bytes)
-  TG_CUDA(cudaMemsetAsync(dflags.p, 0, 16, st));
-  TG_CUDA(cudaMemsetAsync(selected_dev, 0, (size_t)nphys, st));
-  const int64_t n = chk->sel ? chk->nsel : nphys;
-  unsigned long long* dcount = dflags.as<unsigned long long>();
-  unsigned int* dbad = reinterpret_cast<unsigned int*>(dcount + 1);
-  if (n > 0)
-    k_vec_filter_dec<<<grid_size(device_sm_count(device), n, 256, 8), 256, 0, st>>>(cols, f, d, sel_dev, chk->nsel, nphys,
-                                                                                     selected_dev, dcount, dbad);
-  unsigned long long flags[2] = {0, 0};
-  TG_CUDA(cudaMemcpyAsync(flags, dflags.p, 16, cudaMemcpyDeviceToHost, st));
-  TG_CUDA(cudaStreamSynchronize(st));
-  TG_CUDA(cudaGetLastError());
-  if ((unsigned int)flags[1]) return fail(TG_ERR_INVALID, kMalformedCell);
-  // host buffers are written only once the cells are known to be well-formed
-  if (!on_device && nphys) {
-    TG_CUDA(cudaMemcpyAsync(selected, selected_dev, (size_t)nphys, cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaStreamSynchronize(st));
-  }
-  if (n_selected) *n_selected = (int64_t)flags[0];
-  return TG_OK;
+  return run_filter(device, on_device, chk, needed, nullptr, d, f, selected, n_selected, stream);
 }
 
 }  // extern "C"

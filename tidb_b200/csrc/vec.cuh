@@ -1,8 +1,8 @@
 // vec.cuh — what the VecEval translation units share (vec.cu: 8-byte and DECIMAL columns; vec_string.cu: var-length
-// string columns): column arguments, the result bitmap store, the DECIMAL CNF items and the host-side check of a
-// tg_vec_filter_ex CNF.
+// string columns): column arguments, the result bitmap store, the DECIMAL CNF items, the host-side check of a
+// tg_vec_filter_ex CNF and the host path every VecEval call runs through.
 #pragma once
-#include <memory>
+#include <functional>
 #include "common.cuh"
 #include "chunk_io.cuh"
 #include "decimal.cuh"
@@ -70,28 +70,63 @@ __device__ __forceinline__ bool eval_dec_items(const DecFilter& d, const DevCols
   return s;
 }
 
-// a column argument made device-resident (copies host buffers when on_device == 0); `elem` is the width the kernel
-// reads: 8, or 40 for DECIMAL cells
-struct ArgDev {
-  DevBuf data, nulls;
-  VArg v{nullptr, nullptr};
-  int load(int device, int on_device, const tg_column* c, cudaStream_t st, int elem = 8) {
-    if (!c) return TG_OK;
-    if (c->elem_len != elem) return fail(TG_ERR_UNSUPPORTED, elem == 8 ? "VecEval kernels take 8-byte columns" : "DECIMAL operands are 40-byte cells");
-    if (on_device) { v.data = c->data; v.nulls = c->null_bitmap; return TG_OK; }
-    TG_TRY(upload_column(device, st, c->data, c->null_bitmap, c->length, elem, data, nulls, nullptr));
-    v.data = data.p;
-    if (c->null_bitmap) v.nulls = nulls.as<uint8_t>();
-    return TG_OK;
-  }
-};
-
-extern const char* const kMalformedCell;
-
 // The INT / REAL / DECIMAL items of a tg_vec_filter_ex CNF (the items whose `skip` entry is set are the caller's): checks
 // them without a device, marks their operand columns in `needed` and sorts them into d (DECIMAL) and f (the rest).
 int check_filter_items(int on_device, const tg_chunk* chk, const int32_t* col_types, const tg_filter_item* items,
                        int32_t n_items, const uint8_t* dec_consts, const std::vector<char>& skip, DecFilter& d,
                        DevFilter& f, std::vector<char>& needed);
+
+// ---- the host path of a VecEval call (vec.cu run_vec) --------------------------------------------------------------
+// the string columns of a call: data[c] points at the byte of offset base[c] (an uploaded column starts there)
+struct StrCols {
+  const int64_t* offs[TG_MAX_COLS];
+  const uint8_t* data[TG_MAX_COLS];
+  int64_t base[TG_MAX_COLS];
+};
+
+// what a kernel reports back, zeroed before the launch and read once after it: a filter's selected rows and up to two
+// fault words, each meaning one VecFault of the call
+struct VecFlags { unsigned long long count; unsigned int fault[2]; };
+enum VecFault { FAULT_OVERFLOW, FAULT_BAD_CELL, FAULT_BAD_OFFSETS };
+
+// what a launch gets: the call's columns and outputs on the device, and `n` rows to evaluate (the sel vector's when the
+// chunk has one, else its physical rows; never 0)
+struct VecLaunch {
+  int device, nsm, ncols;
+  cudaStream_t st;
+  DevCols cols;                  // fixed-width columns, and the NULL bitmaps of all needed columns
+  StrCols sc;                    // var-length columns
+  const long long* sel;
+  int64_t nsel, nphys, n;
+  uint8_t* selected;             // a filter's output
+  long long* result;             // a column call's outputs
+  uint8_t* rnulls;
+  VecFlags* flags;               // NULL for a call with neither a count nor a fault word
+  // operand c of a column call, or no column when the call has fewer
+  VArg arg(int c) const { return c < ncols ? VArg{cols.data[c], cols.nulls[c]} : VArg{nullptr, nullptr}; }
+};
+using VecKernel = std::function<int(const VecLaunch&)>;
+
+// Runs one VecEval call once its arguments are checked: the device, its guard and the stream; the needed columns of chk
+// borrowed when device-resident, else uploaded; the outputs (a filter's `selected`, or a column call's result / rnulls
+// for chk's physical rows) in device scratch for host buffers; the flags; the launch; the read-back.  A set fault word
+// fails the call with its VecFault's status, and host outputs and *n_selected are written only when none is set.
+int run_vec(int device, int on_device, const tg_chunk* chk, const std::vector<char>& needed, uint8_t* selected,
+            int64_t* n_selected, void* result, uint8_t* rnulls, void* stream, std::initializer_list<VecFault> faults,
+            const VecKernel& launch);
+
+// run_vec for a column call: operand a, and b when given (already checked to have a's length)
+int run_column(int device, int on_device, const tg_column* a, const tg_column* b, void* result, uint8_t* rnulls,
+               void* stream, std::initializer_list<VecFault> faults, const VecKernel& launch);
+
+// the STRING items of a call (vec_string.cu), and k_vec_string over them: a filter's when v has `selected`, then its
+// DECIMAL items d and INT / REAL items f; else one item's column result
+struct StrPrep;
+int launch_string(const VecLaunch& v, StrPrep& prep, const DecFilter& d, const DevFilter& f);
+
+// tg_vec_filter, _ex and _ex2 once each has checked its CNF: k_vec_string when there are STRING items (prep is given),
+// else k_vec_filter_dec when d has items, else k_vec_filter
+int run_filter(int device, int on_device, const tg_chunk* chk, const std::vector<char>& needed, StrPrep* prep,
+               const DecFilter& d, const DevFilter& f, uint8_t* selected, int64_t* n_selected, void* stream);
 
 }  // namespace tg

@@ -19,13 +19,6 @@ static constexpr int kStageCap = 2048;                 // bytes of one warp's bu
 static constexpr int kStageStride = kStageCap + 16;    // + room to keep the global alignment mod 16
 static constexpr int kWarpsPerBlock = 8;
 
-// the string columns of a call: data[c] points at the byte of offset base[c] (an uploaded column starts there)
-struct StrCols {
-  const int64_t* offs[TG_MAX_COLS];
-  const uint8_t* data[TG_MAX_COLS];
-  int64_t base[TG_MAX_COLS];
-};
-
 // one STRING item: a comparison (op, lhs `op` rhs column or the constant k) or a LIKE match of lhs against the compiled
 // pattern (pw, pt, klen entries).  Device pointers into the call's one constant upload.
 struct StrItem {
@@ -164,9 +157,6 @@ k_vec_string(StrCols sc, DevCols cols, const __grid_constant__ StrFilter sf, con
   if (malformed) *bad_cell = 1u;
 }
 
-static const char* kBadOffsets =
-    "malformed string offsets: offsets[r] > offsets[r+1], or an offset outside [offsets[0], offsets[length]], at a row the call evaluates";
-
 // TG_TYPE_VARCHAR, VARSTRING, STRING and the BLOB / TEXT types (ENUM, SET, JSON and BIT are var-length, not strings)
 static bool is_string_type(int32_t tp) {
   return tp == TG_TYPE_VARCHAR || tp == TG_TYPE_VARSTRING || tp == TG_TYPE_STRING ||
@@ -201,6 +191,7 @@ static bool like_bytes_ok(const std::vector<int32_t>& w, const std::vector<uint8
 struct StrPrep {
   StrFilter sf{};
   std::vector<uint8_t> blob;
+  DevBuf dev;
   size_t put(const void* p, size_t bytes) {
     const size_t at = (blob.size() + 15) & ~(size_t)15;
     blob.resize(at + bytes);
@@ -236,7 +227,7 @@ struct StrPrep {
     return TG_OK;
   }
   // upload the blob; item pointers become device pointers into dev
-  int upload(int device, cudaStream_t st, DevBuf& dev) {
+  int upload(int device, cudaStream_t st) {
     TG_TRY(dev.ensure(device, blob.size() + 16));
     if (!blob.empty()) TG_CUDA(cudaMemcpyAsync(dev.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
     const uint8_t* b = dev.as<uint8_t>();
@@ -249,101 +240,19 @@ struct StrPrep {
   }
 };
 
-// Runs one string call once its arguments are checked: `chk` (no sel for the column calls) with the string columns
-// str_needed, the fixed-width columns needed, the items of prep / d / f.  COLUMN calls write result / rnulls for
-// chk->cols[0].length rows; filter calls write selected and *n_selected.  Host outputs are written only when every offset
-// and cell read was good.
-static int run_string(int device, int on_device, const tg_chunk* chk, const std::vector<char>& str_needed,
-                      const std::vector<char>& needed, StrPrep& prep, const DecFilter& d, const DevFilter& f, bool column,
-                      uint8_t* selected, int64_t* n_selected, int64_t* result, uint8_t* result_nulls, void* stream) {
-  TG_TRY(require_device("VecEval"));
-  DeviceGuard g(device);
-  if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t nphys = chk->cols[0].length;
-  std::vector<std::unique_ptr<ArgDev>> args;
-  std::vector<std::unique_ptr<DevBuf>> sbufs;
-  DevCols cols{};
-  StrCols sc{};
-  for (int c = 0; c < chk->ncols; c++) {
-    args.emplace_back(new ArgDev());
-    const tg_column& col = chk->cols[c];
-    cols.elem_len[c] = col.elem_len;
-    if (str_needed[c]) {
-      if (on_device) {
-        sc.offs[c] = col.offsets; sc.data[c] = col.data; sc.base[c] = 0; cols.nulls[c] = col.null_bitmap;
-      } else {
-        for (int k = 0; k < 3; k++) sbufs.emplace_back(new DevBuf());
-        DevBuf& o = *sbufs[sbufs.size() - 3]; DevBuf& dd = *sbufs[sbufs.size() - 2]; DevBuf& nb = *sbufs.back();
-        TG_TRY(upload_varlen_column(device, st, col, o, dd, nb, nullptr));
-        sc.offs[c] = o.as<int64_t>(); sc.data[c] = dd.as<uint8_t>(); sc.base[c] = col.offsets[0];
-        cols.nulls[c] = col.null_bitmap ? nb.as<uint8_t>() : nullptr;
-      }
-    } else if (needed[c]) {
-      TG_TRY(args[c]->load(device, on_device, &col, st, col.elem_len));
-      cols.data[c] = args[c]->v.data; cols.nulls[c] = args[c]->v.nulls;
-    }
-  }
-  DevBuf dconst, dsel_idx, dout, dnul, dflags;
-  TG_TRY(prep.upload(device, st, dconst));
-  const long long* sel_dev = reinterpret_cast<const long long*>(chk->sel);
-  uint8_t* selected_dev = selected;
-  long long* res_dev = reinterpret_cast<long long*>(result);
-  uint8_t* nul_dev = result_nulls;
-  const size_t nb = (size_t)((nphys + 7) / 8);
-  if (!on_device) {
-    if (chk->sel) {
-      TG_TRY(dsel_idx.ensure(device, (size_t)chk->nsel * 8 + 16));
-      TG_CUDA(cudaMemcpyAsync(dsel_idx.p, chk->sel, (size_t)chk->nsel * 8, cudaMemcpyHostToDevice, st));
-      sel_dev = dsel_idx.as<long long>();
-    }
-    if (column) {
-      TG_TRY(dout.ensure(device, (size_t)nphys * 8 + 16)); TG_TRY(dnul.ensure(device, nb + 16));
-      res_dev = dout.as<long long>(); nul_dev = dnul.as<uint8_t>();
-    } else {
-      TG_TRY(dout.ensure(device, (size_t)nphys + 16));
-      selected_dev = dout.as<uint8_t>();
-    }
-  }
-  TG_TRY(dflags.ensure(device, 16));   // the count (8 bytes), the bad-offsets flag, the malformed-cell flag (4 bytes each)
-  TG_CUDA(cudaMemsetAsync(dflags.p, 0, 16, st));
-  if (!column) TG_CUDA(cudaMemsetAsync(selected_dev, 0, (size_t)nphys, st));
-  const int64_t n = chk->sel ? chk->nsel : nphys;
-  unsigned long long* dcount = dflags.as<unsigned long long>();
-  unsigned int* dbad = reinterpret_cast<unsigned int*>(dcount + 1);
+int launch_string(const VecLaunch& v, StrPrep& prep, const DecFilter& d, const DevFilter& f) {
+  TG_TRY(prep.upload(v.device, v.st));
   bool two = false;
   for (int q = 0; q < prep.sf.n; q++) two |= prep.sf.items[q].rhs >= 0;
   const size_t smem = (size_t)kWarpsPerBlock * kStageStride * (two ? 2 : 1);
-  const int grid = grid_size(device_sm_count(device), n, 32 * kWarpsPerBlock, 8);
-  if (n > 0) {
-    if (column)
-      k_vec_string<true><<<grid, 32 * kWarpsPerBlock, smem, st>>>(sc, cols, prep.sf, d, f, nullptr, 0, nphys, nullptr, dcount,
-                                                                  res_dev, nul_dev, dbad, dbad + 1);
-    else
-      k_vec_string<false><<<grid, 32 * kWarpsPerBlock, smem, st>>>(sc, cols, prep.sf, d, f, sel_dev, chk->nsel, nphys, selected_dev,
-                                                                   dcount, nullptr, nullptr, dbad, dbad + 1);
-  }
-  unsigned long long flags[2] = {0, 0};
-  TG_CUDA(cudaMemcpyAsync(flags, dflags.p, 16, cudaMemcpyDeviceToHost, st));
-  TG_CUDA(cudaStreamSynchronize(st));
-  TG_CUDA(cudaGetLastError());
-  if ((unsigned int)flags[1]) return fail(TG_ERR_INVALID, kBadOffsets);
-  if ((unsigned int)(flags[1] >> 32)) return fail(TG_ERR_INVALID, kMalformedCell);
-  // host buffers are written only once every offset and cell read is known to be good
-  if (!on_device && nphys) {
-    if (column) {
-      TG_CUDA(cudaMemcpyAsync(result, res_dev, (size_t)nphys * 8, cudaMemcpyDeviceToHost, st));
-      TG_CUDA(cudaMemcpyAsync(result_nulls, nul_dev, nb, cudaMemcpyDeviceToHost, st));
-    } else {
-      TG_CUDA(cudaMemcpyAsync(selected, selected_dev, (size_t)nphys, cudaMemcpyDeviceToHost, st));
-    }
-    TG_CUDA(cudaStreamSynchronize(st));
-  }
-  if (!column && n_selected) *n_selected = (int64_t)flags[0];
+  const int grid = grid_size(v.nsm, v.n, 32 * kWarpsPerBlock, 8);
+  const auto kernel = v.selected ? k_vec_string<false> : k_vec_string<true>;
+  kernel<<<grid, 32 * kWarpsPerBlock, smem, v.st>>>(v.sc, v.cols, prep.sf, d, f, v.sel, v.nsel, v.nphys, v.selected, &v.flags->count,
+                                                    v.result, v.rnulls, &v.flags->fault[0], &v.flags->fault[1]);
   return TG_OK;
 }
 
-// tg_vec_compare_string / tg_vec_like: the column a (and b) as a one- or two-column chunk with one STRING item
+// tg_vec_compare_string / tg_vec_like: the column a (and b) with one STRING item
 static int run_string_column(int device, int on_device, int kind, int op, int32_t collation, const tg_column* a,
                              const tg_column* b, const uint8_t* bytes, int64_t len, int32_t escape, int64_t* result,
                              uint8_t* result_nulls, void* stream) {
@@ -353,11 +262,8 @@ static int run_string_column(int device, int on_device, int kind, int op, int32_
   if (b) TG_TRY(check_str_column(*b, on_device));
   StrPrep prep;
   TG_TRY(prep.add(kind, op, 0, b ? 1 : -1, collation, bytes, len, escape));
-  const tg_column cols[2] = {*a, b ? *b : *a};
-  const tg_chunk chk{b ? 2 : 1, 0, cols, nullptr, 0};
-  const std::vector<char> str_needed(chk.ncols, 1), needed(chk.ncols, 0);
-  return run_string(device, on_device, &chk, str_needed, needed, prep, DecFilter{}, DevFilter{}, true, nullptr, nullptr,
-                    result, result_nulls, stream);
+  return run_column(device, on_device, a, b, result, result_nulls, stream, {FAULT_BAD_OFFSETS},
+                    [&](const VecLaunch& v) { return launch_string(v, prep, DecFilter{}, DevFilter{}); });
 }
 
 }  // namespace tg
@@ -386,7 +292,7 @@ int tg_vec_filter_ex2(int device, int on_device, const tg_chunk* chk, const int3
   if (chk->ncols <= 0 || chk->ncols > TG_MAX_COLS || !chk->cols) return fail(TG_ERR_UNSUPPORTED, "chunk must have 1..16 columns");
   const int64_t nphys = chk->cols[0].length;
   StrPrep prep;
-  std::vector<char> is_str(n_items, 0), str_needed(chk->ncols, 0), needed(chk->ncols, 0);
+  std::vector<char> is_str(n_items, 0), needed(chk->ncols, 0);
   for (int i = 0; i < n_items; i++) {
     const tg_filter_item& it = items[i];
     if (it.is_real != TG_FILTER_STRING) continue;
@@ -402,7 +308,7 @@ int tg_vec_filter_ex2(int device, int on_device, const tg_chunk* chk, const int3
       const tg_column& col = chk->cols[c];
       TG_TRY(check_str_column(col, on_device));
       if (col.length != nphys) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
-      str_needed[c] = 1;
+      needed[c] = 1;
     }
     TG_TRY(prep.add(sa.kind, it.op, it.lhs_col, rhs, sa.collation, sa.bytes, sa.len, sa.escape));
   }
@@ -415,8 +321,7 @@ int tg_vec_filter_ex2(int device, int on_device, const tg_chunk* chk, const int3
     if (is_string_type(col_types[items[i].lhs_col]) || (items[i].rhs_col >= 0 && is_string_type(col_types[items[i].rhs_col])))
       return fail(TG_ERR_UNSUPPORTED, "a string column in an INT / REAL / DECIMAL filter item");
   }
-  if (prep.sf.n == 0) return tg_vec_filter_ex(device, on_device, chk, col_types, items, n_items, dec_consts, selected, n_selected, stream);
-  return run_string(device, on_device, chk, str_needed, needed, prep, d, f, false, selected, n_selected, nullptr, nullptr, stream);
+  return run_filter(device, on_device, chk, needed, prep.sf.n ? &prep : nullptr, d, f, selected, n_selected, stream);
 }
 
 }  // extern "C"

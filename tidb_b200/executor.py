@@ -286,9 +286,9 @@ def _split_head(pending: List[Chunk], required_rows: int) -> Chunk:
 class SelectionExec(Executor):
     """GPU replacement of executor.SelectionExec (pkg/executor/select.go:746-785): pulls child chunks, evaluates the
     CNF filter list with expression.VectorizedFilter semantics (chunk_executor.go:413: a row is selected iff every item is
-    non-NULL true) on the device (tg_vec_filter; tg_vec_filter_ex when an item compares DECIMAL cells; tg_vec_filter_ex2
-    when an item compares or matches strings) and hands the selected rows on, at most `required_rows` per Next; string
-    payload columns are handed on bit for bit.  Child chunks are batched (`batch_rows`) so that one launch filters
+    non-NULL true) on the device (tg_vec_filter_ex2, told the child schema's types, so INT, REAL, DECIMAL and STRING items
+    mix in one call) and hands the selected rows on, at most `required_rows` per Next; string payload columns are handed
+    on bit for bit.  Child chunks are batched (`batch_rows`) so that one launch filters
     many 1024-row chunks."""
 
     def __init__(self, child: Executor, filters: Sequence, device: int = 0, batch_rows: int = 64 * MAX_CHUNK_SIZE):
@@ -322,20 +322,10 @@ class SelectionExec(Executor):
         selected = np.zeros(n, dtype=np.uint8)
         nsel = C.c_int64(0)
         cs = dense.to_struct()
-        arr = filter_array(self.filters)
-        if any(f.is_string for f in self.filters):
-            # STRING items read var-length columns: tg_vec_filter_ex2, with one tg_str_arg per item
-            tps = (C.c_int32 * len(self.schema))(*[t.tp for t in self.schema])
-            abi.check(self._lib.tg_vec_filter_ex2(self.device, 0, C.byref(cs), tps, arr, len(self.filters), dec_const_array(self.filters),
-                                                  str_arg_array(self.filters), selected.ctypes.data_as(C.c_void_p), C.byref(nsel), None))
-        elif any(f.is_decimal for f in self.filters):
-            # DECIMAL items compare MyDecimal cells: tg_vec_filter_ex, told the child schema's types
-            tps = (C.c_int32 * len(self.schema))(*[t.tp for t in self.schema])
-            consts = dec_const_array(self.filters)
-            abi.check(self._lib.tg_vec_filter_ex(self.device, 0, C.byref(cs), tps, arr, len(self.filters), consts,
-                                                 selected.ctypes.data_as(C.c_void_p), C.byref(nsel), None))
-        else:
-            abi.check(self._lib.tg_vec_filter(self.device, 0, C.byref(cs), arr, len(self.filters), selected.ctypes.data_as(C.c_void_p), C.byref(nsel), None))
+        tps = (C.c_int32 * len(self.schema))(*[t.tp for t in self.schema])
+        abi.check(self._lib.tg_vec_filter_ex2(self.device, 0, C.byref(cs), tps, filter_array(self.filters), len(self.filters),
+                                              dec_const_array(self.filters), str_arg_array(self.filters),
+                                              selected.ctypes.data_as(C.c_void_p), C.byref(nsel), None))
         self.launches += 1
         keep = selected.astype(bool)
         assert int(keep.sum()) == nsel.value
