@@ -496,6 +496,70 @@ typedef struct tg_agg_distinct_stats {
 } tg_agg_distinct_stats;
 int tg_agg_get_distinct_stats(tg_agg* a, tg_agg_distinct_stats* out);
 
+/* tg_agg_desc_ex2 plus FieldType.GetCollate() (a MySQL collation id) per child column, for GROUP BY over string columns.
+ * col_collation NULL, or a plan without a string column: tg_agg_supported_ex3 / tg_agg_open_ex3 answer exactly like
+ * tg_agg_supported_ex2 / tg_agg_open_ex2.
+ *   String column: col_types TG_TYPE_VARCHAR, TG_TYPE_VARSTRING, TG_TYPE_STRING or one of the four BLOB / TEXT types
+ *     (ENUM, SET, JSON and BIT are TG_ERR_UNSUPPORTED wherever they are used).
+ *   GROUP BY: a string GROUP BY column needs col_collation 63 (binary), 46 (utf8mb4_bin), 83 (utf8_bin), 65 (ascii_bin),
+ *     47 (latin1_bin) or 309 (utf8mb4_0900_bin); any other id is TG_ERR_UNSUPPORTED.  The group key is
+ *     collator.ImmutableKey (codec.go HashGroupKey): the bytes under 63 and 309, the bytes with trailing 0x20 cut under
+ *     46, 83, 65 and 47 ("a", "a " and "a  " form one group, "a\t" its own).  NULL is its own group, apart from ''.  Keys
+ *     are equal only when their key bytes are.  String columns count toward the 4 GROUP BY columns and mix with integer
+ *     and DOUBLE ones.
+ *   Functions over a string column: FIRSTROW of a string GROUP BY column, and COUNT without DISTINCT (only the NULL
+ *     bitmap is read).  SUM, AVG, MIN, MAX, any DISTINCT function and a string operand of arg_expr are
+ *     TG_ERR_UNSUPPORTED.  FIRSTROW of a string GROUP BY column returns the raw bytes, trailing spaces included, of the
+ *     group's earliest row in push order (within a chunk, logical row order: `sel` order when it has one), as
+ *     firstRow4String with one worker (aggfuncs/func_first_row.go); NULL for the NULL group.  Under 46, 83, 65 and 47
+ *     with several GROUP BY columns, rows of one key value in different groups may differ in their trailing spaces, so
+ *     such a FIRSTROW also takes, per key column, one free column slot (child columns + DISTINCT argument columns +
+ *     such columns <= 16) and one of the 12 aggregate slots and one state word (a per-group MIN the library adds and
+ *     does not return); a plan past those limits is TG_ERR_UNSUPPORTED.  A push to such a plan fails with
+ *     TG_ERR_UNSUPPORTED when a row of that column has 2^23 or more trailing spaces, or when the handle's input would
+ *     reach 2^41 rows.  FIRSTROW of a string column that is not a GROUP BY column stays TG_ERR_UNSUPPORTED.
+ *   Pushes: a string column has elem_len -1 and length + 1 offsets, under the Columns and Offsets rules of
+ *     tg_vec_filter_ex2 (offsets need not start at 0; a bad row is TG_ERR_INVALID).  A host push checks the offsets of
+ *     every row it holds before it stages anything; a device push (offsets 8-byte aligned) checks every row on the
+ *     device before the dictionaries see the batch.  A rejected push leaves groups, DISTINCT sets and dictionaries
+ *     unchanged.  A push that fails once a dictionary has run its encode pass on the batch (an allocation failure while
+ *     a dictionary or the group table grows, a too-wide trailing-space count above) fails with its status, and every
+ *     later push and finish fails with TG_ERR_STATE.  A failure before that pass (a bad row, an allocation before the
+ *     first round) leaves the handle usable.
+ *   Results: a string result column (FIRSTROW of a string column) is read with tg_agg_next_ex or tg_agg_result_dev_ex;
+ *     tg_agg_next and tg_agg_result_dev return TG_ERR_INVALID for such a plan and write nothing.
+ * The library keeps one device dictionary per string GROUP BY column for the life of the handle: an id per key value,
+ * the raw bytes of its earliest row, and a hash table that grows on demand (tg_agg_get_string_stats). */
+typedef struct tg_agg_desc_ex3 {
+  tg_agg_desc_ex2 ex2;            /* everything tg_agg_desc_ex2 says, unchanged                  */
+  const int32_t* col_collation;   /* FieldType.GetCollate() per child column; NULL = not given   */
+} tg_agg_desc_ex3;
+int tg_agg_supported_ex3(const tg_agg_desc_ex3* desc);
+int tg_agg_open_ex3(const tg_agg_desc_ex3* desc, tg_agg** out);
+
+/* A caller-owned var-length result column: offsets has room for capacity_rows + 1 values, data for data_cap bytes. */
+typedef struct tg_mut_varlen { int64_t* offsets; uint8_t* data; int64_t data_cap; } tg_mut_varlen;
+/* tg_agg_next with string results.  var_out has one entry per result column; only the string ones are read (their
+ * tg_mut_column has elem_len -1 and its data pointer is ignored; its null_bitmap follows the usual rules).  Serves the
+ * largest n <= min(max_rows, capacity_rows, rows left) whose bytes fit data_cap in every string column, and writes
+ * offsets[0..n] from 0 and the bytes.  If not even one row fits: TG_ERR_CAPACITY, nothing written, the read position
+ * unchanged.  For a plan without string results it is tg_agg_next, and var_out may be NULL. */
+int tg_agg_next_ex(tg_agg* a, tg_mut_chunk* out, tg_mut_varlen* var_out, int64_t max_rows, int64_t* nrows);
+/* tg_agg_result_dev plus out_offsets: for a string result, out_cols[k] is its device bytes and out_offsets[k] its device
+ * offsets (rows + 1 int64 values from 0); NULL for every other result. */
+int tg_agg_result_dev_ex(tg_agg* a, int64_t* out_rows, void** out_cols, void** out_nulls, void** out_offsets);
+
+/* the encode pass of the string GROUP BY columns (k_str_dict_encode), cumulative over the handle: dictionary entries,
+ * arena bytes and table slots of all dictionaries, table growths, kernel launches of the pass (growth and arena copies
+ * included), and its device time (CUDA events).  All 0 for a plan without a string GROUP BY column. */
+typedef struct tg_agg_string_stats {
+  int64_t dict_entries, dict_bytes, dict_slots, dict_grows, launches;
+  double encode_ms;
+} tg_agg_string_stats;
+int tg_agg_get_string_stats(tg_agg* a, tg_agg_string_stats* out);
+/* tg_agg_stats.paths bit 7 (0x80): the encode pass of a string GROUP BY column ran (k_str_dict_encode) */
+enum { TG_AGG_PATH_STRING_KEY = 0x80 };
+
 /* ---------------------------------------------------------------------------------------------
  * VecEval* kernels             replace pkg/expression builtin_*_vec.go signatures
  * All operate on one column-at-a-time over host or device buffers (`on_device` flag).

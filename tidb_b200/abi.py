@@ -139,6 +139,22 @@ class TgAggDescEx2(C.Structure):
     _fields_ = [("ex", TgAggDescEx), ("has_distinct", C.POINTER(C.c_uint8))]
 
 
+class TgAggDescEx3(C.Structure):
+    """tg_agg_desc_ex3: tg_agg_desc_ex2 plus FieldType.GetCollate() per child column (NULL = not given)"""
+    _fields_ = [("ex2", TgAggDescEx2), ("col_collation", C.POINTER(C.c_int32))]
+
+
+class TgMutVarlen(C.Structure):
+    """tg_mut_varlen: a caller-owned var-length result column (capacity_rows + 1 offsets, data_cap bytes)"""
+    _fields_ = [("offsets", C.c_void_p), ("data", C.c_void_p), ("data_cap", C.c_int64)]
+
+
+class TgAggStringStats(C.Structure):
+    """tg_agg_string_stats: the encode pass of the string GROUP BY columns, cumulative over the handle's pushes"""
+    _fields_ = [("dict_entries", C.c_int64), ("dict_bytes", C.c_int64), ("dict_slots", C.c_int64), ("dict_grows", C.c_int64),
+                ("launches", C.c_int64), ("encode_ms", C.c_double)]
+
+
 class TgAggDistinctStats(C.Structure):
     """tg_agg_distinct_stats: the dedup pass of the DISTINCT functions, cumulative over the handle's pushes"""
     _fields_ = [("pairs", C.c_int64), ("set_slots", C.c_int64), ("set_grows", C.c_int64), ("launches", C.c_int64),
@@ -158,6 +174,7 @@ JOIN_PATH_SCATTER_BULK, JOIN_PATH_SCATTER = 1 << 5, 1 << 6   # 1 << 4 is unassig
 JOIN_PATH_CELL_GATHER = 1 << 7
 AGG_PATH_NOGROUP, AGG_PATH_V2_GLOBAL, AGG_PATH_V2_LOCAL, AGG_PATH_MULTI_KEY = 1 << 0, 1 << 1, 1 << 2, 1 << 3
 AGG_PATH_V1_LOCAL, AGG_PATH_V1_GLOBAL, AGG_PATH_MERGE = 1 << 4, 1 << 5, 1 << 6
+AGG_PATH_STRING_KEY = 1 << 7
 
 
 # every symbol include/tidbgpu.h declares; tests/test_abi_exports.py checks the .so exports them all
@@ -171,6 +188,7 @@ EXPORTED_SYMBOLS = [
     "tg_join_close", "tg_join_probe_dev", "tg_join_probe_dev_seg", "tg_join_get_stats",
     "tg_agg_supported", "tg_agg_supported_ex", "tg_agg_supported_ex2", "tg_agg_open", "tg_agg_open_ex", "tg_agg_open_ex2", "tg_agg_push",
     "tg_agg_push_dev", "tg_agg_finish", "tg_agg_next", "tg_agg_close", "tg_agg_result_dev", "tg_agg_get_stats", "tg_agg_get_distinct_stats",
+    "tg_agg_supported_ex3", "tg_agg_open_ex3", "tg_agg_next_ex", "tg_agg_result_dev_ex", "tg_agg_get_string_stats",
     "tg_vec_compare_int", "tg_vec_compare_real", "tg_vec_arith_int", "tg_vec_arith_real",
     "tg_vec_filter", "tg_vec_compare_decimal", "tg_vec_filter_ex", "tg_decimal_normalize", "tg_topn",
     "tg_vec_filter_ex2", "tg_vec_compare_string", "tg_vec_like",

@@ -17,8 +17,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(CSRC, "libtidbgpu.so")
-SOURCES = ["runtime.cu", "chunk_io.cu", "join.cu", "agg.cu", "vec.cu", "vec_string.cu", "partition.cu", "codec.cu", "topn.cu"]
-HEADERS = ["common.cuh", "chunk_io.cuh", "join_kernels.cuh", "partition_kernels.cuh", "tma.cuh", "agg_update.cuh", "decimal.cuh", "vec.cuh", "string.cuh", os.path.join("..", "..", "include", "tidbgpu.h")]
+SOURCES = ["runtime.cu", "chunk_io.cu", "join.cu", "agg.cu", "str_dict.cu", "vec.cu", "vec_string.cu", "partition.cu", "codec.cu", "topn.cu"]
+HEADERS = ["common.cuh", "chunk_io.cuh", "join_kernels.cuh", "partition_kernels.cuh", "tma.cuh", "agg_update.cuh", "decimal.cuh", "vec.cuh", "string.cuh", "str_dict.cuh", os.path.join("..", "..", "include", "tidbgpu.h")]
 ARCH = "arch=compute_90a,code=sm_90a"
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", ARCH, "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "--expt-relaxed-constexpr"]

@@ -192,15 +192,28 @@ def chunk_array(chunks: Sequence[Chunk]):
 
 
 class MutChunk:
-    """Caller-owned output chunk (tg_mut_chunk): numpy buffers the library fills."""
+    """Caller-owned output chunk (tg_mut_chunk): numpy buffers the library fills.  A var-length column (elem_len -1) has
+    capacity + 1 int64 offsets and `data_cap` bytes, described to the library by `varlen` (one tg_mut_varlen per
+    column, zeros for the fixed-width ones)."""
 
-    def __init__(self, elem_lens: Sequence[int], capacity_rows: int, dtypes: Optional[Sequence] = None):
+    def __init__(self, elem_lens: Sequence[int], capacity_rows: int, dtypes: Optional[Sequence] = None, data_cap: int = 0):
         self.capacity = int(capacity_rows)
+        self.elem_lens = list(elem_lens)
         self.data = []
         self.bitmaps = []
+        self.offsets: List[Optional[np.ndarray]] = []
+        self.varlen = (abi.TgMutVarlen * max(len(elem_lens), 1))()
         for i, el in enumerate(elem_lens):
-            dt = dtypes[i] if dtypes is not None else (np.int64 if el == 8 else np.float32)
-            self.data.append(np.zeros(max(self.capacity, 1), dtype=dt))
+            if el == VARLEN:
+                self.data.append(np.zeros(max(int(data_cap), 1), dtype=np.uint8))
+                self.offsets.append(np.zeros(max(self.capacity, 1) + 1, dtype=np.int64))
+                self.varlen[i].offsets = self.offsets[i].ctypes.data
+                self.varlen[i].data = self.data[i].ctypes.data
+                self.varlen[i].data_cap = int(data_cap)
+            else:
+                dt = dtypes[i] if dtypes is not None else (np.int64 if el == 8 else np.float32)
+                self.data.append(np.zeros(max(self.capacity, 1), dtype=dt))
+                self.offsets.append(None)
             self.bitmaps.append(np.zeros((max(self.capacity, 1) + 7) // 8, dtype=np.uint8))
         self._cols = (abi.TgMutColumn * max(len(elem_lens), 1))()
         for i, el in enumerate(elem_lens):
@@ -213,5 +226,23 @@ class MutChunk:
         self.struct.capacity_rows = self.capacity
 
     def columns(self, nrows: int):
-        """-> list of (values ndarray[:nrows], nulls bool ndarray[:nrows])"""
-        return [(d[:nrows].copy(), unpack_nulls(b, nrows)) for d, b in zip(self.data, self.bitmaps)]
+        """-> list of (values ndarray[:nrows], nulls bool ndarray[:nrows]); a var-length column's values are its rows as
+        bytes (None where NULL) in an object array"""
+        out = []
+        for i, (d, b) in enumerate(zip(self.data, self.bitmaps)):
+            nl = unpack_nulls(b, nrows)
+            if self.offsets[i] is None:
+                out.append((d[:nrows].copy(), nl))
+            else:
+                o = self.offsets[i]
+                out.append((np.array([None if nl[r] else d[o[r]:o[r + 1]].tobytes() for r in range(nrows)], dtype=object), nl))
+        return out
+
+    def column(self, i: int, nrows: int) -> Column:
+        """output column i of the first nrows rows as a Column (var-length columns keep their offsets)"""
+        nl = unpack_nulls(self.bitmaps[i], nrows)
+        nl = nl if nl.any() else None
+        if self.offsets[i] is None:
+            return Column(self.data[i][:nrows].copy(), nl)
+        o = self.offsets[i][:nrows + 1].copy()
+        return Column(self.data[i][:o[-1]].copy(), nl, o)

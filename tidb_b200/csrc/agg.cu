@@ -20,6 +20,8 @@
 #include "tma.cuh"
 #include "decimal.cuh"
 #include "chunk_io.cuh"
+#include "string.cuh"
+#include "str_dict.cuh"
 
 namespace tg {
 
@@ -966,6 +968,28 @@ struct AggImpl : DeviceHandle {
   bool broken = false;                  // a push failed after a set was touched: every later push / finish fails
   tg_agg_distinct_stats dstats{};
 
+  // string columns (tg_agg_desc_ex3): a string GROUP BY column is encoded to ids by its dictionary (str_dict.cuh) before
+  // the DISTINCT sets and the update kernels see the batch; its FIRSTROW finalizes to the id, then gathers the bytes
+  std::vector<int> coll;                // per child column: StrColl of its collation (COLL_NONE: not given / not one)
+  std::vector<char> is_str;             // a string column the plan reads (GROUP BY key or COUNT argument)
+  std::vector<char> needed_fixed;       // `needed` without the string columns (validate_chunk / device_view)
+  std::vector<int> dict_of;             // per child column: its dictionary, -1
+  std::vector<std::unique_ptr<StrDict>> dicts;
+  std::vector<std::unique_ptr<DevBuf>> sids, doffs;   // per child column: the id column of a batch, a batch's offsets
+  DevBuf sflag;                         // bad-offsets flag of a device push
+  int64_t str_ords = 0;                 // logical rows encoded so far: the ordinal of the next batch's first row
+  double encode_ms = 0;
+  std::vector<int> out_dict;            // per result: the dictionary of a string result, -1
+  // FIRSTROW of a PAD-collation string key with several GROUP BY columns: the dictionary's earliest row of a key value
+  // is not each group's, so the encode pass writes a tail column (ordinal << kTailBits | trailing spaces cut) and a
+  // hidden unsigned MIN per group keeps its earliest row's: that row's raw bytes are the key plus that many spaces
+  int n_out = 0;                        // functions of the descriptor; spec.n counts the hidden MINs after them
+  std::vector<int> tail_col;            // per child column: the virtual column of its tail values, -1
+  std::vector<int> tail_fn;             // per result: the hidden MIN of its tail values, -1
+  std::vector<std::unique_ptr<DevBuf>> stails;   // per child column: a batch's tail values
+  std::vector<std::unique_ptr<DevBuf>> out_soffs, out_sbytes;
+  std::vector<std::vector<int64_t>> host_soffs;   // the string results' offsets, read back once at finish
+
   // table
   DevBuf tbl_mem;
   AggTable tbl{};
@@ -1055,7 +1079,28 @@ static int distinct_rules(const AggImpl* a, const tg_agg_func& f) {
   return TG_OK;
 }
 
-static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, const int32_t* col_dec, const uint8_t* has_distinct = nullptr) {
+// TG_TYPE_VARCHAR, VARSTRING, STRING and the BLOB / TEXT types (ENUM, SET, JSON and BIT are var-length, not strings)
+static bool agg_string_type(int32_t tp) {
+  return tp == TG_TYPE_VARCHAR || tp == TG_TYPE_VARSTRING || tp == TG_TYPE_STRING || (tp >= TG_TYPE_TINY_BLOB && tp <= TG_TYPE_BLOB);
+}
+
+// A function over a string column (tg_agg_desc_ex3): TG_OK when it is offloaded, else the status and message
+static int str_arg_rules(const AggImpl* a, const tg_agg_func& f) {
+  if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "a string column is not offloaded in an argument expression");
+  switch (f.name) {
+    case TG_AGG_COUNT:   // reads the null bitmap only
+      if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "COUNT over a string column is offloaded in Complete mode only");
+      if (f.ret_type == TG_TYPE_NEWDECIMAL) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG / MIN / MAX only");
+      return TG_OK;
+    case TG_AGG_FIRSTROW:
+      if (a->dict_of[f.arg_col] < 0) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW of a string column is offloaded only for GROUP BY columns");
+      return TG_OK;
+    default: return fail(TG_ERR_UNSUPPORTED, "only FIRSTROW (of a GROUP BY column) and COUNT are offloaded over string columns");
+  }
+}
+
+static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, const int32_t* col_dec, const uint8_t* has_distinct = nullptr,
+                     const int32_t* col_coll = nullptr) {
   if (!d) return fail(TG_ERR_INVALID, "desc is NULL");
   if (d->n_cols <= 0 || d->n_cols > TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "child schema must have 1..16 columns");
   a->ncols = d->n_cols;
@@ -1071,6 +1116,10 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
   }
   a->dec_decode.assign(d->n_cols, 0);
   a->needed.assign(d->n_cols, 0);
+  a->coll.assign(d->n_cols, COLL_NONE);
+  a->dict_of.assign(d->n_cols, -1);
+  for (int i = 0; i < d->n_cols; i++) if (col_coll && agg_string_type(a->types[i])) a->coll[i] = coll_of_id(col_coll[i]);
+  int ndicts = 0;
   if (d->n_group_by > TG_MAX_GROUP_COLS) return fail(TG_ERR_UNSUPPORTED, "GPU hash aggregation handles up to 4 GROUP BY columns");
   a->group_col = -1; a->gk_kind = GK_NONE; a->nkw = 0;
   a->group_cols.clear(); a->group_kinds.clear();
@@ -1079,10 +1128,16 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
     int g = d->group_by_cols[q];
     if (g < 0 || g >= a->ncols) return fail(TG_ERR_INVALID, "group-by column out of range");
     int kind;
+    const bool str = col_coll && agg_string_type(a->types[g]);
     if (is_int_family(a->types[g])) kind = GK_I64;
     else if (a->types[g] == TG_TYPE_DOUBLE) kind = GK_F64;
+    else if (str) {   // encoded to a dense int64 id column (encode_strings)
+      if (a->coll[g] == COLL_NONE) return fail(TG_ERR_UNSUPPORTED, "string GROUP BY collation not offloaded (binary, *_bin and utf8mb4_0900_bin are)");
+      kind = GK_I64;
+      if (a->dict_of[g] < 0) a->dict_of[g] = ndicts++;
+    }
     else return fail(TG_ERR_UNSUPPORTED, "GROUP BY column type is not offloaded (int family / double only)");
-    if (a->elem[g] != 8) return fail(TG_ERR_UNSUPPORTED, "GROUP BY columns must be 8-byte columns");
+    if (a->elem[g] != 8 && !str) return fail(TG_ERR_UNSUPPORTED, "GROUP BY columns must be 8-byte columns");
     if (q == 0) { a->group_col = g; a->gk_kind = kind; }
     a->group_cols.push_back(g); a->group_kinds.push_back(kind);
     any_nullable |= !(a->flags[g] & TG_FLAG_NOT_NULL);
@@ -1095,6 +1150,7 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
   a->out_nullable.assign(d->n_funcs, 0);
   a->out_elem.assign(d->n_funcs, 8);
   a->fdistinct.assign(d->n_funcs, 0);
+  a->out_dict.assign(d->n_funcs, -1);
   for (int k = 0; k < d->n_funcs; k++) {
     const tg_agg_func& f = d->funcs[k];
     AggFuncDev& o = a->spec.f[k];
@@ -1105,6 +1161,11 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
       if (f.name != TG_AGG_MIN && f.name != TG_AGG_MAX) { TG_TRY(distinct_rules(a, f)); a->fdistinct[k] = 1; }
     }
     const bool distinct = a->fdistinct[k] != 0;
+    const bool str_arg = col_coll && f.arg_col >= 0 && f.arg_col < a->ncols && agg_string_type(a->types[f.arg_col]);
+    if (str_arg) {
+      TG_TRY(str_arg_rules(a, f));
+      if (f.name == TG_AGG_FIRSTROW) a->out_dict[k] = a->dict_of[f.arg_col];
+    }
     // a DECIMAL(p <= 18, s) argument column (tg_agg_desc_ex): decoded to int64 value * 10^s on every batch, then the integer
     // update paths run unchanged
     const bool dec_arg = f.arg_col >= 0 && f.arg_col < a->ncols && a->types[f.arg_col] == TG_TYPE_NEWDECIMAL;
@@ -1138,7 +1199,7 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
     if (f.arg_expr != TG_ARGEXPR_COL && f.arg_col2 >= 0 && f.arg_col2 < d->n_cols && !(a->flags[f.arg_col2] & TG_FLAG_NOT_NULL)) arg_nullable = true;
     // a DISTINCT argument is NULL on every row that brought no new value: COUNT needs its own count, AVG its divisor
     if (distinct) arg_nullable = true;
-    if (f.arg_col >= 0) { if (a->elem[f.arg_col] != 8 && !dec_arg) return fail(TG_ERR_UNSUPPORTED, "aggregate arguments must be 8-byte columns"); a->needed[f.arg_col] = 1; }
+    if (f.arg_col >= 0) { if (a->elem[f.arg_col] != 8 && !dec_arg && !str_arg) return fail(TG_ERR_UNSUPPORTED, "aggregate arguments must be 8-byte columns"); a->needed[f.arg_col] = 1; }
     int atype = f.arg_col >= 0 ? a->types[f.arg_col] : TG_TYPE_LONGLONG;
     o.is_real = atype == TG_TYPE_DOUBLE;
     o.is_unsigned = f.arg_col >= 0 && !dec_arg && (a->flags[f.arg_col] & TG_FLAG_UNSIGNED) != 0;   // a decoded DECIMAL is a signed int64
@@ -1231,6 +1292,30 @@ static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, 
   if (a->ncols + (int)a->dist_cols.size() > TG_MAX_COLS)
     return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates need one free column slot per argument column (child columns + DISTINCT columns <= 16)");
   a->dist_gkw = d->n_group_by + (any_nullable ? 1 : 0);
+  // FIRSTROW of a PAD string key under several GROUP BY columns: one tail column and one hidden MIN per such column
+  a->n_out = d->n_funcs;
+  a->tail_col.assign(d->n_cols, -1);
+  a->tail_fn.assign(d->n_funcs, -1);
+  std::vector<int> min_of(d->n_cols, -1);
+  int nvirt = a->ncols + (int)a->dist_cols.size();
+  for (int k = 0; k < d->n_funcs; k++) {
+    const int c = d->funcs[k].arg_col;
+    if (a->out_dict[k] < 0 || a->coll[c] != COLL_PAD_BIN || d->n_group_by < 2) continue;
+    if (min_of[c] < 0) {
+      if (nvirt >= TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW of a PAD string key with several GROUP BY columns needs a free column slot (child columns + DISTINCT columns + such keys <= 16)");
+      if (a->spec.n >= TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW of a PAD string key with several GROUP BY columns takes a hidden aggregate slot (at most 12 in all)");
+      a->tail_col[c] = nvirt++;
+      min_of[c] = a->spec.n++;
+      a->spec.f[min_of[c]] = AggFuncDev{TG_AGG_MIN, a->tail_col[c], 0, 1, a->nstates++, -1, 0, -1, TG_ARGEXPR_COL, -1, 0, -1, -1, 0.0, 0};
+      a->out_nullable.push_back(0); a->out_elem.push_back(8); a->out_dict.push_back(-1); a->fdistinct.push_back(0);
+    }
+    a->tail_fn[k] = min_of[c];
+  }
+  if (a->nstates > 2 * TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "the aggregate list needs more than 24 state words (a DECIMAL SUM / AVG takes up to 3, up to 4 over a product)");
+  a->is_str.assign(d->n_cols, 0);
+  a->needed_fixed = a->needed;
+  for (int c = 0; c < d->n_cols; c++)
+    if (a->needed[c] && col_coll && agg_string_type(a->types[c])) { a->is_str[c] = 1; a->needed_fixed[c] = 0; }
   a->device = d->device;
   a->expected_groups = d->expected_groups;
   return TG_OK;
@@ -1640,18 +1725,65 @@ static int update_after_decode(AggImpl* a, DevCols& cols, int64_t n) {
 }
 
 static int broken_fail() {
-  return fail(TG_ERR_STATE, "an earlier push failed after the DISTINCT sets had taken its values: this handle's results are lost");
+  return fail(TG_ERR_STATE, "an earlier push failed after the DISTINCT sets or string dictionaries had taken its values: this handle's results are lost");
 }
 
-// aggregate n device-resident rows; a fused argument expression that overflowed fails the call (types.ErrOverflow).  A bad
-// DECIMAL cell fails the push before the DISTINCT sets see it; any later failure leaves a set holding values whose rows
-// were not aggregated, so the handle refuses every later push and finish instead of counting them twice or never.
-static int update_device(AggImpl* a, const DevCols& in, int64_t n) {
+// every string GROUP BY column of the batch -> its dictionary's ids (str_dict.cuh), through the grow-and-retry of the
+// other find-or-insert passes; then the id column, with the column's own NULL bitmap, stands in for the string column.
+// Row i of the batch has the ordinal str_ords + i, so a key's earliest row is the first in push order.
+static int encode_strings(AggImpl* a, DevCols& cols, const StrColDev* sv, int64_t n, bool& touched) {
+  if (a->dicts.empty() || n == 0) return TG_OK;
+  if ((unsigned long long)(a->str_ords + n) >> (64 - kTailBits))
+    return fail(TG_ERR_UNSUPPORTED, "a string-key aggregation is offloaded for fewer than 2^41 input rows");
+  TG_CUDA(cudaEventRecord(a->ev0, a->stream));
+  for (int c = 0; c < a->ncols; c++) {
+    const int j = a->dict_of[c];
+    if (j < 0) continue;
+    StrDict& d = *a->dicts[j];
+    TG_TRY(str_dict_prepare(d, a->device, n, a->expected_groups, a->stream));
+    TG_TRY(a->sids[c]->ensure(a->device, (size_t)n * 8 + 16));
+    long long* ids = a->sids[c]->as<long long>();
+    unsigned long long* tails = nullptr;
+    if (a->tail_col[c] >= 0) { TG_TRY(a->stails[c]->ensure(a->device, (size_t)n * 8 + 16)); tails = a->stails[c]->as<unsigned long long>(); }
+    touched = true;   // from the first round on, the dictionary may hold entries of this batch
+    TG_TRY(grow_and_retry(a, a->deferred, n, false, "string dictionary", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+      a->stats.kernel_launches++;
+      return str_dict_round(d, sv[c], n, a->str_ords, kAggMaxProbe, ids, deferred, only, nd, tails, a->nsm, a->stream);
+    }, [&](unsigned long long nd) { return str_dict_grow(d, nd, a->device, a->nsm, a->stream); }));
+    if (tails) {
+      bool wide = false;
+      TG_TRY(str_dict_tail_overflow(d, wide, a->stream));
+      if (wide) return fail(TG_ERR_UNSUPPORTED, "a string GROUP BY value with 2^23 or more trailing spaces under a PAD collation, whose FIRSTROW is asked with several GROUP BY columns");
+      cols.data[a->tail_col[c]] = tails;
+      cols.nulls[a->tail_col[c]] = nullptr;
+      cols.elem_len[a->tail_col[c]] = 8;
+    }
+    TG_TRY(str_dict_commit(d, sv[c], ids, n, a->str_ords, a->device, a->nsm, a->stream));
+    cols.data[c] = ids;
+    cols.elem_len[c] = 8;
+  }
+  a->str_ords += n;
+  a->stats.paths |= TG_AGG_PATH_STRING_KEY;
+  TG_CUDA(cudaEventRecord(a->ev1, a->stream));
+  TG_CUDA(cudaStreamSynchronize(a->stream));
+  TG_CUDA(cudaGetLastError());
+  a->encode_ms += a->elapsed_ms();
+  return TG_OK;
+}
+
+// aggregate n device-resident rows (sv: the string columns, by child column; nullptr without any); a fused argument
+// expression that overflowed fails the call (types.ErrOverflow).  A bad DECIMAL cell fails the push before the
+// dictionaries and the DISTINCT sets see it; a failure once a dictionary round has run, or any later one with DISTINCT
+// sets, leaves a dictionary or a set holding values whose rows were not aggregated, so the handle refuses every later
+// push and finish instead of counting them twice or never.
+static int update_device(AggImpl* a, const DevCols& in, const StrColDev* sv, int64_t n) {
   if (a->broken) return broken_fail();
   DevCols cols = in;
   TG_TRY(decode_decimal_args(a, cols, n));
-  const int rc = update_after_decode(a, cols, n);
-  if (rc != TG_OK && !a->dist_cols.empty()) a->broken = true;
+  bool touched = false;
+  int rc = encode_strings(a, cols, sv, n, touched);
+  if (rc == TG_OK) rc = update_after_decode(a, cols, n);
+  if (rc != TG_OK && (!a->dist_cols.empty() || touched)) a->broken = true;
   return rc;
 }
 
@@ -1659,15 +1791,33 @@ static int aflush(AggImpl* a) {
   HostStage& st = a->stage;
   if (st.rows == 0) return TG_OK;
   DevCols v{};
+  StrColDev sv[TG_MAX_COLS] = {};
   for (int c = 0; c < a->ncols; c++) {
     v.elem_len[c] = a->elem[c];
     if (!a->needed[c]) continue;
+    if (a->is_str[c]) {   // staged offsets (from 0) and bytes
+      TG_TRY(a->doffs[c]->ensure(a->device, (size_t)(st.rows + 1) * 8 + 16));
+      TG_CUDA(cudaMemcpyAsync(a->doffs[c]->p, st.offs[c]->p, (size_t)(st.rows + 1) * 8, cudaMemcpyHostToDevice, a->stream));
+      TG_TRY(upload_column(a->device, a->stream, st.data[c]->p, nullptr, (int64_t)st.data[c]->used, 1, *a->dcols[c], *a->dnulls[c],
+                           &a->stats.h2d_bytes));
+      a->stats.h2d_bytes += (st.rows + 1) * 8;
+      if (st.has_nulls[c]) {
+        const size_t nb = (size_t)((st.rows + 7) / 8);
+        TG_TRY(a->dnulls[c]->ensure(a->device, nb + 16));
+        if (nb) TG_CUDA(cudaMemcpyAsync(a->dnulls[c]->p, st.nulls[c]->p, nb, cudaMemcpyHostToDevice, a->stream));
+        a->stats.h2d_bytes += (int64_t)nb;
+      }
+      v.data[c] = a->dcols[c]->p;
+      if (st.has_nulls[c]) v.nulls[c] = a->dnulls[c]->as<uint8_t>();
+      sv[c] = StrColDev{a->doffs[c]->as<int64_t>(), a->dcols[c]->as<uint8_t>(), 0, v.nulls[c]};
+      continue;
+    }
     TG_TRY(upload_column(a->device, a->stream, st.data[c]->p, st.has_nulls[c] ? st.nulls[c]->p : nullptr, st.rows, a->elem[c],
                          *a->dcols[c], *a->dnulls[c], &a->stats.h2d_bytes));
     v.data[c] = a->dcols[c]->p;
     if (st.has_nulls[c]) v.nulls[c] = a->dnulls[c]->as<uint8_t>();
   }
-  int rc = update_device(a, v, st.rows);
+  int rc = update_device(a, v, sv, st.rows);
   st.reset();
   return rc;
 }
@@ -1681,7 +1831,18 @@ static int afinalize(AggImpl* a) {
   // agg_hash_executor.go:654: empty input and no GROUP BY → one row of default values (COUNT 0, rest NULL)
   bool default_row = a->stats.input_rows == 0 && a->group_col < 0;
   if (a->nslots == 0) {
-    if (!default_row) { a->out_rows = 0; return TG_OK; }
+    if (!default_row) {   // no input rows: no groups, and a string result has the one offset 0
+      a->out_rows = 0;
+      for (int k = 0; k < nf; k++) {
+        if (a->out_dict[k] < 0) continue;
+        TG_TRY(a->out_soffs[k]->ensure(a->device, 16));
+        TG_TRY(a->out_sbytes[k]->ensure(a->device, 16));
+        TG_CUDA(cudaMemsetAsync(a->out_soffs[k]->p, 0, 8, a->stream));
+        a->host_soffs[k].assign(1, 0);
+      }
+      TG_CUDA(cudaStreamSynchronize(a->stream));
+      return TG_OK;
+    }
     TG_CUDA(cudaMemsetAsync(sc, 0, 64, a->stream));
     TG_TRY(alloc_table(a, 1024, a->tbl_mem, a->tbl));
     a->nslots = 1024;
@@ -1725,6 +1886,18 @@ static int afinalize(AggImpl* a) {
     TG_TRY(a->out_bitmaps[k]->ensure(a->device, (size_t)((a->out_rows + 7) / 8) + 16));
     if (a->out_rows) { launch_pack_bitmap(ao.valid[k], a->out_rows, a->out_bitmaps[k]->as<uint8_t>(), a->nsm, a->stream); a->stats.kernel_launches++; }
   }
+  // string results: the ids k_agg_finalize wrote -> offsets and bytes from the dictionary, the offsets also on the host
+  for (int k = 0; k < nf; k++) {
+    const int j = a->out_dict[k];
+    if (j < 0) continue;
+    int64_t total = 0;
+    const unsigned long long* tails = a->tail_fn[k] >= 0 ? a->out_cols[a->tail_fn[k]]->as<unsigned long long>() : nullptr;
+    TG_TRY(str_dict_gather(*a->dicts[j], a->out_cols[k]->as<long long>(), ao.valid[k], tails, a->out_rows, *a->out_soffs[k], *a->out_sbytes[k],
+                           &total, a->device, a->nsm, a->stream));
+    a->stats.kernel_launches += 5;
+    a->host_soffs[k].assign((size_t)a->out_rows + 1, 0);
+    TG_CUDA(cudaMemcpyAsync(a->host_soffs[k].data(), a->out_soffs[k]->p, (size_t)(a->out_rows + 1) * 8, cudaMemcpyDeviceToHost, a->stream));
+  }
   TG_CUDA(cudaEventRecord(a->ev1, a->stream));
   TG_CUDA(cudaStreamSynchronize(a->stream));
   TG_CUDA(cudaGetLastError());
@@ -1749,12 +1922,19 @@ int tg_agg_supported_ex2(const tg_agg_desc_ex2* desc) {
                    desc ? desc->has_distinct : nullptr);
 }
 
-static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int32_t* col_dec, const uint8_t* has_distinct, tg_agg** out) {
+int tg_agg_supported_ex3(const tg_agg_desc_ex3* desc) {
+  AggImpl tmp;
+  return agg_setup(&tmp, desc ? &desc->ex2.ex.base : nullptr, desc ? desc->ex2.ex.col_flen : nullptr, desc ? desc->ex2.ex.col_decimal : nullptr,
+                   desc ? desc->ex2.has_distinct : nullptr, desc ? desc->col_collation : nullptr);
+}
+
+static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int32_t* col_dec, const uint8_t* has_distinct, tg_agg** out,
+                    const int32_t* col_coll = nullptr) {
   if (!out) return fail(TG_ERR_INVALID, "out is NULL");
   *out = nullptr;
   std::unique_ptr<tg_agg> shell(new tg_agg());
   std::unique_ptr<AggImpl> a(new AggImpl());
-  TG_TRY(agg_setup(a.get(), desc, col_flen, col_dec, has_distinct));
+  TG_TRY(agg_setup(a.get(), desc, col_flen, col_dec, has_distinct, col_coll));
   int ndev = 0;
   TG_TRY(require_device("the GPU hash aggregation", &ndev));
   if (a->device < 0 || a->device >= ndev) return fail(TG_ERR_INVALID, "device ordinal out of range");
@@ -1764,7 +1944,11 @@ static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int3
   a->stage.init(a->ncols);
   for (int c = 0; c < a->ncols; c++) {
     a->dcols.emplace_back(new DevBuf()); a->dnulls.emplace_back(new DevBuf()); a->dscaled.emplace_back(new DevBuf());
+    a->sids.emplace_back(new DevBuf()); a->doffs.emplace_back(new DevBuf()); a->stails.emplace_back(new DevBuf());
+    if (a->dict_of[c] >= 0) { a->dicts.emplace_back(new StrDict()); a->dicts.back()->coll = a->coll[c]; }
   }
+  for (int k = 0; k < a->spec.n; k++) { a->out_soffs.emplace_back(new DevBuf()); a->out_sbytes.emplace_back(new DevBuf()); }
+  a->host_soffs.resize(a->spec.n);
   for (size_t j = 0; j < a->dist_cols.size(); j++) a->dsets.emplace_back(new AggImpl::SetMem());
   shell->impl = a.release();
   *out = shell.release();
@@ -1782,11 +1966,23 @@ int tg_agg_open_ex2(const tg_agg_desc_ex2* desc, tg_agg** out) {
                   desc ? desc->has_distinct : nullptr, out);
 }
 
+int tg_agg_open_ex3(const tg_agg_desc_ex3* desc, tg_agg** out) {
+  return agg_open(desc ? &desc->ex2.ex.base : nullptr, desc ? desc->ex2.ex.col_flen : nullptr, desc ? desc->ex2.ex.col_decimal : nullptr,
+                  desc ? desc->ex2.has_distinct : nullptr, out, desc ? desc->col_collation : nullptr);
+}
+
 int tg_agg_push(tg_agg* h, const tg_chunk* chk) {
   TG_LOCK(h, AggImpl, a);
   if (a->finished) return fail(TG_ERR_STATE, "push after finish");
   if (a->broken) return broken_fail();
-  TG_TRY(validate_chunk(a->ncols, a->needed, a->elem, chk));
+  TG_TRY(validate_chunk(a->ncols, a->needed_fixed, a->elem, chk));
+  // string columns: every row's offsets are checked before anything is staged (staging copies the rows' bytes)
+  const int64_t phys = chk->ncols ? chk->cols[0].length : 0;
+  for (int c = 0; c < a->ncols; c++) {
+    if (!a->is_str[c]) continue;
+    TG_TRY(check_varlen_rows(chk->cols[c], chk));
+    if (chk->cols[c].length != phys) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
+  }
   TG_TRY(stage_append(a->stage, a->needed, a->elem, chk));
   if (a->stage.rows >= kStageBatchRows) TG_TRY(aflush(a));
   return TG_OK;
@@ -1796,9 +1992,33 @@ int tg_agg_push_dev(tg_agg* h, const tg_chunk* chk) {
   TG_LOCK(h, AggImpl, a);
   if (a->finished) return fail(TG_ERR_STATE, "push after finish");
   DevCols v;
-  TG_TRY(device_view(chk, a->ncols, a->needed, a->elem, v));
+  TG_TRY(device_view(chk, a->ncols, a->needed_fixed, a->elem, v));
+  const int64_t n = logical_rows(chk);
+  StrColDev sv[TG_MAX_COLS] = {};
+  bool any_str = false;
+  for (int c = 0; c < a->ncols; c++) {
+    if (!a->is_str[c]) continue;
+    const tg_column& col = chk->cols[c];
+    if (col.elem_len != -1 || !col.offsets) return fail(TG_ERR_INVALID, "a string column is var-length: elem_len -1 and offsets");
+    if (col.length != n) return fail(TG_ERR_INVALID, "chunk columns have different lengths");
+    if (reinterpret_cast<uintptr_t>(col.offsets) & 7) return fail(TG_ERR_INVALID, "device string offsets must be 8-byte aligned");
+    v.data[c] = col.data; v.nulls[c] = col.null_bitmap;
+    sv[c] = StrColDev{col.offsets, col.data, 0, col.null_bitmap};
+    any_str = true;
+  }
+  if (any_str && n > 0) {   // every row's offsets, on the device, before a dictionary sees the batch
+    TG_TRY(a->sflag.ensure(a->device, 16));
+    TG_CUDA(cudaMemsetAsync(a->sflag.p, 0, 4, a->stream));
+    for (int c = 0; c < a->ncols; c++)
+      if (a->is_str[c]) { str_check_offsets(sv[c].offs, sv[c].data, n, a->sflag.as<unsigned int>(), a->nsm, a->stream); a->stats.kernel_launches++; }
+    unsigned int bad = 0;
+    TG_CUDA(cudaMemcpyAsync(&bad, a->sflag.p, 4, cudaMemcpyDeviceToHost, a->stream));
+    TG_CUDA(cudaStreamSynchronize(a->stream));
+    TG_CUDA(cudaGetLastError());
+    if (bad) return fail(TG_ERR_INVALID, "a string column has a row with bad offsets (offsets[r] > offsets[r+1], or outside [offsets[0], offsets[length]])");
+  }
   TG_TRY(aflush(a));
-  return update_device(a, v, logical_rows(chk));
+  return update_device(a, v, sv, n);
 }
 
 int tg_agg_finish(tg_agg* h) {
@@ -1811,18 +2031,23 @@ int tg_agg_finish(tg_agg* h) {
   return TG_OK;
 }
 
+static bool has_string_result(const AggImpl* a) {
+  return std::find_if(a->out_dict.begin(), a->out_dict.end(), [](int j) { return j >= 0; }) != a->out_dict.end();
+}
+
 int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) {
   TG_LOCK(h, AggImpl, a);
   if (!out || !nrows) return fail(TG_ERR_INVALID, "out / nrows is NULL");
+  if (has_string_result(a)) return fail(TG_ERR_INVALID, "the plan has a string result: read it with tg_agg_next_ex");
   *nrows = 0;
   if (!a->finished) return fail(TG_ERR_STATE, "next before finish (hash aggregation is a pipeline breaker)");
-  if (out->ncols != a->spec.n) return fail(TG_ERR_INVALID, "output chunk column count does not match the aggregate list");
+  if (out->ncols != a->n_out) return fail(TG_ERR_INVALID, "output chunk column count does not match the aggregate list");
   int64_t lo = a->consumed;
   int64_t want = std::min<int64_t>(std::min<int64_t>(max_rows, out->capacity_rows), a->out_rows - lo);
   if (want <= 0) return TG_OK;
   // every output column is checked before the first copy is enqueued: a rejected call writes nothing
   TG_TRY(check_out_columns(a->out_bitmaps, a->out_elem, out));
-  for (int k = 0; k < a->spec.n; k++) {
+  for (int k = 0; k < a->n_out; k++) {
     const size_t el = (size_t)a->out_elem[k];
     TG_CUDA(cudaMemcpyAsync(out->cols[k].data, a->out_cols[k]->as<uint8_t>() + (size_t)lo * el, (size_t)want * el, cudaMemcpyDeviceToHost, a->stream));
     a->stats.d2h_bytes += want * (int64_t)el;
@@ -1835,11 +2060,91 @@ int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) 
   return TG_OK;
 }
 
-int tg_agg_result_dev(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls) {
+// tg_agg_next_ex of a plan with a string result
+static int agg_next_varlen(AggImpl* a, tg_mut_chunk* out, tg_mut_varlen* var_out, int64_t max_rows, int64_t* nrows) {
+  if (!out || !nrows || !var_out) return fail(TG_ERR_INVALID, "out / var_out / nrows is NULL");
+  *nrows = 0;
+  if (!a->finished) return fail(TG_ERR_STATE, "next before finish (hash aggregation is a pipeline breaker)");
+  if (out->ncols != a->n_out) return fail(TG_ERR_INVALID, "output chunk column count does not match the aggregate list");
+  const int64_t lo = a->consumed;
+  int64_t want = std::min<int64_t>(std::min<int64_t>(max_rows, out->capacity_rows), a->out_rows - lo);
+  if (want <= 0) return TG_OK;
+  // every output column is checked before the first copy is enqueued: a rejected call writes nothing
+  for (int k = 0; k < a->n_out; k++) {
+    const bool str = a->out_dict[k] >= 0;
+    if (out->cols[k].elem_len != (str ? -1 : a->out_elem[k]))
+      return fail(TG_ERR_INVALID, "output column elem_len does not match its result column (-1 for a string result, 40 for a DECIMAL one, else 8)");
+    if (a->out_bitmaps[k]->p && !out->cols[k].null_bitmap) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");
+    if (!str) continue;
+    const tg_mut_varlen& vo = var_out[k];
+    if (!vo.offsets || (vo.data_cap > 0 && !vo.data) || vo.data_cap < 0) return fail(TG_ERR_INVALID, "a string result needs offsets and data_cap bytes of data");
+    // the largest prefix of rows whose bytes fit data_cap
+    const int64_t* ho = a->host_soffs[k].data() + lo;
+    int64_t fit = std::upper_bound(ho, ho + want + 1, ho[0] + vo.data_cap) - ho - 1;
+    want = std::min<int64_t>(want, fit);
+  }
+  if (want <= 0) return fail(TG_ERR_CAPACITY, "the next result row's string bytes do not fit data_cap");
+  for (int k = 0; k < a->n_out; k++) {
+    if (a->out_dict[k] >= 0) {
+      const int64_t* ho = a->host_soffs[k].data() + lo;
+      const int64_t bytes = ho[want] - ho[0];
+      if (bytes) TG_CUDA(cudaMemcpyAsync(var_out[k].data, a->out_sbytes[k]->as<uint8_t>() + ho[0], (size_t)bytes, cudaMemcpyDeviceToHost, a->stream));
+      for (int64_t r = 0; r <= want; r++) var_out[k].offsets[r] = ho[r] - ho[0];
+      a->stats.d2h_bytes += bytes + (want + 1) * 8;
+      continue;
+    }
+    const size_t el = (size_t)a->out_elem[k];
+    TG_CUDA(cudaMemcpyAsync(out->cols[k].data, a->out_cols[k]->as<uint8_t>() + (size_t)lo * el, (size_t)want * el, cudaMemcpyDeviceToHost, a->stream));
+    a->stats.d2h_bytes += want * (int64_t)el;
+  }
+  TG_TRY(download_bitmaps(a->out_bitmaps, out, lo, want, a->stream, nullptr));
+  a->consumed += want;
+  *nrows = want;
+  return TG_OK;
+}
+
+int tg_agg_next_ex(tg_agg* h, tg_mut_chunk* out, tg_mut_varlen* var_out, int64_t max_rows, int64_t* nrows) {
+  {
+    TG_LOCK(h, AggImpl, a);
+    if (has_string_result(a)) return agg_next_varlen(a, out, var_out, max_rows, nrows);
+  }
+  return tg_agg_next(h, out, max_rows, nrows);
+}
+
+int tg_agg_result_dev_ex(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls, void** out_offsets) {
   TG_LOCK(h, AggImpl, a);
   if (!a->finished) return fail(TG_ERR_STATE, "result before finish");
   if (out_rows) *out_rows = a->out_rows;
-  for (int k = 0; k < a->spec.n; k++) {
+  for (int k = 0; k < a->n_out; k++) {
+    const bool str = a->out_dict[k] >= 0;
+    if (out_cols) out_cols[k] = str ? a->out_sbytes[k]->p : a->out_cols[k]->p;
+    if (out_nulls) out_nulls[k] = a->out_bitmaps[k]->p;
+    if (out_offsets) out_offsets[k] = str ? a->out_soffs[k]->p : nullptr;
+  }
+  return TG_OK;
+}
+
+int tg_agg_get_string_stats(tg_agg* h, tg_agg_string_stats* out) {
+  TG_LOCK(h, AggImpl, a);
+  if (!out) return fail(TG_ERR_INVALID, "out is NULL");
+  *out = tg_agg_string_stats{};
+  for (const auto& d : a->dicts) {
+    out->dict_entries += d->entries;
+    out->dict_bytes += (int64_t)d->arena_used;
+    out->dict_slots += (int64_t)d->nslots;
+    out->dict_grows += d->grows;
+    out->launches += d->launches;
+  }
+  out->encode_ms = a->encode_ms;
+  return TG_OK;
+}
+
+int tg_agg_result_dev(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls) {
+  TG_LOCK(h, AggImpl, a);
+  if (has_string_result(a)) return fail(TG_ERR_INVALID, "the plan has a string result: read it with tg_agg_result_dev_ex");
+  if (!a->finished) return fail(TG_ERR_STATE, "result before finish");
+  if (out_rows) *out_rows = a->out_rows;
+  for (int k = 0; k < a->n_out; k++) {
     if (out_cols) out_cols[k] = a->out_cols[k]->p;
     if (out_nulls) out_nulls[k] = a->out_bitmaps[k]->p;
   }

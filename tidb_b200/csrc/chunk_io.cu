@@ -26,13 +26,39 @@ int stage_append(HostStage& st, const std::vector<char>& needed, const std::vect
     const tg_column& col = chk->cols[c];
     int el = elem[c];
     PinBuf& d = *st.data[c];
-    TG_TRY(d.reserve((size_t)(st.rows + n) * el));
-    uint8_t* dst = d.p + (size_t)st.rows * el;
-    if (!chk->sel) std::memcpy(dst, col.data, (size_t)n * el);
-    else if (el == 8) { auto* o = reinterpret_cast<uint64_t*>(dst); auto* in = reinterpret_cast<const uint64_t*>(col.data); for (int64_t i = 0; i < n; i++) o[i] = in[chk->sel[i]]; }
-    else if (el == 4) { auto* o = reinterpret_cast<uint32_t*>(dst); auto* in = reinterpret_cast<const uint32_t*>(col.data); for (int64_t i = 0; i < n; i++) o[i] = in[chk->sel[i]]; }
-    else { auto* in = reinterpret_cast<const uint8_t*>(col.data); for (int64_t i = 0; i < n; i++) std::memcpy(dst + (size_t)i * el, in + (size_t)chk->sel[i] * el, el); }
-    d.used = (size_t)(st.rows + n) * el;
+    if (el < 0) {   // var-length: the rows' bytes appended, their offsets rebased onto the staged bytes
+      PinBuf& ob = *st.offs[c];
+      TG_TRY(ob.reserve((size_t)(st.rows + n + 1) * 8));
+      int64_t* o = reinterpret_cast<int64_t*>(ob.p);
+      if (st.rows == 0) o[0] = 0;
+      const int64_t at = o[st.rows];
+      int64_t add = 0;
+      if (!chk->sel) add = col.offsets[n] - col.offsets[0];
+      else for (int64_t i = 0; i < n; i++) add += col.offsets[chk->sel[i] + 1] - col.offsets[chk->sel[i]];
+      TG_TRY(d.reserve((size_t)(at + add)));
+      if (!chk->sel) {
+        if (add) std::memcpy(d.p + at, col.data + col.offsets[0], (size_t)add);
+        for (int64_t i = 0; i < n; i++) o[st.rows + i + 1] = at + col.offsets[i + 1] - col.offsets[0];
+      } else {
+        int64_t w = at;
+        for (int64_t i = 0; i < n; i++) {
+          const int64_t s0 = col.offsets[chk->sel[i]], len = col.offsets[chk->sel[i] + 1] - s0;
+          if (len) std::memcpy(d.p + w, col.data + s0, (size_t)len);
+          w += len;
+          o[st.rows + i + 1] = w;
+        }
+      }
+      d.used = (size_t)(at + add);
+      ob.used = (size_t)(st.rows + n + 1) * 8;
+    } else {
+      TG_TRY(d.reserve((size_t)(st.rows + n) * el));
+      uint8_t* dst = d.p + (size_t)st.rows * el;
+      if (!chk->sel) std::memcpy(dst, col.data, (size_t)n * el);
+      else if (el == 8) { auto* o = reinterpret_cast<uint64_t*>(dst); auto* in = reinterpret_cast<const uint64_t*>(col.data); for (int64_t i = 0; i < n; i++) o[i] = in[chk->sel[i]]; }
+      else if (el == 4) { auto* o = reinterpret_cast<uint32_t*>(dst); auto* in = reinterpret_cast<const uint32_t*>(col.data); for (int64_t i = 0; i < n; i++) o[i] = in[chk->sel[i]]; }
+      else { auto* in = reinterpret_cast<const uint8_t*>(col.data); for (int64_t i = 0; i < n; i++) std::memcpy(dst + (size_t)i * el, in + (size_t)chk->sel[i] * el, el); }
+      d.used = (size_t)(st.rows + n) * el;
+    }
     // null bitmap: materialised lazily, the first time a chunk brings one
     PinBuf& nb = *st.nulls[c];
     bool bring = col.null_bitmap != nullptr;
@@ -86,6 +112,22 @@ int upload_varlen_column(int device, cudaStream_t s, const tg_column& c, DevBuf&
     if (nb) TG_CUDA(cudaMemcpyAsync(nulls.p, c.null_bitmap, nb, cudaMemcpyHostToDevice, s));
   }
   if (h2d_bytes) *h2d_bytes += (int64_t)(ob + bytes + nb);
+  return TG_OK;
+}
+
+int check_varlen_rows(const tg_column& c, const tg_chunk* chk) {
+  if (c.elem_len != -1 || !c.offsets) return fail(TG_ERR_INVALID, "a string column is var-length: elem_len -1 and offsets");
+  if (c.length < 0) return fail(TG_ERR_INVALID, "negative column length");
+  const int64_t lo = c.offsets[0], hi = c.offsets[c.length];
+  if (hi < lo) return fail(TG_ERR_INVALID, "string column offsets[length] < offsets[0]");
+  if (hi > lo && !c.data) return fail(TG_ERR_INVALID, "string column without data");
+  const int64_t n = logical_rows(chk);
+  for (int64_t i = 0; i < n; i++) {
+    const int64_t r = chk->sel ? chk->sel[i] : i;
+    if (r < 0 || r >= c.length) return fail(TG_ERR_INVALID, "sel entry out of range");
+    const int64_t o0 = c.offsets[r], o1 = c.offsets[r + 1];
+    if (o0 > o1 || o0 < lo || o1 > hi) return fail(TG_ERR_INVALID, "string column row " + std::to_string(r) + " has bad offsets");
+  }
   return TG_OK;
 }
 

@@ -18,21 +18,26 @@ int64_t logical_rows(const tg_chunk* chk);
 // chunk has rows, data
 int validate_chunk(int ncols, const std::vector<char>& needed, const std::vector<int>& elem, const tg_chunk* chk);
 
-// pinned host staging of pushed chunks, one buffer per column (only needed columns are filled)
+// pinned host staging of pushed chunks, one buffer per column (only needed columns are filled).  A var-length column
+// (elem -1) stages its rows' bytes in `data` and rows + 1 offsets into them, starting at 0, in `offs`.
 struct HostStage {
-  std::vector<std::unique_ptr<PinBuf>> data, nulls;
+  std::vector<std::unique_ptr<PinBuf>> data, nulls, offs;
   std::vector<char> has_nulls;
   int64_t rows = 0;
   void init(int ncols) {
-    data.clear(); nulls.clear();
-    for (int i = 0; i < ncols; i++) { data.emplace_back(new PinBuf()); nulls.emplace_back(new PinBuf()); }
+    data.clear(); nulls.clear(); offs.clear();
+    for (int i = 0; i < ncols; i++) { data.emplace_back(new PinBuf()); nulls.emplace_back(new PinBuf()); offs.emplace_back(new PinBuf()); }
     has_nulls.assign(ncols, 0);
     rows = 0;
   }
-  void reset() { rows = 0; std::fill(has_nulls.begin(), has_nulls.end(), 0); for (auto& d : data) d->used = 0; for (auto& d : nulls) d->used = 0; }
+  void reset() {
+    rows = 0; std::fill(has_nulls.begin(), has_nulls.end(), 0);
+    for (auto& d : data) d->used = 0; for (auto& d : nulls) d->used = 0; for (auto& d : offs) d->used = 0;
+  }
 };
 
-// append the logical rows of a validated host chunk to the staging (gathers through sel)
+// append the logical rows of a validated host chunk to the staging (gathers through sel).  A var-length column's
+// offsets must already be checked at those rows (check_varlen_rows): its bytes are copied here on the host.
 int stage_append(HostStage& st, const std::vector<char>& needed, const std::vector<int>& elem, const tg_chunk* chk);
 
 // `rows` host cells of `elem` bytes → data, and their NULL bitmap (when `bitmap` is set) → nulls, on stream s; each
@@ -48,6 +53,11 @@ int upload_column(int device, cudaStream_t s, const void* src, const uint8_t* bi
 // it is given.
 int upload_varlen_column(int device, cudaStream_t s, const tg_column& c, DevBuf& offs, DevBuf& data, DevBuf& nulls,
                          int64_t* h2d_bytes);
+
+// a var-length host column at the rows a chunk holds (its sel rows, else every physical row): offsets present,
+// offsets[length] >= offsets[0], data present when there are bytes, and each row r with offsets[r] <= offsets[r+1],
+// both within [offsets[0], offsets[length]]; TG_ERR_INVALID otherwise
+int check_varlen_rows(const tg_column& c, const tg_chunk* chk);
 
 // borrow a validated device-resident chunk (no sel vector) as a column view of its needed columns; no copy
 int device_view(const tg_chunk* chk, int ncols, const std::vector<char>& needed, const std::vector<int>& elem, DevCols& v);

@@ -13,20 +13,29 @@ from . import abi
 from .plan import AggPlan, JoinPlan
 
 
-def dev_chunk(cols: Sequence[torch.Tensor], nulls: Optional[Sequence[Optional[torch.Tensor]]] = None):
+def dev_chunk(cols: Sequence, nulls: Optional[Sequence[Optional[torch.Tensor]]] = None):
     """tg_chunk whose pointers are device addresses of 1-D int64/float64/float32 CUDA tensors, or (n, 40) uint8 tensors of
-    MyDecimal cells (a DECIMAL column)."""
+    MyDecimal cells (a DECIMAL column), or (offsets, bytes) pairs of an int64 and a uint8 CUDA tensor (a string column:
+    row r is bytes[offsets[r]:offsets[r + 1]])."""
     n = len(cols)
     arr = (abi.TgColumn * max(n, 1))()
     for i, t in enumerate(cols):
+        nb = nulls[i] if nulls is not None else None
+        arr[i].null_bitmap = nb.data_ptr() if nb is not None else None
+        if isinstance(t, tuple):
+            offs, data = t
+            assert offs.is_cuda and data.is_cuda and offs.dtype == torch.int64 and data.dtype == torch.uint8
+            arr[i].length = offs.shape[0] - 1
+            arr[i].offsets = offs.data_ptr()
+            arr[i].data = data.data_ptr() if data.numel() else None
+            arr[i].elem_len = -1
+            continue
         dec = t.dim() == 2 and t.dtype == torch.uint8 and t.shape[1] == 40
         assert t.is_cuda and (t.dim() == 1 or dec) and t.is_contiguous()
         arr[i].length = t.shape[0]
         arr[i].data = t.data_ptr()
         arr[i].elem_len = 40 if dec else t.element_size()
         arr[i].offsets = None
-        nb = nulls[i] if nulls is not None else None
-        arr[i].null_bitmap = nb.data_ptr() if nb is not None else None
     s = abi.TgChunk()
     s.ncols = n
     s.cols = C.cast(arr, C.POINTER(abi.TgColumn))
@@ -90,15 +99,19 @@ class DeviceJoin:
 
 
 class DeviceAgg:
+    """One tg_agg handle driven with device-resident chunks.  A string column is pushed as an (offsets, bytes) tensor
+    pair; finish() returns, for a string result, the device pointer of its bytes, and its offsets in `offsets`."""
+
     def __init__(self, plan: AggPlan):
         self.lib = abi.load_lib()
         self.plan = plan
-        desc, self._keep = plan.to_struct_ex2()
+        desc, self._keep = plan.to_struct_ex3()
         self.h = C.c_void_p()
-        abi.check(self.lib.tg_agg_open_ex2(C.byref(desc), C.byref(self.h)))
+        abi.check(self.lib.tg_agg_open_ex3(C.byref(desc), C.byref(self.h)))
         self.n_out = len(plan.funcs)
+        self.offsets: List[int] = [0] * self.n_out
 
-    def push(self, cols: Sequence[torch.Tensor], nulls=None) -> None:
+    def push(self, cols: Sequence, nulls=None) -> None:
         ck = dev_chunk(cols, nulls)
         abi.check(self.lib.tg_agg_push_dev(self.h, C.byref(ck)))
 
@@ -106,9 +119,16 @@ class DeviceAgg:
         abi.check(self.lib.tg_agg_finish(self.h))
         out_cols = (C.c_void_p * self.n_out)()
         out_nulls = (C.c_void_p * self.n_out)()
+        out_offs = (C.c_void_p * self.n_out)()
         rows = C.c_int64(0)
-        abi.check(self.lib.tg_agg_result_dev(self.h, C.byref(rows), out_cols, out_nulls))
+        abi.check(self.lib.tg_agg_result_dev_ex(self.h, C.byref(rows), out_cols, out_nulls, out_offs))
+        self.offsets = [p or 0 for p in out_offs]
         return rows.value, [p or 0 for p in out_cols], [p or 0 for p in out_nulls]
+
+    def string_stats(self) -> abi.TgAggStringStats:
+        s = abi.TgAggStringStats()
+        abi.check(self.lib.tg_agg_get_string_stats(self.h, C.byref(s)))
+        return s
 
     def stats(self) -> abi.TgAggStats:
         s = abi.TgAggStats()

@@ -17,7 +17,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 from . import abi
-from .chunk import DECIMAL_DTYPE, Chunk, Column, MutChunk, concat_columns
+from .chunk import DECIMAL_DTYPE, VARLEN, Chunk, Column, MutChunk, concat_columns
 from .plan import AggPlan, FieldType, JoinPlan
 
 MAX_CHUNK_SIZE = 1024  # tidb_max_chunk_size default (vardef/tidb_vars.go:1464)
@@ -203,10 +203,12 @@ class HashAggExec(Executor):
     def open(self) -> None:
         super().open()
         self._lib = abi.load_lib()
-        desc, self._keep = self.plan.to_struct_ex2()
+        desc, self._keep = self.plan.to_struct_ex3()
         self._h = C.c_void_p()
-        abi.check(self._lib.tg_agg_open_ex2(C.byref(desc), C.byref(self._h)))
+        abi.check(self._lib.tg_agg_open_ex3(C.byref(desc), C.byref(self._h)))
         self._prepared = False
+        self._str = self.plan.string_results()
+        self._data_cap = 64 << 10
 
     def next(self, required_rows: int = MAX_CHUNK_SIZE) -> Chunk:
         if not self._prepared:
@@ -219,12 +221,28 @@ class HashAggExec(Executor):
                 abi.check(self._lib.tg_agg_push(self._h, C.byref(cs)))
             abi.check(self._lib.tg_agg_finish(self._h))
             self._prepared = True
-        if self._out is None or self._out.capacity < required_rows:
-            self._out = _out_chunk(self.schema, max(required_rows, 8))
-        n = C.c_int64(0)
-        abi.check(self._lib.tg_agg_next(self._h, C.byref(self._out.struct), C.c_int64(required_rows), C.byref(n)))
-        cols = self._out.columns(n.value)
-        return Chunk([Column(v, nl if nl.any() else None) for v, nl in cols])
+        if not any(self._str):
+            if self._out is None or self._out.capacity < required_rows:
+                self._out = _out_chunk(self.schema, max(required_rows, 8))
+            n = C.c_int64(0)
+            abi.check(self._lib.tg_agg_next(self._h, C.byref(self._out.struct), C.c_int64(required_rows), C.byref(n)))
+            cols = self._out.columns(n.value)
+            return Chunk([Column(v, nl if nl.any() else None) for v, nl in cols])
+        # string results (FIRSTROW of a string GROUP BY column): var-length output columns, whose byte buffers grow
+        # until the next row fits
+        while True:
+            if self._out is None or self._out.capacity < required_rows:
+                els = [VARLEN if s else np.dtype(np_dtype_of(t)).itemsize for s, t in zip(self._str, self.schema)]
+                self._out = MutChunk(els, max(required_rows, 8), [np.uint8 if s else np_dtype_of(t) for s, t in zip(self._str, self.schema)],
+                                     self._data_cap)
+            n = C.c_int64(0)
+            rc = self._lib.tg_agg_next_ex(self._h, C.byref(self._out.struct), self._out.varlen, C.c_int64(required_rows), C.byref(n))
+            if rc != abi.TG_ERR_CAPACITY:
+                break
+            self._data_cap *= 4
+            self._out = None
+        abi.check(rc)
+        return Chunk([self._out.column(i, n.value) for i in range(len(self._str))])
 
     def stats(self) -> abi.TgAggStats:
         s = abi.TgAggStats()
@@ -234,6 +252,11 @@ class HashAggExec(Executor):
     def distinct_stats(self) -> abi.TgAggDistinctStats:
         s = abi.TgAggDistinctStats()
         abi.check(self._lib.tg_agg_get_distinct_stats(self._h, C.byref(s)))
+        return s
+
+    def string_stats(self) -> abi.TgAggStringStats:
+        s = abi.TgAggStringStats()
+        abi.check(self._lib.tg_agg_get_string_stats(self._h, C.byref(s)))
         return s
 
     def close(self) -> None:

@@ -20,12 +20,13 @@ UNSPECIFIED_LENGTH = -1   # types.UnspecifiedLength
 
 @dataclass
 class FieldType:
-    """types.FieldType reduced to what the path needs: MySQL type code + flag bits, and GetFlen() / GetDecimal() (the
-    precision and scale of a DECIMAL column; -1 = not given)."""
+    """types.FieldType reduced to what the path needs: MySQL type code + flag bits, GetFlen() / GetDecimal() (the
+    precision and scale of a DECIMAL column; -1 = not given) and GetCollate() (the MySQL collation id of a string column)."""
     tp: int = abi.TYPE_LONGLONG
     flag: int = 0
     flen: int = UNSPECIFIED_LENGTH
     decimal: int = UNSPECIFIED_LENGTH
+    collation: int = abi.COLLATION_UTF8MB4_BIN
 
     @property
     def not_null(self) -> bool:
@@ -265,6 +266,18 @@ class AggPlan:
         if any(f.distinct for f in self.funcs):
             a = (C.c_uint8 * len(self.funcs))(*[int(f.distinct) for f in self.funcs]); keep.append(a); d.has_distinct = a
         return d, keep
+
+    def to_struct_ex3(self) -> Tuple[abi.TgAggDescEx3, list]:
+        """tg_agg_desc_ex3: to_struct_ex2() plus the collation id of every child column"""
+        ex2, keep = self.to_struct_ex2()
+        d = abi.TgAggDescEx3()
+        d.ex2 = ex2
+        a = _i32([t.collation for t in self.col_types]); keep.append(a); d.col_collation = a
+        return d, keep
+
+    def string_results(self) -> List[bool]:
+        """per function: its result is a string column (FIRSTROW of a string column)"""
+        return [f.name == abi.AGG_FIRSTROW and f.arg_col >= 0 and self.col_types[f.arg_col].tp in abi.STRING_TYPES for f in self.funcs]
 
 
 # ---------------------------------------------------------------------------------------------------------------
