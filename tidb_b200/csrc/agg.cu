@@ -938,10 +938,15 @@ struct tg_agg {
   AggImpl* impl = nullptr;
 };
 
-struct AggImpl : DeviceHandle {
+// What the gate compiles from a descriptor (agg_compile): the child schema, the group keys, the device functions and
+// their state words, and the shape of every result.  tg_agg_supported* compiles one on the stack; a handle keeps its own.
+struct AggPlan {
   int ncols = 0;
   std::vector<int> types, elem;
   std::vector<uint32_t> flags;
+  std::vector<int> col_flen, col_dec;   // tg_agg_desc_ex: precision / scale per child column, -1 = not given
+  std::vector<char> str_col;            // a string column of a descriptor with collations (tg_agg_desc_ex3)
+  std::vector<int> coll;                // per child column: StrColl of its collation (COLL_NONE: not given / not one)
   std::vector<char> needed;
   int group_col = -1;          // -1: no GROUP BY (several GROUP BY columns: the first one)
   int gk_kind = GK_NONE;
@@ -949,36 +954,23 @@ struct AggImpl : DeviceHandle {
   int nkw = 0;                 // > 0: multi-key table (key words per slot)
   AggSpec spec{};
   int nstates = 0;
-  std::vector<char> out_nullable;
-  std::vector<int> out_elem;   // bytes per result cell: 8, or 40 for a DECIMAL (MyDecimal) column
-  std::vector<int> col_flen, col_dec;   // tg_agg_desc_ex: precision / scale per child column, -1 = not given
   std::vector<char> dec_decode;         // DECIMAL argument column of SUM / AVG / MIN / MAX: k_dec_to_scaled runs on every batch
-  std::vector<std::unique_ptr<DevBuf>> dscaled;   // its int64 value * 10^scale, one pooled scratch column per such column
   bool wide = false;        // a DECIMAL SUM / AVG of a product: the WIDE kernel instantiations
   bool dec_out = false;     // a DECIMAL result column: k_agg_finalize<true, wide>
+  std::vector<char> out_nullable;
+  std::vector<int> out_elem;   // bytes per result cell: 8, or 40 for a DECIMAL (MyDecimal) column
 
   // DISTINCT arguments (tg_agg_desc_ex2): set j dedups child column dist_cols[j] and feeds the virtual column ncols + j
   // (the column's values, null bitmap = the set's mark bits), which the DISTINCT functions read as their argument
   std::vector<char> fdistinct;          // per function: COUNT / SUM / AVG with HasDistinct
   std::vector<int> dist_cols;
   int dist_gkw = 0;                     // group key words of a set record (the value word follows)
-  struct SetMem { DevBuf mem, mark; DistinctSet t{}; };
-  std::vector<std::unique_ptr<SetMem>> dsets;
-  DevBuf dcounters;                     // k_agg_distinct_mark: [0] rows deferred [1] pairs inserted
-  bool broken = false;                  // a push failed after a set was touched: every later push / finish fails
-  tg_agg_distinct_stats dstats{};
 
   // string columns (tg_agg_desc_ex3): a string GROUP BY column is encoded to ids by its dictionary (str_dict.cuh) before
   // the DISTINCT sets and the update kernels see the batch; its FIRSTROW finalizes to the id, then gathers the bytes
-  std::vector<int> coll;                // per child column: StrColl of its collation (COLL_NONE: not given / not one)
   std::vector<char> is_str;             // a string column the plan reads (GROUP BY key or COUNT argument)
   std::vector<char> needed_fixed;       // `needed` without the string columns (validate_chunk / device_view)
   std::vector<int> dict_of;             // per child column: its dictionary, -1
-  std::vector<std::unique_ptr<StrDict>> dicts;
-  std::vector<std::unique_ptr<DevBuf>> sids, doffs;   // per child column: the id column of a batch, a batch's offsets
-  DevBuf sflag;                         // bad-offsets flag of a device push
-  int64_t str_ords = 0;                 // logical rows encoded so far: the ordinal of the next batch's first row
-  double encode_ms = 0;
   std::vector<int> out_dict;            // per result: the dictionary of a string result, -1
   // FIRSTROW of a PAD-collation string key with several GROUP BY columns: the dictionary's earliest row of a key value
   // is not each group's, so the encode pass writes a tail column (ordinal << kTailBits | trailing spaces cut) and a
@@ -986,6 +978,22 @@ struct AggImpl : DeviceHandle {
   int n_out = 0;                        // functions of the descriptor; spec.n counts the hidden MINs after them
   std::vector<int> tail_col;            // per child column: the virtual column of its tail values, -1
   std::vector<int> tail_fn;             // per result: the hidden MIN of its tail values, -1
+};
+
+struct AggImpl : DeviceHandle, AggPlan {
+  std::vector<std::unique_ptr<DevBuf>> dscaled;   // per DECIMAL argument column: its int64 value * 10^scale, pooled scratch
+
+  struct SetMem { DevBuf mem, mark; DistinctSet t{}; };
+  std::vector<std::unique_ptr<SetMem>> dsets;
+  DevBuf dcounters;                     // k_agg_distinct_mark: [0] rows deferred [1] pairs inserted
+  bool broken = false;                  // a push failed after a set was touched: every later push / finish fails
+  tg_agg_distinct_stats dstats{};
+
+  std::vector<std::unique_ptr<StrDict>> dicts;
+  std::vector<std::unique_ptr<DevBuf>> sids, doffs;   // per child column: the id column of a batch, a batch's offsets
+  DevBuf sflag;                         // bad-offsets flag of a device push
+  int64_t str_ords = 0;                 // logical rows encoded so far: the ordinal of the next batch's first row
+  double encode_ms = 0;
   std::vector<std::unique_ptr<DevBuf>> stails;   // per child column: a batch's tail values
   std::vector<std::unique_ptr<DevBuf>> out_soffs, out_sbytes;
   std::vector<std::vector<int64_t>> host_soffs;   // the string results' offsets, read back once at finish
@@ -1013,44 +1021,49 @@ struct AggImpl : DeviceHandle {
 
 namespace tg {
 
-static int dec_expr_rules(const AggImpl* a, const tg_agg_func& f);
 static long long pow10_i64(int k) { long long p = 1; while (k-- > 0) p *= 10; return p; }
 
-// A function over a DECIMAL column (tg_agg_desc_ex): TG_OK when it is offloaded, else the status and message
-static int dec_arg_rules(const AggImpl* a, const tg_agg_func& f) {
-  const int c = f.arg_col, p = a->col_flen[c], s = a->col_dec[c];
-  if (p < 0 || s < 0) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL argument column needs its precision and scale (tg_agg_desc_ex col_flen / col_decimal)");
-  if (p > 18) return fail(TG_ERR_UNSUPPORTED, "DECIMAL arguments are offloaded up to precision 18 (one int64 at the column's scale)");
-  if (p < 1 || s > p) return fail(TG_ERR_INVALID, "a DECIMAL column needs 1 <= flen and 0 <= decimal <= flen");
-  if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "aggregates over DECIMAL columns are offloaded in Complete mode only (no DECIMAL partial results)");
-  if (f.arg_expr == TG_ARGEXPR_MUL || f.arg_expr == TG_ARGEXPR_MUL_CSUB) return dec_expr_rules(a, f);
-  if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL column is not offloaded in this argument expression");
-  switch (f.name) {
-    case TG_AGG_COUNT:   // reads the null bitmap only
-      return f.ret_type == TG_TYPE_NEWDECIMAL ? fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG / MIN / MAX only") : TG_OK;
-    case TG_AGG_SUM: case TG_AGG_AVG: case TG_AGG_MIN: case TG_AGG_MAX:
-      if (f.ret_type != TG_TYPE_NEWDECIMAL) return fail(TG_ERR_UNSUPPORTED, "SUM / AVG / MIN / MAX over a DECIMAL column need a DECIMAL ret_type");
-      if (f.name == TG_AGG_AVG ? (f.ret_frac < s || f.ret_frac > 30) : f.ret_frac != s)
-        return fail(TG_ERR_INVALID, f.name == TG_AGG_AVG ? "DECIMAL AVG scale must be the column's scale .. 30"
-                                                        : "DECIMAL SUM / MIN / MAX of a DECIMAL column have the column's scale");
-      return TG_OK;
-    default: return fail(TG_ERR_UNSUPPORTED, "this aggregate function is not offloaded over a DECIMAL column");
-  }
+// TG_TYPE_VARCHAR, VARSTRING, STRING and the BLOB / TEXT types (ENUM, SET, JSON and BIT are var-length, not strings)
+static bool agg_string_type(int32_t tp) {
+  return tp == TG_TYPE_VARCHAR || tp == TG_TYPE_VARSTRING || tp == TG_TYPE_STRING || (tp >= TG_TYPE_TINY_BLOB && tp <= TG_TYPE_BLOB);
+}
+
+// What a function's argument is, once the schema is read: the class decides which rules the function runs
+enum ArgClass { ARG_NONE, ARG_INT, ARG_REAL, ARG_DEC, ARG_DEC_PRODUCT, ARG_STR, ARG_OTHER };
+static int arg_class(const AggPlan* p, const tg_agg_func& f) {
+  if (f.arg_col < 0 || f.arg_col >= p->ncols) return ARG_NONE;
+  const int t = p->types[f.arg_col];
+  if (p->str_col[f.arg_col]) return ARG_STR;
+  if (t == TG_TYPE_NEWDECIMAL) return f.arg_expr == TG_ARGEXPR_MUL || f.arg_expr == TG_ARGEXPR_MUL_CSUB ? ARG_DEC_PRODUCT : ARG_DEC;
+  if (t == TG_TYPE_DOUBLE) return ARG_REAL;
+  return is_int_family(t) ? ARG_INT : ARG_OTHER;
+}
+
+// A DECIMAL result keeps the argument's scale s, except AVG, which rounds to s .. 30 digits (typeInfer4Sum / typeInfer4Avg)
+static int ret_frac_rule(const tg_agg_func& f, int s, const char* avg_msg, const char* msg) {
+  if (f.name == TG_AGG_AVG ? (f.ret_frac < s || f.ret_frac > 30) : f.ret_frac != s) return fail(TG_ERR_INVALID, f.name == TG_AGG_AVG ? avg_msg : msg);
+  return TG_OK;
+}
+
+// A DECIMAL argument column is decoded to one int64 at its scale: it needs its precision (1..18) and scale
+static int dec_col_rules(const AggPlan* p, int c) {
+  const int prec = p->col_flen[c], s = p->col_dec[c];
+  if (prec < 0 || s < 0) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL argument column needs its precision and scale (tg_agg_desc_ex col_flen / col_decimal)");
+  if (prec > 18) return fail(TG_ERR_UNSUPPORTED, "DECIMAL arguments are offloaded up to precision 18 (one int64 at the column's scale)");
+  if (prec < 1 || s > prec) return fail(TG_ERR_INVALID, "a DECIMAL column needs 1 <= flen and 0 <= decimal <= flen");
+  return TG_OK;
 }
 
 // SUM / AVG of a * b or a * (c - b) over two DECIMAL(p <= 18) columns (dec_arg_rules has checked a and the mode): the exact
 // product (DecimalMul, mydecimal.go:2041) has scale s = s_a + s_b, and c - b (DecimalSub) is exact at scale s_b
-static int dec_expr_rules(const AggImpl* a, const tg_agg_func& f) {
+static int dec_product_rules(const AggPlan* p, const tg_agg_func& f) {
   const int c2 = f.arg_col2;
-  if (c2 < 0 || c2 >= a->ncols || a->types[c2] != TG_TYPE_NEWDECIMAL)
+  if (c2 < 0 || c2 >= p->ncols || p->types[c2] != TG_TYPE_NEWDECIMAL)
     return fail(TG_ERR_UNSUPPORTED, "a DECIMAL argument expression takes two DECIMAL columns");
-  const int p2 = a->col_flen[c2], s2 = a->col_dec[c2];
-  if (p2 < 0 || s2 < 0) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL argument column needs its precision and scale (tg_agg_desc_ex col_flen / col_decimal)");
-  if (p2 > 18) return fail(TG_ERR_UNSUPPORTED, "DECIMAL arguments are offloaded up to precision 18 (one int64 at the column's scale)");
-  if (p2 < 1 || s2 > p2) return fail(TG_ERR_INVALID, "a DECIMAL column needs 1 <= flen and 0 <= decimal <= flen");
+  TG_TRY(dec_col_rules(p, c2));
   if (f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) return fail(TG_ERR_UNSUPPORTED, "argument expressions are fused for SUM / AVG only");
   if (f.ret_type != TG_TYPE_NEWDECIMAL) return fail(TG_ERR_UNSUPPORTED, "SUM / AVG of a DECIMAL product need a DECIMAL ret_type");
-  const int s = a->col_dec[f.arg_col] + s2;
+  const int s2 = p->col_dec[c2], s = p->col_dec[f.arg_col] + s2;
   // TiDB types the product with frac min(s, 30) but keeps digitsFrac min(s, 31) in the value: past 30 the two disagree
   if (s > 30) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL product is offloaded up to scale 30 (s_a + s_b)");
   if (f.arg_expr == TG_ARGEXPR_MUL_CSUB) {   // c * 10^s_b - b must fit int64: |c| * 10^s_b <= 10^18 keeps it below 2 * 10^18
@@ -1059,33 +1072,55 @@ static int dec_expr_rules(const AggImpl* a, const tg_agg_func& f) {
     if (!std::isfinite(c) || c != std::trunc(c) || std::fabs(c) > lim)
       return fail(TG_ERR_UNSUPPORTED, "a DECIMAL c - b takes an integer constant c with |c| * 10^scale(b) <= 10^18");
   }
-  if (f.name == TG_AGG_AVG ? (f.ret_frac < s || f.ret_frac > 30) : f.ret_frac != s)
-    return fail(TG_ERR_INVALID, f.name == TG_AGG_AVG ? "DECIMAL AVG of a product: scale must be s_a + s_b .. 30"
-                                                    : "DECIMAL SUM of a product has the scale s_a + s_b");
-  return TG_OK;
+  return ret_frac_rule(f, s, "DECIMAL AVG of a product: scale must be s_a + s_b .. 30", "DECIMAL SUM of a product has the scale s_a + s_b");
+}
+
+// A function over a DECIMAL column (tg_agg_desc_ex), alone or in a product: TG_OK when it is offloaded
+static int dec_arg_rules(const AggPlan* p, const tg_agg_func& f) {
+  TG_TRY(dec_col_rules(p, f.arg_col));
+  if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "aggregates over DECIMAL columns are offloaded in Complete mode only (no DECIMAL partial results)");
+  if (f.arg_expr == TG_ARGEXPR_MUL || f.arg_expr == TG_ARGEXPR_MUL_CSUB) return dec_product_rules(p, f);
+  if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL column is not offloaded in this argument expression");
+  switch (f.name) {
+    case TG_AGG_COUNT:   // reads the null bitmap only
+      return f.ret_type == TG_TYPE_NEWDECIMAL ? fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG / MIN / MAX only") : TG_OK;
+    case TG_AGG_SUM: case TG_AGG_AVG: case TG_AGG_MIN: case TG_AGG_MAX:
+      if (f.ret_type != TG_TYPE_NEWDECIMAL) return fail(TG_ERR_UNSUPPORTED, "SUM / AVG / MIN / MAX over a DECIMAL column need a DECIMAL ret_type");
+      return ret_frac_rule(f, p->col_dec[f.arg_col], "DECIMAL AVG scale must be the column's scale .. 30",
+                           "DECIMAL SUM / MIN / MAX of a DECIMAL column have the column's scale");
+    default: return fail(TG_ERR_UNSUPPORTED, "this aggregate function is not offloaded over a DECIMAL column");
+  }
+}
+
+// DECIMAL SUM / AVG of an integer column (typeInfer4Sum / typeInfer4Avg, aggregation/base_func.go); any other ret_type
+// keeps the result type each function has always had here
+static int dec_result_rules(const AggPlan* p, const tg_agg_func& f) {
+  if (f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG only");
+  if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG are offloaded in Complete mode only (no DECIMAL partial results)");
+  if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG take a plain column argument");
+  if (f.arg_col < 0 || f.arg_col >= p->ncols) return fail(TG_ERR_INVALID, "aggregate argument column out of range");
+  const int t = p->types[f.arg_col];
+  if (!is_int_family(t) || t == TG_TYPE_DURATION || p->elem[f.arg_col] != 8)
+    return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG are offloaded over 8-byte integer columns only");
+  return ret_frac_rule(f, 0, "DECIMAL AVG scale must be 0..30", "DECIMAL SUM of an integer column has scale 0");
 }
 
 // COUNT / SUM / AVG with HasDistinct (tg_agg_desc_ex2), checked before the rules of the same function without it, which
 // must accept it too: TG_OK when its dedup pass is offloaded, else the status and message
-static int distinct_rules(const AggImpl* a, const tg_agg_func& f) {
-  if (f.arg_col < 0 || f.arg_col >= a->ncols) return fail(TG_ERR_INVALID, "a DISTINCT aggregate needs an argument column");
+static int distinct_rules(const AggPlan* p, const tg_agg_func& f) {
+  if (f.arg_col < 0 || f.arg_col >= p->ncols) return fail(TG_ERR_INVALID, "a DISTINCT aggregate needs an argument column");
   if (f.name == TG_AGG_FIRSTROW) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW with DISTINCT is not offloaded");
   if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates are offloaded in Complete mode only");
   if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates take a plain column argument");
   if (f.name == TG_AGG_COUNT && f.arg_col2 >= 0) return fail(TG_ERR_UNSUPPORTED, "COUNT(DISTINCT a, b) over several arguments is not offloaded");
-  const int t = a->types[f.arg_col];
-  if (!((is_int_family(t) && a->elem[f.arg_col] == 8) || t == TG_TYPE_DOUBLE || t == TG_TYPE_NEWDECIMAL))
+  const int t = p->types[f.arg_col];
+  if (!((is_int_family(t) && p->elem[f.arg_col] == 8) || t == TG_TYPE_DOUBLE || t == TG_TYPE_NEWDECIMAL))
     return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates are offloaded over integer-family, DOUBLE and DECIMAL(p <= 18) columns");
   return TG_OK;
 }
 
-// TG_TYPE_VARCHAR, VARSTRING, STRING and the BLOB / TEXT types (ENUM, SET, JSON and BIT are var-length, not strings)
-static bool agg_string_type(int32_t tp) {
-  return tp == TG_TYPE_VARCHAR || tp == TG_TYPE_VARSTRING || tp == TG_TYPE_STRING || (tp >= TG_TYPE_TINY_BLOB && tp <= TG_TYPE_BLOB);
-}
-
 // A function over a string column (tg_agg_desc_ex3): TG_OK when it is offloaded, else the status and message
-static int str_arg_rules(const AggImpl* a, const tg_agg_func& f) {
+static int str_arg_rules(const AggPlan* p, const tg_agg_func& f) {
   if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "a string column is not offloaded in an argument expression");
   switch (f.name) {
     case TG_AGG_COUNT:   // reads the null bitmap only
@@ -1093,231 +1128,228 @@ static int str_arg_rules(const AggImpl* a, const tg_agg_func& f) {
       if (f.ret_type == TG_TYPE_NEWDECIMAL) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG / MIN / MAX only");
       return TG_OK;
     case TG_AGG_FIRSTROW:
-      if (a->dict_of[f.arg_col] < 0) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW of a string column is offloaded only for GROUP BY columns");
+      if (p->dict_of[f.arg_col] < 0) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW of a string column is offloaded only for GROUP BY columns");
       return TG_OK;
     default: return fail(TG_ERR_UNSUPPORTED, "only FIRSTROW (of a GROUP BY column) and COUNT are offloaded over string columns");
   }
 }
 
-static int agg_setup(AggImpl* a, const tg_agg_desc* d, const int32_t* col_flen, const int32_t* col_dec, const uint8_t* has_distinct = nullptr,
-                     const int32_t* col_coll = nullptr) {
-  if (!d) return fail(TG_ERR_INVALID, "desc is NULL");
-  if (d->n_cols <= 0 || d->n_cols > TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "child schema must have 1..16 columns");
-  a->ncols = d->n_cols;
-  a->types.assign(d->col_types, d->col_types + d->n_cols);
-  a->flags.resize(d->n_cols);
-  for (int i = 0; i < d->n_cols; i++) a->flags[i] = d->col_flags ? d->col_flags[i] : 0;
-  a->elem.resize(d->n_cols);
-  for (int i = 0; i < d->n_cols; i++) a->elem[i] = fixed_len(a->types[i]);
-  a->col_flen.assign(d->n_cols, -1); a->col_dec.assign(d->n_cols, -1);
-  for (int i = 0; i < d->n_cols; i++) {
-    if (col_flen) a->col_flen[i] = col_flen[i];
-    if (col_dec) a->col_dec[i] = col_dec[i];
+static AggFuncDev func_dev(const tg_agg_func& f) {   // no state words yet, an 8-byte result
+  return AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, -1, 0, -1, -1, f.arg_const, 0};
+}
+
+// The state words of one function: its value in `words` words (1; 2 or 3 for the 128 / 192-bit sum of a DECIMAL SUM /
+// AVG: dec3_apply / sdec3_apply find them one state stride apart, so they are consecutive), then a non-NULL count
+static void add_states(AggPlan* p, AggFuncDev& o, int words, bool count) {
+  o.s0 = p->nstates++;
+  if (words > 1) o.s2 = p->nstates++;
+  if (words > 2) o.s3 = p->nstates++;
+  if (count) o.s1 = p->nstates++;
+}
+
+static bool nullable_col(const AggPlan* p, int c) { return !(p->flags[c] & TG_FLAG_NOT_NULL); }
+
+static int compile_schema(AggPlan* p, const tg_agg_desc_ex3& d) {
+  const tg_agg_desc& b = d.ex2.ex.base;
+  if (b.n_cols <= 0 || b.n_cols > TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "child schema must have 1..16 columns");
+  p->ncols = b.n_cols;
+  for (int c = 0; c < b.n_cols; c++) {
+    const int t = b.col_types[c];
+    const bool str = d.col_collation && agg_string_type(t);
+    p->types.push_back(t);
+    p->flags.push_back(b.col_flags ? b.col_flags[c] : 0);
+    p->elem.push_back(fixed_len(t));
+    p->col_flen.push_back(d.ex2.ex.col_flen ? d.ex2.ex.col_flen[c] : -1);
+    p->col_dec.push_back(d.ex2.ex.col_decimal ? d.ex2.ex.col_decimal[c] : -1);
+    p->str_col.push_back(str);
+    p->coll.push_back(str ? coll_of_id(d.col_collation[c]) : COLL_NONE);
   }
-  a->dec_decode.assign(d->n_cols, 0);
-  a->needed.assign(d->n_cols, 0);
-  a->coll.assign(d->n_cols, COLL_NONE);
-  a->dict_of.assign(d->n_cols, -1);
-  for (int i = 0; i < d->n_cols; i++) if (col_coll && agg_string_type(a->types[i])) a->coll[i] = coll_of_id(col_coll[i]);
-  int ndicts = 0;
-  if (d->n_group_by > TG_MAX_GROUP_COLS) return fail(TG_ERR_UNSUPPORTED, "GPU hash aggregation handles up to 4 GROUP BY columns");
-  a->group_col = -1; a->gk_kind = GK_NONE; a->nkw = 0;
-  a->group_cols.clear(); a->group_kinds.clear();
+  p->needed.assign(b.n_cols, 0);
+  p->dec_decode.assign(b.n_cols, 0);
+  p->dict_of.assign(b.n_cols, -1);
+  return TG_OK;
+}
+
+static int compile_group_keys(AggPlan* p, const tg_agg_desc& b) {
+  if (b.n_group_by > TG_MAX_GROUP_COLS) return fail(TG_ERR_UNSUPPORTED, "GPU hash aggregation handles up to 4 GROUP BY columns");
   bool any_nullable = false;
-  for (int q = 0; q < d->n_group_by; q++) {
-    int g = d->group_by_cols[q];
-    if (g < 0 || g >= a->ncols) return fail(TG_ERR_INVALID, "group-by column out of range");
-    int kind;
-    const bool str = col_coll && agg_string_type(a->types[g]);
-    if (is_int_family(a->types[g])) kind = GK_I64;
-    else if (a->types[g] == TG_TYPE_DOUBLE) kind = GK_F64;
-    else if (str) {   // encoded to a dense int64 id column (encode_strings)
-      if (a->coll[g] == COLL_NONE) return fail(TG_ERR_UNSUPPORTED, "string GROUP BY collation not offloaded (binary, *_bin and utf8mb4_0900_bin are)");
-      kind = GK_I64;
-      if (a->dict_of[g] < 0) a->dict_of[g] = ndicts++;
-    }
-    else return fail(TG_ERR_UNSUPPORTED, "GROUP BY column type is not offloaded (int family / double only)");
-    if (a->elem[g] != 8 && !str) return fail(TG_ERR_UNSUPPORTED, "GROUP BY columns must be 8-byte columns");
-    if (q == 0) { a->group_col = g; a->gk_kind = kind; }
-    a->group_cols.push_back(g); a->group_kinds.push_back(kind);
-    any_nullable |= !(a->flags[g] & TG_FLAG_NOT_NULL);
-    a->needed[g] = 1;
+  int ndicts = 0;
+  for (int q = 0; q < b.n_group_by; q++) {
+    const int g = b.group_by_cols[q];
+    if (g < 0 || g >= p->ncols) return fail(TG_ERR_INVALID, "group-by column out of range");
+    const int t = p->types[g];
+    if (!is_int_family(t) && t != TG_TYPE_DOUBLE && !p->str_col[g]) return fail(TG_ERR_UNSUPPORTED, "GROUP BY column type is not offloaded (int family / double only)");
+    if (p->str_col[g]) {   // encoded to a dense int64 id column (encode_strings)
+      if (p->coll[g] == COLL_NONE) return fail(TG_ERR_UNSUPPORTED, "string GROUP BY collation not offloaded (binary, *_bin and utf8mb4_0900_bin are)");
+      if (p->dict_of[g] < 0) p->dict_of[g] = ndicts++;
+    } else if (p->elem[g] != 8) return fail(TG_ERR_UNSUPPORTED, "GROUP BY columns must be 8-byte columns");
+    const int kind = t == TG_TYPE_DOUBLE ? GK_F64 : GK_I64;
+    if (q == 0) { p->group_col = g; p->gk_kind = kind; }
+    p->group_cols.push_back(g); p->group_kinds.push_back(kind);
+    any_nullable |= nullable_col(p, g);
+    p->needed[g] = 1;
   }
-  if (d->n_group_by > 1) a->nkw = d->n_group_by + (any_nullable ? 1 : 0);
-  if (d->n_funcs <= 0 || d->n_funcs > TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "1..12 aggregate functions are offloaded");
-  a->spec.n = d->n_funcs;
-  a->nstates = 0;
-  a->out_nullable.assign(d->n_funcs, 0);
-  a->out_elem.assign(d->n_funcs, 8);
-  a->fdistinct.assign(d->n_funcs, 0);
-  a->out_dict.assign(d->n_funcs, -1);
-  for (int k = 0; k < d->n_funcs; k++) {
-    const tg_agg_func& f = d->funcs[k];
-    AggFuncDev& o = a->spec.f[k];
-    o = AggFuncDev{f.name, f.arg_col, 0, 0, -1, -1, 0, f.arg_col2, f.arg_expr, -1, 0, -1, -1, f.arg_const, 0};
-    if (has_distinct && has_distinct[k]) {
-      if (f.arg_col < 0) return fail(TG_ERR_INVALID, "a DISTINCT aggregate needs an argument column");
-      // MIN / MAX: DISTINCT changes nothing (buildMaxMin ignores HasDistinct)
-      if (f.name != TG_AGG_MIN && f.name != TG_AGG_MAX) { TG_TRY(distinct_rules(a, f)); a->fdistinct[k] = 1; }
-    }
-    const bool distinct = a->fdistinct[k] != 0;
-    const bool str_arg = col_coll && f.arg_col >= 0 && f.arg_col < a->ncols && agg_string_type(a->types[f.arg_col]);
-    if (str_arg) {
-      TG_TRY(str_arg_rules(a, f));
-      if (f.name == TG_AGG_FIRSTROW) a->out_dict[k] = a->dict_of[f.arg_col];
-    }
-    // a DECIMAL(p <= 18, s) argument column (tg_agg_desc_ex): decoded to int64 value * 10^s on every batch, then the integer
-    // update paths run unchanged
-    const bool dec_arg = f.arg_col >= 0 && f.arg_col < a->ncols && a->types[f.arg_col] == TG_TYPE_NEWDECIMAL;
-    if (dec_arg) TG_TRY(dec_arg_rules(a, f));
-    // DECIMAL SUM / AVG of an integer column (typeInfer4Sum / typeInfer4Avg, aggregation/base_func.go); any other ret_type
-    // keeps the result type each function has always had here
-    const bool dec = f.ret_type == TG_TYPE_NEWDECIMAL;
-    if (dec && !dec_arg) {
-      if (f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) return fail(TG_ERR_UNSUPPORTED, "a DECIMAL result is offloaded for SUM / AVG only");
-      if (f.mode != TG_AGGMODE_COMPLETE) return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG are offloaded in Complete mode only (no DECIMAL partial results)");
-      if (f.arg_expr != TG_ARGEXPR_COL) return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG take a plain column argument");
-      if (f.arg_col < 0 || f.arg_col >= a->ncols) return fail(TG_ERR_INVALID, "aggregate argument column out of range");
-      const int t = a->types[f.arg_col];
-      if (!is_int_family(t) || t == TG_TYPE_DURATION || a->elem[f.arg_col] != 8)
-        return fail(TG_ERR_UNSUPPORTED, "DECIMAL SUM / AVG are offloaded over 8-byte integer columns only");
-      if (f.name == TG_AGG_SUM && f.ret_frac != 0) return fail(TG_ERR_INVALID, "DECIMAL SUM of an integer column has scale 0");
-      if (f.name == TG_AGG_AVG && (f.ret_frac < 0 || f.ret_frac > 30)) return fail(TG_ERR_INVALID, "DECIMAL AVG scale must be 0..30");
-    }
-    if (f.arg_expr != TG_ARGEXPR_COL) {
-      if (f.arg_expr != TG_ARGEXPR_MUL && f.arg_expr != TG_ARGEXPR_MUL_CSUB) return fail(TG_ERR_INVALID, "unknown aggregate argument expression");
-      if ((f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) || f.mode != TG_AGGMODE_COMPLETE)
-        return fail(TG_ERR_UNSUPPORTED, "argument expressions are fused for SUM / AVG in Complete mode only");
-      if (!dec_arg && (f.arg_col < 0 || f.arg_col2 < 0 || f.arg_col2 >= d->n_cols || a->types[f.arg_col] != TG_TYPE_DOUBLE || a->types[f.arg_col2] != TG_TYPE_DOUBLE))
-        return fail(TG_ERR_UNSUPPORTED, "argument expressions take two DOUBLE columns");
-      a->needed[f.arg_col2] = 1;
-    }
-    if (f.mode != TG_AGGMODE_COMPLETE && f.mode != TG_AGGMODE_FINAL) return fail(TG_ERR_UNSUPPORTED, "only Complete and Final aggregate modes are offloaded");
-    o.final_mode = f.mode == TG_AGGMODE_FINAL;
-    if (f.arg_col >= a->ncols || f.arg_col2 >= a->ncols) return fail(TG_ERR_INVALID, "aggregate argument column out of range");
-    bool arg_nullable = f.arg_col >= 0 && !(a->flags[f.arg_col] & TG_FLAG_NOT_NULL);
-    if (f.arg_expr != TG_ARGEXPR_COL && f.arg_col2 >= 0 && f.arg_col2 < d->n_cols && !(a->flags[f.arg_col2] & TG_FLAG_NOT_NULL)) arg_nullable = true;
-    // a DISTINCT argument is NULL on every row that brought no new value: COUNT needs its own count, AVG its divisor
-    if (distinct) arg_nullable = true;
-    if (f.arg_col >= 0) { if (a->elem[f.arg_col] != 8 && !dec_arg && !str_arg) return fail(TG_ERR_UNSUPPORTED, "aggregate arguments must be 8-byte columns"); a->needed[f.arg_col] = 1; }
-    int atype = f.arg_col >= 0 ? a->types[f.arg_col] : TG_TYPE_LONGLONG;
-    o.is_real = atype == TG_TYPE_DOUBLE;
-    o.is_unsigned = f.arg_col >= 0 && !dec_arg && (a->flags[f.arg_col] & TG_FLAG_UNSIGNED) != 0;   // a decoded DECIMAL is a signed int64
-    if (dec_arg && f.name != TG_AGG_COUNT) { o.dec_scale = a->col_dec[f.arg_col]; a->dec_decode[f.arg_col] = 1; }
-    else if (dec) o.dec_scale = 0;
-    if (distinct && dec_arg) a->dec_decode[f.arg_col] = 1;   // COUNT(DISTINCT dec) too: the set is keyed on the value
-    const bool dec_expr = dec_arg && f.arg_expr != TG_ARGEXPR_COL;   // SUM / AVG of a DECIMAL product (dec_expr_rules)
-    if (dec_expr) {
-      const int sb = a->col_dec[f.arg_col2];
-      o.dec_scale += sb;
-      a->dec_decode[f.arg_col2] = 1;
-      if (f.arg_expr == TG_ARGEXPR_MUL_CSUB) o.dec_c = (long long)f.arg_const * pow10_i64(sb);
-    }
-    switch (f.name) {
-      case TG_AGG_COUNT:
-        if (o.final_mode) { if (f.arg_col < 0) return fail(TG_ERR_INVALID, "final COUNT needs the partial count column"); o.s0 = a->nstates++; }
-        else if (f.arg_col >= 0 && arg_nullable) o.s0 = a->nstates++;   // NOT NULL COUNT(x) == COUNT(*) == rows[]
-        break;
-      case TG_AGG_SUM:
-        if (dec) {   // states: low word, high word (a product: middle and top word), non-NULL count (NOT NULL arguments count with rows[])
-          o.s0 = a->nstates++; o.s2 = a->nstates++;
-          if (dec_expr) o.s3 = a->nstates++;
-          if (arg_nullable) o.s1 = a->nstates++;
-          a->out_nullable[k] = 1; a->out_elem[k] = TG_DEC_CELL_BYTES;
-          break;
-        }
-        // SUM(int) yields DECIMAL in TiDB (aggregation/base_func.go:223-245): offloaded only when ret_type asks for it
-        if (f.arg_col < 0 || atype != TG_TYPE_DOUBLE) return fail(TG_ERR_UNSUPPORTED, "SUM is offloaded for DOUBLE arguments only (SUM(int) is DECIMAL)");
-        o.s0 = a->nstates++;
-        if (arg_nullable) o.s1 = a->nstates++;
-        a->out_nullable[k] = 1;
-        break;
-      case TG_AGG_AVG:
-        if (dec) {
-          o.s0 = a->nstates++; o.s2 = a->nstates++;
-          if (dec_expr) o.s3 = a->nstates++;
-          if (arg_nullable) o.s1 = a->nstates++;
-          o.dec_frac = f.ret_frac;
-          a->out_nullable[k] = 1; a->out_elem[k] = TG_DEC_CELL_BYTES;
-          break;
-        }
-        if (o.final_mode) {
-          if (f.arg_col < 0 || f.arg_col2 < 0 || a->types[f.arg_col2] != TG_TYPE_DOUBLE || !is_int_family(a->types[f.arg_col]))
-            return fail(TG_ERR_UNSUPPORTED, "final AVG takes (count BIGINT, sum DOUBLE)");
-          a->needed[f.arg_col2] = 1;
-          o.s0 = a->nstates++; o.s1 = a->nstates++;
-        } else {
-          if (f.arg_col < 0 || atype != TG_TYPE_DOUBLE) return fail(TG_ERR_UNSUPPORTED, "AVG is offloaded for DOUBLE arguments only");
-          o.s0 = a->nstates++;
-          if (arg_nullable) o.s1 = a->nstates++;
-        }
-        a->out_nullable[k] = 1;
-        break;
-      case TG_AGG_MIN: case TG_AGG_MAX:
-        if (f.arg_col < 0 || !(dec_arg || is_int_family(atype) || atype == TG_TYPE_DOUBLE)) return fail(TG_ERR_UNSUPPORTED, "MIN/MAX are offloaded for int family / DOUBLE / DECIMAL");
-        o.s0 = a->nstates++;
-        if (arg_nullable) o.s1 = a->nstates++;
-        a->out_nullable[k] = 1;
-        if (dec_arg) a->out_elem[k] = TG_DEC_CELL_BYTES;   // the signed int64 MIN / MAX at the column's scale
-        break;
-      case TG_AGG_FIRSTROW: {
-        int gi = -1;
-        for (size_t q = 0; q < a->group_cols.size(); q++) if (a->group_cols[q] == f.arg_col) gi = (int)q;
-        if (f.arg_col < 0 || gi < 0) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW is offloaded only for GROUP BY columns (deterministic)");
-        a->out_nullable[k] = !(a->flags[f.arg_col] & TG_FLAG_NOT_NULL);
-        o.arg_col2 = gi | ((a->nkw > (int)a->group_cols.size() ? (int)a->group_cols.size() : 0) << 8);
-        break;
+  p->dist_gkw = b.n_group_by + (any_nullable ? 1 : 0);
+  if (b.n_group_by > 1) p->nkw = p->dist_gkw;
+  return TG_OK;
+}
+
+// The rules of function k that do not depend on its function name: its argument's class decides which ones run
+static int func_rules(AggPlan* p, const tg_agg_desc_ex3& d, int k) {
+  const tg_agg_func& f = d.ex2.ex.base.funcs[k];
+  if (d.ex2.has_distinct && d.ex2.has_distinct[k]) {
+    if (f.arg_col < 0) return fail(TG_ERR_INVALID, "a DISTINCT aggregate needs an argument column");
+    // MIN / MAX: DISTINCT changes nothing (buildMaxMin ignores HasDistinct)
+    if (f.name != TG_AGG_MIN && f.name != TG_AGG_MAX) { TG_TRY(distinct_rules(p, f)); p->fdistinct[k] = 1; }
+  }
+  const int cls = arg_class(p, f);
+  const bool dec_arg = cls == ARG_DEC || cls == ARG_DEC_PRODUCT;
+  if (cls == ARG_STR) {
+    TG_TRY(str_arg_rules(p, f));
+    if (f.name == TG_AGG_FIRSTROW) p->out_dict[k] = p->dict_of[f.arg_col];
+  }
+  if (dec_arg) TG_TRY(dec_arg_rules(p, f));
+  else if (f.ret_type == TG_TYPE_NEWDECIMAL) TG_TRY(dec_result_rules(p, f));
+  if (f.arg_expr != TG_ARGEXPR_COL) {
+    if (f.arg_expr != TG_ARGEXPR_MUL && f.arg_expr != TG_ARGEXPR_MUL_CSUB) return fail(TG_ERR_INVALID, "unknown aggregate argument expression");
+    if ((f.name != TG_AGG_SUM && f.name != TG_AGG_AVG) || f.mode != TG_AGGMODE_COMPLETE)
+      return fail(TG_ERR_UNSUPPORTED, "argument expressions are fused for SUM / AVG in Complete mode only");
+    if (!dec_arg && (cls != ARG_REAL || f.arg_col2 < 0 || f.arg_col2 >= p->ncols || p->types[f.arg_col2] != TG_TYPE_DOUBLE))
+      return fail(TG_ERR_UNSUPPORTED, "argument expressions take two DOUBLE columns");
+    p->needed[f.arg_col2] = 1;
+  }
+  if (f.mode != TG_AGGMODE_COMPLETE && f.mode != TG_AGGMODE_FINAL) return fail(TG_ERR_UNSUPPORTED, "only Complete and Final aggregate modes are offloaded");
+  if (f.arg_col >= p->ncols || f.arg_col2 >= p->ncols) return fail(TG_ERR_INVALID, "aggregate argument column out of range");
+  if (cls != ARG_NONE) {
+    if (p->elem[f.arg_col] != 8 && !dec_arg && cls != ARG_STR) return fail(TG_ERR_UNSUPPORTED, "aggregate arguments must be 8-byte columns");
+    p->needed[f.arg_col] = 1;
+  }
+  return TG_OK;
+}
+
+// The device function, state words and result shape of function k, with the rules that depend on its function name
+static int compile_func(AggPlan* p, const tg_agg_desc_ex3& d, int k) {
+  const tg_agg_func& f = d.ex2.ex.base.funcs[k];
+  AggFuncDev& o = p->spec.f[k] = func_dev(f);
+  TG_TRY(func_rules(p, d, k));
+  const int cls = arg_class(p, f);   // the argument columns are in range now: ARG_NONE is arg_col < 0
+  // a DECIMAL(p <= 18, s) argument column: decoded to int64 value * 10^s on every batch, then the integer update paths run
+  const bool dec_arg = cls == ARG_DEC || cls == ARG_DEC_PRODUCT, dec = f.ret_type == TG_TYPE_NEWDECIMAL;
+  // a DISTINCT argument is NULL on every row that brought no new value: COUNT needs its own count, AVG its divisor
+  const bool distinct = p->fdistinct[k] != 0;
+  const bool nullable = distinct || (cls != ARG_NONE && nullable_col(p, f.arg_col)) ||
+                        (f.arg_expr != TG_ARGEXPR_COL && f.arg_col2 >= 0 && nullable_col(p, f.arg_col2));
+  o.final_mode = f.mode == TG_AGGMODE_FINAL;
+  o.is_real = cls == ARG_REAL;
+  o.is_unsigned = cls != ARG_NONE && !dec_arg && (p->flags[f.arg_col] & TG_FLAG_UNSIGNED) != 0;   // a decoded DECIMAL is a signed int64
+  if (dec_arg && (f.name != TG_AGG_COUNT || distinct)) p->dec_decode[f.arg_col] = 1;   // COUNT(DISTINCT dec): the set is keyed on the value
+  if (dec_arg && f.name != TG_AGG_COUNT) o.dec_scale = p->col_dec[f.arg_col];
+  else if (dec) o.dec_scale = 0;
+  if (cls == ARG_DEC_PRODUCT) {
+    const int sb = p->col_dec[f.arg_col2];
+    o.dec_scale += sb;
+    p->dec_decode[f.arg_col2] = 1;
+    if (f.arg_expr == TG_ARGEXPR_MUL_CSUB) o.dec_c = (long long)f.arg_const * pow10_i64(sb);
+  }
+  p->dec_out |= o.dec_scale >= 0;
+  switch (f.name) {
+    case TG_AGG_COUNT:
+      if (o.final_mode && cls == ARG_NONE) return fail(TG_ERR_INVALID, "final COUNT needs the partial count column");
+      if (o.final_mode || (cls != ARG_NONE && nullable)) add_states(p, o, 1, false);   // NOT NULL COUNT(x) == COUNT(*) == rows[]
+      return TG_OK;
+    case TG_AGG_SUM: case TG_AGG_AVG:
+      p->out_nullable[k] = 1;
+      if (dec) {   // the exact sum (a product's in 3 words), non-NULL count (NOT NULL arguments count with rows[])
+        add_states(p, o, cls == ARG_DEC_PRODUCT ? 3 : 2, nullable);
+        p->wide |= cls == ARG_DEC_PRODUCT;
+        if (f.name == TG_AGG_AVG) o.dec_frac = f.ret_frac;
+        p->out_elem[k] = TG_DEC_CELL_BYTES;
+      } else if (f.name == TG_AGG_AVG && o.final_mode) {
+        if (cls == ARG_NONE || f.arg_col2 < 0 || p->types[f.arg_col2] != TG_TYPE_DOUBLE || !is_int_family(p->types[f.arg_col]))
+          return fail(TG_ERR_UNSUPPORTED, "final AVG takes (count BIGINT, sum DOUBLE)");
+        p->needed[f.arg_col2] = 1;
+        add_states(p, o, 1, true);
+      } else {   // SUM(int) yields DECIMAL in TiDB (aggregation/base_func.go:223-245): offloaded only when ret_type asks for it
+        if (cls != ARG_REAL) return fail(TG_ERR_UNSUPPORTED, f.name == TG_AGG_SUM ? "SUM is offloaded for DOUBLE arguments only (SUM(int) is DECIMAL)"
+                                                                                 : "AVG is offloaded for DOUBLE arguments only");
+        add_states(p, o, 1, nullable);
       }
-      default: return fail(TG_ERR_UNSUPPORTED, "aggregate function is not offloaded");
+      return TG_OK;
+    case TG_AGG_MIN: case TG_AGG_MAX:
+      if (!dec_arg && cls != ARG_INT && cls != ARG_REAL) return fail(TG_ERR_UNSUPPORTED, "MIN/MAX are offloaded for int family / DOUBLE / DECIMAL");
+      add_states(p, o, 1, nullable);
+      p->out_nullable[k] = 1;
+      if (dec_arg) p->out_elem[k] = TG_DEC_CELL_BYTES;   // the signed int64 MIN / MAX at the column's scale
+      return TG_OK;
+    case TG_AGG_FIRSTROW: {
+      int gi = -1;   // the last GROUP BY item of the column
+      for (size_t q = 0; q < p->group_cols.size(); q++) if (p->group_cols[q] == f.arg_col) gi = (int)q;
+      if (cls == ARG_NONE || gi < 0) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW is offloaded only for GROUP BY columns (deterministic)");
+      p->out_nullable[k] = nullable_col(p, f.arg_col);
+      o.arg_col2 = gi | ((p->nkw > (int)p->group_cols.size() ? (int)p->group_cols.size() : 0) << 8);
+      return TG_OK;
     }
+    default: return fail(TG_ERR_UNSUPPORTED, "aggregate function is not offloaded");
   }
-  a->wide = a->dec_out = false;
-  for (int k = 0; k < d->n_funcs; k++) {
-    const AggFuncDev& o = a->spec.f[k];
-    // dec3_apply / sdec3_apply find the middle and top words one and two state strides after the low word
-    if (o.s3 >= 0 && (o.s2 != o.s0 + 1 || o.s3 != o.s0 + 2)) return fail(TG_ERR_CUDA, "internal: the 192-bit sum's state words are not consecutive");
-    a->wide |= o.s3 >= 0;
-    a->dec_out |= o.dec_scale >= 0;
+}
+
+// One dedup set per DISTINCT argument column; its functions read the virtual column ncols + j (free DevCols slots)
+static int compile_distinct(AggPlan* p) {
+  for (int k = 0; k < p->n_out; k++) {
+    if (!p->fdistinct[k]) continue;
+    int& c = p->spec.f[k].arg_col;
+    const size_t j = std::find(p->dist_cols.begin(), p->dist_cols.end(), c) - p->dist_cols.begin();
+    if (j == p->dist_cols.size()) p->dist_cols.push_back(c);
+    c = p->ncols + (int)j;
   }
-  if (a->nstates > 2 * TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "the aggregate list needs more than 24 state words (a DECIMAL SUM / AVG takes up to 3, up to 4 over a product)");
-  // one dedup set per DISTINCT argument column; its functions read the virtual column ncols + j (free DevCols slots)
-  a->dist_cols.clear();
-  for (int k = 0; k < d->n_funcs; k++) {
-    if (!a->fdistinct[k]) continue;
-    const int c = d->funcs[k].arg_col;
-    const size_t j = std::find(a->dist_cols.begin(), a->dist_cols.end(), c) - a->dist_cols.begin();
-    if (j == a->dist_cols.size()) a->dist_cols.push_back(c);
-    a->spec.f[k].arg_col = a->ncols + (int)j;
-  }
-  if (a->ncols + (int)a->dist_cols.size() > TG_MAX_COLS)
+  if (p->ncols + (int)p->dist_cols.size() > TG_MAX_COLS)
     return fail(TG_ERR_UNSUPPORTED, "DISTINCT aggregates need one free column slot per argument column (child columns + DISTINCT columns <= 16)");
-  a->dist_gkw = d->n_group_by + (any_nullable ? 1 : 0);
-  // FIRSTROW of a PAD string key under several GROUP BY columns: one tail column and one hidden MIN per such column
-  a->n_out = d->n_funcs;
-  a->tail_col.assign(d->n_cols, -1);
-  a->tail_fn.assign(d->n_funcs, -1);
-  std::vector<int> min_of(d->n_cols, -1);
-  int nvirt = a->ncols + (int)a->dist_cols.size();
-  for (int k = 0; k < d->n_funcs; k++) {
-    const int c = d->funcs[k].arg_col;
-    if (a->out_dict[k] < 0 || a->coll[c] != COLL_PAD_BIN || d->n_group_by < 2) continue;
+  return TG_OK;
+}
+
+// FIRSTROW of a PAD string key under several GROUP BY columns: one tail column and one hidden MIN per such column
+static int compile_tail_mins(AggPlan* p, int n_group_by) {
+  p->tail_col.assign(p->ncols, -1);
+  p->tail_fn.assign(p->n_out, -1);
+  std::vector<int> min_of(p->ncols, -1);
+  int nvirt = p->ncols + (int)p->dist_cols.size();
+  for (int k = 0; k < p->n_out; k++) {
+    const int c = p->spec.f[k].arg_col;
+    if (p->out_dict[k] < 0 || p->coll[c] != COLL_PAD_BIN || n_group_by < 2) continue;
     if (min_of[c] < 0) {
       if (nvirt >= TG_MAX_COLS) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW of a PAD string key with several GROUP BY columns needs a free column slot (child columns + DISTINCT columns + such keys <= 16)");
-      if (a->spec.n >= TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW of a PAD string key with several GROUP BY columns takes a hidden aggregate slot (at most 12 in all)");
-      a->tail_col[c] = nvirt++;
-      min_of[c] = a->spec.n++;
-      a->spec.f[min_of[c]] = AggFuncDev{TG_AGG_MIN, a->tail_col[c], 0, 1, a->nstates++, -1, 0, -1, TG_ARGEXPR_COL, -1, 0, -1, -1, 0.0, 0};
-      a->out_nullable.push_back(0); a->out_elem.push_back(8); a->out_dict.push_back(-1); a->fdistinct.push_back(0);
+      if (p->spec.n >= TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "FIRSTROW of a PAD string key with several GROUP BY columns takes a hidden aggregate slot (at most 12 in all)");
+      p->tail_col[c] = nvirt++;
+      min_of[c] = p->spec.n++;
+      AggFuncDev& o = p->spec.f[min_of[c]] = func_dev(tg_agg_func{TG_AGG_MIN, TG_AGGMODE_COMPLETE, p->tail_col[c], 0, 0, -1, TG_ARGEXPR_COL, 0, 0, 0.0});
+      o.is_unsigned = 1;
+      add_states(p, o, 1, false);
+      p->out_nullable.push_back(0); p->out_elem.push_back(8); p->out_dict.push_back(-1); p->fdistinct.push_back(0);
     }
-    a->tail_fn[k] = min_of[c];
+    p->tail_fn[k] = min_of[c];
   }
-  if (a->nstates > 2 * TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "the aggregate list needs more than 24 state words (a DECIMAL SUM / AVG takes up to 3, up to 4 over a product)");
-  a->is_str.assign(d->n_cols, 0);
-  a->needed_fixed = a->needed;
-  for (int c = 0; c < d->n_cols; c++)
-    if (a->needed[c] && col_coll && agg_string_type(a->types[c])) { a->is_str[c] = 1; a->needed_fixed[c] = 0; }
-  a->device = d->device;
-  a->expected_groups = d->expected_groups;
+  return TG_OK;
+}
+
+// The gate: compiles a descriptor into a fresh *p, or returns the status and message of the first rule it breaks
+static int agg_compile(AggPlan* p, const tg_agg_desc_ex3& d) {
+  const tg_agg_desc& b = d.ex2.ex.base;
+  TG_TRY(compile_schema(p, d));
+  TG_TRY(compile_group_keys(p, b));
+  if (b.n_funcs <= 0 || b.n_funcs > TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "1..12 aggregate functions are offloaded");
+  p->spec.n = p->n_out = b.n_funcs;
+  p->out_nullable.assign(b.n_funcs, 0);
+  p->out_elem.assign(b.n_funcs, 8);
+  p->fdistinct.assign(b.n_funcs, 0);
+  p->out_dict.assign(b.n_funcs, -1);
+  for (int k = 0; k < b.n_funcs; k++) TG_TRY(compile_func(p, d, k));
+  TG_TRY(compile_distinct(p));
+  TG_TRY(compile_tail_mins(p, b.n_group_by));
+  if (p->nstates > 2 * TG_MAX_AGG) return fail(TG_ERR_UNSUPPORTED, "the aggregate list needs more than 24 state words (a DECIMAL SUM / AVG takes up to 3, up to 4 over a product)");
+  p->is_str.assign(p->ncols, 0);
+  p->needed_fixed = p->needed;
+  for (int c = 0; c < p->ncols; c++)
+    if (p->needed[c] && p->str_col[c]) { p->is_str[c] = 1; p->needed_fixed[c] = 0; }
   return TG_OK;
 }
 
@@ -1905,42 +1937,34 @@ static int afinalize(AggImpl* a) {
   return TG_OK;
 }
 
-}  // namespace tg
+// every descriptor version as a tg_agg_desc_ex3 whose arrays that version lacks are NULL
+static tg_agg_desc_ex3 ex3_view(const tg_agg_desc& d) { tg_agg_desc_ex3 v{}; v.ex2.ex.base = d; return v; }
+static tg_agg_desc_ex3 ex3_view(const tg_agg_desc_ex& d) { tg_agg_desc_ex3 v{}; v.ex2.ex = d; return v; }
+static tg_agg_desc_ex3 ex3_view(const tg_agg_desc_ex2& d) { tg_agg_desc_ex3 v{}; v.ex2 = d; return v; }
+static tg_agg_desc_ex3 ex3_view(const tg_agg_desc_ex3& d) { return d; }
 
-extern "C" {
-
-int tg_agg_supported(const tg_agg_desc* desc) { AggImpl tmp; return agg_setup(&tmp, desc, nullptr, nullptr); }
-
-int tg_agg_supported_ex(const tg_agg_desc_ex* desc) {
-  AggImpl tmp;
-  return agg_setup(&tmp, desc ? &desc->base : nullptr, desc ? desc->col_flen : nullptr, desc ? desc->col_decimal : nullptr);
+template <class Desc> static int agg_supported(const Desc* desc) {
+  if (!desc) return fail(TG_ERR_INVALID, "desc is NULL");
+  AggPlan p;
+  return agg_compile(&p, ex3_view(*desc));
 }
 
-int tg_agg_supported_ex2(const tg_agg_desc_ex2* desc) {
-  AggImpl tmp;
-  return agg_setup(&tmp, desc ? &desc->ex.base : nullptr, desc ? desc->ex.col_flen : nullptr, desc ? desc->ex.col_decimal : nullptr,
-                   desc ? desc->has_distinct : nullptr);
-}
-
-int tg_agg_supported_ex3(const tg_agg_desc_ex3* desc) {
-  AggImpl tmp;
-  return agg_setup(&tmp, desc ? &desc->ex2.ex.base : nullptr, desc ? desc->ex2.ex.col_flen : nullptr, desc ? desc->ex2.ex.col_decimal : nullptr,
-                   desc ? desc->ex2.has_distinct : nullptr, desc ? desc->col_collation : nullptr);
-}
-
-static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int32_t* col_dec, const uint8_t* has_distinct, tg_agg** out,
-                    const int32_t* col_coll = nullptr) {
+template <class Desc> static int agg_open(const Desc* desc, tg_agg** out) {
   if (!out) return fail(TG_ERR_INVALID, "out is NULL");
   *out = nullptr;
+  if (!desc) return fail(TG_ERR_INVALID, "desc is NULL");
+  const tg_agg_desc_ex3 d = ex3_view(*desc);
   std::unique_ptr<tg_agg> shell(new tg_agg());
   std::unique_ptr<AggImpl> a(new AggImpl());
-  TG_TRY(agg_setup(a.get(), desc, col_flen, col_dec, has_distinct, col_coll));
+  TG_TRY(agg_compile(a.get(), d));
+  a->device = d.ex2.ex.base.device;
+  a->expected_groups = d.ex2.ex.base.expected_groups;
   int ndev = 0;
   TG_TRY(require_device("the GPU hash aggregation", &ndev));
   if (a->device < 0 || a->device >= ndev) return fail(TG_ERR_INVALID, "device ordinal out of range");
   DeviceGuard g(a->device);
   if (!g.ok) return fail(TG_ERR_CUDA, "cudaSetDevice failed");
-  TG_TRY(a->open(a->device, desc->stream));
+  TG_TRY(a->open(a->device, d.ex2.ex.base.stream));
   a->stage.init(a->ncols);
   for (int c = 0; c < a->ncols; c++) {
     a->dcols.emplace_back(new DevBuf()); a->dnulls.emplace_back(new DevBuf()); a->dscaled.emplace_back(new DevBuf());
@@ -1955,21 +1979,18 @@ static int agg_open(const tg_agg_desc* desc, const int32_t* col_flen, const int3
   return TG_OK;
 }
 
-int tg_agg_open(const tg_agg_desc* desc, tg_agg** out) { return agg_open(desc, nullptr, nullptr, nullptr, out); }
+}  // namespace tg
 
-int tg_agg_open_ex(const tg_agg_desc_ex* desc, tg_agg** out) {
-  return agg_open(desc ? &desc->base : nullptr, desc ? desc->col_flen : nullptr, desc ? desc->col_decimal : nullptr, nullptr, out);
-}
+extern "C" {
 
-int tg_agg_open_ex2(const tg_agg_desc_ex2* desc, tg_agg** out) {
-  return agg_open(desc ? &desc->ex.base : nullptr, desc ? desc->ex.col_flen : nullptr, desc ? desc->ex.col_decimal : nullptr,
-                  desc ? desc->has_distinct : nullptr, out);
-}
-
-int tg_agg_open_ex3(const tg_agg_desc_ex3* desc, tg_agg** out) {
-  return agg_open(desc ? &desc->ex2.ex.base : nullptr, desc ? desc->ex2.ex.col_flen : nullptr, desc ? desc->ex2.ex.col_decimal : nullptr,
-                  desc ? desc->ex2.has_distinct : nullptr, out, desc ? desc->col_collation : nullptr);
-}
+int tg_agg_supported(const tg_agg_desc* desc) { return agg_supported(desc); }
+int tg_agg_supported_ex(const tg_agg_desc_ex* desc) { return agg_supported(desc); }
+int tg_agg_supported_ex2(const tg_agg_desc_ex2* desc) { return agg_supported(desc); }
+int tg_agg_supported_ex3(const tg_agg_desc_ex3* desc) { return agg_supported(desc); }
+int tg_agg_open(const tg_agg_desc* desc, tg_agg** out) { return agg_open(desc, out); }
+int tg_agg_open_ex(const tg_agg_desc_ex* desc, tg_agg** out) { return agg_open(desc, out); }
+int tg_agg_open_ex2(const tg_agg_desc_ex2* desc, tg_agg** out) { return agg_open(desc, out); }
+int tg_agg_open_ex3(const tg_agg_desc_ex3* desc, tg_agg** out) { return agg_open(desc, out); }
 
 int tg_agg_push(tg_agg* h, const tg_chunk* chk) {
   TG_LOCK(h, AggImpl, a);
@@ -2035,34 +2056,12 @@ static bool has_string_result(const AggImpl* a) {
   return std::find_if(a->out_dict.begin(), a->out_dict.end(), [](int j) { return j >= 0; }) != a->out_dict.end();
 }
 
-int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) {
+// tg_agg_next (ex false, var_out NULL: a plan with a string result is refused) and tg_agg_next_ex
+static int agg_next(tg_agg* h, tg_mut_chunk* out, tg_mut_varlen* var_out, int64_t max_rows, int64_t* nrows, bool ex) {
   TG_LOCK(h, AggImpl, a);
-  if (!out || !nrows) return fail(TG_ERR_INVALID, "out / nrows is NULL");
-  if (has_string_result(a)) return fail(TG_ERR_INVALID, "the plan has a string result: read it with tg_agg_next_ex");
-  *nrows = 0;
-  if (!a->finished) return fail(TG_ERR_STATE, "next before finish (hash aggregation is a pipeline breaker)");
-  if (out->ncols != a->n_out) return fail(TG_ERR_INVALID, "output chunk column count does not match the aggregate list");
-  int64_t lo = a->consumed;
-  int64_t want = std::min<int64_t>(std::min<int64_t>(max_rows, out->capacity_rows), a->out_rows - lo);
-  if (want <= 0) return TG_OK;
-  // every output column is checked before the first copy is enqueued: a rejected call writes nothing
-  TG_TRY(check_out_columns(a->out_bitmaps, a->out_elem, out));
-  for (int k = 0; k < a->n_out; k++) {
-    const size_t el = (size_t)a->out_elem[k];
-    TG_CUDA(cudaMemcpyAsync(out->cols[k].data, a->out_cols[k]->as<uint8_t>() + (size_t)lo * el, (size_t)want * el, cudaMemcpyDeviceToHost, a->stream));
-    a->stats.d2h_bytes += want * (int64_t)el;
-  }
-  // any RequiredRows >= 1 is served (download_bitmaps re-aligns bitmaps that start inside a byte); d2h_bytes counts the
-  // result cells only
-  TG_TRY(download_bitmaps(a->out_bitmaps, out, lo, want, a->stream, nullptr));
-  a->consumed += want;
-  *nrows = want;
-  return TG_OK;
-}
-
-// tg_agg_next_ex of a plan with a string result
-static int agg_next_varlen(AggImpl* a, tg_mut_chunk* out, tg_mut_varlen* var_out, int64_t max_rows, int64_t* nrows) {
-  if (!out || !nrows || !var_out) return fail(TG_ERR_INVALID, "out / var_out / nrows is NULL");
+  const bool str = has_string_result(a);
+  if (!out || !nrows || (str && ex && !var_out)) return fail(TG_ERR_INVALID, str && ex ? "out / var_out / nrows is NULL" : "out / nrows is NULL");
+  if (str && !ex) return fail(TG_ERR_INVALID, "the plan has a string result: read it with tg_agg_next_ex");
   *nrows = 0;
   if (!a->finished) return fail(TG_ERR_STATE, "next before finish (hash aggregation is a pipeline breaker)");
   if (out->ncols != a->n_out) return fail(TG_ERR_INVALID, "output chunk column count does not match the aggregate list");
@@ -2070,18 +2069,18 @@ static int agg_next_varlen(AggImpl* a, tg_mut_chunk* out, tg_mut_varlen* var_out
   int64_t want = std::min<int64_t>(std::min<int64_t>(max_rows, out->capacity_rows), a->out_rows - lo);
   if (want <= 0) return TG_OK;
   // every output column is checked before the first copy is enqueued: a rejected call writes nothing
-  for (int k = 0; k < a->n_out; k++) {
-    const bool str = a->out_dict[k] >= 0;
-    if (out->cols[k].elem_len != (str ? -1 : a->out_elem[k]))
+  if (!str) TG_TRY(check_out_columns(a->out_bitmaps, a->out_elem, out));
+  for (int k = 0; str && k < a->n_out; k++) {
+    const bool sk = a->out_dict[k] >= 0;
+    if (out->cols[k].elem_len != (sk ? -1 : a->out_elem[k]))
       return fail(TG_ERR_INVALID, "output column elem_len does not match its result column (-1 for a string result, 40 for a DECIMAL one, else 8)");
     if (a->out_bitmaps[k]->p && !out->cols[k].null_bitmap) return fail(TG_ERR_INVALID, "output column can be NULL but the caller passed no null bitmap");
-    if (!str) continue;
+    if (!sk) continue;
     const tg_mut_varlen& vo = var_out[k];
     if (!vo.offsets || (vo.data_cap > 0 && !vo.data) || vo.data_cap < 0) return fail(TG_ERR_INVALID, "a string result needs offsets and data_cap bytes of data");
     // the largest prefix of rows whose bytes fit data_cap
     const int64_t* ho = a->host_soffs[k].data() + lo;
-    int64_t fit = std::upper_bound(ho, ho + want + 1, ho[0] + vo.data_cap) - ho - 1;
-    want = std::min<int64_t>(want, fit);
+    want = std::min<int64_t>(want, std::upper_bound(ho, ho + want + 1, ho[0] + vo.data_cap) - ho - 1);
   }
   if (want <= 0) return fail(TG_ERR_CAPACITY, "the next result row's string bytes do not fit data_cap");
   for (int k = 0; k < a->n_out; k++) {
@@ -2097,22 +2096,18 @@ static int agg_next_varlen(AggImpl* a, tg_mut_chunk* out, tg_mut_varlen* var_out
     TG_CUDA(cudaMemcpyAsync(out->cols[k].data, a->out_cols[k]->as<uint8_t>() + (size_t)lo * el, (size_t)want * el, cudaMemcpyDeviceToHost, a->stream));
     a->stats.d2h_bytes += want * (int64_t)el;
   }
+  // any RequiredRows >= 1 is served (download_bitmaps re-aligns bitmaps that start inside a byte); d2h_bytes counts the
+  // result cells only
   TG_TRY(download_bitmaps(a->out_bitmaps, out, lo, want, a->stream, nullptr));
   a->consumed += want;
   *nrows = want;
   return TG_OK;
 }
 
-int tg_agg_next_ex(tg_agg* h, tg_mut_chunk* out, tg_mut_varlen* var_out, int64_t max_rows, int64_t* nrows) {
-  {
-    TG_LOCK(h, AggImpl, a);
-    if (has_string_result(a)) return agg_next_varlen(a, out, var_out, max_rows, nrows);
-  }
-  return tg_agg_next(h, out, max_rows, nrows);
-}
-
-int tg_agg_result_dev_ex(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls, void** out_offsets) {
+// tg_agg_result_dev (ex false: a plan with a string result is refused) and tg_agg_result_dev_ex
+static int agg_result_dev(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls, void** out_offsets, bool ex) {
   TG_LOCK(h, AggImpl, a);
+  if (!ex && has_string_result(a)) return fail(TG_ERR_INVALID, "the plan has a string result: read it with tg_agg_result_dev_ex");
   if (!a->finished) return fail(TG_ERR_STATE, "result before finish");
   if (out_rows) *out_rows = a->out_rows;
   for (int k = 0; k < a->n_out; k++) {
@@ -2122,6 +2117,20 @@ int tg_agg_result_dev_ex(tg_agg* h, int64_t* out_rows, void** out_cols, void** o
     if (out_offsets) out_offsets[k] = str ? a->out_soffs[k]->p : nullptr;
   }
   return TG_OK;
+}
+
+int tg_agg_next(tg_agg* h, tg_mut_chunk* out, int64_t max_rows, int64_t* nrows) { return agg_next(h, out, nullptr, max_rows, nrows, false); }
+
+int tg_agg_next_ex(tg_agg* h, tg_mut_chunk* out, tg_mut_varlen* var_out, int64_t max_rows, int64_t* nrows) {
+  return agg_next(h, out, var_out, max_rows, nrows, true);
+}
+
+int tg_agg_result_dev(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls) {
+  return agg_result_dev(h, out_rows, out_cols, out_nulls, nullptr, false);
+}
+
+int tg_agg_result_dev_ex(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls, void** out_offsets) {
+  return agg_result_dev(h, out_rows, out_cols, out_nulls, out_offsets, true);
 }
 
 int tg_agg_get_string_stats(tg_agg* h, tg_agg_string_stats* out) {
@@ -2136,18 +2145,6 @@ int tg_agg_get_string_stats(tg_agg* h, tg_agg_string_stats* out) {
     out->launches += d->launches;
   }
   out->encode_ms = a->encode_ms;
-  return TG_OK;
-}
-
-int tg_agg_result_dev(tg_agg* h, int64_t* out_rows, void** out_cols, void** out_nulls) {
-  TG_LOCK(h, AggImpl, a);
-  if (has_string_result(a)) return fail(TG_ERR_INVALID, "the plan has a string result: read it with tg_agg_result_dev_ex");
-  if (!a->finished) return fail(TG_ERR_STATE, "result before finish");
-  if (out_rows) *out_rows = a->out_rows;
-  for (int k = 0; k < a->n_out; k++) {
-    if (out_cols) out_cols[k] = a->out_cols[k]->p;
-    if (out_nulls) out_nulls[k] = a->out_bitmaps[k]->p;
-  }
   return TG_OK;
 }
 
