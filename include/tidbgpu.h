@@ -314,7 +314,9 @@ enum {
   /* 1 << 4 is unassigned: older headers name a removed kernel with it, so a new path must not reuse it              */
   TG_JOIN_PATH_SCATTER_BULK = 1 << 5,   /* bulk partition scatter (k_partition_scatter_bulk)                     */
   TG_JOIN_PATH_SCATTER = 1 << 6,        /* LSU partition scatter over the whole input (k_partition_scatter)      */
-  TG_JOIN_PATH_CELL_GATHER = 0x80       /* 1 << 7: DECIMAL output cells gathered from row ids (k_gather_cells)      */
+  TG_JOIN_PATH_CELL_GATHER = 0x80,      /* 1 << 7: DECIMAL output cells gathered from row ids (k_gather_cells)      */
+  TG_JOIN_PATH_PROBE_INDEX = 0x100      /* 1 << 8: in-place segment probe through the table's slice index
+                                           (k_probe_inner_u1_seg_inplace_pidx)                                        */
 };
 int tg_join_get_stats(tg_join* j, tg_join_stats* out);
 

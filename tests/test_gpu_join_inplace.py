@@ -17,6 +17,7 @@ SENTINEL = -(1 << 63)
 INT = FieldType(abi.TYPE_LONGLONG, abi.FLAG_NOT_NULL)
 PART = dict(TG_PROBE_PARTITION="1", TG_PROBE_PARTS="8", TG_PROBE_PART_MIN_MB="0", TG_PROBE_PART_MIN_ROWS="0")
 INPLACE, LEAN, FILL, SCATTER = "k_probe_inner_u1_seg_inplace", "k_probe_inner_u1_seg_lean", "k_inplace_fill", "k_partition_scatter_bulk"
+PIDX = "k_probe_inner_u1_seg_inplace_pidx"   # the in-place probe through the slice index (its name contains INPLACE)
 # kernels one partitioned probe of dense input enqueues (stats.kernel_launches): k_segment_bases, the scatter, the segment
 # probe and the gated k_probe_inner_u1_w; in place adds k_inplace_holes, the three scan kernels and k_inplace_fill
 LAUNCHES = {True: 9, False: 4}
@@ -78,12 +79,15 @@ def ran(names, kernel):
     return any(kernel in n for n in names)
 
 
-def assert_mode(names, launches, inplace):
+def assert_mode(names, launches, inplace, index=False):
+    """the call took the in-place probe (else the lean one); in place, through the table's slice index (PIDX) or not"""
     assert launches == LAUNCHES[inplace], (launches, inplace)
     # a torch.profiler capture can come back without its kernel records (only the runtime API calls): the scatter runs in
     # both modes, so a capture that names it holds the kernels; test_profiler_names_the_mode_kernels requires one
     if ran(names, SCATTER):
-        assert ran(names, INPLACE) == inplace and ran(names, FILL) == inplace and ran(names, LEAN) != inplace, names
+        linear = any(INPLACE in n and PIDX not in n for n in names)
+        assert linear == (inplace and not index) and ran(names, PIDX) == (inplace and index), names
+        assert ran(names, FILL) == inplace and ran(names, LEAN) != inplace, names
 
 
 class Dev:
@@ -180,7 +184,7 @@ def test_skewed_probe_overflows_a_segment(monkeypatch):
     assert st.paths & abi.JOIN_PATH_PROBE_DIRECT
 
 
-@pytest.mark.parametrize("ncols,lused,rused", [
+OUTPUT_SHAPES = [   # (probe columns, lused, rused); test_gpu_slice_index runs them through the slice index
     (2, None, None),            # NPC 1, NKD 2 (probe and build key), NMD 1
     (2, [0, 1], [1]),           # the pruned 3-column plan: NKD 1
     (2, [1], [0, 1]),           # NKD 1 fed by the build key only
@@ -188,16 +192,26 @@ def test_skewed_probe_overflows_a_segment(monkeypatch):
     (3, [0, 1, 2], [0]),        # NPC 2, NMD 0
     (4, [0, 1, 2, 3], [1]),     # NPC 3, NKD 1
     (2, [1], [1]),              # no output fed by the key (NKD 0): not eligible
-])
-@pytest.mark.parametrize("match", [1.0, 0.6])
-def test_output_shapes(ncols, lused, rused, match, monkeypatch):
-    setenv(monkeypatch, "1")
-    bk, bv, pcols = make_sides(30_000, 200_003, match, seed=5, ncols=ncols)
-    got, names, launches, _ = run_dev(bk, bv, pcols, lused, rused)
+]
+
+
+def run_shape(ncols, lused, rused, match, nb, npr, seed):
+    """one forced in-place call of the output shape against its reference -> (kernel names, launches, stats, whether the
+    shape is eligible for the in-place probe: an output fed by the join key)"""
+    bk, bv, pcols = make_sides(nb, npr, match, seed=seed, ncols=ncols)
+    got, names, launches, st = run_dev(bk, bv, pcols, lused, rused)
     lu = list(range(ncols)) if lused is None else lused
     ru = [0, 1] if rused is None else rused
     check(got, expected(bk, bv, pcols, lu, ru))
-    assert_mode(names, launches, 0 in lu or 0 in ru)
+    return names, launches, st, 0 in lu or 0 in ru
+
+
+@pytest.mark.parametrize("ncols,lused,rused", OUTPUT_SHAPES)
+@pytest.mark.parametrize("match", [1.0, 0.6])
+def test_output_shapes(ncols, lused, rused, match, monkeypatch):
+    setenv(monkeypatch, "1")
+    names, launches, _, eligible = run_shape(ncols, lused, rused, match, 30_000, 200_003, seed=5)
+    assert_mode(names, launches, eligible)
 
 
 @pytest.mark.parametrize("mode", ["1", "0", None])

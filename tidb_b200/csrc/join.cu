@@ -933,14 +933,12 @@ struct LaunchInplace {
       int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
       int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
       if (j->pidx.P == (uint32_t)(n / seg.cap)) {
-        // the slice index of this table, cut for this P: one CTA per SM holding one slice's pilots
-        static bool attr = false;
-        if (!attr) {
-          TG_CUDA(cudaFuncSetAttribute(k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)kPidxMaxPilotBytes));
-          attr = true;
-        }
+        // the slice index of this table, cut for this P: one CTA per SM holding one slice's pilots.  The shared-memory
+        // limit is an attribute of the current device, so it is raised on every launch, as the aggregation does.
+        TG_CUDA(cudaFuncSetAttribute(k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)kPidxMaxPilotBytes));
         k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD><<<j->nsm, kPidxThreads, j->pidx.B, j->stream>>>(n, j->tv, j->pidx, fo, cur, seg, tile_cnt);
+        j->stats.paths |= TG_JOIN_PATH_PROBE_INDEX;
         return TG_OK;
       }
       k_probe_inner_u1_seg_inplace<NPC, NKD, NMD><<<grid, 256, 0, j->stream>>>(n, j->tv, fo, cur, seg, tile_cnt);
@@ -993,9 +991,11 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
     // random HBM traffic, which only pays while a slice stays L2 resident (probe_slices; U1 tables are built dense
     // enough for that, build_table).  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
     // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
+    // Fewer than PTILE rows leave the scatter nothing to do: the whole input would be the tail, and the gated launch,
+    // which probes the tail from row n_main on, reads n_main = 0 as "no tail".  Such a probe takes the direct launch.
     int P = 0;
     int64_t C = 0;
-    if (n > 0 && tune.partition && src16 && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
+    if (n_main > 0 && tune.partition && src16 && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
       P = probe_slices(table_bytes, j->device, tune.parts);
       C = ((int64_t)((double)n_main / P * 1.05) + 16384 + 127) / 128 * 128;
       if (!(P >= 2 && (int64_t)P * C / 128 < (1ll << 31))) P = 0;
