@@ -434,7 +434,7 @@ static ProbeTuning probe_tuning() {
   ProbeTuning t;
   t.ctas_per_sm = env_int("TG_PROBE_CTAS_PER_SM", 0);   // 0 = exactly the resident CTA count (occupancy query)
   t.partition = env_int("TG_PROBE_PARTITION", 1) != 0;   // regroup big probes into L2-sized partitions first (0 = never)
-  t.parts = env_int("TG_PROBE_PARTS", 0);           // 0 = auto (probe_slices), at most TG_MAX_PARTS
+  t.parts = env_int("TG_PROBE_PARTS", 0);           // 0 = auto (probe_slices), at most TG_MAX_SLICES
   t.part_min_mb = env_int("TG_PROBE_PART_MIN_MB", 64);
   t.part_min_rows = env_int("TG_PROBE_PART_MIN_ROWS", 1 << 22);
   t.inplace = env_int("TG_PROBE_INPLACE", -1);      // -1 = by the last match fraction (kInplaceMinMatch), 0 / 1 = never / always
@@ -455,9 +455,10 @@ static size_t l2_slice_target(int device) {
   if (device >= 0 && device < 64) cache[device] = t;
   return t;
 }
-// P for a table of `table_bytes`: slices of at most l2_slice_target, at most TG_MAX_PARTS (TG_PROBE_PARTS > 0 overrides)
+// P for a table of `table_bytes`: slices of at most l2_slice_target, at most TG_MAX_PARTS (TG_PROBE_PARTS > 0 overrides, up
+// to TG_MAX_SLICES)
 static int probe_slices(size_t table_bytes, int device, int parts_override) {
-  if (parts_override > 0) return std::min(parts_override, TG_MAX_PARTS);
+  if (parts_override > 0) return std::min(parts_override, TG_MAX_SLICES);
   const size_t target = l2_slice_target(device);
   return (int)std::min<size_t>((table_bytes + target - 1) / target, TG_MAX_PARTS);
 }
@@ -487,11 +488,11 @@ static int build_slice_index(JoinImpl* j, const Slot* slots, unsigned long long 
   const uint32_t P = (uint32_t)probe_slices((size_t)nslots * sizeof(Slot), j->device, tune.parts);
   if (P < 2) return TG_OK;
   DevBuf cnt;
-  TG_TRY(cnt.ensure(j->device, (size_t)(TG_MAX_PARTS + 1) * 8));
+  TG_TRY(cnt.ensure(j->device, (size_t)(TG_MAX_SLICES + 1) * 8));
   unsigned long long* pcnt = cnt.as<unsigned long long>();
-  TG_CUDA(cudaMemsetAsync(pcnt, 0, (size_t)(TG_MAX_PARTS + 1) * 8, j->stream));
+  TG_CUDA(cudaMemsetAsync(pcnt, 0, (size_t)(TG_MAX_SLICES + 1) * 8, j->stream));
   k_pidx_part_count<<<grid_size(j->nsm, (int64_t)nslots, 256, 8), 256, 0, j->stream>>>(slots, nslots, P, pcnt);
-  unsigned long long hc[TG_MAX_PARTS];
+  unsigned long long hc[TG_MAX_SLICES];
   TG_CUDA(cudaMemcpyAsync(hc, pcnt, P * 8, cudaMemcpyDeviceToHost, j->stream));
   TG_CUDA(cudaStreamSynchronize(j->stream));
   unsigned long long mx = 0;
@@ -502,7 +503,8 @@ static int build_slice_index(JoinImpl* j, const Slot* slots, unsigned long long 
   ix.B = ((uint32_t)std::ceil((double)mx / kPidxKeysPerBucket) + 16) & ~15u;
   int optin = 0;
   cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, j->device);
-  if (ix.B > kPidxMaxPilotBytes || ix.B > (uint32_t)optin) return TG_OK;   // slices too big: the linear-probe kernels
+  if (ix.B > kPidxMaxPilotBytes || ix.B + 16 > (uint32_t)optin) return TG_OK;   // slices too big: the linear-probe kernels
+  ix.nbuf = 2 * ix.B <= kPidxMaxPilotBytes && 2 * (ix.B + 8) <= (uint32_t)optin ? 2 : 1;
   const size_t nb = (size_t)P * ix.B, ns = (size_t)P * ix.S;
   TG_TRY(j->pidx_slots.ensure(j->device, ns * sizeof(Slot)));
   TG_TRY(j->pidx_pilot.ensure(j->device, nb));
@@ -526,7 +528,7 @@ static int build_slice_index(JoinImpl* j, const Slot* slots, unsigned long long 
   const unsigned gb = (unsigned)grid_size(j->nsm, (int64_t)nb, 256, 8);
   for (uint32_t size = kPidxMaxBucket; size >= 1; size--)   // largest buckets first
     k_pidx_place<<<gb, 256, 0, j->stream>>>(slots, ix, off, list.as<uint32_t>(), size, owner.as<uint32_t>(), j->pidx_pilot.as<uint8_t>());
-  unsigned long long* bad = pcnt + TG_MAX_PARTS;
+  unsigned long long* bad = pcnt + TG_MAX_SLICES;
   k_pidx_write<<<g, 256, 0, j->stream>>>(slots, nslots, ix, islots, 0, bad);
   k_pidx_write<<<g, 256, 0, j->stream>>>(slots, nslots, ix, islots, 1, bad);
   j->stats.kernel_launches += 8 + kPidxMaxBucket;
@@ -933,11 +935,12 @@ struct LaunchInplace {
       int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
       int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
       if (j->pidx.P == (uint32_t)(n / seg.cap)) {
-        // the slice index of this table, cut for this P: one CTA per SM holding one slice's pilots.  The shared-memory
-        // limit is an attribute of the current device, so it is raised on every launch, as the aggregation does.
-        TG_CUDA(cudaFuncSetAttribute(k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)kPidxMaxPilotBytes));
-        k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD><<<j->nsm, kPidxThreads, j->pidx.B, j->stream>>>(n, j->tv, j->pidx, fo, cur, seg, tile_cnt);
+        // the slice index of this table, cut for this P: one CTA per SM holding nbuf slices' pilots and their mbarriers.
+        // The shared-memory limit is an attribute of the current device, so it is raised on every launch, as the
+        // aggregation does.
+        const int smem = (int)(j->pidx.nbuf * (j->pidx.B + 8));
+        TG_CUDA(cudaFuncSetAttribute(k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD><<<j->nsm, kPidxThreads, smem, j->stream>>>(n, j->tv, j->pidx, fo, cur, seg, tile_cnt);
         j->stats.paths |= TG_JOIN_PATH_PROBE_INDEX;
         return TG_OK;
       }
@@ -1022,10 +1025,10 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
             TG_TRY(j->part_cols[c]->ensure(j->device, (size_t)P * C * 8 + 64));
           }
         }
-        TG_TRY(j->part_scratch.ensure(j->device, (size_t)3 * TG_MAX_PARTS * 8 + 64));
-        unsigned long long* cursors = j->part_scratch.as<unsigned long long>();     // fill count per segment
-        long long* bases = reinterpret_cast<long long*>(cursors + TG_MAX_PARTS);   // first row of each segment
-        unsigned long long* flag = cursors + 2 * TG_MAX_PARTS;                      // overflow
+        TG_TRY(j->part_scratch.ensure(j->device, (size_t)3 * TG_MAX_SLICES * 8 + 64));
+        unsigned long long* cursors = j->part_scratch.as<unsigned long long>();      // fill count per segment
+        long long* bases = reinterpret_cast<long long*>(cursors + TG_MAX_SLICES);   // first row of each segment
+        unsigned long long* flag = cursors + 2 * TG_MAX_SLICES;                      // overflow
         PartDst d{};
         d.nparts = P; d.ncols = nc;
         d.src[0] = pkey;
@@ -1071,7 +1074,7 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
     }
     TG_TRY(gather_cells(j, rb, &pcells, cur));   // after the hole fill and the gated fallback: *cur rows from row 0
     if (sync_count) {
-      unsigned long long got = 0, part[2 * TG_MAX_PARTS + 1];   // fill counts | segment bases | overflow flag
+      unsigned long long got = 0, part[2 * TG_MAX_SLICES + 1];   // fill counts | segment bases | overflow flag
       const bool learn = P && !in_seg;
       if (learn) TG_CUDA(cudaMemcpyAsync(part, j->part_scratch.p, sizeof(part), cudaMemcpyDeviceToHost, j->stream));
       TG_CUDA(cudaMemcpyAsync(&got, cur, 8, cudaMemcpyDeviceToHost, j->stream));
@@ -1080,7 +1083,7 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
       j->stats.output_rows += (int64_t)got;
       if (P && n > 0) j->seg_match = (double)got / (double)n;
       if (learn) {
-        j->seg_parts = part[2 * TG_MAX_PARTS] ? 0 : P;
+        j->seg_parts = part[2 * TG_MAX_SLICES] ? 0 : P;
         j->seg_rows = n_main;
         j->seg_fill_max = (int64_t)*std::max_element(part, part + P);
       }

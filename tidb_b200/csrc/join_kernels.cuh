@@ -854,7 +854,8 @@ static constexpr int kPidxThreads = 1024;   // CTA of the index probe: the CTA's
 struct SliceIndex {
   const Slot* slots;        // [P][S]
   const uint8_t* pilot;     // [P][B], B a multiple of 16
-  uint32_t P, S, B, pad;
+  uint32_t P, S, B;
+  uint32_t nbuf;            // pilot buffers of the index probe: 2 when 2·B fits kPidxMaxPilotBytes (join.cu), else 1
 };
 
 __host__ __device__ __forceinline__ uint32_t pidx_slot(uint64_t h, uint32_t q, uint32_t S) {
@@ -865,7 +866,7 @@ __host__ __device__ __forceinline__ uint32_t pidx_bucket(uint64_t h, uint32_t B)
 // keys per partition (block-aggregated in shared memory)
 __global__ void __launch_bounds__(256) k_pidx_part_count(const Slot* __restrict__ slots, unsigned long long nslots, uint32_t P,
                                                          unsigned long long* __restrict__ pcnt) {
-  __shared__ unsigned int c[64];   // P <= TG_MAX_PARTS (partition_kernels.cuh: 16)
+  __shared__ unsigned int c[64];   // P <= TG_MAX_SLICES (partition_kernels.cuh: 32)
   for (int i = threadIdx.x; i < 64; i += blockDim.x) c[i] = 0;
   __syncthreads();
   for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nslots; i += (unsigned long long)gridDim.x * blockDim.x) {
@@ -941,34 +942,56 @@ __global__ void __launch_bounds__(256) k_pidx_write(const Slot* __restrict__ slo
 }
 
 // In-place segment probe through the slice index: the contract of k_probe_inner_u1_seg_inplace (tile_cnt, one cursor
-// atomic per warp, compaction of partly matched tiles), but CTA-cooperative: one CTA of kPidxThreads per SM loads the
-// pilots of slice p into shared memory, its warps sweep segment p's tiles, and a barrier precedes the next slice.  A full
-// tile reads its keys, one pilot byte and ONE 16-byte slot per row; a tile with a sentinel-valued key or a key whose
-// bucket has no pilot, and a segment's partial last tile, take inplace_tile_generic on the linear-probe table.
+// atomic per warp, compaction of partly matched tiles), but CTA-cooperative: one CTA of kPidxThreads per SM holds slice
+// pilots in shared memory, in ix.nbuf buffers (2 when two slices' pilots fit kPidxMaxPilotBytes, else 1).  Buffer b is
+// filled by one cp.async.bulk that completes on full[b]; a warp waits for slice p's pilots, sweeps its own tiles of segment
+// p and moves on to slice p + 1 at once; the last warp done with a buffer refills it with slice p + nbuf.  So with two
+// buffers no barrier spans the CTA: the next slice's pilots land while slow warps finish the current one.  Tile i of
+// segment p goes to warp (p·tiles_per_seg + i) mod warps: the warps that take one tile more than the others differ from
+// slice to slice.  A full tile reads its keys, one pilot byte and ONE 16-byte slot per row; a tile with a sentinel-valued
+// key or a key whose bucket has no pilot, and a segment's partial last tile, take inplace_tile_generic on the
+// linear-probe table.
 template <int NPC, int NKD, int NMD>
 __global__ void __launch_bounds__(kPidxThreads, 1)
 k_probe_inner_u1_seg_inplace_pidx(int64_t n, TableView t, SliceIndex ix, FastOut out, unsigned long long* __restrict__ out_cursor,
                                   SegSpec seg, uint32_t* __restrict__ tile_cnt) {
   static_assert(NKD >= 1, "the probe key is read from the first key destination");
-  constexpr int R = 4, G = 2, NP = NPC > 0 ? NPC : 1;
-  extern __shared__ __align__(16) uint8_t spil[];
+  constexpr int R = 4, G = 2, NP = NPC > 0 ? NPC : 1, NW = kPidxThreads / 32;
+  extern __shared__ __align__(16) uint8_t spil[];   // [nbuf][B] pilots, then nbuf "full" mbarriers
+  __shared__ uint32_t s_done[2];                     // warps done with buffer b, summed over the sweep
   if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) return;
   const int lane = threadIdx.x & 31;
-  const int64_t warps_total = (int64_t)gridDim.x * (kPidxThreads / 32);
-  const int64_t warp_id = (int64_t)blockIdx.x * (kPidxThreads / 32) + (threadIdx.x >> 5);
+  const int64_t warps_total = (int64_t)gridDim.x * NW;
+  const int64_t warp_id = (int64_t)blockIdx.x * NW + (threadIdx.x >> 5);
   const int64_t* __restrict__ pkey = reinterpret_cast<const int64_t*>(out.key_dst[0]);
   const int nseg = (int)(n / 128 / seg.tiles_per_seg);
+  const int nbuf = (int)ix.nbuf;
+  uint64_t* full = reinterpret_cast<uint64_t*>(spil + (size_t)nbuf * ix.B);
+  auto load = [&](int p) {   // one thread: slice p's pilots into buffer p % nbuf
+    const int b = p % nbuf;
+    mbar_arrive_expect_tx(&full[b], ix.B);
+    bulk_g2s(spil + (size_t)b * ix.B, ix.pilot + (size_t)p * ix.B, ix.B, &full[b], l2_policy_evict_normal());
+  };
+  if (threadIdx.x == 0) {
+    s_done[0] = s_done[1] = 0;
+    for (int b = 0; b < nbuf; b++) mbar_init(&full[b], 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int p = 0; p < nbuf && p < nseg; p++) load(p);
   unsigned long long kept = 0;
   for (int p = 0; p < nseg; p++) {
-    __syncthreads();   // every warp is done with the previous slice's pilots
-    const uint4* src = reinterpret_cast<const uint4*>(ix.pilot + (size_t)p * ix.B);
-    for (uint32_t i = threadIdx.x; i < ix.B / 16; i += kPidxThreads) reinterpret_cast<uint4*>(spil)[i] = __ldcs(src + i);
-    __syncthreads();
+    const int b = p % nbuf;
+    const uint32_t use = (uint32_t)(p / nbuf);   // how many slices buffer b held before this one
+    mbar_wait(&full[b], use & 1u);
+    const uint8_t* __restrict__ pil = spil + (size_t)b * ix.B;
     const unsigned long long c = seg.cnt[p];
     const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
     const int64_t t0 = (int64_t)p * seg.tiles_per_seg, t1 = t0 + seg.tiles_per_seg;
+    const int64_t r = t0 % warps_total;
     const Slot* __restrict__ islots = ix.slots + (size_t)p * ix.S;
-    for (int64_t tile = t0 + warp_id; tile < t1; tile += warps_total) {
+    for (int64_t tile = t0 + (warp_id >= r ? warp_id - r : warp_id - r + warps_total); tile < t1; tile += warps_total) {
       const int64_t base = tile * 128;
       uint32_t m = 0;
       if (limit - base >= 128) {
@@ -982,7 +1005,7 @@ k_probe_inner_u1_seg_inplace_pidx(int64_t n, TableView t, SliceIndex ix, FastOut
         bool generic = false;
 #pragma unroll
         for (int j = 0; j < R; j++) {
-          q[j] = spil[pidx_bucket(hash64((uint64_t)k[j]), ix.B)];
+          q[j] = pil[pidx_bucket(hash64((uint64_t)k[j]), ix.B)];
           generic |= (k[j] == kEmptyKey) | (q[j] == kPilotNone);
         }
         if (__any_sync(0xffffffffu, generic)) {
@@ -1025,6 +1048,9 @@ k_probe_inner_u1_seg_inplace_pidx(int64_t n, TableView t, SliceIndex ix, FastOut
       if (lane == 0) tile_cnt[tile] = m;
       kept += m;
     }
+    // this warp's pilot reads of buffer b are done (their values fed its gathers); the last of the NW warps refills it
+    __syncwarp();
+    if (lane == 0 && atomicAdd(&s_done[b], 1u) == (use + 1) * NW - 1 && p + nbuf < nseg) load(p + nbuf);
   }
   if (lane == 0 && kept) atomicAdd(out_cursor, kept);
 }

@@ -9,7 +9,8 @@
 
 namespace tg {
 
-#define TG_MAX_PARTS 16
+#define TG_MAX_PARTS 16   // destinations of the count kernels (register arrays, k_partition_count4's 8-bit packed counters)
+#define TG_MAX_SLICES 32  // destinations of the scatters: up to 32 L2 slices of a join probe (join.cu), TG_MAX_PARTS GPUs
 #define TG_PART_MAX_COLS 8
 #define PT_BLOCK 256
 #define PT_ITEMS 8
@@ -18,7 +19,7 @@ namespace tg {
 struct PartDst {
   int32_t nparts, ncols;
   const void* src[TG_PART_MAX_COLS];
-  void* dst[TG_MAX_PARTS][TG_PART_MAX_COLS];   // column base per destination
+  void* dst[TG_MAX_SLICES][TG_PART_MAX_COLS];  // column base per destination
   // row offset inside the destination buffers where this launch starts writing, per destination
   const long long* dst_base;                   // device array [nparts]; nullptr = `base_const` for every destination
   long long base_const;
@@ -89,7 +90,7 @@ static __global__ void k_partition_offsets(const unsigned long long* counts, uin
 
 // count-free partitioning: zero the fill counters and the overflow flag, lay the segments out back to back
 static __global__ void k_segment_bases(unsigned long long* cursors, long long* bases, unsigned long long* flag, int nparts, long long cap) {
-  if (threadIdx.x < TG_MAX_PARTS) { cursors[threadIdx.x] = 0; bases[threadIdx.x] = (long long)threadIdx.x * cap; }
+  if (threadIdx.x < TG_MAX_SLICES) { cursors[threadIdx.x] = 0; bases[threadIdx.x] = (long long)threadIdx.x * cap; }
   if (threadIdx.x == 0) *flag = 0;
   (void)nparts;
 }
@@ -99,14 +100,14 @@ __global__ void __launch_bounds__(PT_BLOCK)
 k_partition_scatter(const long long* __restrict__ key, const uint8_t* __restrict__ nulls, int64_t n, PartDst d,
                     unsigned long long* __restrict__ cursors) {
   __shared__ unsigned long long s_val[PT_TILE];
-  __shared__ uint32_t s_cnt[TG_MAX_PARTS], s_off[TG_MAX_PARTS + 1], s_room[TG_MAX_PARTS];
-  __shared__ unsigned long long s_gbase[TG_MAX_PARTS], s_spill[TG_MAX_PARTS];   // s_spill: first spill row of the rows that did not fit, ~0 = dropped
+  __shared__ uint32_t s_cnt[TG_MAX_SLICES], s_off[TG_MAX_SLICES + 1], s_room[TG_MAX_SLICES];
+  __shared__ unsigned long long s_gbase[TG_MAX_SLICES], s_spill[TG_MAX_SLICES];   // s_spill: first spill row of the rows that did not fit, ~0 = dropped
   const int lane = threadIdx.x & 31;
   const uint32_t P = (uint32_t)d.nparts;
   const int64_t ntiles = (n + PT_TILE - 1) / PT_TILE;
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int64_t base = tile * PT_TILE;
-    if (threadIdx.x < TG_MAX_PARTS) s_cnt[threadIdx.x] = 0;
+    if (threadIdx.x < TG_MAX_SLICES) s_cnt[threadIdx.x] = 0;
     __syncthreads();
     // phase 1: destination of every row + rank inside (tile, destination), warp-aggregated
     uint32_t part[PT_ITEMS], rank[PT_ITEMS];
@@ -193,14 +194,14 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 template <bool HIGH, int NC, int ITEMS>
 __global__ void __launch_bounds__(PT_BLOCK)
 k_partition_scatter_bulk(int64_t ntiles, PartDst d, unsigned long long* __restrict__ cursors) {
-  constexpr int STAGES = 2, TILE = PT_BLOCK * ITEMS, SROWS = TILE + 2 * TG_MAX_PARTS;
+  constexpr int STAGES = 2, TILE = PT_BLOCK * ITEMS, SROWS = TILE + 2 * TG_MAX_SLICES;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned long long* ring = reinterpret_cast<unsigned long long*>(smem_raw);      // [STAGES][NC][TILE]
   unsigned long long* stage = ring + (size_t)STAGES * NC * TILE;                   // [NC][SROWS]
   uint64_t* full = reinterpret_cast<uint64_t*>(stage + (size_t)NC * SROWS);
-  __shared__ uint32_t s_cnt[TG_MAX_PARTS], s_off[TG_MAX_PARTS], s_len[TG_MAX_PARTS];
-  __shared__ unsigned long long s_gbase[TG_MAX_PARTS], s_spg[TG_MAX_PARTS];
-  __shared__ uint32_t s_spn[TG_MAX_PARTS];    // rows of this tile's run that go to the spill area, starting at spill row s_spg
+  __shared__ uint32_t s_cnt[TG_MAX_SLICES], s_off[TG_MAX_SLICES], s_len[TG_MAX_SLICES];
+  __shared__ unsigned long long s_gbase[TG_MAX_SLICES], s_spg[TG_MAX_SLICES];
+  __shared__ uint32_t s_spn[TG_MAX_SLICES];    // rows of this tile's run that go to the spill area, starting at spill row s_spg
   const int tid = threadIdx.x, lane = tid & 31;
   const uint32_t P = (uint32_t)d.nparts;
   const unsigned long long pol = l2_policy_evict_first();
@@ -223,7 +224,7 @@ k_partition_scatter_bulk(int64_t ntiles, PartDst d, unsigned long long* __restri
     const int64_t tile = (int64_t)blockIdx.x + it * gridDim.x;
     if (tile >= ntiles) break;
     const int s = (int)(it % STAGES);
-    if (tid < TG_MAX_PARTS) s_cnt[tid] = 0;
+    if (tid < TG_MAX_SLICES) s_cnt[tid] = 0;
     mbar_wait(&full[s], (uint32_t)((it / STAGES) & 1));
     __syncthreads();
     const unsigned long long* in = ring + (size_t)s * NC * TILE;
@@ -383,7 +384,7 @@ inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d,
   constexpr int ITEMS = 4, TILE = PT_BLOCK * ITEMS;
   int64_t ntiles = n / TILE;
   if (ntiles > 0) {
-    size_t smem = (size_t)2 * NC * TILE * 8 + (size_t)NC * (TILE + 2 * TG_MAX_PARTS) * 8 + 2 * 8 + 16;
+    size_t smem = (size_t)2 * NC * TILE * 8 + (size_t)NC * (TILE + 2 * TG_MAX_SLICES) * 8 + 2 * 8 + 16;
     TG_CUDA(cudaFuncSetAttribute(k_partition_scatter_bulk<HIGH, NC, ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (smem + 1024)));
     // a scatter that runs NEXT TO a probe kernel (exchange of step k+1 under the probe of step k) should leave the SMs'

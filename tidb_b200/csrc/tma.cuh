@@ -46,6 +46,11 @@ __device__ __forceinline__ unsigned long long l2_policy_evict_first() {
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
+__device__ __forceinline__ unsigned long long l2_policy_evict_normal() {
+  unsigned long long p;
+  asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
 __device__ __forceinline__ unsigned long long l2_policy_evict_last() {
   unsigned long long p;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));

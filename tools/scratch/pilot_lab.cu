@@ -13,10 +13,13 @@
 //                                                          for each (load factor, mean keys per bucket) pair; default
 //                                                          0.9 2  0.8 3  0.75 4)
 //        tools/scratch/pilot_lab --host [ALPHA LAMBDA]   (CPU only: placement statistics of the pilot index)
+//        tools/scratch/pilot_lab --slices                (GPU: 16 against 32 slices — the index probe and the scatter of the
+//                                                         library at the bench shape, DESIGN.md §4.1 "16 against 32")
 //
 // The index is built on the host here (sequential, largest bucket first, one byte per pilot, 255 = not placed: such a
 // key's tile takes the library's generic path on the linear-probe table).  Results: DESIGN.md §4.1 "Pilot index".
 #include "join_kernels.cuh"
+#include "partition_kernels.cuh"
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
@@ -28,7 +31,7 @@ using namespace tg;
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { printf("CUDA %s at %d\n", cudaGetErrorString(e_), __LINE__); exit(1); } } while (0)
 
 static const uint64_t ODD = 0x9E3779B97F4A7C15ull;
-static const int P = 16;
+static int P = 16;   // slices (--slices sets 16 and 32 in turn)
 
 // slot of a key within its slice under pilot q
 __host__ __device__ __forceinline__ uint32_t pilot_slot(uint64_t h, uint32_t q, uint32_t S) {
@@ -45,7 +48,7 @@ struct Index {
 
 // sequential hash-and-displace per slice, largest bucket first; pilot 255 = not placed
 static Index build_index(const std::vector<uint64_t>& keys, const std::vector<uint64_t>& payload, double alpha, double lambda,
-                         bool fill_slots) {
+                         bool fill_slots, bool library_sizing = false) {
   std::vector<std::vector<uint32_t>> part(P);
   for (uint32_t i = 0; i < keys.size(); i++) part[slot32(hash64(keys[i]), P)].push_back(i);
   size_t mx = 0;
@@ -53,6 +56,10 @@ static Index build_index(const std::vector<uint64_t>& keys, const std::vector<ui
   Index ix;
   ix.S = (uint32_t)std::ceil(mx / alpha);
   ix.B = ((uint32_t)std::ceil(mx / lambda) + 15) & ~15u;   // whole uint4 rows for the shared-memory copy
+  if (library_sizing) {   // build_slice_index (join.cu)
+    ix.S = (uint32_t)std::ceil((double)mx / alpha) + 1;
+    ix.B = ((uint32_t)std::ceil((double)mx / lambda) + 16) & ~15u;
+  }
   ix.pilot.assign((size_t)P * ix.B, 255);
   if (fill_slots) ix.slots.assign((size_t)P * ix.S, Slot{kEmptyKey, 0});
   std::vector<uint8_t> taken(ix.S);
@@ -96,7 +103,7 @@ static Index build_index(const std::vector<uint64_t>& keys, const std::vector<ui
 
 // ---- (b) prototype: pilot → slot → one LDG.128 → compare ---------------------------------------------------------------
 struct PilotView {
-  const Slot* slots; const uint8_t* pilot; uint32_t S, B;
+  const Slot* slots; const uint8_t* pilot; uint32_t S, B, P;
 };
 
 template <bool SMEM>
@@ -116,7 +123,7 @@ __device__ __forceinline__ void pilot_tile(int64_t base, int64_t limit, const Pi
 #pragma unroll
   for (int j = 0; j < R; j++) {
     const uint64_t h = hash64((uint64_t)k[j]);
-    const uint32_t p = slot32(h, P), b = bucket_of(h, ix.B);
+    const uint32_t p = slot32(h, ix.P), b = bucket_of(h, ix.B);
     q[j] = SMEM ? spil[b] : __ldg(ix.pilot + (size_t)p * ix.B + b);
     odd |= (k[j] == kEmptyKey) | (q[j] == 255u);
   }
@@ -126,7 +133,7 @@ __device__ __forceinline__ void pilot_tile(int64_t base, int64_t limit, const Pi
 #pragma unroll
   for (int j = 0; j < R; j++) {
     const uint64_t h = hash64((uint64_t)k[j]);
-    const Slot v = load_slot(ix.slots + (size_t)slot32(h, P) * ix.S + pilot_slot(h, q[j], ix.S));
+    const Slot v = load_slot(ix.slots + (size_t)slot32(h, ix.P) * ix.S + pilot_slot(h, q[j], ix.S));
     meta[j] = v.meta;
     if (v.key == k[j]) hit |= 1u << j;
   }
@@ -227,7 +234,247 @@ static void host_stats(const std::vector<double>& as, const std::vector<double>&
     }
 }
 
+// ---- --slices: 16 against 32 slices at the bench shape (DESIGN.md §4.1, "32 slices") -------------------------------
+// The library's k_probe_inner_u1_seg_inplace_pidx as it was with 16 slices: one pilot buffer, and every slice behind two
+// CTA-wide barriers (the CTA loads the pilots while no gather is in flight).  Variant (a) runs it with half-size slices.
+template <int NPC, int NKD, int NMD>
+__global__ void __launch_bounds__(1024, 1)
+k_pidx_barrier(int64_t n, TableView t, SliceIndex ix, FastOut out, unsigned long long* __restrict__ out_cursor,
+                                  SegSpec seg, uint32_t* __restrict__ tile_cnt) {
+  static_assert(NKD >= 1, "the probe key is read from the first key destination");
+  constexpr int R = 4, G = 2, NP = NPC > 0 ? NPC : 1;
+  extern __shared__ __align__(16) uint8_t spil[];
+  if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) return;
+  const int lane = threadIdx.x & 31;
+  const int64_t warps_total = (int64_t)gridDim.x * (1024 / 32);
+  const int64_t warp_id = (int64_t)blockIdx.x * (1024 / 32) + (threadIdx.x >> 5);
+  const int64_t* __restrict__ pkey = reinterpret_cast<const int64_t*>(out.key_dst[0]);
+  const int nseg = (int)(n / 128 / seg.tiles_per_seg);
+  unsigned long long kept = 0;
+  for (int p = 0; p < nseg; p++) {
+    __syncthreads();   // every warp is done with the previous slice's pilots
+    const uint4* src = reinterpret_cast<const uint4*>(ix.pilot + (size_t)p * ix.B);
+    for (uint32_t i = threadIdx.x; i < ix.B / 16; i += 1024) reinterpret_cast<uint4*>(spil)[i] = __ldcs(src + i);
+    __syncthreads();
+    const unsigned long long c = seg.cnt[p];
+    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+    const int64_t t0 = (int64_t)p * seg.tiles_per_seg, t1 = t0 + seg.tiles_per_seg;
+    const Slot* __restrict__ islots = ix.slots + (size_t)p * ix.S;
+    for (int64_t tile = t0 + warp_id; tile < t1; tile += warps_total) {
+      const int64_t base = tile * 128;
+      uint32_t m = 0;
+      if (limit - base >= 128) {
+        int64_t k[R];
+#pragma unroll
+        for (int g = 0; g < G; g++) {
+          const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + base + g * 64 + 2 * lane));
+          k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
+        }
+        uint32_t q[R];
+        bool generic = false;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+          q[j] = spil[pidx_bucket(hash64((uint64_t)k[j]), ix.B)];
+          generic |= (k[j] == kEmptyKey) | (q[j] == kPilotNone);
+        }
+        if (__any_sync(0xffffffffu, generic)) {
+          m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
+        } else {
+          unsigned long long meta[R];
+          unsigned hit = 0;
+#pragma unroll
+          for (int j = 0; j < R; j++) {
+            const Slot v = load_slot(islots + pidx_slot(hash64((uint64_t)k[j]), q[j], ix.S));
+            meta[j] = v.meta;
+            if (v.key == k[j]) hit |= 1u << j;
+          }
+          if (__all_sync(0xffffffffu, hit == 0xFu)) {
+            m = 128;
+#pragma unroll
+            for (int g = 0; g < G; g++) {
+              const int64_t o = base + g * 64 + 2 * lane;
+              const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
+#pragma unroll
+              for (int d = 1; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
+#pragma unroll
+              for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
+            }
+          } else {
+            unsigned long long pv[R][NP];
+            inplace_load_pv<NPC>(base, out, pv, lane);
+            unsigned bal[R];
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+              bal[j] = __ballot_sync(0xffffffffu, (hit >> j) & 1u);
+              m += __popc(bal[j]);
+            }
+            inplace_store<NPC, NKD, NMD>(base, k, meta, pv, bal, out, lane);
+          }
+        }
+      } else if (limit > base) {
+        m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
+      }
+      if (lane == 0) tile_cnt[tile] = m;
+      kept += m;
+    }
+  }
+  if (lane == 0 && kept) atomicAdd(out_cursor, kept);
+}
+
+
+template <int ITEMS>
+static void scatter(int sms, int64_t rows, const PartDst& d, unsigned long long* cursors, long long* bases, unsigned long long* flag,
+                    int P, long long C) {
+  constexpr int NC = 2, TILE = PT_BLOCK * ITEMS;
+  const size_t smem = (size_t)2 * NC * TILE * 8 + (size_t)NC * (TILE + 2 * TG_MAX_SLICES) * 8 + 2 * 8 + 16;
+  static bool set = false;
+  if (!set) { CK(cudaFuncSetAttribute(k_partition_scatter_bulk<true, NC, ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); set = true; }
+  const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (smem + 1024)));   // launch_scatter_nc
+  const int64_t ntiles = rows / TILE;   // whole tiles of this ITEMS only
+  k_segment_bases<<<1, 32>>>(cursors, bases, flag, P, C);
+  k_partition_scatter_bulk<true, NC, ITEMS><<<(int)std::min<int64_t>(ntiles, (int64_t)sms * per_sm), PT_BLOCK, smem>>>(ntiles, d, cursors);
+}
+
+// One configuration: P slices, its segments (scattered from the same probe columns), its index.
+struct Cut {
+  int P; long long C; unsigned long long *key0, *pv0, *scr; Index ix; Slot* d_ix; uint8_t* d_pil; SliceIndex si;
+};
+
+static int slices_gate() {
+  const int64_t nb = 10000000, np = 100000000;
+  cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, 0));
+  const int sms = prop.multiProcessorCount;
+  printf("card %s, %d SMs, L2 %d MiB, shared memory per block (opt-in) %zu B\n", prop.name, sms, prop.l2CacheSize >> 20, prop.sharedMemPerBlockOptin);
+  // bench.py's columns: build keys id * ODD (ids a permutation), payload id * 7; probe keys uniform ids * ODD, payload the row
+  std::vector<uint64_t> bk(nb), bv(nb), ids(nb), pk(np), pv(np);
+  std::iota(ids.begin(), ids.end(), 0);
+  std::mt19937_64 rng(42);
+  std::shuffle(ids.begin(), ids.end(), rng);
+  for (int64_t i = 0; i < nb; i++) { bk[i] = ids[i] * ODD; bv[i] = ids[i] * 7; }
+  std::uniform_int_distribution<uint64_t> U(0, nb - 1);
+  for (int64_t i = 0; i < np; i++) { pk[i] = U(rng) * ODD; pv[i] = (uint64_t)i; }
+  unsigned long long *d_bk, *d_bv, *d_pk, *d_pv, *d_key1, *d_meta, *d_cur;
+  uint32_t* d_tc;
+  Slot* d_lp;
+  const unsigned long long nslots = (unsigned long long)(nb / 0.5 + 32) & ~3ull;
+  const long long cmax = (long long)(np / 16 * 1.05) + 16384 + 128;
+  CK(cudaMalloc(&d_bk, nb * 8)); CK(cudaMalloc(&d_bv, nb * 8)); CK(cudaMalloc(&d_pk, np * 8)); CK(cudaMalloc(&d_pv, np * 8));
+  CK(cudaMalloc(&d_key1, 16 * cmax * 8)); CK(cudaMalloc(&d_meta, 16 * cmax * 8)); CK(cudaMalloc(&d_cur, 8));
+  CK(cudaMalloc(&d_tc, 16 * cmax / 128 * 4 + 64)); CK(cudaMalloc(&d_lp, (nslots + 2) * sizeof(Slot)));
+  CK(cudaMemcpy(d_bk, bk.data(), nb * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(d_bv, bv.data(), nb * 8, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(d_pk, pk.data(), np * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(d_pv, pv.data(), np * 8, cudaMemcpyHostToDevice));
+  k_table_init<<<(nslots + 256) / 256, 256>>>(d_lp, nslots + 2, nslots);
+  k_lp_insert<<<(nb + 255) / 256, 256>>>(d_bk, d_bv, nb, d_lp, nslots);
+  CK(cudaDeviceSynchronize());
+  const TableView t{d_lp, nslots, nullptr, 0, -1, TABLE_U1, 0};
+  const int64_t nrows = np / 2048 * 2048;   // whole scatter tiles at ITEMS 4 and 8: the same rows for both
+  Cut cut[2];
+  for (int c = 0; c < 2; c++) {
+    Cut& k = cut[c];
+    P = k.P = 16 << c;
+    const long long C0 = ((long long)((double)np / P * 1.05) + 16384 + 127) / 128 * 128;
+    CK(cudaMalloc(&k.key0, P * C0 * 8)); CK(cudaMalloc(&k.pv0, P * C0 * 8)); CK(cudaMalloc(&k.scr, (3 * TG_MAX_SLICES + 8) * 8));
+    PartDst d{};
+    d.nparts = P; d.ncols = 2; d.src[0] = d_pk; d.src[1] = d_pv;
+    for (int q = 0; q < P; q++) { d.dst[q][0] = k.key0; d.dst[q][1] = k.pv0; }
+    unsigned long long* cursors = k.scr;
+    long long* bases = reinterpret_cast<long long*>(k.scr + TG_MAX_SLICES);
+    unsigned long long* flag = k.scr + 2 * TG_MAX_SLICES;
+    d.dst_base = bases; d.capacity = C0; d.overflow = flag;
+    scatter<4>(sms, nrows, d, cursors, bases, flag, P, C0);
+    unsigned long long fill[TG_MAX_SLICES];
+    CK(cudaMemcpy(fill, cursors, P * 8, cudaMemcpyDeviceToHost));
+    const double f = (double)*std::max_element(fill, fill + P);
+    k.C = std::min(((long long)(f + 8.0 * std::sqrt(f)) + 4096 + 127) / 128 * 128, C0);   // inplace_seg_cap
+    d.capacity = k.C;
+    scatter<4>(sms, nrows, d, cursors, bases, flag, P, k.C);
+    unsigned long long ov = 0;
+    CK(cudaMemcpy(&ov, flag, 8, cudaMemcpyDeviceToHost));
+    k.ix = build_index(bk, bv, 0.7, 4.0, true, true);
+    CK(cudaMalloc(&k.d_ix, k.ix.slots.size() * sizeof(Slot))); CK(cudaMalloc(&k.d_pil, k.ix.pilot.size()));
+    CK(cudaMemcpy(k.d_ix, k.ix.slots.data(), k.ix.slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(k.d_pil, k.ix.pilot.data(), k.ix.pilot.size(), cudaMemcpyHostToDevice));
+    k.si = SliceIndex{k.d_ix, k.d_pil, (uint32_t)P, k.ix.S, k.ix.B, 1};
+    printf("P %d: segment capacity %lld (largest fill %.0f, overflow %llu), S %u (%.2f MiB per slice), B %u (%.1f KiB of pilots), unplaced keys %lld\n",
+           P, k.C, f, ov, k.ix.S, k.ix.S * 16.0 / (1 << 20), k.ix.B, k.ix.B / 1024.0, k.ix.bad_keys);
+    fflush(stdout);
+  }
+  auto scatter_run = [&](int v) {   // v: 0 = P16 ITEMS 4, 1 = P32 ITEMS 4, 2 = P32 ITEMS 8, 3 = P16 ITEMS 8
+    Cut& k = cut[v == 1 || v == 2];
+    PartDst d{};
+    d.nparts = k.P; d.ncols = 2; d.src[0] = d_pk; d.src[1] = d_pv;
+    for (int q = 0; q < k.P; q++) { d.dst[q][0] = k.key0; d.dst[q][1] = k.pv0; }
+    d.dst_base = reinterpret_cast<long long*>(k.scr + TG_MAX_SLICES); d.capacity = k.C; d.overflow = k.scr + 2 * TG_MAX_SLICES;
+    if (v == 0 || v == 1) scatter<4>(sms, nrows, d, k.scr, reinterpret_cast<long long*>(k.scr + TG_MAX_SLICES), k.scr + 2 * TG_MAX_SLICES, k.P, k.C);
+    else scatter<8>(sms, nrows, d, k.scr, reinterpret_cast<long long*>(k.scr + TG_MAX_SLICES), k.scr + 2 * TG_MAX_SLICES, k.P, k.C);
+  };
+  // probe variants: 0 = P16 barrier kernel (the library with 16 slices), 1 = (a) P32 barrier kernel, one buffer,
+  // 2 = (b) P32 library kernel, two buffers, 3 = P32 library kernel, one buffer, 4 = P16 library kernel, one buffer
+  const int NV = 5;
+  const char* pname[NV] = {"P16, barriers, 1 buffer (parent)", "(a) P32, barriers, 1 buffer", "(b) P32, library, 2 buffers",
+                           "P32, library, 1 buffer", "P16, library, 1 buffer"};
+  CK(cudaFuncSetAttribute(k_pidx_barrier<1, 2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 << 10));
+  CK(cudaFuncSetAttribute(k_probe_inner_u1_seg_inplace_pidx<1, 2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 << 10));
+  auto probe_run = [&](int v) {
+    Cut& k = cut[v >= 1 && v <= 3];
+    FastOut out{};
+    out.n_pcols = 1; out.n_key_dst = 2; out.n_meta_dst = 1;
+    out.psrc[0] = k.pv0; out.pdst[0] = k.pv0; out.key_dst[0] = k.key0; out.key_dst[1] = d_key1; out.meta_dst[0] = d_meta;
+    const SegSpec sg{k.scr, (uint32_t)(k.C / 128), 0, k.C, nullptr, 0};
+    const int64_t n = (int64_t)k.P * k.C;
+    CK(cudaMemsetAsync(d_cur, 0, 8));
+    SliceIndex si = k.si;
+    if (v <= 1) { k_pidx_barrier<1, 2, 1><<<sms, 1024, si.B>>>(n, t, si, out, d_cur, sg, d_tc); return; }
+    si.nbuf = v == 2 ? 2 : 1;
+    k_probe_inner_u1_seg_inplace_pidx<1, 2, 1><<<sms, 1024, si.nbuf * (si.B + 8)>>>(n, t, si, out, d_cur, sg, d_tc);
+  };
+  // correctness: every variant matches every probe row and writes the build payload of the key at the row's position
+  for (int v = 0; v < NV; v++) {
+    Cut& k = cut[v >= 1 && v <= 3];
+    CK(cudaMemset(d_meta, 0, 16 * cmax * 8)); CK(cudaMemset(d_key1, 0, 16 * cmax * 8));
+    probe_run(v); CK(cudaDeviceSynchronize()); CK(cudaGetLastError());
+    unsigned long long cur, fill[TG_MAX_SLICES];
+    CK(cudaMemcpy(&cur, d_cur, 8, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(fill, k.scr, k.P * 8, cudaMemcpyDeviceToHost));
+    std::vector<uint64_t> m(k.P * k.C), k0(k.P * k.C), k1(k.P * k.C);
+    CK(cudaMemcpy(m.data(), d_meta, m.size() * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(k0.data(), k.key0, m.size() * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(k1.data(), d_key1, m.size() * 8, cudaMemcpyDeviceToHost));
+    long long bad = 0, rows = 0;
+    for (int p = 0; p < k.P; p++)
+      for (unsigned long long i = 0; i < fill[p]; i++, rows++) {
+        const size_t o = (size_t)p * k.C + i;
+        bad += (m[o] * ODD != k0[o] * 7) | (k1[o] != k0[o]);
+      }
+    printf("%-36s rows %llu (want %lld, segment rows %lld), wrong rows %lld\n", pname[v], cur, (long long)np, rows, bad);
+    fflush(stdout);
+  }
+  cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+  auto timed = [&](auto&& fn, int nv, const char* const* names, const char* what) {
+    std::vector<std::vector<float>> ms(nv);
+    for (int v = 0; v < nv; v++) { fn(v); fn(v); }
+    for (int it = 0; it < 30; it++)
+      for (int v = 0; v < nv; v++) {
+        CK(cudaEventRecord(e0)); fn(v); CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
+        float x; CK(cudaEventElapsedTime(&x, e0, e1)); ms[v].push_back(x);
+      }
+    CK(cudaGetLastError());
+    printf("\n%s, ms per launch, median of 30 alternating launches (min, max):\n", what);
+    for (int v = 0; v < nv; v++) {
+      std::sort(ms[v].begin(), ms[v].end());
+      printf("  %-36s %.3f  (%.3f, %.3f)  %+.1f %%\n", names[v], ms[v][15], ms[v][0], ms[v][29], 100.0 * (ms[v][15] / ms[0][15] - 1));
+    }
+    fflush(stdout);
+  };
+  const char* sname[4] = {"P16, ITEMS 4 (parent)", "P32, ITEMS 4", "P32, ITEMS 8", "P16, ITEMS 8"};
+  for (int round = 0; round < 2; round++) {
+    timed(scatter_run, 4, sname, "k_partition_scatter_bulk<true,2,ITEMS> (k_segment_bases + scatter, 100 M rows, 2 columns)");
+    timed(probe_run, NV, pname, "index probe <1,2,1> (100 M rows, 100 % match)");
+  }
+  return 0;
+}
+
 int main(int argc, char** argv) {
+  if (argc > 1 && !strcmp(argv[1], "--slices")) return slices_gate();
   if (argc > 1 && !strcmp(argv[1], "--host")) {
     if (argc == 4) host_stats({atof(argv[2])}, {atof(argv[3])});
     else host_stats({0.8, 0.85, 0.9}, {4.0, 5.0, 6.0});
@@ -291,7 +538,7 @@ int main(int argc, char** argv) {
     CK(cudaMalloc(&d_ix, ix.slots.size() * sizeof(Slot))); CK(cudaMalloc(&d_pil, ix.pilot.size()));
     CK(cudaMemcpy(d_ix, ix.slots.data(), ix.slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(d_pil, ix.pilot.data(), ix.pilot.size(), cudaMemcpyHostToDevice));
-    PilotView pv{d_ix, d_pil, ix.S, ix.B};
+    PilotView pv{d_ix, d_pil, ix.S, ix.B, (uint32_t)P};
     const size_t smem = ix.B;
     const int nv = smem <= prop.sharedMemPerBlockOptin ? 3 : 2;   // the shared-memory variant needs the slice's pilots in one CTA
     if (nv == 3) CK(cudaFuncSetAttribute(k_pilot_sm<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
