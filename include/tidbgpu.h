@@ -315,8 +315,10 @@ enum {
   TG_JOIN_PATH_SCATTER_BULK = 1 << 5,   /* bulk partition scatter (k_partition_scatter_bulk)                     */
   TG_JOIN_PATH_SCATTER = 1 << 6,        /* LSU partition scatter over the whole input (k_partition_scatter)      */
   TG_JOIN_PATH_CELL_GATHER = 0x80,      /* 1 << 7: DECIMAL output cells gathered from row ids (k_gather_cells)      */
-  TG_JOIN_PATH_PROBE_INDEX = 0x100      /* 1 << 8: in-place segment probe through the table's slice index
+  TG_JOIN_PATH_PROBE_INDEX = 0x100,     /* 1 << 8: in-place segment probe through the table's slice index
                                            (k_probe_inner_u1_seg_inplace_pidx)                                        */
+  TG_JOIN_SCATTER_TILE_4K = 0x200       /* 1 << 9, not a kernel family but a qualifier of TG_JOIN_PATH_SCATTER_BULK: the
+                                           bulk scatter ran with 4096-row tiles (dense input), else with 1024-row tiles   */
 };
 int tg_join_get_stats(tg_join* j, tg_join_stats* out);
 

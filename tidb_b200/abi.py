@@ -173,6 +173,7 @@ JOIN_PATH_PROBE_UQ, JOIN_PATH_PROBE_GENERAL, JOIN_PATH_PROBE_DIRECT, JOIN_PATH_P
 JOIN_PATH_SCATTER_BULK, JOIN_PATH_SCATTER = 1 << 5, 1 << 6   # 1 << 4 is unassigned
 JOIN_PATH_CELL_GATHER = 1 << 7
 JOIN_PATH_PROBE_INDEX = 1 << 8   # the in-place segment probe took the slice index (k_probe_inner_u1_seg_inplace_pidx)
+JOIN_SCATTER_TILE_4K = 1 << 9    # qualifies JOIN_PATH_SCATTER_BULK: 4096-row tiles (dense input), else 1024-row tiles
 AGG_PATH_NOGROUP, AGG_PATH_V2_GLOBAL, AGG_PATH_V2_LOCAL, AGG_PATH_MULTI_KEY = 1 << 0, 1 << 1, 1 << 2, 1 << 3
 AGG_PATH_V1_LOCAL, AGG_PATH_V1_GLOBAL, AGG_PATH_MERGE = 1 << 4, 1 << 5, 1 << 6
 AGG_PATH_STRING_KEY = 1 << 7

@@ -986,7 +986,7 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
     const size_t table_bytes = (size_t)j->tv.nslots * sizeof(Slot);
     bool src16 = aligned16(pkey);
     for (int c = 0; c < fo.n_pcols; c++) src16 = src16 && aligned16(fo.psrc[c]);
-    const int64_t PTILE = 1024;   // rows per scatter tile (k_partition_scatter_bulk<.., 4>)
+    const int64_t PTILE = scatter_tile_rows(true, in_seg != nullptr, 1 + fo.n_pcols);   // rows per scatter tile: 4096, or 1024
     const int64_t n_main = n / PTILE * PTILE;
     // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments of C rows.
     // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
@@ -1061,7 +1061,7 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
           TG_TRY(launch_probe_seg(j, j->part_cols[0]->as<int64_t>(), (int64_t)P * C, pf, cur, tune, seg));
           j->stats.kernel_launches++;
         }
-        // gated fallback: probes the ORIGINAL input only after an overflow; the < 1024-row tail the scatter left behind
+        // gated fallback: probes the ORIGINAL input only after an overflow; the < PTILE-row tail the scatter left behind
         // (dense input only) rides on the same launch — it is probed whatever the flag says, and appended at R
         if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n_main, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 1, in_seg->cap, flag, 0}));
         else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{nullptr, 0, 1, 0, flag, n_main < n ? n_main : 0}));

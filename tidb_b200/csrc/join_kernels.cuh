@@ -446,7 +446,7 @@ struct SegSpec {
   long long cap;
   const unsigned long long* gate;    // nullptr = unconditional
   long long ungated_from;            // k_probe_inner_u1_w, dense input: when the gate says "do not run", rows >= ungated_from
-                                     // (a multiple of 128) are probed all the same — the < 1024-row tail the partition pass
+                                     // (a multiple of 128) are probed all the same — the < 1 scatter tile the partition pass
                                      // leaves behind rides on the gated fallback launch instead of costing a launch of its own
 };
 

@@ -191,10 +191,10 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 // Threads only touch shared memory: per row one LDS + one atomic (rank) and, per column, one LDS + one STS.
 // Count-free mode (d.capacity > 0): destinations are fixed-size segments and the global cursor atomics are the only
 // bookkeeping — no histogram pass over the keys.  Full TILE-row tiles only; the caller handles the tail.
-template <bool HIGH, int NC, int ITEMS>
-__global__ void __launch_bounds__(PT_BLOCK)
+template <bool HIGH, int NC, int ITEMS, int THREADS = PT_BLOCK>
+__global__ void __launch_bounds__(THREADS)
 k_partition_scatter_bulk(int64_t ntiles, PartDst d, unsigned long long* __restrict__ cursors) {
-  constexpr int STAGES = 2, TILE = PT_BLOCK * ITEMS, SROWS = TILE + 2 * TG_MAX_SLICES;
+  constexpr int STAGES = 2, TILE = THREADS * ITEMS, SROWS = TILE + 2 * TG_MAX_SLICES;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned long long* ring = reinterpret_cast<unsigned long long*>(smem_raw);      // [STAGES][NC][TILE]
   unsigned long long* stage = ring + (size_t)STAGES * NC * TILE;                   // [NC][SROWS]
@@ -238,8 +238,8 @@ k_partition_scatter_bulk(int64_t ntiles, PartDst d, unsigned long long* __restri
     uint32_t pr[ITEMS];   // destination << 16 | rank inside (tile, destination); 0xffff.... = padding row
 #pragma unroll
     for (int j = 0; j < ITEMS; j++) {
-      if (j * PT_BLOCK + tid < valid) {
-        uint64_t h = hash64(in[j * PT_BLOCK + tid]);
+      if (j * THREADS + tid < valid) {
+        uint64_t h = hash64(in[j * THREADS + tid]);
         uint32_t p = HIGH ? mulhi32((uint32_t)(h >> 32), P) : part_of(h, P);
         pr[j] = (p << 16) | atomicAdd(&s_cnt[p], 1u);
       } else pr[j] = 0xffffffffu;
@@ -273,7 +273,7 @@ k_partition_scatter_bulk(int64_t ntiles, PartDst d, unsigned long long* __restri
     for (int c = 0; c < NC; c++) {
 #pragma unroll
       for (int j = 0; j < ITEMS; j++)
-        if (pr[j] != 0xffffffffu) stage[(size_t)c * SROWS + s_off[pr[j] >> 16] + (pr[j] & 0xffffu)] = in[(size_t)c * TILE + j * PT_BLOCK + tid];
+        if (pr[j] != 0xffffffffu) stage[(size_t)c * SROWS + s_off[pr[j] >> 16] + (pr[j] & 0xffffu)] = in[(size_t)c * TILE + j * THREADS + tid];
     }
     fence_async_smem();              // generic-proxy STS → visible to the async proxy that executes the bulk stores
     __syncthreads();                 // staging complete, ring stage s fully consumed (LDS results fed the STS above)
@@ -376,16 +376,26 @@ inline int launch_partition_count(int device, cudaStream_t st, const long long* 
   return TG_OK;
 }
 
-template <bool HIGH, int NC>
-inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d, unsigned long long* cursors, int64_t* launches, int ctas_per_sm,
-                             int32_t* paths) {
+// Rows per tile of k_partition_scatter_bulk for `ncols` columns.  The L2 partition pass of a join (HIGH) over dense input
+// with at most 2 columns takes 4096-row tiles of 512 threads: a quarter of the per-tile bookkeeping (barriers, cursor
+// atomics, the staging drain) per row, at one CTA per SM (193 KiB of shared memory at 2 columns); the pass got faster with
+// every doubling of the tile (DESIGN.md §4.1, "4096-row scatter tiles").  Everything else takes 1024-row tiles of 256
+// threads: segmented input, whose segment capacities are multiples of 1024 rows; the exchange across GPUs, whose
+// mailboxes are sized in 1024-row tiles; and 3–4 columns, whose 4096-row tile does not fit in shared memory.
+inline int64_t scatter_tile_rows(bool high, bool segmented, int ncols) {
+  return high && !segmented && ncols <= 2 ? 4096 : 1024;
+}
+
+template <bool HIGH, int NC, int ITEMS, int THREADS>
+inline int launch_scatter_tiles(int device, cudaStream_t st, int64_t n, PartDst& d, unsigned long long* cursors, int64_t* launches, int ctas_per_sm,
+                                int32_t* paths) {
   int nsm = device_sm_count(device);
-  // 1024-row tiles: 4 CTAs per SM for NC <= 2
-  constexpr int ITEMS = 4, TILE = PT_BLOCK * ITEMS;
+  constexpr int TILE = THREADS * ITEMS;
   int64_t ntiles = n / TILE;
   if (ntiles > 0) {
     size_t smem = (size_t)2 * NC * TILE * 8 + (size_t)NC * (TILE + 2 * TG_MAX_SLICES) * 8 + 2 * 8 + 16;
-    TG_CUDA(cudaFuncSetAttribute(k_partition_scatter_bulk<HIGH, NC, ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    TG_CUDA(cudaFuncSetAttribute(k_partition_scatter_bulk<HIGH, NC, ITEMS, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // 4 CTAs per SM with 1024-row tiles of <= 2 columns, 1 with 4096-row tiles
     int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (smem + 1024)));
     // a scatter that runs NEXT TO a probe kernel (exchange of step k+1 under the probe of step k) should leave the SMs'
     // L1 to the probe: TG_SCATTER_CTAS_PER_SM caps the CTAs (and with them the shared-memory carve-out) per SM
@@ -393,9 +403,9 @@ inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d,
     if (!HIGH && cap_env > 0 && per_sm > cap_env) per_sm = cap_env;
     if (ctas_per_sm > 0 && per_sm > ctas_per_sm) per_sm = ctas_per_sm;
     int grid = (int)std::min<int64_t>(ntiles, (int64_t)nsm * per_sm);
-    k_partition_scatter_bulk<HIGH, NC, ITEMS><<<grid, PT_BLOCK, smem, st>>>(ntiles, d, cursors);
+    k_partition_scatter_bulk<HIGH, NC, ITEMS, THREADS><<<grid, THREADS, smem, st>>>(ntiles, d, cursors);
     if (launches) (*launches)++;
-    if (paths) *paths |= TG_JOIN_PATH_SCATTER_BULK;
+    if (paths) *paths |= TG_JOIN_PATH_SCATTER_BULK | (TILE == 4096 ? TG_JOIN_SCATTER_TILE_4K : 0);
   }
   int64_t done = ntiles * TILE;
   if (done < n) {
@@ -406,6 +416,16 @@ inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d,
     if (launches) (*launches)++;
   }
   return TG_OK;
+}
+
+template <bool HIGH, int NC>
+inline int launch_scatter_nc(int device, cudaStream_t st, int64_t n, PartDst& d, unsigned long long* cursors, int64_t* launches, int ctas_per_sm,
+                             int32_t* paths) {
+  if constexpr (HIGH && NC <= 2) {
+    if (scatter_tile_rows(HIGH, d.in_cnt != nullptr, NC) == 4096)
+      return launch_scatter_tiles<HIGH, NC, 8, 512>(device, st, n, d, cursors, launches, ctas_per_sm, paths);
+  }
+  return launch_scatter_tiles<HIGH, NC, 4, PT_BLOCK>(device, st, n, d, cursors, launches, ctas_per_sm, paths);
 }
 
 // d.src[0] must be the key column; falls back to the LSU kernel for NULL-able keys, unaligned sources or > 4 columns.

@@ -15,6 +15,10 @@
 //        tools/scratch/pilot_lab --host [ALPHA LAMBDA]   (CPU only: placement statistics of the pilot index)
 //        tools/scratch/pilot_lab --slices                (GPU: 16 against 32 slices — the index probe and the scatter of the
 //                                                         library at the bench shape, DESIGN.md §4.1 "16 against 32")
+//        tools/scratch/pilot_lab --scatter               (GPU: the L2 partition pass at 16 and 32 slices — 1024- to 4096-row
+//                                                         tiles, 256 to 1024 threads, ballot ranks, two staging buffers, a
+//                                                         one-stage ring and a plain copy of the same bytes, DESIGN.md §4.1
+//                                                         "4096-row scatter tiles")
 //
 // The index is built on the host here (sequential, largest bucket first, one byte per pilot, 255 = not placed: such a
 // key's tile takes the library's generic path on the linear-probe table).  Results: DESIGN.md §4.1 "Pilot index".
@@ -473,8 +477,241 @@ static int slices_gate() {
   return 0;
 }
 
+// ---- --scatter: the per-tile serial work of the L2 partition pass (DESIGN.md §4.1, "2048-row scatter tiles") ----------
+// k_scatter_lab restates k_partition_scatter_bulk<true, 2, ITEMS, THREADS> for dense input and a capacity without spill,
+// with STAGES input buffers and two switches.  RANK: a row's rank inside (tile, destination) comes from five warp ballots of its destination's bits (the
+// lanes of the same destination, and in lane q the warp's rows for destination q, kept in a register) and one CTA scan over
+// the per-warp counts, instead of one shared atomicAdd per row; the ranks are deterministic.  DBL: two staging buffers, so
+// tile k+1 stages while the bulk stores of tile k still read (cp.async.bulk.wait_group.read 1 instead of 0).
+template <int ITEMS, bool RANK, bool DBL, int THREADS = PT_BLOCK, int STAGES = 2>
+__global__ void __launch_bounds__(THREADS)
+k_scatter_lab(int64_t ntiles, PartDst d, unsigned long long* __restrict__ cursors) {
+  constexpr int NC = 2, TILE = THREADS * ITEMS, SROWS = TILE + 2 * TG_MAX_SLICES, NW = THREADS / 32;
+  constexpr int NBUF = DBL ? 2 : 1;
+  static_assert(!RANK || THREADS == PT_BLOCK, "ballot ranks: 8 warps");
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  unsigned long long* ring = reinterpret_cast<unsigned long long*>(smem_raw);      // [STAGES][NC][TILE]
+  unsigned long long* stage0 = ring + (size_t)STAGES * NC * TILE;                  // [NBUF][NC][SROWS]
+  uint64_t* full = reinterpret_cast<uint64_t*>(stage0 + (size_t)NBUF * NC * SROWS);
+  __shared__ uint32_t s_cnt[TG_MAX_SLICES], s_off[TG_MAX_SLICES], s_len[TG_MAX_SLICES];
+  __shared__ uint32_t s_w[NW][TG_MAX_SLICES];   // RANK: the warp's rows per destination, then the warp's first rank
+  __shared__ unsigned long long s_gbase[TG_MAX_SLICES];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t P = (uint32_t)d.nparts;
+  const unsigned long long pol = l2_policy_evict_first();
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; s++) mbar_init(&full[s], 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  auto issue = [&](int64_t it) {
+    int64_t tile = (int64_t)blockIdx.x + it * gridDim.x;
+    if (tile >= ntiles) return;
+    int s = (int)(it % STAGES);
+    mbar_arrive_expect_tx(&full[s], (uint32_t)(NC * TILE * 8));
+#pragma unroll
+    for (int c = 0; c < NC; c++)
+      bulk_g2s(ring + ((size_t)s * NC + c) * TILE, reinterpret_cast<const unsigned long long*>(d.src[c]) + tile * TILE, TILE * 8, &full[s], pol);
+  };
+  if (tid == 0) for (int it = 0; it < STAGES; it++) issue(it);
+  for (int64_t it = 0;; it++) {
+    const int64_t tile = (int64_t)blockIdx.x + it * gridDim.x;
+    if (tile >= ntiles) break;
+    const int s = (int)(it % STAGES);
+    unsigned long long* stage = stage0 + (size_t)(DBL ? (it & 1) : 0) * NC * SROWS;
+    if (!RANK && tid < TG_MAX_SLICES) s_cnt[tid] = 0;
+    mbar_wait(&full[s], (uint32_t)((it / STAGES) & 1));
+    __syncthreads();
+    const unsigned long long* in = ring + (size_t)s * NC * TILE;
+    uint32_t pr[ITEMS], wcnt = 0;   // wcnt (RANK): in lane q, this warp's rows for destination q so far
+#pragma unroll
+    for (int j = 0; j < ITEMS; j++) {
+      const uint64_t h = hash64(in[j * THREADS + tid]);
+      const uint32_t p = mulhi32((uint32_t)(h >> 32), P);
+      if constexpr (RANK) {
+        unsigned peers = 0xffffffffu, mine = 0xffffffffu;
+#pragma unroll
+        for (int b = 0; b < 5; b++) {
+          const unsigned bal = __ballot_sync(0xffffffffu, (p >> b) & 1u);
+          peers &= ((p >> b) & 1u) ? bal : ~bal;
+          mine &= ((lane >> b) & 1) ? bal : ~bal;
+        }
+        const uint32_t before = __shfl_sync(0xffffffffu, wcnt, (int)p);
+        pr[j] = (p << 16) | (before + __popc(peers & ((1u << lane) - 1)));
+        wcnt += __popc(mine);
+      } else {
+        pr[j] = (p << 16) | atomicAdd(&s_cnt[p], 1u);
+      }
+    }
+    if (RANK) s_w[warp][lane] = wcnt;
+    __syncthreads();
+    if (tid < 32) {
+      uint32_t c = 0;
+      if (tid < (int)P) {
+        if constexpr (RANK) {
+          for (int w = 0; w < NW; w++) { const uint32_t t = s_w[w][tid]; s_w[w][tid] = c; c += t; }
+        } else c = s_cnt[tid];
+      }
+      uint32_t len = c;
+      unsigned long long g = 0;
+      if (tid < (int)P) {
+        const unsigned long long old = c ? atomicAdd(&cursors[tid], (unsigned long long)c) : 0ull;
+        const unsigned long long avail = old < (unsigned long long)d.capacity ? (unsigned long long)d.capacity - old : 0ull;
+        if ((unsigned long long)c > avail) { len = (uint32_t)avail; *d.overflow = 1ull; }
+        g = old + (unsigned long long)d.dst_base[tid];
+      }
+      uint32_t w = tid < (int)P ? (((uint32_t)(g & 1) + c + 1) & ~1u) : 0, incl = w;
+      for (int o = 1; o < 32; o <<= 1) { uint32_t u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
+      if (tid < (int)P) { s_off[tid] = incl - w + (uint32_t)(g & 1); s_gbase[tid] = g; s_len[tid] = len; }
+    }
+    if (tid < (int)P * NC) {
+      if (DBL) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // the stores of tile k-2 have read this buffer
+      else bulk_wait_read_all();
+    }
+    __syncthreads();
+#pragma unroll
+    for (int c = 0; c < NC; c++) {
+#pragma unroll
+      for (int j = 0; j < ITEMS; j++) {
+        const uint32_t p = pr[j] >> 16;
+        stage[(size_t)c * SROWS + s_off[p] + (RANK ? s_w[warp][p] : 0u) + (pr[j] & 0xffffu)] = in[(size_t)c * TILE + j * THREADS + tid];
+      }
+    }
+    fence_async_smem();
+    __syncthreads();
+    if (tid == 0) issue(it + STAGES);
+    if (tid < (int)P * NC) {
+      const uint32_t p = tid / NC, c = tid % NC;
+      const unsigned long long g = s_gbase[p];
+      const uint32_t len = s_len[p], so = s_off[p];
+      unsigned long long* dst = reinterpret_cast<unsigned long long*>(d.dst[p][c]);
+      const unsigned long long* src = stage + (size_t)c * SROWS;
+      const uint32_t head = (uint32_t)(g & 1) & (len > 0 ? 1u : 0u);
+      const uint32_t mid = (len - head) & ~1u;
+      if (mid) bulk_s2g(dst + g + head, src + so + head, mid * 8);
+      bulk_commit();
+      if (head) dst[g] = src[so];
+      if ((len - head) & 1u) dst[g + len - 1] = src[so + len - 1];
+    }
+  }
+  if (tid < (int)P * NC) bulk_wait_read_all();
+}
+
+// per segment, the sum of a mix of (key, payload) over its filled rows: equal sums = the same rows in every segment
+static __global__ void k_seg_sum(const unsigned long long* key, const unsigned long long* pv, const unsigned long long* fill, long long C,
+                                 int P, unsigned long long* out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (int64_t)P * C; i += (int64_t)gridDim.x * blockDim.x) {
+    const int p = (int)(i / C);
+    if (i - (int64_t)p * C < (int64_t)fill[p]) atomicAdd(&out[p], hash64(key[i] ^ (pv[i] * 0xD6E8FEB86659FD93ull)));
+  }
+}
+
+static int scatter_gate() {
+  const int64_t np = 100000000, nb = 10000000;
+  cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, 0));
+  const int sms = prop.multiProcessorCount;
+  printf("card %s, %d SMs, L2 %d MiB\n", prop.name, sms, prop.l2CacheSize >> 20);
+  // bench.py's probe columns: uniform build ids * ODD, payload the row
+  std::vector<uint64_t> pk(np), pv(np);
+  std::mt19937_64 rng(42);
+  std::uniform_int_distribution<uint64_t> U(0, nb - 1);
+  for (int64_t i = 0; i < np; i++) { pk[i] = U(rng) * ODD; pv[i] = (uint64_t)i; }
+  const int64_t nrows = np / 2048 * 2048;   // whole tiles at ITEMS 4 and 8
+  unsigned long long *d_pk, *d_pv, *d_c0, *d_c1, *d_key0, *d_pv0, *scr, *sum;
+  const long long cmax = (long long)(np / 16 * 1.05) + 16384 + 128;
+  CK(cudaMalloc(&d_pk, np * 8)); CK(cudaMalloc(&d_pv, np * 8)); CK(cudaMalloc(&d_c0, np * 8)); CK(cudaMalloc(&d_c1, np * 8));
+  CK(cudaMalloc(&d_key0, 16 * cmax * 8)); CK(cudaMalloc(&d_pv0, 16 * cmax * 8));
+  CK(cudaMalloc(&scr, (3 * TG_MAX_SLICES + 8) * 8)); CK(cudaMalloc(&sum, TG_MAX_SLICES * 8));
+  CK(cudaMemcpy(d_pk, pk.data(), np * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(d_pv, pv.data(), np * 8, cudaMemcpyHostToDevice));
+  unsigned long long* cursors = scr;
+  long long* bases = reinterpret_cast<long long*>(scr + TG_MAX_SLICES);
+  unsigned long long* flag = scr + 2 * TG_MAX_SLICES;
+  const int NV = 13;
+  const char* name[NV] = {"library ITEMS 4 (parent)", "library ITEMS 8", "lab ITEMS 8", "(a) ITEMS 8, ballot ranks",
+                          "(b) ITEMS 8, 2 staging buffers", "(a)+(b) ITEMS 8", "(b) ITEMS 4, 2 staging buffers", "copy of the same bytes",
+                          "(c) 512 threads x 4 (2048 rows)", "(c) 1024 threads x 2 (2048 rows)", "(d) ITEMS 8, 1-stage ring",
+                          "(c)+(d) 512 x 4, 1-stage ring", "(c) 512 threads x 8 (4096 rows)"};
+  auto lab = [&](auto kernel, int items, int nbuf, const PartDst& d, int threads = PT_BLOCK, int stages = 2) {
+    const size_t tile = (size_t)threads * items;
+    const size_t smem = (size_t)stages * 2 * tile * 8 + (size_t)nbuf * 2 * (tile + 2 * TG_MAX_SLICES) * 8 + 2 * 8 + 16;
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (smem + 1024)));   // launch_scatter_nc
+    const int64_t ntiles = nrows / (int64_t)tile;
+    kernel<<<(int)std::min<int64_t>(ntiles, (int64_t)sms * per_sm), threads, smem>>>(ntiles, d, cursors);
+  };
+  for (int P : {16, 32}) {
+    const long long C0 = ((long long)((double)nrows / P * 1.05) + 16384 + 127) / 128 * 128;
+    PartDst d{};
+    d.nparts = P; d.ncols = 2; d.src[0] = d_pk; d.src[1] = d_pv;
+    for (int q = 0; q < P; q++) { d.dst[q][0] = d_key0; d.dst[q][1] = d_pv0; }
+    d.dst_base = bases; d.capacity = C0; d.overflow = flag;
+    scatter<4>(sms, nrows, d, cursors, bases, flag, P, C0);
+    unsigned long long fill[TG_MAX_SLICES];
+    CK(cudaMemcpy(fill, cursors, P * 8, cudaMemcpyDeviceToHost));
+    const double f = (double)*std::max_element(fill, fill + P);
+    d.capacity = std::min(((long long)(f + 8.0 * std::sqrt(f)) + 4096 + 127) / 128 * 128, C0);   // inplace_seg_cap
+    auto run = [&](int v) {
+      if (v == 7) {
+        CK(cudaMemcpyAsync(d_c0, d_pk, nrows * 8, cudaMemcpyDeviceToDevice)); CK(cudaMemcpyAsync(d_c1, d_pv, nrows * 8, cudaMemcpyDeviceToDevice));
+        return;
+      }
+      if (v < 2) { (v ? scatter<8> : scatter<4>)(sms, nrows, d, cursors, bases, flag, P, d.capacity); return; }
+      k_segment_bases<<<1, 32>>>(cursors, bases, flag, P, d.capacity);
+      if (v == 2) lab(k_scatter_lab<8, false, false>, 8, 1, d);
+      else if (v == 3) lab(k_scatter_lab<8, true, false>, 8, 1, d);
+      else if (v == 4) lab(k_scatter_lab<8, false, true>, 8, 2, d);
+      else if (v == 5) lab(k_scatter_lab<8, true, true>, 8, 2, d);
+      else if (v == 6) lab(k_scatter_lab<4, false, true>, 4, 2, d);
+      else if (v == 8) lab(k_scatter_lab<4, false, false, 512>, 4, 1, d, 512);
+      else if (v == 9) lab(k_scatter_lab<2, false, false, 1024>, 2, 1, d, 1024);
+      else if (v == 10) lab(k_scatter_lab<8, false, false, 256, 1>, 8, 1, d, 256, 1);
+      else if (v == 11) lab(k_scatter_lab<4, false, false, 512, 1>, 4, 1, d, 512, 1);
+      else lab(k_scatter_lab<8, false, false, 512>, 8, 1, d, 512);
+    };
+    // correctness: every variant leaves the same rows in every segment as the parent's kernel, and no overflow
+    std::vector<unsigned long long> ref(P);
+    for (int v = 0; v < NV; v++) {
+      if (v == 7) continue;
+      run(v);
+      CK(cudaMemsetAsync(sum, 0, TG_MAX_SLICES * 8));
+      k_seg_sum<<<sms * 8, 256>>>(d_key0, d_pv0, cursors, d.capacity, P, sum);
+      CK(cudaDeviceSynchronize()); CK(cudaGetLastError());
+      std::vector<unsigned long long> got(P), fl(P);
+      unsigned long long ov = 0;
+      CK(cudaMemcpy(got.data(), sum, P * 8, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(fl.data(), cursors, P * 8, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(&ov, flag, 8, cudaMemcpyDeviceToHost));
+      if (v == 0) ref = got;
+      unsigned long long rows = 0;
+      for (int p = 0; p < P; p++) rows += fl[p];
+      printf("P %d %-32s rows %llu (want %lld), overflow %llu, segments %s\n", P, name[v], rows, (long long)nrows, ov, got == ref ? "same" : "DIFFERENT");
+    }
+    fflush(stdout);
+    cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    for (int round = 0; round < 2; round++) {
+      std::vector<std::vector<float>> ms(NV);
+      for (int v = 0; v < NV; v++) { run(v); run(v); }
+      for (int it = 0; it < 30; it++)
+        for (int v = 0; v < NV; v++) {
+          CK(cudaEventRecord(e0)); run(v); CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
+          float x; CK(cudaEventElapsedTime(&x, e0, e1)); ms[v].push_back(x);
+        }
+      CK(cudaGetLastError());
+      printf("\nP %d, round %d: %lld rows x 2 columns, ms per launch, median of 30 alternating launches (min, max), TB/s of 32 B/row:\n",
+             P, round, (long long)nrows);
+      for (int v = 0; v < NV; v++) {
+        std::sort(ms[v].begin(), ms[v].end());
+        printf("  %-32s %.3f  (%.3f, %.3f)  %.2f TB/s  %+.1f %%\n", name[v], ms[v][15], ms[v][0], ms[v][29],
+               32.0 * nrows / (ms[v][15] * 1e-3) / 1e12, 100.0 * (ms[v][15] / ms[0][15] - 1));
+      }
+      fflush(stdout);
+    }
+  }
+  return 0;
+}
+
 int main(int argc, char** argv) {
   if (argc > 1 && !strcmp(argv[1], "--slices")) return slices_gate();
+  if (argc > 1 && !strcmp(argv[1], "--scatter")) return scatter_gate();
   if (argc > 1 && !strcmp(argv[1], "--host")) {
     if (argc == 4) host_stats({atof(argv[2])}, {atof(argv[3])});
     else host_stats({0.8, 0.85, 0.9}, {4.0, 5.0, 6.0});
