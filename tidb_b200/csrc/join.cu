@@ -873,10 +873,11 @@ static bool build_fast_out(const JoinImpl* j, const OutCols& oc, const DevCols& 
   return true;
 }
 
-// (NPC, NKD, NMD) dispatch
-template <template <int, int, int> class F, typename... A>
-static int dispatch_shape(const FastOut& fo, A&&... a) {
-#define TG_SHAPE(P, K, M) if (fo.n_pcols == P && fo.n_key_dst == K && fo.n_meta_dst == M) return F<P, K, M>::run(a...);
+// (NPC, NKD, NMD) dispatch: f(npc, nkd, nmd), the shape of fo as std::integral_constant values
+template <typename F>
+static int dispatch_shape(const FastOut& fo, F&& f) {
+  using std::integral_constant;
+#define TG_SHAPE(P, K, M) if (fo.n_pcols == P && fo.n_key_dst == K && fo.n_meta_dst == M) return f(integral_constant<int, P>(), integral_constant<int, K>(), integral_constant<int, M>());
 #define TG_SHAPE_KM(P) TG_SHAPE(P, 0, 0) TG_SHAPE(P, 0, 1) TG_SHAPE(P, 1, 0) TG_SHAPE(P, 1, 1) TG_SHAPE(P, 2, 0) TG_SHAPE(P, 2, 1)
   TG_SHAPE_KM(0) TG_SHAPE_KM(1) TG_SHAPE_KM(2) TG_SHAPE_KM(3)
 #undef TG_SHAPE_KM
@@ -884,245 +885,236 @@ static int dispatch_shape(const FastOut& fo, A&&... a) {
   return fail(TG_ERR_CUDA, "internal: fused probe shape not instantiated");
 }
 
-template <int NPC, int NKD, int NMD>
-struct LaunchWarp {
-  static int run(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t, const SegSpec& seg) {
-    constexpr int R = 4;
-    static int resident = 0;   // CTAs of this instantiation one SM holds (register-bound)
-    if (!resident) {
-      int nb = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_probe_inner_u1_w<R, NPC, NKD, NMD>, 256, 0) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 3; }
-      resident = nb;
-      if (getenv("TG_DEBUG")) fprintf(stderr, "[tidbgpu] k_probe_inner_u1_w<%d,%d,%d>: %d resident CTAs per SM\n", NPC, NKD, NMD, nb);
-    }
-    int64_t tiles = (n + 32 * R - 1) / (32 * R);
-    int64_t ctas = (tiles + 7) / 8;
-    int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
-    int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
-    k_probe_inner_u1_w<R, NPC, NKD, NMD><<<grid, 256, 0, j->stream>>>(pkey, n, j->tv, fo, cur, seg);
-    return TG_OK;
+// Launch the persistent fused probe kernel K with `ctas` CTAs at most, and one wave at most: TG_PROBE_CTAS_PER_SM, or the
+// CTAs of K one SM holds (register-bound: queried once per instantiation, 3 if the query fails), per SM
+template <auto K, typename... A>
+static int launch_resident(JoinImpl* j, const char* name, const FastOut& fo, int64_t ctas, const ProbeTuning& t, A... args) {
+  static int resident = 0;
+  if (!resident) {
+    int nb = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, K, 256, 0) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 3; }
+    resident = nb;
+    if (getenv("TG_DEBUG")) fprintf(stderr, "[tidbgpu] %s<%d,%d,%d>: %d resident CTAs per SM\n", name, fo.n_pcols, fo.n_key_dst, fo.n_meta_dst, nb);
   }
-};
-template <int NPC, int NKD, int NMD>
-struct LaunchSeg {
-  static int run(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t, const SegSpec& seg) {
-    static int resident = 0;
-    if (!resident) {
-      int nb = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_probe_inner_u1_seg_lean<NPC, NKD, NMD>, 256, 0) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 3; }
-      resident = nb;
-    }
-    int64_t ctas = (n / 128 + 7) / 8;
-    int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
-    int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
-    k_probe_inner_u1_seg_lean<NPC, NKD, NMD><<<grid, 256, 0, j->stream>>>(pkey, n, j->tv, fo, cur, seg);
-    return TG_OK;
+  const int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
+  K<<<(int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm), 256, 0, j->stream>>>(args...);
+  return TG_OK;
+}
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// the fast paths write every output column from row rb.rows on, and no NULLs
+static void bind_fast_outputs(JoinImpl* j, ResultBatch& rb, OutCols& oc) {
+  for (int c = 0; c < j->n_out; c++) { oc.data[c] = kernel_out(j, rb, c) + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
+}
+
+// wait for the probe and append the `got` = *cur rows it wrote to rb (copies enqueued before this land as well)
+static int read_cursor(JoinImpl* j, ResultBatch& rb, const unsigned long long* cur, unsigned long long& got) {
+  TG_CUDA(cudaMemcpyAsync(&got, cur, 8, cudaMemcpyDeviceToHost, j->stream));
+  TG_CUDA(cudaStreamSynchronize(j->stream));
+  TG_CUDA(cudaGetLastError());
+  rb.rows += (int64_t)got;
+  j->stats.output_rows += (int64_t)got;
+  return TG_OK;
+}
+
+static void ensure_tmp_valid(JoinImpl* j) {
+  if ((int)j->tmp_valid.size() != j->n_out) { j->tmp_valid.clear(); for (int i = 0; i < j->n_out; i++) j->tmp_valid.emplace_back(new DevBuf()); }
+}
+
+// ---- fused path: the warp kernels, behind an optional L2 partition pass ------------------------------------
+// The partition pass of one call: P segments of C rows (P = 0: no pass, the direct launch), the n_main rows it scatters in
+// tiles of ptile, and whether the segment probe runs in place
+struct FusedPlan { int P; int64_t C; int64_t ptile, n_main; bool inplace; };
+
+static FusedPlan fused_plan(const JoinImpl* j, const ResultBatch& rb, const int64_t* pkey, int64_t n, const FastOut& fo,
+                            const ProbeTuning& tune, bool seg_input) {
+  FusedPlan fp{};
+  const size_t table_bytes = (size_t)j->tv.nslots * sizeof(Slot);
+  bool src16 = aligned16(pkey);
+  for (int c = 0; c < fo.n_pcols; c++) src16 = src16 && aligned16(fo.psrc[c]);
+  fp.ptile = scatter_tile_rows(true, seg_input, 1 + fo.n_pcols);   // rows per scatter tile: 4096, or 1024
+  fp.n_main = n / fp.ptile * fp.ptile;
+  // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments of C rows.
+  // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
+  // [p/P, (p+1)/P) while the probe kernel sweeps the segment.  The pass trades 32 B/row of extra streaming traffic for
+  // random HBM traffic, which only pays while a slice stays L2 resident (probe_slices; U1 tables are built dense
+  // enough for that, build_table).  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
+  // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
+  // Fewer than ptile rows leave the scatter nothing to do: the whole input would be the tail, and the gated launch,
+  // which probes the tail from row n_main on, reads n_main = 0 as "no tail".  Such a probe takes the direct launch.
+  if (fp.n_main > 0 && tune.partition && src16 && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
+    fp.P = probe_slices(table_bytes, j->device, tune.parts);
+    fp.C = ((int64_t)((double)fp.n_main / fp.P * 1.05) + 16384 + 127) / 128 * 128;
+    if (!(fp.P >= 2 && (int64_t)fp.P * fp.C / 128 < (1ll << 31))) fp.P = 0;
   }
-};
-template <int NPC, int NKD, int NMD>
-struct LaunchInplace {
-  static int run(JoinImpl* j, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t, const SegSpec& seg, uint32_t* tile_cnt) {
-    if constexpr (NKD == 0) {
-      return fail(TG_ERR_CUDA, "internal: the in-place segment probe needs an output fed by the join key");
-    } else {
-      static int resident = 0;
-      if (!resident) {
-        int nb = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_probe_inner_u1_seg_inplace<NPC, NKD, NMD>, 256, 0) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 3; }
-        resident = nb;
-      }
-      int64_t ctas = (n / 128 + 7) / 8;
-      int per_sm = t.ctas_per_sm > 0 ? t.ctas_per_sm : resident;
-      int grid = (int)std::min<int64_t>(ctas, (int64_t)j->nsm * per_sm);
-      if (j->pidx.P == (uint32_t)(n / seg.cap)) {
+  // In place (k_probe_inner_u1_seg_inplace): the scatter writes the probe columns straight into the output columns, which
+  // then take the segment layout, P·C rows.  It moves fewer bytes than the lean segment probe only when nearly every
+  // 128-row tile matches in full, so it follows the match fraction of the last partitioned call whose count the host read
+  // (the first call takes it); a mispredicted call is slower, never wrong.  Dense input and a fresh batch only: the
+  // segment layout starts at the allocation.
+  fp.inplace = fp.P && !seg_input && rb.rows == 0 && fo.n_key_dst >= 1 &&
+               (tune.inplace >= 0 ? tune.inplace != 0 : j->seg_match >= kInplaceMinMatch);
+  if (fp.inplace) fp.C = inplace_seg_cap(j, fp.P, fp.n_main, fp.C);
+  return fp;
+}
+
+// the partition pass: the probe key and payload columns into P segments of C rows (the output columns themselves when in
+// place, else part_cols); `seg` describes them, gated on the pass's overflow flag
+static int scatter_segments(JoinImpl* j, const FusedPlan& fp, const int64_t* pkey, const FastOut& fo, const SegSpec* in_seg, SegSpec& seg) {
+  const int nc = 1 + fo.n_pcols;
+  if (!fp.inplace) {
+    for (int c = 0; c < nc; c++) {
+      if (!j->part_cols[c]) j->part_cols[c].reset(new DevBuf());
+      TG_TRY(j->part_cols[c]->ensure(j->device, (size_t)fp.P * fp.C * 8 + 64));
+    }
+  }
+  TG_TRY(j->part_scratch.ensure(j->device, (size_t)3 * TG_MAX_SLICES * 8 + 64));
+  unsigned long long* cursors = j->part_scratch.as<unsigned long long>();      // fill count per segment
+  long long* bases = reinterpret_cast<long long*>(cursors + TG_MAX_SLICES);   // first row of each segment
+  unsigned long long* flag = cursors + 2 * TG_MAX_SLICES;                      // overflow
+  PartDst d{};
+  d.nparts = fp.P; d.ncols = nc;
+  d.src[0] = pkey;
+  for (int c = 0; c < fo.n_pcols; c++) d.src[1 + c] = fo.psrc[c];
+  for (int c = 0; c < nc; c++)
+    for (int q = 0; q < fp.P; q++) d.dst[q][c] = fp.inplace ? (c == 0 ? (void*)fo.key_dst[0] : (void*)fo.pdst[c - 1]) : j->part_cols[c]->p;
+  k_segment_bases<<<1, 32, 0, j->stream>>>(cursors, bases, flag, fp.P, fp.C);
+  j->stats.kernel_launches++;
+  d.dst_base = bases; d.capacity = fp.C; d.overflow = flag;
+  if (in_seg) { d.in_cnt = in_seg->cnt; d.in_cap = in_seg->cap; d.in_tiles_per_seg = (uint32_t)(in_seg->cap / fp.ptile); }
+  TG_TRY(launch_partition_scatter<true>(j->device, j->stream, reinterpret_cast<const long long*>(pkey), nullptr, fp.n_main, d, cursors,
+                                        &j->stats.kernel_launches, 0, &j->stats.paths));
+  seg = SegSpec{cursors, (uint32_t)(fp.C / 128), 0, fp.C, flag};
+  return TG_OK;
+}
+
+// the segment probe: in place, then the output made dense (the rows at or beyond R = *cur fill the holes below R); or lean,
+// from the segment copies in part_cols
+static int probe_segments(JoinImpl* j, const FusedPlan& fp, const FastOut& fo, unsigned long long* cur, const ProbeTuning& tune, const SegSpec& seg) {
+  const int64_t rows = (int64_t)fp.P * fp.C, ntiles = rows / 128;
+  j->stats.paths |= TG_JOIN_PATH_PROBE_SEG;
+  if (fp.inplace) {
+    TG_TRY(j->tile_cnt.ensure(j->device, (size_t)ntiles * 4 + 16));
+    TG_TRY(j->tmp_cnt.ensure(j->device, (size_t)(2 * ntiles + 1) * 4));
+    uint32_t* tile_cnt = j->tile_cnt.as<uint32_t>();
+    TG_TRY(dispatch_shape(fo, [&](auto npc, auto nkd, auto nmd) -> int {
+      if constexpr (nkd == 0) {
+        return fail(TG_ERR_CUDA, "internal: the in-place segment probe needs an output fed by the join key");
+      } else if (j->pidx.P == (uint32_t)fp.P) {
         // the slice index of this table, cut for this P: one CTA per SM holding nbuf slices' pilots and their mbarriers.
         // The shared-memory limit is an attribute of the current device, so it is raised on every launch, as the
         // aggregation does.
         const int smem = (int)(j->pidx.nbuf * (j->pidx.B + 8));
-        TG_CUDA(cudaFuncSetAttribute(k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        k_probe_inner_u1_seg_inplace_pidx<NPC, NKD, NMD><<<j->nsm, kPidxThreads, smem, j->stream>>>(n, j->tv, j->pidx, fo, cur, seg, tile_cnt);
+        TG_CUDA(cudaFuncSetAttribute(k_probe_inner_u1_seg_inplace_pidx<npc, nkd, nmd>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        k_probe_inner_u1_seg_inplace_pidx<npc, nkd, nmd><<<j->nsm, kPidxThreads, smem, j->stream>>>(rows, j->tv, j->pidx, fo, cur, seg, tile_cnt);
         j->stats.paths |= TG_JOIN_PATH_PROBE_INDEX;
         return TG_OK;
-      }
-      k_probe_inner_u1_seg_inplace<NPC, NKD, NMD><<<grid, 256, 0, j->stream>>>(n, j->tv, fo, cur, seg, tile_cnt);
-      return TG_OK;
-    }
-  }
-};
-static int launch_probe_warp(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t,
-                             const SegSpec& seg = SegSpec{nullptr, 0, 0, 0, nullptr}) {
-  j->stats.paths |= TG_JOIN_PATH_PROBE_DIRECT;
-  return dispatch_shape<LaunchWarp>(fo, j, pkey, n, fo, cur, t, seg);
-}
-static int launch_probe_seg(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& t, const SegSpec& seg) {
-  j->stats.paths |= TG_JOIN_PATH_PROBE_SEG;
-  return dispatch_shape<LaunchSeg>(fo, j, pkey, n, fo, cur, t, seg);
-}
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
-// probe `n` device-resident rows; results are appended to rb (rb.rows advanced)
-static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBatch& rb, bool sync_count, const SegSpec* in_seg = nullptr) {
-  const Side& p = j->probe;
-  DevCols pview = pcells;
-  TG_TRY(kernel_view(j, p, pview, n));
-  j->stats.probe_rows += n;
-  KeySpec ks = j->probe_key;
-  if (j->multi_key) {
-    if (in_seg) return fail(TG_ERR_UNSUPPORTED, "segmented device chunks: joins on several key columns take the general path");
-    TG_TRY(composite_key(j, p, pview, n, j->pkey_syn, j->pkey_syn_nn));
-    ks.data = j->pkey_syn.p; ks.nulls = j->pkey_syn_nn.as<uint8_t>();
-  } else { ks.data = pview.data[p.key_col]; ks.nulls = pview.nulls[p.key_col]; }
-  TG_TRY(j->out_cursor.ensure(j->device, 64));
-  OutCols oc{};
-  fill_outspec_probe(j, oc);
-  FastOut fo{};
-  // the output shape decides the path before any output is allocated: the fused warp kernels, else the single-pass
-  // unique-key kernel, else the general path.  build_fast_out runs again once the output pointers are known.
-  const bool fast = fast_path_ok(j, pview) && build_fast_out(j, oc, pview, fo);
-  if (in_seg && !fast) return fail(TG_ERR_UNSUPPORTED, "segmented device chunks are only accepted by the fused fast path (unique build keys, <= 1 payload, no filters, an output shape the warp kernels cover)");
-  if (fast) {
-    const ProbeTuning& tune = probe_tuning();
-    const int64_t* pkey = reinterpret_cast<const int64_t*>(ks.data);
-    const size_t table_bytes = (size_t)j->tv.nslots * sizeof(Slot);
-    bool src16 = aligned16(pkey);
-    for (int c = 0; c < fo.n_pcols; c++) src16 = src16 && aligned16(fo.psrc[c]);
-    const int64_t PTILE = scatter_tile_rows(true, in_seg != nullptr, 1 + fo.n_pcols);   // rows per scatter tile: 4096, or 1024
-    const int64_t n_main = n / PTILE * PTILE;
-    // L2 partition pass, count-free: regroup the probe rows by the TOP hash bits into P fixed-capacity segments of C rows.
-    // slot = mulhi(hash, nslots) is monotone in the hash, so segment p only touches the contiguous table slice
-    // [p/P, (p+1)/P) while the probe kernel sweeps the segment.  The pass trades 32 B/row of extra streaming traffic for
-    // random HBM traffic, which only pays while a slice stays L2 resident (probe_slices; U1 tables are built dense
-    // enough for that, build_table).  A skewed probe side that overflows a segment raises `flag`; the partitioned probe
-    // launch then exits at once and the gated direct launch behind it does the work — no host round trip.
-    // Fewer than PTILE rows leave the scatter nothing to do: the whole input would be the tail, and the gated launch,
-    // which probes the tail from row n_main on, reads n_main = 0 as "no tail".  Such a probe takes the direct launch.
-    int P = 0;
-    int64_t C = 0;
-    if (n_main > 0 && tune.partition && src16 && n >= (int64_t)tune.part_min_rows && table_bytes > ((size_t)tune.part_min_mb << 20)) {
-      P = probe_slices(table_bytes, j->device, tune.parts);
-      C = ((int64_t)((double)n_main / P * 1.05) + 16384 + 127) / 128 * 128;
-      if (!(P >= 2 && (int64_t)P * C / 128 < (1ll << 31))) P = 0;
-    }
-    // In place (k_probe_inner_u1_seg_inplace): the scatter writes the probe columns straight into the output columns, which
-    // then take the segment layout, P·C rows.  It moves fewer bytes than the lean segment probe only when nearly every
-    // 128-row tile matches in full, so it follows the match fraction of the last partitioned call whose count the host read
-    // (the first call takes it); a mispredicted call is slower, never wrong.  Dense input and a fresh batch only: the
-    // segment layout starts at the allocation.
-    const bool inplace = P && !in_seg && rb.rows == 0 && fo.n_key_dst >= 1 &&
-                         (tune.inplace >= 0 ? tune.inplace != 0 : j->seg_match >= kInplaceMinMatch);
-    if (inplace) C = inplace_seg_cap(j, P, n_main, C);
-    TG_TRY(ensure_result(j, rb, inplace ? std::max<int64_t>(n, (int64_t)P * C) : rb.rows + n, rb.rows > 0, rb.rows));
-    for (int c = 0; c < j->n_out; c++) { oc.data[c] = kernel_out(j, rb, c) + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
-    build_fast_out(j, oc, pview, fo);
-    unsigned long long* cur = j->out_cursor.as<unsigned long long>();
-    TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
-    if (n > 0) {
-      if (P) {
-        const int nc = 1 + fo.n_pcols;
-        if (!inplace) {
-          for (int c = 0; c < nc; c++) {
-            if (!j->part_cols[c]) j->part_cols[c].reset(new DevBuf());
-            TG_TRY(j->part_cols[c]->ensure(j->device, (size_t)P * C * 8 + 64));
-          }
-        }
-        TG_TRY(j->part_scratch.ensure(j->device, (size_t)3 * TG_MAX_SLICES * 8 + 64));
-        unsigned long long* cursors = j->part_scratch.as<unsigned long long>();      // fill count per segment
-        long long* bases = reinterpret_cast<long long*>(cursors + TG_MAX_SLICES);   // first row of each segment
-        unsigned long long* flag = cursors + 2 * TG_MAX_SLICES;                      // overflow
-        PartDst d{};
-        d.nparts = P; d.ncols = nc;
-        d.src[0] = pkey;
-        for (int c = 0; c < fo.n_pcols; c++) d.src[1 + c] = fo.psrc[c];
-        for (int c = 0; c < nc; c++)
-          for (int q = 0; q < P; q++) d.dst[q][c] = inplace ? (c == 0 ? (void*)fo.key_dst[0] : (void*)fo.pdst[c - 1]) : j->part_cols[c]->p;
-        k_segment_bases<<<1, 32, 0, j->stream>>>(cursors, bases, flag, P, C);
-        d.dst_base = bases; d.capacity = C; d.overflow = flag;
-        if (in_seg) { d.in_cnt = in_seg->cnt; d.in_cap = in_seg->cap; d.in_tiles_per_seg = (uint32_t)(in_seg->cap / PTILE); }
-        TG_TRY(launch_partition_scatter<true>(j->device, j->stream, reinterpret_cast<const long long*>(pkey), nullptr, n_main, d, cursors,
-                                              &j->stats.kernel_launches, 0, &j->stats.paths));
-        const SegSpec seg{cursors, (uint32_t)(C / 128), 0, C, flag};
-        if (inplace) {
-          // probe in place, then make the output dense: the rows at or beyond R = *cur fill the holes below R
-          const int64_t ntiles = (int64_t)P * C / 128;
-          TG_TRY(j->tile_cnt.ensure(j->device, (size_t)ntiles * 4 + 16));
-          TG_TRY(j->tmp_cnt.ensure(j->device, (size_t)(2 * ntiles + 1) * 4));
-          j->stats.paths |= TG_JOIN_PATH_PROBE_SEG;
-          TG_TRY(dispatch_shape<LaunchInplace>(fo, j, (int64_t)P * C, fo, cur, tune, seg, j->tile_cnt.as<uint32_t>()));
-          k_inplace_holes<<<grid_size(j->nsm, ntiles, 256, 4), 256, 0, j->stream>>>(j->tile_cnt.as<uint32_t>(), ntiles, cur, flag, j->tmp_cnt.as<uint32_t>());
-          int64_t nblocks = 0;
-          TG_TRY(enqueue_scan(j, 2 * ntiles, &nblocks));
-          k_inplace_fill<<<j->nsm * 8, 256, 0, j->stream>>>(j->tile_cnt.as<uint32_t>(), ntiles, j->tmp_off.as<unsigned long long>(), cur, flag, fo);
-          j->stats.kernel_launches += 3;
-        } else {
-          FastOut pf = fo;
-          for (int c = 0; c < fo.n_pcols; c++) pf.psrc[c] = j->part_cols[1 + c]->as<unsigned long long>();
-          // the 128-bit stores of the segment kernel need 16-byte aligned output columns: every caller passes a fresh
-          // batch (rb.rows == 0), so the columns start at the allocation
-          TG_TRY(launch_probe_seg(j, j->part_cols[0]->as<int64_t>(), (int64_t)P * C, pf, cur, tune, seg));
-          j->stats.kernel_launches++;
-        }
-        // gated fallback: probes the ORIGINAL input only after an overflow; the < PTILE-row tail the scatter left behind
-        // (dense input only) rides on the same launch — it is probed whatever the flag says, and appended at R
-        if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n_main, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 1, in_seg->cap, flag, 0}));
-        else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{nullptr, 0, 1, 0, flag, n_main < n ? n_main : 0}));
-        j->stats.kernel_launches += 2;
       } else {
-        if (in_seg) TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune, SegSpec{in_seg->cnt, in_seg->tiles_per_seg, 0, in_seg->cap, nullptr}));
-        else TG_TRY(launch_probe_warp(j, pkey, n, fo, cur, tune));
-        j->stats.kernel_launches++;
+        return launch_resident<k_probe_inner_u1_seg_inplace<npc, nkd, nmd>>(j, "k_probe_inner_u1_seg_inplace", fo, (rows / 128 + 7) / 8, tune,
+                                                                            rows, j->tv, fo, cur, seg, tile_cnt);
       }
-    }
-    TG_TRY(gather_cells(j, rb, &pcells, cur));   // after the hole fill and the gated fallback: *cur rows from row 0
-    if (sync_count) {
-      unsigned long long got = 0, part[2 * TG_MAX_SLICES + 1];   // fill counts | segment bases | overflow flag
-      const bool learn = P && !in_seg;
-      if (learn) TG_CUDA(cudaMemcpyAsync(part, j->part_scratch.p, sizeof(part), cudaMemcpyDeviceToHost, j->stream));
-      TG_CUDA(cudaMemcpyAsync(&got, cur, 8, cudaMemcpyDeviceToHost, j->stream));
-      TG_CUDA(cudaStreamSynchronize(j->stream));
-      rb.rows += (int64_t)got;
-      j->stats.output_rows += (int64_t)got;
-      if (P && n > 0) j->seg_match = (double)got / (double)n;
-      if (learn) {
-        j->seg_parts = part[2 * TG_MAX_SLICES] ? 0 : P;
-        j->seg_rows = n_main;
-        j->seg_fill_max = (int64_t)*std::max_element(part, part + P);
-      }
-    }
+    }));
+    k_inplace_holes<<<grid_size(j->nsm, ntiles, 256, 4), 256, 0, j->stream>>>(tile_cnt, ntiles, cur, seg.gate, j->tmp_cnt.as<uint32_t>());
+    int64_t nblocks = 0;
+    TG_TRY(enqueue_scan(j, 2 * ntiles, &nblocks));
+    k_inplace_fill<<<j->nsm * 8, 256, 0, j->stream>>>(tile_cnt, ntiles, j->tmp_off.as<unsigned long long>(), cur, seg.gate, fo);
+    j->stats.kernel_launches += 3;
     return TG_OK;
   }
-  // single-pass path: inner join on unique build keys with filters / several payload columns (k_probe_inner_uq)
-  if (uq_path_ok(j, pview)) {
-    TG_TRY(ensure_result(j, rb, rb.rows + n, rb.rows > 0, rb.rows));
-    for (int c = 0; c < j->n_out; c++) { oc.data[c] = kernel_out(j, rb, c) + (size_t)rb.rows * 8; oc.valid[c] = nullptr; if (rb.bitmaps[c]->p) rb.bitmaps[c]->release(); }
-    unsigned long long* cur = j->out_cursor.as<unsigned long long>();
-    TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
-    if (n > 0) {
-      int64_t tiles = (n + 256 * UQ_R - 1) / (256 * UQ_R);
-      int grid = (int)std::min<int64_t>(tiles, (int64_t)j->nsm * 8);
-      k_probe_inner_uq<<<grid, 256, 0, j->stream>>>(ks, pview, p.filter, n, j->tv, oc, cur);
-      j->stats.kernel_launches++;
-      j->stats.paths |= TG_JOIN_PATH_PROBE_UQ;
-    }
-    TG_TRY(gather_cells(j, rb, &pcells, cur));
-    // the output row count decides rb.rows (and the next append position): always needed on the host
-    unsigned long long got = 0;
-    TG_CUDA(cudaMemcpyAsync(&got, cur, 8, cudaMemcpyDeviceToHost, j->stream));
-    TG_CUDA(cudaStreamSynchronize(j->stream));
-    TG_CUDA(cudaGetLastError());
-    rb.rows += (int64_t)got;
-    j->stats.output_rows += (int64_t)got;
-    return TG_OK;
+  FastOut pf = fo;
+  for (int c = 0; c < fo.n_pcols; c++) pf.psrc[c] = j->part_cols[1 + c]->as<unsigned long long>();
+  // the 128-bit stores of the segment kernel need 16-byte aligned output columns: every caller passes a fresh
+  // batch (rb.rows == 0), so the columns start at the allocation
+  const int64_t* pkey = j->part_cols[0]->as<int64_t>();
+  TG_TRY(dispatch_shape(pf, [&](auto npc, auto nkd, auto nmd) {
+    return launch_resident<k_probe_inner_u1_seg_lean<npc, nkd, nmd>>(j, "k_probe_inner_u1_seg_lean", pf, (rows / 128 + 7) / 8, tune,
+                                                                     pkey, rows, j->tv, pf, cur, seg);
+  }));
+  j->stats.kernel_launches++;
+  return TG_OK;
+}
+
+// the warp kernel over the caller's input (n rows, segmented as in_seg when given).  gate != nullptr: it runs only when
+// *gate is set (the partition pass overflowed a segment), except that dense rows from ungated_from on are probed either way
+static int probe_direct(JoinImpl* j, const int64_t* pkey, int64_t n, const FastOut& fo, unsigned long long* cur, const ProbeTuning& tune,
+                        const SegSpec* in_seg, const unsigned long long* gate, int64_t ungated_from) {
+  const SegSpec seg = in_seg ? SegSpec{in_seg->cnt, in_seg->tiles_per_seg, gate != nullptr, in_seg->cap, gate, 0}
+                             : SegSpec{nullptr, 0, gate != nullptr, 0, gate, ungated_from};
+  constexpr int R = 4;
+  const int64_t tiles = (n + 32 * R - 1) / (32 * R);
+  j->stats.paths |= TG_JOIN_PATH_PROBE_DIRECT;
+  TG_TRY(dispatch_shape(fo, [&](auto npc, auto nkd, auto nmd) {
+    return launch_resident<k_probe_inner_u1_w<R, npc, nkd, nmd>>(j, "k_probe_inner_u1_w", fo, (tiles + 7) / 8, tune, pkey, n, j->tv, fo, cur, seg);
+  }));
+  j->stats.kernel_launches++;
+  return TG_OK;
+}
+
+static int probe_fused(JoinImpl* j, const DevCols& pcells, const DevCols& pview, const KeySpec& ks, int64_t n, ResultBatch& rb,
+                       bool sync_count, const SegSpec* in_seg, OutCols& oc, FastOut& fo) {
+  const ProbeTuning& tune = probe_tuning();
+  const int64_t* pkey = reinterpret_cast<const int64_t*>(ks.data);
+  const FusedPlan fp = fused_plan(j, rb, pkey, n, fo, tune, in_seg != nullptr);
+  TG_TRY(ensure_result(j, rb, fp.inplace ? std::max<int64_t>(n, (int64_t)fp.P * fp.C) : rb.rows + n, rb.rows > 0, rb.rows));
+  bind_fast_outputs(j, rb, oc);
+  build_fast_out(j, oc, pview, fo);
+  unsigned long long* cur = j->out_cursor.as<unsigned long long>();
+  TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
+  if (fp.P) {
+    SegSpec seg;
+    TG_TRY(scatter_segments(j, fp, pkey, fo, in_seg, seg));
+    TG_TRY(probe_segments(j, fp, fo, cur, tune, seg));
+    // gated fallback: probes the ORIGINAL input only after an overflow; the < ptile-row tail the scatter left behind
+    // (dense input only) rides on the same launch — it is probed whatever the flag says, and appended at R
+    TG_TRY(probe_direct(j, pkey, in_seg ? fp.n_main : n, fo, cur, tune, in_seg, seg.gate, fp.n_main < n ? fp.n_main : 0));
+  } else if (n > 0) {
+    TG_TRY(probe_direct(j, pkey, n, fo, cur, tune, in_seg, nullptr, 0));
   }
-  // general path, in sub-batches
+  TG_TRY(gather_cells(j, rb, &pcells, cur));   // after the hole fill and the gated fallback: *cur rows from row 0
+  if (!sync_count) return TG_OK;
+  unsigned long long got = 0, part[2 * TG_MAX_SLICES + 1];   // fill counts | segment bases | overflow flag
+  const bool learn = fp.P && !in_seg;
+  if (learn) TG_CUDA(cudaMemcpyAsync(part, j->part_scratch.p, sizeof(part), cudaMemcpyDeviceToHost, j->stream));
+  TG_TRY(read_cursor(j, rb, cur, got));
+  if (fp.P) j->seg_match = (double)got / (double)n;
+  if (learn) {
+    j->seg_parts = part[2 * TG_MAX_SLICES] ? 0 : fp.P;
+    j->seg_rows = fp.n_main;
+    j->seg_fill_max = (int64_t)*std::max_element(part, part + fp.P);
+  }
+  return TG_OK;
+}
+
+// single-pass path: inner join on unique build keys with filters / several payload columns (k_probe_inner_uq)
+static int probe_uq(JoinImpl* j, const DevCols& pcells, const DevCols& pview, const KeySpec& ks, int64_t n, ResultBatch& rb, OutCols& oc) {
+  TG_TRY(ensure_result(j, rb, rb.rows + n, rb.rows > 0, rb.rows));
+  bind_fast_outputs(j, rb, oc);
+  unsigned long long* cur = j->out_cursor.as<unsigned long long>();
+  TG_CUDA(cudaMemsetAsync(cur, 0, 8, j->stream));
+  if (n > 0) {
+    int64_t tiles = (n + 256 * UQ_R - 1) / (256 * UQ_R);
+    int grid = (int)std::min<int64_t>(tiles, (int64_t)j->nsm * 8);
+    k_probe_inner_uq<<<grid, 256, 0, j->stream>>>(ks, pview, j->probe.filter, n, j->tv, oc, cur);
+    j->stats.kernel_launches++;
+    j->stats.paths |= TG_JOIN_PATH_PROBE_UQ;
+  }
+  TG_TRY(gather_cells(j, rb, &pcells, cur));
+  // the output row count decides rb.rows (and the next append position): always needed on the host
+  unsigned long long got = 0;
+  return read_cursor(j, rb, cur, got);
+}
+
+// general path (any join type, NULLs, filters, duplicates): count → scan → write, in sub-batches
+static int probe_general(JoinImpl* j, const DevCols& pcells, const DevCols& pview, const KeySpec& ks, int64_t n, ResultBatch& rb, OutCols& oc) {
+  const Side& p = j->probe;
   std::vector<char> nullable;
   out_nullable(j, pview, nullable);
-  if ((int)j->tmp_valid.size() != j->n_out) { j->tmp_valid.clear(); for (int i = 0; i < j->n_out; i++) j->tmp_valid.emplace_back(new DevBuf()); }
-  int64_t out_start = rb.rows;
+  ensure_tmp_valid(j);
   // valid bytes are produced for the whole call, so size them after counting all sub-batches: run count+scan
   // per sub-batch, remembering totals, then write.  Sub-batching keeps the temporaries bounded.
-  for (int64_t lo = 0; lo < n || (lo == 0 && n == 0); lo += kGeneralBatchRows) {
+  for (int64_t lo = 0; lo < n; lo += kGeneralBatchRows) {
     int64_t m = std::min<int64_t>(kGeneralBatchRows, n - lo);
-    if (m <= 0) break;
     DevCols sub = pview;
     if (lo) {
       if (lo % 8) return fail(TG_ERR_CUDA, "internal: sub-batch offset not byte aligned");
@@ -1144,8 +1136,6 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
     TG_TRY(scan_counts(j, m, &total));
     if (total) {
       TG_TRY(ensure_result(j, rb, rb.rows + (int64_t)total, true, rb.rows));
-      OutCols oc{};
-      fill_outspec_probe(j, oc);
       for (int c = 0; c < j->n_out; c++) {
         oc.data[c] = kernel_out(j, rb, c);
         oc.valid[c] = nullptr;
@@ -1162,13 +1152,37 @@ static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBat
       j->stats.output_rows += (int64_t)total;
     }
   }
-  (void)out_start;
   if ((int)rb.cols.size() != j->n_out) TG_TRY(ensure_result(j, rb, 8, false, 0));
   TG_TRY(finish_bitmaps(j, rb, nullable));
   TG_TRY(gather_cells(j, rb, &pcells, nullptr));
   TG_CUDA(cudaStreamSynchronize(j->stream));
   TG_CUDA(cudaGetLastError());
   return TG_OK;
+}
+
+// probe `n` device-resident rows; results are appended to rb (rb.rows advanced)
+static int probe_device(JoinImpl* j, const DevCols& pcells, int64_t n, ResultBatch& rb, bool sync_count, const SegSpec* in_seg = nullptr) {
+  const Side& p = j->probe;
+  DevCols pview = pcells;
+  TG_TRY(kernel_view(j, p, pview, n));
+  j->stats.probe_rows += n;
+  KeySpec ks = j->probe_key;
+  if (j->multi_key) {
+    if (in_seg) return fail(TG_ERR_UNSUPPORTED, "segmented device chunks: joins on several key columns take the general path");
+    TG_TRY(composite_key(j, p, pview, n, j->pkey_syn, j->pkey_syn_nn));
+    ks.data = j->pkey_syn.p; ks.nulls = j->pkey_syn_nn.as<uint8_t>();
+  } else { ks.data = pview.data[p.key_col]; ks.nulls = pview.nulls[p.key_col]; }
+  TG_TRY(j->out_cursor.ensure(j->device, 64));
+  OutCols oc{};
+  fill_outspec_probe(j, oc);
+  FastOut fo{};
+  // the output shape decides the path before any output is allocated: the fused warp kernels, else the single-pass
+  // unique-key kernel, else the general path.  build_fast_out runs again once the output pointers are known.
+  const bool fast = fast_path_ok(j, pview) && build_fast_out(j, oc, pview, fo);
+  if (in_seg && !fast) return fail(TG_ERR_UNSUPPORTED, "segmented device chunks are only accepted by the fused fast path (unique build keys, <= 1 payload, no filters, an output shape the warp kernels cover)");
+  if (fast) return probe_fused(j, pcells, pview, ks, n, rb, sync_count, in_seg, oc, fo);
+  if (uq_path_ok(j, pview)) return probe_uq(j, pcells, pview, ks, n, rb, oc);
+  return probe_general(j, pcells, pview, ks, n, rb, oc);
 }
 
 // ScanRowTable after the probe side is exhausted (hash_join_v2.go:877)
@@ -1187,7 +1201,7 @@ static int scan_build_side(JoinImpl* j, ResultBatch& rb) {
   bool probe_is_left = j->build_is_right;
   OutCols oc{};
   oc.n = j->n_out;
-  if ((int)j->tmp_valid.size() != j->n_out) { j->tmp_valid.clear(); for (int i = 0; i < j->n_out; i++) j->tmp_valid.emplace_back(new DevBuf()); }
+  ensure_tmp_valid(j);
   TG_TRY(ensure_result(j, rb, rb.rows + (int64_t)total, false, 0));
   for (int o = 0; o < j->n_out; o++) {
     bool from_left = o < j->n_lused;

@@ -377,6 +377,45 @@ struct FastOut {
   unsigned long long* meta_dst[TG_FAST_MAX_METADST]; // output that carries the build payload
 };
 
+// Warp-tile output stores at the rows the warp reserved from wbase on.  Paired: the whole tile matched and wbase is even;
+// rows 2g, 2g+1 of a lane are adjacent input rows, so the input order is kept and a lane writes 16 bytes per column (half
+// the store instructions of the compacting store).
+template <int R, int NPC, int NKD, int NMD>
+__device__ __forceinline__ void store_tile_paired(unsigned long long wbase, const int64_t (&k)[R], const unsigned long long (&meta)[R],
+                                                  const unsigned long long (&pv)[R][NPC > 0 ? NPC : 1], const FastOut& out, int lane) {
+#pragma unroll
+  for (int g = 0; g < R / 2; g++) {
+    const unsigned long long o = wbase + (unsigned long long)(g * 64 + 2 * lane);
+    const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
+#pragma unroll
+    for (int d = 0; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
+#pragma unroll
+    for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
+#pragma unroll
+    for (int c = 0; c < NPC; c++) __stcs(reinterpret_cast<ulonglong2*>(out.pdst[c] + o), make_ulonglong2(pv[2 * g][c], pv[2 * g + 1][c]));
+  }
+}
+
+// compacting: row j of a lane goes to its rank among the warp's matched rows j (bal[j]), behind the matched rows before j
+template <int R, int NPC, int NKD, int NMD>
+__device__ __forceinline__ void store_tile_compact(unsigned long long wbase, const int64_t (&k)[R], const unsigned long long (&meta)[R],
+                                                   const unsigned long long (&pv)[R][NPC > 0 ? NPC : 1], const unsigned (&bal)[R],
+                                                   const FastOut& out, int lane) {
+#pragma unroll
+  for (int j = 0; j < R; j++) {
+    if ((bal[j] >> lane) & 1u) {
+      const unsigned long long o = wbase + __popc(bal[j] & ((1u << lane) - 1));
+#pragma unroll
+      for (int d = 0; d < NKD; d++) __stcs(out.key_dst[d] + o, (unsigned long long)k[j]);
+#pragma unroll
+      for (int d = 0; d < NMD; d++) __stcs(out.meta_dst[d] + o, meta[j]);
+#pragma unroll
+      for (int c = 0; c < NPC; c++) __stcs(out.pdst[c] + o, pv[j][c]);
+    }
+    wbase += __popc(bal[j]);
+  }
+}
+
 // R rows per lane, keys and payloads already in registers: gather, resolve, compact, store.
 // `in[j]` = row j of this lane exists (tail tiles).
 template <int R, int NPC, int NKD, int NMD, bool PAIRED = false>
@@ -388,6 +427,7 @@ __device__ __forceinline__ void probe_rows_u1(const int64_t (&k)[R], const unsig
   // (the table holds one spare slot behind it); only its first slot counts.
 #pragma unroll
   for (int j = 0; j < R; j++) load_pair(t.slots + sl0[j], v[j], w[j]);
+  unsigned long long meta[R];
   unsigned bal[R];
   uint32_t total = 0;
 #pragma unroll
@@ -398,41 +438,15 @@ __device__ __forceinline__ void probe_rows_u1(const int64_t (&k)[R], const unsig
     else if (w[j].key == k[j]) { v[j] = w[j]; m = true; }
     else if (v[j].key == kEmptyKey || w[j].key == kEmptyKey) m = false;
     else m = probe_run(t.slots, t.nslots, k[j], sl0[j] + 2, v[j].meta);   // the home slots hold other keys
+    meta[j] = v[j].meta;
     bal[j] = __ballot_sync(0xffffffffu, m);
     total += __popc(bal[j]);
   }
   unsigned long long wbase = 0;
   if (lane == 0 && total) wbase = atomicAdd(out_cursor, (unsigned long long)total);
   wbase = __shfl_sync(0xffffffffu, wbase, 0);
-  if (PAIRED && total == 32u * R && (wbase & 1ull) == 0) {
-    // rows 2g, 2g+1 of a lane are adjacent input rows and the whole warp tile matched: keep the input order and write
-    // 16 bytes per lane and column (half the store instructions of the compacting path below)
-#pragma unroll
-    for (int g = 0; g < R / 2; g++) {
-      const unsigned long long o = wbase + (unsigned long long)(g * 64 + 2 * lane);
-      const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
-#pragma unroll
-      for (int d = 0; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
-#pragma unroll
-      for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(v[2 * g].meta, v[2 * g + 1].meta));
-#pragma unroll
-      for (int c = 0; c < NPC; c++) __stcs(reinterpret_cast<ulonglong2*>(out.pdst[c] + o), make_ulonglong2(pv[2 * g][c], pv[2 * g + 1][c]));
-    }
-    return;
-  }
-#pragma unroll
-  for (int j = 0; j < R; j++) {
-    if ((bal[j] >> lane) & 1u) {
-      const unsigned long long o = wbase + __popc(bal[j] & ((1u << lane) - 1));
-#pragma unroll
-      for (int d = 0; d < NKD; d++) __stcs(out.key_dst[d] + o, (unsigned long long)k[j]);
-#pragma unroll
-      for (int d = 0; d < NMD; d++) __stcs(out.meta_dst[d] + o, v[j].meta);
-#pragma unroll
-      for (int c = 0; c < NPC; c++) __stcs(out.pdst[c] + o, pv[j][c]);
-    }
-    wbase += __popc(bal[j]);
-  }
+  if (PAIRED && total == 32u * R && (wbase & 1ull) == 0) store_tile_paired<R, NPC, NKD, NMD>(wbase, k, meta, pv, out, lane);
+  else store_tile_compact<R, NPC, NKD, NMD>(wbase, k, meta, pv, bal, out, lane);
 }
 
 // Optional input shape of the warp kernel: the probe rows regrouped by L2 partition into fixed-capacity segments
@@ -450,6 +464,19 @@ struct SegSpec {
                                      // leaves behind rides on the gated fallback launch instead of costing a launch of its own
 };
 
+// true when the launch's gate says "do not run"
+__device__ __forceinline__ bool gated_off(const SegSpec& seg) {
+  return seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0));
+}
+
+// one past the last row of segment p: p·cap + min(cnt[p], cap).  p keeps the caller's integer type, and with it the
+// caller's address arithmetic.
+template <typename I>
+__device__ __forceinline__ int64_t seg_end(const SegSpec& seg, I p) {
+  const unsigned long long c = seg.cnt[p];
+  return (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+}
+
 // warp-autonomous: no shared memory, no block barrier; each warp owns tiles of 32×R rows.
 // Launch with exactly the resident CTA count (occupancy × SMs): every extra wave of a persistent grid-stride kernel
 // re-sweeps all partitions of a partition-ordered input and re-fetches the table slices.
@@ -459,7 +486,7 @@ k_probe_inner_u1_w(const int64_t* __restrict__ pkey, int64_t n, TableView t, Fas
                    unsigned long long* __restrict__ out_cursor, SegSpec seg) {
   const int64_t tile_rows = 32 * R;
   int64_t first_tile = 0;
-  if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) {
+  if (gated_off(seg)) {
     if (seg.ungated_from <= 0 || seg.cnt) return;
     first_tile = seg.ungated_from / tile_rows;
   }
@@ -471,9 +498,7 @@ k_probe_inner_u1_w(const int64_t* __restrict__ pkey, int64_t n, TableView t, Fas
     const int64_t base = tile * tile_rows;
     int64_t limit = n;
     if (seg.cnt) {
-      const uint32_t p = (uint32_t)tile / seg.tiles_per_seg;
-      const unsigned long long c = seg.cnt[p];
-      limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+      limit = seg_end(seg, (uint32_t)tile / seg.tiles_per_seg);
       if (base >= limit) continue;
     }
     int64_t k[R];
@@ -504,6 +529,29 @@ k_probe_inner_u1_w(const int64_t* __restrict__ pkey, int64_t n, TableView t, Fas
 // masked.  A full tile takes a lean path — no per-row `in` flags, no slot array, sentinel-valued keys detected once per
 // tile (then the tile takes the generic path).  3 CTAs per SM (80 registers): launch exactly the resident CTA count.
 // ---------------------------------------------------------------------------------------------
+
+// the keys of the 128-row tile at `base`: lane owns rows 2·lane, 2·lane+1 of each 64-row group, one 128-bit load per group
+__device__ __forceinline__ void load_tile_keys(const int64_t* __restrict__ pkey, int64_t base, int lane, int64_t (&k)[4]) {
+#pragma unroll
+  for (int g = 0; g < 2; g++) {
+    const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + base + g * 64 + 2 * lane));
+    k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
+  }
+}
+
+// the same for a tile that may end early: in[j] = row j lies below `limit`; a row past it gets the sentinel key
+__device__ __forceinline__ void load_tile_keys(const int64_t* __restrict__ pkey, int64_t base, int64_t limit, int lane, int64_t (&k)[4],
+                                               bool (&in)[4]) {
+#pragma unroll
+  for (int g = 0; g < 2; g++) {
+    const int64_t i = base + g * 64 + 2 * lane;
+    const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + i));
+    in[2 * g] = i < limit; in[2 * g + 1] = i + 1 < limit;
+    k[2 * g] = in[2 * g] ? (int64_t)kk.x : kEmptyKey;
+    k[2 * g + 1] = in[2 * g + 1] ? (int64_t)kk.y : kEmptyKey;
+  }
+}
+
 template <int NPC, int NKD, int NMD>
 __device__ __forceinline__ void probe_tile_generic(const int64_t* __restrict__ pkey, int64_t base, int64_t limit, const TableView& t,
                                                    const FastOut& out, unsigned long long* __restrict__ out_cursor, int lane) {
@@ -512,14 +560,7 @@ __device__ __forceinline__ void probe_tile_generic(const int64_t* __restrict__ p
   unsigned long long pv[R][NPC > 0 ? NPC : 1];
   unsigned long long sl[R];
   bool in[R];
-#pragma unroll
-  for (int g = 0; g < R / 2; g++) {
-    const int64_t i = base + g * 64 + 2 * lane;
-    const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + i));
-    in[2 * g] = i < limit; in[2 * g + 1] = i + 1 < limit;
-    k[2 * g] = in[2 * g] ? (int64_t)kk.x : kEmptyKey;
-    k[2 * g + 1] = in[2 * g + 1] ? (int64_t)kk.y : kEmptyKey;
-  }
+  load_tile_keys(pkey, base, limit, lane, k, in);
 #pragma unroll
   for (int g = 0; g < R / 2; g++) {
     const int64_t i = base + g * 64 + 2 * lane;
@@ -534,12 +575,53 @@ __device__ __forceinline__ void probe_tile_generic(const int64_t* __restrict__ p
   probe_rows_u1<R, NPC, NKD, NMD, true>(k, pv, sl, in, t, out, out_cursor, lane);
 }
 
+// A full tile without the sentinel key: gather each row's home pair, then continue the linear probe of every row whose home
+// pair holds two other keys, one aligned pair per row and step.  The rows of a lane walk their runs side by side, so a step
+// costs one L2 round trip however many rows are still walking (dense tables: one of the 128 rows of a tile nearly always
+// has a run).  Bit j of the result: row j matched, its build payload in meta[j].
+__device__ __forceinline__ unsigned gather_walk(const int64_t (&k)[4], const TableView& t, unsigned long long (&meta)[4]) {
+  constexpr int R = 4;
+  Slot v[R], w[R];
+#pragma unroll
+  for (int j = 0; j < R; j++) load_pair(t.slots + home_slot(hash64((uint64_t)k[j]), t.nslots), v[j], w[j]);
+  unsigned run = 0, hit = 0;   // bit j: row j's home pair holds two other keys / row j matched
+#pragma unroll
+  for (int j = 0; j < R; j++) {
+    meta[j] = 0;
+    if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; }
+    else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; }
+    else if (v[j].key != kEmptyKey && w[j].key != kEmptyKey) run |= 1u << j;
+  }
+  if (run) {
+    uint32_t sl[R];
+#pragma unroll
+    for (int j = 0; j < R; j++) {
+      const unsigned long long s = home_slot(hash64((uint64_t)k[j]), t.nslots) + 2;
+      sl[j] = s == t.nslots ? 0u : (uint32_t)s;
+    }
+    do {
+#pragma unroll
+      for (int j = 0; j < R; j++) if ((run >> j) & 1u) load_pair(t.slots + sl[j], v[j], w[j]);
+#pragma unroll
+      for (int j = 0; j < R; j++) {
+        if (!((run >> j) & 1u)) continue;
+        if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; run &= ~(1u << j); }
+        else if (v[j].key == kEmptyKey) run &= ~(1u << j);
+        else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; run &= ~(1u << j); }
+        else if (w[j].key == kEmptyKey) run &= ~(1u << j);
+        else { sl[j] += 2; if (sl[j] == t.nslots) sl[j] = 0; }
+      }
+    } while (run);
+  }
+  return hit;
+}
+
 template <int NPC, int NKD, int NMD>
 __global__ void __launch_bounds__(256, 3)
 k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView t, FastOut out,
                           unsigned long long* __restrict__ out_cursor, SegSpec seg) {
   constexpr int R = 4, G = 2, NP = NPC > 0 ? NPC : 1;
-  if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) return;
+  if (gated_off(seg)) return;
   const int lane = threadIdx.x & 31;
   const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
   const int64_t warp_id = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -551,11 +633,10 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
   for (int64_t tile = warp_id; tile < ntiles; tile += warps_total) {
     int64_t k[R];
     unsigned long long pv[R][NP];
+    load_tile_keys(pkey, tile * 128, lane, k);
 #pragma unroll
     for (int g = 0; g < G; g++) {
       const int64_t i = tile * 128 + g * 64 + 2 * lane;
-      const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + i));
-      k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
 #pragma unroll
       for (int c = 0; c < NPC; c++) {
         const ulonglong2 pp = __ldcs(reinterpret_cast<const ulonglong2*>(out.psrc[c] + i));
@@ -563,51 +644,15 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
       }
     }
     const int64_t base = tile * 128;
-    const uint32_t p = (uint32_t)tile / seg.tiles_per_seg;
-    const unsigned long long c = seg.cnt[p];
-    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+    const int64_t limit = seg_end(seg, (uint32_t)tile / seg.tiles_per_seg);
     if (limit - base < 128) continue;                       // empty or partial tile: pass 2
     const bool sentinel = (k[0] == kEmptyKey) | (k[1] == kEmptyKey) | (k[2] == kEmptyKey) | (k[3] == kEmptyKey);
     if (__any_sync(0xffffffffu, sentinel)) {                // the key value used as the empty marker: generic path for this tile
       probe_tile_generic<NPC, NKD, NMD>(pkey, base, limit, t, out, out_cursor, lane);
       continue;
     }
-    Slot v[R], w[R];
-#pragma unroll
-    for (int j = 0; j < R; j++) load_pair(t.slots + home_slot(hash64((uint64_t)k[j]), t.nslots), v[j], w[j]);
     unsigned long long meta[R];
-    unsigned hit = 0, run = 0;   // bit j: row j matched / row j's home pair holds two other keys
-#pragma unroll
-    for (int j = 0; j < R; j++) {
-      meta[j] = 0;
-      if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; }
-      else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; }
-      else if (v[j].key != kEmptyKey && w[j].key != kEmptyKey) run |= 1u << j;
-    }
-    if (run) {
-      // continue the linear probe of every such row behind its home pair, one aligned pair per row and step: the rows of a
-      // lane walk their runs side by side, so a step costs one L2 round trip however many rows are still walking (dense
-      // tables: one of the 128 rows of a tile nearly always has a run)
-      uint32_t sl[R];
-#pragma unroll
-      for (int j = 0; j < R; j++) {
-        const unsigned long long s = home_slot(hash64((uint64_t)k[j]), t.nslots) + 2;
-        sl[j] = s == t.nslots ? 0u : (uint32_t)s;
-      }
-      do {
-#pragma unroll
-        for (int j = 0; j < R; j++) if ((run >> j) & 1u) load_pair(t.slots + sl[j], v[j], w[j]);
-#pragma unroll
-        for (int j = 0; j < R; j++) {
-          if (!((run >> j) & 1u)) continue;
-          if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; run &= ~(1u << j); }
-          else if (v[j].key == kEmptyKey) run &= ~(1u << j);
-          else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; run &= ~(1u << j); }
-          else if (w[j].key == kEmptyKey) run &= ~(1u << j);
-          else { sl[j] += 2; if (sl[j] == t.nslots) sl[j] = 0; }
-        }
-      } while (run);
-    }
+    const unsigned hit = gather_walk(k, t, meta);
     unsigned bal[R];
     uint32_t total = 0;
 #pragma unroll
@@ -618,33 +663,8 @@ k_probe_inner_u1_seg_lean(const int64_t* __restrict__ pkey, int64_t n, TableView
     unsigned long long wbase = 0;
     if (lane == 0 && total) wbase = atomicAdd(out_cursor, (unsigned long long)total);
     wbase = __shfl_sync(0xffffffffu, wbase, 0);
-    if (total == 128u && (wbase & 1ull) == 0) {
-#pragma unroll
-      for (int g = 0; g < G; g++) {
-        const unsigned long long o = wbase + (unsigned long long)(g * 64 + 2 * lane);
-        const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
-#pragma unroll
-        for (int d = 0; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
-#pragma unroll
-        for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
-#pragma unroll
-        for (int cc = 0; cc < NPC; cc++) __stcs(reinterpret_cast<ulonglong2*>(out.pdst[cc] + o), make_ulonglong2(pv[2 * g][cc], pv[2 * g + 1][cc]));
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < R; j++) {
-        if ((bal[j] >> lane) & 1u) {
-          const unsigned long long o = wbase + __popc(bal[j] & ((1u << lane) - 1));
-#pragma unroll
-          for (int d = 0; d < NKD; d++) __stcs(out.key_dst[d] + o, (unsigned long long)k[j]);
-#pragma unroll
-          for (int d = 0; d < NMD; d++) __stcs(out.meta_dst[d] + o, meta[j]);
-#pragma unroll
-          for (int cc = 0; cc < NPC; cc++) __stcs(out.pdst[cc] + o, pv[j][cc]);
-        }
-        wbase += __popc(bal[j]);
-      }
-    }
+    if (total == 128u && (wbase & 1ull) == 0) store_tile_paired<R, NPC, NKD, NMD>(wbase, k, meta, pv, out, lane);
+    else store_tile_compact<R, NPC, NKD, NMD>(wbase, k, meta, pv, bal, out, lane);
   }
   // pass 2: the partial tile of each segment
   const int64_t nseg = ntiles / seg.tiles_per_seg;
@@ -713,14 +733,7 @@ __device__ __forceinline__ uint32_t inplace_tile_generic(int64_t base, int64_t l
   int64_t k[R];
   unsigned long long pv[R][NPC > 0 ? NPC : 1], meta[R];
   bool in[R];
-#pragma unroll
-  for (int g = 0; g < R / 2; g++) {
-    const int64_t i = base + g * 64 + 2 * lane;
-    const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(out.key_dst[0] + i));
-    in[2 * g] = i < limit; in[2 * g + 1] = i + 1 < limit;
-    k[2 * g] = in[2 * g] ? (int64_t)kk.x : kEmptyKey;
-    k[2 * g + 1] = in[2 * g + 1] ? (int64_t)kk.y : kEmptyKey;
-  }
+  load_tile_keys(reinterpret_cast<const int64_t*>(out.key_dst[0]), base, limit, lane, k, in);
   inplace_load_pv<NPC>(base, out, pv, lane);
   unsigned bal[R];
   uint32_t total = 0;
@@ -743,13 +756,44 @@ __device__ __forceinline__ uint32_t inplace_tile_generic(int64_t base, int64_t l
   return total;
 }
 
+// The end of a full in-place tile whose rows are resolved (bit j of hit: row j matched, its build payload in meta[j]).  When
+// all 128 rows matched, the probe columns are already in place: only the extra key copies and the build payload are written.
+// Else the tile is compacted to its front.  Returns the rows the tile keeps.
+template <int NPC, int NKD, int NMD>
+__device__ __forceinline__ uint32_t inplace_finish(int64_t base, const int64_t (&k)[4], const unsigned long long (&meta)[4], unsigned hit,
+                                                   const FastOut& out, int lane) {
+  if (__all_sync(0xffffffffu, hit == 0xFu)) {
+#pragma unroll
+    for (int g = 0; g < 2; g++) {
+      const int64_t o = base + g * 64 + 2 * lane;
+      const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
+#pragma unroll
+      for (int d = 1; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
+#pragma unroll
+      for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
+    }
+    return 128;
+  }
+  unsigned long long pv[4][NPC > 0 ? NPC : 1];
+  inplace_load_pv<NPC>(base, out, pv, lane);
+  unsigned bal[4];
+  uint32_t m = 0;
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    bal[j] = __ballot_sync(0xffffffffu, (hit >> j) & 1u);
+    m += __popc(bal[j]);
+  }
+  inplace_store<NPC, NKD, NMD>(base, k, meta, pv, bal, out, lane);
+  return m;
+}
+
 template <int NPC, int NKD, int NMD>
 __global__ void __launch_bounds__(256, 3)
 k_probe_inner_u1_seg_inplace(int64_t n, TableView t, FastOut out, unsigned long long* __restrict__ out_cursor, SegSpec seg,
                              uint32_t* __restrict__ tile_cnt) {
   static_assert(NKD >= 1, "the probe key is read from the first key destination");
-  constexpr int R = 4, G = 2, NP = NPC > 0 ? NPC : 1;
-  if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) return;
+  constexpr int R = 4;
+  if (gated_off(seg)) return;
   const int lane = threadIdx.x & 31;
   const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
   const int64_t warp_id = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -758,78 +802,18 @@ k_probe_inner_u1_seg_inplace(int64_t n, TableView t, FastOut out, unsigned long 
   unsigned long long kept = 0;
   for (int64_t tile = warp_id; tile < ntiles; tile += warps_total) {
     const int64_t base = tile * 128;
-    const uint32_t p = (uint32_t)tile / seg.tiles_per_seg;
-    const unsigned long long c = seg.cnt[p];
-    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+    const int64_t limit = seg_end(seg, (uint32_t)tile / seg.tiles_per_seg);
     uint32_t m = 0;
     if (limit - base >= 128) {
       int64_t k[R];
-#pragma unroll
-      for (int g = 0; g < G; g++) {
-        const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + base + g * 64 + 2 * lane));
-        k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
-      }
+      load_tile_keys(pkey, base, lane, k);
       const bool sentinel = (k[0] == kEmptyKey) | (k[1] == kEmptyKey) | (k[2] == kEmptyKey) | (k[3] == kEmptyKey);
       if (__any_sync(0xffffffffu, sentinel)) {
         m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
       } else {
-        // gather and run walk exactly as k_probe_inner_u1_seg_lean
-        Slot v[R], w[R];
-#pragma unroll
-        for (int j = 0; j < R; j++) load_pair(t.slots + home_slot(hash64((uint64_t)k[j]), t.nslots), v[j], w[j]);
         unsigned long long meta[R];
-        unsigned hit = 0, run = 0;
-#pragma unroll
-        for (int j = 0; j < R; j++) {
-          meta[j] = 0;
-          if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; }
-          else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; }
-          else if (v[j].key != kEmptyKey && w[j].key != kEmptyKey) run |= 1u << j;
-        }
-        if (run) {
-          uint32_t sl[R];
-#pragma unroll
-          for (int j = 0; j < R; j++) {
-            const unsigned long long s = home_slot(hash64((uint64_t)k[j]), t.nslots) + 2;
-            sl[j] = s == t.nslots ? 0u : (uint32_t)s;
-          }
-          do {
-#pragma unroll
-            for (int j = 0; j < R; j++) if ((run >> j) & 1u) load_pair(t.slots + sl[j], v[j], w[j]);
-#pragma unroll
-            for (int j = 0; j < R; j++) {
-              if (!((run >> j) & 1u)) continue;
-              if (v[j].key == k[j]) { hit |= 1u << j; meta[j] = v[j].meta; run &= ~(1u << j); }
-              else if (v[j].key == kEmptyKey) run &= ~(1u << j);
-              else if (w[j].key == k[j]) { hit |= 1u << j; meta[j] = w[j].meta; run &= ~(1u << j); }
-              else if (w[j].key == kEmptyKey) run &= ~(1u << j);
-              else { sl[j] += 2; if (sl[j] == t.nslots) sl[j] = 0; }
-            }
-          } while (run);
-        }
-        if (__all_sync(0xffffffffu, hit == 0xFu)) {
-          // every row matched: the probe columns are already in place
-          m = 128;
-#pragma unroll
-          for (int g = 0; g < G; g++) {
-            const int64_t o = base + g * 64 + 2 * lane;
-            const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
-#pragma unroll
-            for (int d = 1; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
-#pragma unroll
-            for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
-          }
-        } else {
-          unsigned long long pv[R][NP];
-          inplace_load_pv<NPC>(base, out, pv, lane);
-          unsigned bal[R];
-#pragma unroll
-          for (int j = 0; j < R; j++) {
-            bal[j] = __ballot_sync(0xffffffffu, (hit >> j) & 1u);
-            m += __popc(bal[j]);
-          }
-          inplace_store<NPC, NKD, NMD>(base, k, meta, pv, bal, out, lane);
-        }
+        const unsigned hit = gather_walk(k, t, meta);
+        m = inplace_finish<NPC, NKD, NMD>(base, k, meta, hit, out, lane);
       }
     } else if (limit > base) {
       m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
@@ -956,10 +940,10 @@ __global__ void __launch_bounds__(kPidxThreads, 1)
 k_probe_inner_u1_seg_inplace_pidx(int64_t n, TableView t, SliceIndex ix, FastOut out, unsigned long long* __restrict__ out_cursor,
                                   SegSpec seg, uint32_t* __restrict__ tile_cnt) {
   static_assert(NKD >= 1, "the probe key is read from the first key destination");
-  constexpr int R = 4, G = 2, NP = NPC > 0 ? NPC : 1, NW = kPidxThreads / 32;
+  constexpr int R = 4, NW = kPidxThreads / 32;
   extern __shared__ __align__(16) uint8_t spil[];   // [nbuf][B] pilots, then nbuf "full" mbarriers
   __shared__ uint32_t s_done[2];                     // warps done with buffer b, summed over the sweep
-  if (seg.gate && ((*seg.gate != 0ull) != (seg.gate_want != 0))) return;
+  if (gated_off(seg)) return;
   const int lane = threadIdx.x & 31;
   const int64_t warps_total = (int64_t)gridDim.x * NW;
   const int64_t warp_id = (int64_t)blockIdx.x * NW + (threadIdx.x >> 5);
@@ -986,8 +970,7 @@ k_probe_inner_u1_seg_inplace_pidx(int64_t n, TableView t, SliceIndex ix, FastOut
     const uint32_t use = (uint32_t)(p / nbuf);   // how many slices buffer b held before this one
     mbar_wait(&full[b], use & 1u);
     const uint8_t* __restrict__ pil = spil + (size_t)b * ix.B;
-    const unsigned long long c = seg.cnt[p];
-    const int64_t limit = (int64_t)p * seg.cap + (int64_t)(c < (unsigned long long)seg.cap ? c : (unsigned long long)seg.cap);
+    const int64_t limit = seg_end(seg, p);
     const int64_t t0 = (int64_t)p * seg.tiles_per_seg, t1 = t0 + seg.tiles_per_seg;
     const int64_t r = t0 % warps_total;
     const Slot* __restrict__ islots = ix.slots + (size_t)p * ix.S;
@@ -996,11 +979,7 @@ k_probe_inner_u1_seg_inplace_pidx(int64_t n, TableView t, SliceIndex ix, FastOut
       uint32_t m = 0;
       if (limit - base >= 128) {
         int64_t k[R];
-#pragma unroll
-        for (int g = 0; g < G; g++) {
-          const ulonglong2 kk = __ldcs(reinterpret_cast<const ulonglong2*>(pkey + base + g * 64 + 2 * lane));
-          k[2 * g] = (int64_t)kk.x; k[2 * g + 1] = (int64_t)kk.y;
-        }
+        load_tile_keys(pkey, base, lane, k);
         uint32_t q[R];
         bool generic = false;
 #pragma unroll
@@ -1019,28 +998,7 @@ k_probe_inner_u1_seg_inplace_pidx(int64_t n, TableView t, SliceIndex ix, FastOut
             meta[j] = v.meta;
             if (v.key == k[j]) hit |= 1u << j;
           }
-          if (__all_sync(0xffffffffu, hit == 0xFu)) {
-            m = 128;
-#pragma unroll
-            for (int g = 0; g < G; g++) {
-              const int64_t o = base + g * 64 + 2 * lane;
-              const ulonglong2 kk = make_ulonglong2((unsigned long long)k[2 * g], (unsigned long long)k[2 * g + 1]);
-#pragma unroll
-              for (int d = 1; d < NKD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.key_dst[d] + o), kk);
-#pragma unroll
-              for (int d = 0; d < NMD; d++) __stcs(reinterpret_cast<ulonglong2*>(out.meta_dst[d] + o), make_ulonglong2(meta[2 * g], meta[2 * g + 1]));
-            }
-          } else {
-            unsigned long long pv[R][NP];
-            inplace_load_pv<NPC>(base, out, pv, lane);
-            unsigned bal[R];
-#pragma unroll
-            for (int j = 0; j < R; j++) {
-              bal[j] = __ballot_sync(0xffffffffu, (hit >> j) & 1u);
-              m += __popc(bal[j]);
-            }
-            inplace_store<NPC, NKD, NMD>(base, k, meta, pv, bal, out, lane);
-          }
+          m = inplace_finish<NPC, NKD, NMD>(base, k, meta, hit, out, lane);
         }
       } else if (limit > base) {
         m = inplace_tile_generic<NPC, NKD, NMD>(base, limit, t, out, lane);
