@@ -153,8 +153,9 @@ __device__ __forceinline__ unsigned long long dec_ext(const AggFuncDev& f, unsig
 // its group
 __device__ __forceinline__ uint32_t agg_home(long long k, unsigned long long nslots) { return slot32(hash64((unsigned long long)k), (uint32_t)nslots); }
 
-// probe-length limit of every find-or-insert into the group table or a DISTINCT set: an item whose probe sequence is
-// longer finds the table overfull and is deferred, and the host grows the table (grow_and_retry)
+// probe-length limit of every find-or-insert into the group table, a DISTINCT set or a string dictionary: an item whose
+// probe sequence is longer is deferred, and the host grows the table, or re-runs the item without the limit when the
+// table is far from full (grow_and_retry)
 constexpr uint32_t kAggMaxProbe = 48;
 
 // find-or-insert `k` in the global table starting at slot s with the slot's current content `cur` already loaded;
@@ -983,7 +984,7 @@ struct AggPlan {
 struct AggImpl : DeviceHandle, AggPlan {
   std::vector<std::unique_ptr<DevBuf>> dscaled;   // per DECIMAL argument column: its int64 value * 10^scale, pooled scratch
 
-  struct SetMem { DevBuf mem, mark; DistinctSet t{}; };
+  struct SetMem { DevBuf mem, mark; DistinctSet t{}; unsigned long long used = 0; };   // used: the pairs the set holds
   std::vector<std::unique_ptr<SetMem>> dsets;
   DevBuf dcounters;                     // k_agg_distinct_mark: [0] rows deferred [1] pairs inserted
   bool broken = false;                  // a push failed after a set was touched: every later push / finish fails
@@ -1423,26 +1424,45 @@ static int mark_range_deferred(AggImpl* a, int64_t lo, int64_t hi) {
   return TG_OK;
 }
 
-// Grow-and-retry, the protocol of every find-or-insert pass into the group table or a DISTINCT set.  launch(deferred,
-// only, nd) runs one round over the pass's `nitems` items (only == nullptr: all of them, else those whose bit is set),
-// sets in `deferred` the bit of every item that found no slot within kAggMaxProbe steps, and reads back their number
-// into nd; grow(nd) makes room for nd new entries.  The next round re-runs just the deferred items.  bits[0] and bits[1]
-// take turns as the bitmap a round writes and the one it reads; `resume`: the items of the first round are the ones
-// already marked in bits[0].
-template <class Launch, class Grow>
-static int grow_and_retry(AggImpl* a, DevBuf (&bits)[2], int64_t nitems, bool resume, const char* what, Launch launch, Grow grow) {
+// A round deferred nd items from a table of `slots` slots with `used` of them taken: true when the table stays at most a
+// quarter full once they join, so a probe ran long because the keys share a home, not because the table is full.  A
+// home depends only on the top 32 bits of a 64-bit hash, so keys that share those bits share a home at every size, and
+// growing would never shorten their run.  Uniform keys at a quarter load start a run long enough to defer an item with a
+// probability below 3e-14 per slot (a Chernoff bound, tests/agg_keys.py), so this does not change how uniform data grows;
+// at half load the same bound is 8e-5 per slot, which a table of millions of slots does reach.
+static bool long_run_not_full(unsigned long long used, unsigned long long nd, unsigned long long slots) {
+  return (used + nd) * 4 <= slots;
+}
+
+// Grow-and-retry, the protocol of every find-or-insert pass into the group table, a DISTINCT set or a string dictionary.
+// launch(deferred, only, max_probe, nd) runs one round over the pass's `nitems` items (only == nullptr: all of them, else
+// those whose bit is set), sets in `deferred` the bit of every item that found no slot within max_probe steps, and reads
+// back their number into nd.  fill(used, slots) reads how many slots the table has and how many are taken.
+// grow(nd, room) makes room for nd new entries; room: the table has it already (long_run_not_full), and grow only
+// extends what else the pass sizes by its entries (a dictionary's per-id arrays).  The next round re-runs just the
+// deferred items: with room, through an unbounded probe (max_probe = slots) on the same table — nothing is ever deleted
+// from it, so a walk past kAggMaxProbe steps still meets an existing key before any empty slot — else with kAggMaxProbe
+// on the grown table.  bits[0] and bits[1] take turns as the bitmap a round writes and the one it reads; `resume`: the
+// items of the first round are the ones already marked in bits[0].
+template <class Launch, class Fill, class Grow>
+static int grow_and_retry(AggImpl* a, DevBuf (&bits)[2], int64_t nitems, bool resume, const char* what, Launch launch, Fill fill, Grow grow) {
   const size_t bytes = (size_t)((nitems + 31) / 32) * 4;
   int cur = resume ? 1 : 0;
   const uint32_t* only = resume ? bits[0].as<uint32_t>() : nullptr;
+  uint32_t max_probe = kAggMaxProbe;
   for (int round = 0;; round++) {
     TG_TRY(bits[cur].ensure(a->device, bytes + 16));
     TG_CUDA(cudaMemsetAsync(bits[cur].p, 0, bytes, a->stream));
     unsigned long long nd = 0;
-    TG_TRY(launch(bits[cur].as<uint32_t>(), only, nd));
+    TG_TRY(launch(bits[cur].as<uint32_t>(), only, max_probe, nd));
     if (nd == 0) return TG_OK;
-    // x4 per round: 40 rounds are never reached
+    // x4 per growth, and an unbounded round only follows a bounded one: 40 rounds are never reached
     if (round == 39) return fail(TG_ERR_CUDA, std::string("internal: ") + what + " failed to converge");
-    TG_TRY(grow(nd));
+    unsigned long long used = 0, slots = 0;
+    if (max_probe == kAggMaxProbe) TG_TRY(fill(used, slots));
+    const bool room = max_probe == kAggMaxProbe && long_run_not_full(used, nd, slots);
+    TG_TRY(grow(nd, room));
+    max_probe = room ? (uint32_t)slots : kAggMaxProbe;
     only = bits[cur].as<uint32_t>();
     cur ^= 1;
   }
@@ -1455,17 +1475,33 @@ static int read_back(AggImpl* a, const unsigned long long* counter, unsigned lon
   return TG_OK;
 }
 
+// occupied slots of the group table, the NULL and sentinel groups included (k_agg_count; synchronises the stream)
+static int table_used(AggImpl* a, unsigned long long* sc, unsigned long long& used) {
+  TG_CUDA(cudaMemsetAsync(sc + SC_COUNT, 0, 8, a->stream));
+  k_agg_count<<<grid_size(a->nsm, (int64_t)a->nslots + 2, 256, 8), 256, 0, a->stream>>>(a->tbl, sc + SC_COUNT);
+  a->stats.kernel_launches++;
+  return read_back(a, sc + SC_COUNT, used);
+}
+
+// grow_and_retry's fill and grow for the group table
+static auto table_fill(AggImpl* a, unsigned long long* sc) {
+  return [a, sc](unsigned long long& used, unsigned long long& slots) -> int { slots = a->nslots; return table_used(a, sc, used); };
+}
+static auto table_grow(AggImpl* a) {
+  return [a](unsigned long long nd, bool room) -> int { return room ? TG_OK : grow_table(a, nd); };
+}
+
 // fold `m` partial-result tuples into the global table, growing it until every tuple found a slot
 static int merge_partials(AggImpl* a, const AggPartials& pp, unsigned long long m, unsigned long long* sc) {
   if (m == 0) return TG_OK;
   DevBuf bits[2];
-  return grow_and_retry(a, bits, (int64_t)m, false, "aggregation merge", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+  return grow_and_retry(a, bits, (int64_t)m, false, "aggregation merge", [&](uint32_t* deferred, const uint32_t* only, uint32_t max_probe, unsigned long long& nd) -> int {
     TG_CUDA(cudaMemsetAsync(sc + SC_MERGE_DEFERRED, 0, 8, a->stream));
-    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<grid_size(a->nsm, (int64_t)m, 256, 8), 256, 0, a->stream>>>(pp, (int64_t)m, a->nstates, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_MERGE_DEFERRED);
+    (a->wide ? k_agg_merge<true> : k_agg_merge<false>)<<<grid_size(a->nsm, (int64_t)m, 256, 8), 256, 0, a->stream>>>(pp, (int64_t)m, a->nstates, a->tbl, a->spec, max_probe, deferred, only, sc + SC_MERGE_DEFERRED);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_MERGE;
     return read_back(a, sc + SC_MERGE_DEFERRED, nd);
-  }, [&](unsigned long long nd) { return grow_table(a, nd); });
+  }, table_fill(a, sc), table_grow(a));
 }
 
 // columnar partial-result tuples of `cap` entries in partials_mem: keys, rows, one array per state, kind
@@ -1491,13 +1527,13 @@ static int update_grouped_mk(AggImpl* a, const DevCols& cols, int64_t n, unsigne
   GroupKeys gk{};
   gk.n = (int)a->group_cols.size(); gk.nkw = a->nkw;
   for (int q = 0; q < gk.n; q++) { gk.data[q] = cols.data[a->group_cols[q]]; gk.nulls[q] = cols.nulls[a->group_cols[q]]; gk.kind[q] = a->group_kinds[q]; }
-  return grow_and_retry(a, a->deferred, n, false, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+  return grow_and_retry(a, a->deferred, n, false, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, uint32_t max_probe, unsigned long long& nd) -> int {
     TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
-    (a->wide ? k_agg_update_mk<true> : k_agg_update_mk<false>)<<<grid_size(a->nsm, n, 256, 8), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_DEFERRED);
+    (a->wide ? k_agg_update_mk<true> : k_agg_update_mk<false>)<<<grid_size(a->nsm, n, 256, 8), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, max_probe, deferred, only, sc + SC_DEFERRED);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_MULTI_KEY;
     return read_back(a, sc + SC_DEFERRED, nd);
-  }, [&](unsigned long long nd) { return grow_table(a, nd); });
+  }, table_fill(a, sc), table_grow(a));
 }
 
 // Round-2 update path (agg_update.cuh): one two-level kernel per round; rows / local groups that found no slot are re-run
@@ -1521,19 +1557,30 @@ static int update_grouped_v2(AggImpl* a, const GroupKey& gk, const DevCols& cols
     TG_TRY(alloc_partials(a, (size_t)p.spill_cap, sc + SC_SPILLED, p.spill));
     TG_CUDA(cudaFuncSetAttribute(a->wide ? k_agg_update2<true, true> : k_agg_update2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
-  // local groups of the first round that found no global slot (p.spill): the table grows for them as well, then merges them
+  // local groups of the first round that found no global slot (p.spill): they count as entries of the table's fill, the
+  // table grows for them as well, then merges them; a table with room for them merges them after the last round
   unsigned long long spilled = 0;
-  auto grow = [&](unsigned long long nd) {
-    TG_TRY(grow_table(a, nd + spilled));
+  auto merge_spill = [&]() {
     const unsigned long long m = spilled;
     spilled = 0;
     return merge_partials(a, p.spill, m, sc);
   };
-  TG_TRY(grow_and_retry(a, a->deferred, n, false, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+  auto fill = [&](unsigned long long& used, unsigned long long& slots) -> int {
+    slots = a->nslots;
+    TG_TRY(table_used(a, sc, used));
+    used += spilled;
+    return TG_OK;
+  };
+  auto grow = [&](unsigned long long nd, bool room) -> int {
+    if (room) return TG_OK;
+    TG_TRY(grow_table(a, nd + spilled));
+    return merge_spill();
+  };
+  TG_TRY(grow_and_retry(a, a->deferred, n, false, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, uint32_t max_probe, unsigned long long& nd) -> int {
     const bool lvl = local && !only;   // the CTA-local level runs in the first round
     TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
     TG_CUDA(cudaMemsetAsync(sc + SC_SPILLED, 0, 8, a->stream));
-    p.deferred = deferred; p.only = only;
+    p.deferred = deferred; p.only = only; p.max_probe = max_probe;
     if (lvl) (a->wide ? k_agg_update2<true, true> : k_agg_update2<true, false>)<<<grid, AGG2_BLOCK, smem, a->stream>>>(p, cols, a->tbl, a->spec);
     else (a->wide ? k_agg_update2<false, true> : k_agg_update2<false, false>)<<<grid, AGG2_BLOCK, 0, a->stream>>>(p, cols, a->tbl, a->spec);
     a->stats.kernel_launches++;
@@ -1546,8 +1593,12 @@ static int update_grouped_v2(AggImpl* a, const GroupKey& gk, const DevCols& cols
     if (lvl) spilled = back[SC_SPILLED];
     if (spilled > p.spill_cap) return fail(TG_ERR_CUDA, "internal: aggregation spill buffer overflow");
     return TG_OK;
-  }, grow));
-  return spilled ? grow(0) : TG_OK;
+  }, fill, grow));
+  if (spilled == 0) return TG_OK;
+  unsigned long long used = 0;
+  TG_TRY(table_used(a, sc, used));
+  if (!long_run_not_full(used, spilled, a->nslots)) TG_TRY(grow_table(a, spilled));
+  return merge_spill();
 }
 
 // rows [lo, hi): CTA-local partial aggregation, then merge of the partial results into the global table
@@ -1595,13 +1646,13 @@ static int update_grouped_v1(AggImpl* a, const GroupKey& gk, const DevCols& cols
     if (done < n) TG_TRY(mark_range_deferred(a, done, n));   // the rest of the batch goes through the global kernel
     else if (nd == 0) return TG_OK;
   }
-  return grow_and_retry(a, a->deferred, n, try_local, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+  return grow_and_retry(a, a->deferred, n, try_local, "aggregation table", [&](uint32_t* deferred, const uint32_t* only, uint32_t max_probe, unsigned long long& nd) -> int {
     TG_CUDA(cudaMemsetAsync(sc + SC_DEFERRED, 0, 8, a->stream));
-    (a->wide ? k_agg_update<true> : k_agg_update<false>)<<<grid_size(a->nsm, n, 256, 8), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, kAggMaxProbe, deferred, only, sc + SC_DEFERRED);
+    (a->wide ? k_agg_update<true> : k_agg_update<false>)<<<grid_size(a->nsm, n, 256, 8), 256, 0, a->stream>>>(gk, cols, n, a->tbl, a->spec, max_probe, deferred, only, sc + SC_DEFERRED);
     a->stats.kernel_launches++;
     a->stats.paths |= TG_AGG_PATH_V1_GLOBAL;
     return read_back(a, sc + SC_DEFERRED, nd);
-  }, [&](unsigned long long nd) { return grow_table(a, nd); });
+  }, table_fill(a, sc), table_grow(a));
 }
 
 // aggregate n device-resident rows
@@ -1718,10 +1769,10 @@ static int distinct_mark(AggImpl* a, DevCols& cols, int64_t n) {
     const int c = a->dist_cols[j];
     if (m.t.nslots == 0) TG_TRY(alloc_set(a, std::max<unsigned long long>(1024, (unsigned long long)std::min<int64_t>(n, 1ll << 22) * 2), m.mem, m.t));
     TG_TRY(m.mark.ensure(a->device, (size_t)((n + 31) / 32) * 4 + 16));
-    TG_TRY(grow_and_retry(a, a->deferred, n, false, "DISTINCT set", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+    TG_TRY(grow_and_retry(a, a->deferred, n, false, "DISTINCT set", [&](uint32_t* deferred, const uint32_t* only, uint32_t max_probe, unsigned long long& nd) -> int {
       TG_CUDA(cudaMemsetAsync(cnt, 0, 16, a->stream));
       k_agg_distinct_mark<<<grid_size(a->nsm, n, 256, 8), 256, 0, a->stream>>>(gk, static_cast<const long long*>(cols.data[c]), cols.nulls[c],
-                                                               a->types[c] == TG_TYPE_DOUBLE, n, m.t, kAggMaxProbe, m.mark.as<uint32_t>(),
+                                                               a->types[c] == TG_TYPE_DOUBLE, n, m.t, max_probe, m.mark.as<uint32_t>(),
                                                                deferred, only, cnt);
       a->stats.kernel_launches++;
       a->dstats.launches++;
@@ -1729,9 +1780,11 @@ static int distinct_mark(AggImpl* a, DevCols& cols, int64_t n) {
       TG_CUDA(cudaMemcpyAsync(back, cnt, 16, cudaMemcpyDeviceToHost, a->stream));
       TG_CUDA(cudaStreamSynchronize(a->stream));
       a->dstats.pairs += (int64_t)back[1];
+      m.used += back[1];
       nd = back[0];
       return TG_OK;
-    }, [&](unsigned long long nd) { return grow_set(a, m, grown_slots(m.t.nslots, nd)); }));
+    }, [&](unsigned long long& used, unsigned long long& slots) -> int { used = m.used; slots = m.t.nslots; return TG_OK; },
+    [&](unsigned long long nd, bool room) -> int { return room ? TG_OK : grow_set(a, m, grown_slots(m.t.nslots, nd)); }));
     cols.data[a->ncols + j] = cols.data[c];
     cols.nulls[a->ncols + j] = m.mark.as<uint8_t>();
     cols.elem_len[a->ncols + j] = 8;
@@ -1778,10 +1831,11 @@ static int encode_strings(AggImpl* a, DevCols& cols, const StrColDev* sv, int64_
     unsigned long long* tails = nullptr;
     if (a->tail_col[c] >= 0) { TG_TRY(a->stails[c]->ensure(a->device, (size_t)n * 8 + 16)); tails = a->stails[c]->as<unsigned long long>(); }
     touched = true;   // from the first round on, the dictionary may hold entries of this batch
-    TG_TRY(grow_and_retry(a, a->deferred, n, false, "string dictionary", [&](uint32_t* deferred, const uint32_t* only, unsigned long long& nd) -> int {
+    TG_TRY(grow_and_retry(a, a->deferred, n, false, "string dictionary", [&](uint32_t* deferred, const uint32_t* only, uint32_t max_probe, unsigned long long& nd) -> int {
       a->stats.kernel_launches++;
-      return str_dict_round(d, sv[c], n, a->str_ords, kAggMaxProbe, ids, deferred, only, nd, tails, a->nsm, a->stream);
-    }, [&](unsigned long long nd) { return str_dict_grow(d, nd, a->device, a->nsm, a->stream); }));
+      return str_dict_round(d, sv[c], n, a->str_ords, max_probe, ids, deferred, only, nd, tails, a->nsm, a->stream);
+    }, [&](unsigned long long& used, unsigned long long& slots) -> int { slots = d.nslots; return str_dict_used(d, used, a->stream); },
+    [&](unsigned long long nd, bool room) -> int { return str_dict_grow(d, nd, room, a->device, a->nsm, a->stream); }));
     if (tails) {
       bool wide = false;
       TG_TRY(str_dict_tail_overflow(d, wide, a->stream));
@@ -1880,11 +1934,7 @@ static int afinalize(AggImpl* a) {
     a->nslots = 1024;
   }
   unsigned long long fill = 0;
-  TG_CUDA(cudaMemsetAsync(sc + SC_COUNT, 0, 8, a->stream));
-  k_agg_count<<<grid_size(a->nsm, (int64_t)a->nslots + 2, 256, 8), 256, 0, a->stream>>>(a->tbl, sc + SC_COUNT);
-  a->stats.kernel_launches++;
-  TG_CUDA(cudaMemcpyAsync(&fill, sc + SC_COUNT, 8, cudaMemcpyDeviceToHost, a->stream));
-  TG_CUDA(cudaStreamSynchronize(a->stream));
+  TG_TRY(table_used(a, sc, fill));
   int64_t cap = (int64_t)fill + 2 + 1;
   AggOut ao{};
   for (int k = 0; k < nf; k++) {

@@ -337,12 +337,19 @@ int str_dict_tail_overflow(StrDict& d, bool& overflow, cudaStream_t s) {
   return TG_OK;
 }
 
-int str_dict_grow(StrDict& d, unsigned long long more, int device, int nsm, cudaStream_t s) {
+int str_dict_used(StrDict& d, unsigned long long& used, cudaStream_t s) {
+  unsigned long long back[8];
+  TG_TRY(read_counters(d, back, s));
+  used = back[0];
+  return TG_OK;
+}
+
+int str_dict_grow(StrDict& d, unsigned long long more, bool room, int device, int nsm, cudaStream_t s) {
   unsigned long long back[8];
   TG_TRY(read_counters(d, back, s));
   // entries deferred for want of per-id room: x4 arrays (the new entries of this batch, ctr[0], are kept)
   if (back[1] > back[5]) TG_TRY(grow_ids(d, std::max<size_t>(d.id_cap * 4, (size_t)back[0] + 1024), (size_t)back[0], device, s));
-  if (back[5] == 0) return TG_OK;   // no probe ran past its limit: the table has room
+  if (back[5] == 0 || room) return TG_OK;   // no probe ran past its limit, or one did in a table with room
   // x4, or more: at most half full once `more` new entries join
   const unsigned long long want = std::max<unsigned long long>(d.nslots * 4, (back[0] + more) * 2);
   DevBuf nm;

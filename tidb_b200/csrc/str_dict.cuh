@@ -54,9 +54,13 @@ int str_dict_round(StrDict& d, const StrColDev& c, int64_t n, int64_t ord0, uint
 // true when the last batch's tails had a trailing-space count that does not fit kTailBits
 int str_dict_tail_overflow(StrDict& d, bool& overflow, cudaStream_t s);
 
-// after a round deferred rows: x4 room in the per-id arrays when new entries found none, and a rehash into a table x4
-// bigger, or half full with `more` new entries, when a probe ran past its limit
-int str_dict_grow(StrDict& d, unsigned long long more, int device, int nsm, cudaStream_t s);
+// the entries the table holds, this batch's new ones included
+int str_dict_used(StrDict& d, unsigned long long& used, cudaStream_t s);
+
+// after a round deferred rows: x4 room in the per-id arrays when new entries found none, and, unless the table has room
+// (the next round walks it without a probe limit), a rehash into a table x4 bigger, or half full with `more` new
+// entries, when a probe ran past its limit
+int str_dict_grow(StrDict& d, unsigned long long more, bool room, int device, int nsm, cudaStream_t s);
 
 // after the last round: each new entry takes the raw bytes of its earliest row of the batch into the arena, so that no
 // entry points into the batch's buffers any more
